@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- poses/s of the SAM-6D pose-estimation matching path on B200 (BASELINE.json config #2).
+"""bench.py -- poses/s of the SAM-6D pose-estimation matching path on H100 (BASELINE.json config #2).
 
 A step = one pass of the hot path (Net.forward after the RGB backbone: FPS, geometric embedding, coarse and fine
 sparse-to-dense point matching, pose solvers) over one batch of 32 synthetic proposals x 2048 scene points x 2048 template
@@ -7,6 +7,7 @@ points, 256-d features, 1024 CAD samples.  Under torchrun every rank runs the sa
 sharded, no data-path collective) and the step ends with the one all-gather of final poses.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]          our arm
+  python bench.py ... --dump-outputs DIR                        also write the last timed step's outputs as DIR/<name>.npy
   python bench.py --impl reference ...                          the reference algorithm on the host cores (oracle port)
 """
 import argparse
@@ -34,11 +35,12 @@ def peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return dict(hbm=d["hbm_gbs"], tensor=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm=6650.0, tensor=1400.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s
+    return dict(hbm=3350.0, tensor=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons during the timed region (B200_PROFILING.md recipe).  NVML when it is importable (a query
+    """SM clock and throttle reasons during the timed region.  NVML when it is importable (a query
     takes ~1 ms, so a 100 ms timed region still gets tens of samples), else the nvidia-smi command line every 0.2 s."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -133,7 +135,7 @@ def cpu_oracle_throughput(reps: int, threads: int, nprop: int = 0):
 
 
 def same_box_reference(dev, B):
-    """SURVEY.md 8(d) / 2.3: the reference formulation on the SAME B200 -- (i) the reference algorithm (oracle port: the
+    """SURVEY.md 8(d) / 2.3: the reference formulation on the SAME GPU -- (i) the reference algorithm (oracle port: the
     reference's own torch ops) on .cuda() with the reference's own pointnet2 CUDA kernels (oracle/_ref) underneath, as
     `ref_gpu_poses_per_s`; (ii) the reference `_ext` FPS / ball-query kernels timed next to ours on the bench shapes.
     Checker / baseline code only: nothing here is on the product path."""
@@ -379,7 +381,7 @@ def run_ism(args):
                 e2e=dict(value=F_ * args.steps / (ms_e2e * 1e-3), unit="frames/s", h2d_bytes_per_step=host[0].numel() * 4 + qh.numel() * 4,
                          d2h_bytes_per_step=F_ * 256 * 4 + F_ * P * 8),
                 gpu_launches=launches,
-                roofline=dict(kernel="whole encoder (tcgen05 GEMMs + attention)", bound="tensor", achieved=ach, peak=pk["tensor"], unit="TFLOP/s",
+                roofline=dict(kernel="whole encoder (wgmma GEMMs + attention)", bound="tensor", achieved=ach, peak=pk["tensor"], unit="TFLOP/s",
                               frac=ach / pk["tensor"], traffic=None, peak_source=pk["source"] + " bf16_tflops_sustained"))
     if not args.no_cpu_baseline:
         from oracle import sam_oracle as so                # CPU leg only: the oracle port is the thing timed here
@@ -395,6 +397,26 @@ def run_ism(args):
     print(json.dumps(line))
 
 
+DUMP_LIMIT = 64 << 20          # bytes written by --dump-outputs in all
+
+
+def dump_outputs(path, arrays):
+    """arrays (name -> tensor) as path/<name>.npy in float32 (float64 for float64 tensors); an array that would take the
+    total past DUMP_LIMIT is replaced by a fixed, seeded sample of its flattened elements, in ascending index order"""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    items = sorted(arrays.items())
+    budget = DUMP_LIMIT // max(1, len(items))
+    for name, t in items:
+        a = t.detach().cpu()
+        a = a.double() if a.dtype == torch.float64 else a.float()
+        a = a.numpy()
+        if a.nbytes > budget:
+            keep = np.sort(np.random.default_rng(0).choice(a.size, budget // a.itemsize, replace=False))
+            a = a.reshape(-1)[keep]
+        np.save(os.path.join(path, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -407,14 +429,18 @@ def main():
     ap.add_argument("--no-graph", action="store_true",
                     help="launch every kernel of a step one by one instead of replaying the captured step (Net.enable_graphs)")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"],
-                    help="bf16: tcgen05 tensor-core kernels (bf16 operands, fp32 accumulate); fp32: CUDA-core exact path")
+                    help="bf16: wgmma tensor-core kernels (bf16 operands, fp32 accumulate); fp32: CUDA-core exact path")
     ap.add_argument("--rgb", action="store_true",
                     help="PEM workload including the RGB branch (SURVEY 8f row N1): ViT-B/16 features of 224x224 crops + pixel "
                          "gather replace the given dense_fm; not the BASELINE configuration, reported as its own workload name")
     ap.add_argument("--workload", default="pem", choices=["pem", "ism", "ycbv", "lmo"],
                     help="pem: BASELINE config #2 (headline); ism: config #3, SAM ViT-H encoder + template scoring; ycbv / lmo: "
                          "configs #5 / #4, strong scaling of one fixed frame set over the ranks")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="pem workload: write the arrays Net.forward returned in the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "pem"):
+        ap.error("--dump-outputs applies to the pem workload of our arm")
     if args.impl == "reference":
         return run_reference(args)
     if args.workload == "ism":
@@ -465,10 +491,13 @@ def main():
     h2d_bytes = sum(v.numel() * v.element_size() for v in host[0].values())
     gen = torch.Generator(device=dev).manual_seed(1 + rank)
 
+    last = {}
+
     def step_resident(i):
         ep = dict(resident[i % 2])
         rand = torch.rand(B, synth.N_PROPOSAL1 * 3, device=dev, generator=gen)
         out = net(ep, rand=rand)
+        last["out"] = {k: v for k, v in out.items() if k not in resident[i % 2]}    # what the forward added: the poses and scores
         poses = sdist.pack_poses(out)
         return sdist.all_gather_poses(poses)
 
@@ -553,6 +582,8 @@ def main():
     if sampler:
         sampler.start()
     ms, launches, _ = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])       # now: later runs replay into the same graph output buffers
     # dominant-kernel roofline: same steps again with CUDA events around every launch of the kernels the roofline report names
     # (the stream over E; the attention kernel that consumes its scores; the geometric-embedding kernel that writes E)
     from sam6d_b200 import pem as _pem
@@ -620,24 +651,18 @@ def main():
                                 achieved=geo_bytes / (lut_ms * 1e-3) / 1e9, peak=pk["hbm"], unit="GB/s",
                                 frac=geo_bytes / (lut_ms * 1e-3) / 1e9 / pk["hbm"], avg_launch_ms=lut_ms,
                                 algorithmic_bytes_per_launch=geo_bytes, share_of_step=sum(lut) / ms,
-                                note="replaces the tcgen05 projections (977 GFLOP min per step, 1.30 ms = 0.53 of the sustained bf16 rate): "
-                                     "the projected embedding of one scalar is tabulated, so the flops are gone rather than run faster")
+                                note="replaces the tensor-core projections (977 GFLOP min per step): the projected embedding of one "
+                                     "scalar is tabulated, so the flops are gone rather than run faster")
         value = world * B * args.steps / (ms * 1e-3)
         e2e_val = world * B * args.steps / (ms_e2e * 1e-3)
         traffic = None
-        prof = os.path.join(ROOT, "profiles", "rpe_scores_traffic.json")
-        if os.path.exists(prof):
-            rec = json.load(open(prof)).get("bf16" if args.precision == "bf16" else "fp32", {})
-            traffic = rec.get("dram_bytes_per_launch")
-            if traffic is not None and rec.get("clouds_per_launch", B) != clouds:      # ncu capture of another launch shape
-                traffic = None
         line = dict(
             metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=n_warm, warmup_run=n_warm_run,
             ms_per_step=ms / args.steps, higher_is_better=True, scaling="weak", vs_baseline=None,
             dtype="bf16" if args.precision == "bf16" else "f32", data="synthetic",
             config=dict(workload=WORKLOAD + ("+vitb_rgb_branch" if args.rgb else ""), proposals_per_gpu=B, scene_points=N_PTS, template_points=N_PTS, sparse_points=net.coarse_npoint,
                         feat_dim=C_FEAT, model_points=N_MODEL, parallelism=f"proposal-sharded x{world}, 1 all-gather of poses",
-                        cache="inputs+intermediates per step (>1 GB) exceed the 126 MB L2; two input sets alternate",
+                        cache="inputs+intermediates per step (>1 GB) exceed the 50 MB L2; two input sets alternate",
                         launch=(f"one CUDA-graph replay per step ({launches // args.steps} kernels each, captured from Net.forward; "
                                 f"{step_graphs.captures} graphs, {step_graphs.replays} replays in this run)") if graphs and step_graphs
                         else "kernel by kernel"),
@@ -646,7 +671,7 @@ def main():
             gpu_launches=launches,
             roofline=dict(kernel=f"{rpe_name[6:]} ({'bf16' if args.precision == 'bf16' else 'fp32'} E; PEM RPE attention, streams the geometric embedding)", bound="hbm",
                           achieved=achieved, peak=pk["hbm"], unit="GB/s", frac=achieved / pk["hbm"], traffic=traffic,
-                          peak_source=pk["source"] + " (MEASURED_PEAKS.json hbm_gbs)" if pk["source"] == "measured" else "fallback 6650 GB/s",
+                          peak_source=pk["source"] + " (MEASURED_PEAKS.json hbm_gbs)" if pk["source"] == "measured" else pk["source"],
                           algorithmic_bytes_per_launch=alg_bytes, clouds_per_launch=clouds, launches_timed=len(kms), avg_launch_ms=k_avg_ms,
                           share_of_step=sum(kms) / ms,
                           attention_frac=attention_frac, attention_avg_ms=(k_avg_ms + att_avg_ms) if att_avg_ms else None,

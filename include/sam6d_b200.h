@@ -1,5 +1,5 @@
 /*
- * sam6d_b200.h -- C ABI of libsam6d_b200.so: the B200 (sm_100a) kernels behind SAM-6D's data-parallel hot path.
+ * sam6d_b200.h -- C ABI of libsam6d_b200.so: the H100 (sm_90a) kernels behind SAM-6D's data-parallel hot path.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer owned by the caller (the Python host passes torch storage);
@@ -63,14 +63,14 @@ int sam6d_gemm_f32(const float* A, const float* W, const float* bias, const floa
                    long long lda, long long ldw, long long ldc, long long ldr, int batch, long long sA, long long sW,
                    long long sC, long long sR, float alpha, int relu, void* stream);
 
-/* Same contract on the 5th-gen tensor cores: bf16 operands (dtype code 0 = fp32 converted while staging, 1 = bf16), fp32
- * accumulation in TMEM (tcgen05.mma M128 N256 K16), C fp32 (0) or bf16 (1).  K % 8 == 0, 16-byte aligned operand rows. */
+/* Same contract on the tensor cores: bf16 operands (dtype code 0 = fp32 converted while staging, 1 = bf16), fp32
+ * accumulation in registers (wgmma m64n256k16), C fp32 (0) or bf16 (1).  K % 8 == 0, 16-byte aligned operand rows. */
 int sam6d_gemm_bf16(const void* A, int a_dtype, const void* W, int w_dtype, const float* bias, const float* R, void* C,
                     int c_dtype, int M, int N, int K, long long lda, long long ldw, long long ldc, long long ldr, int batch,
                     long long sA, long long sW, long long sC, long long sR, float alpha, int relu, void* stream);
 
 /* Persistent TMA-fed version for plain (non-batched) bf16 operands: cp.async.bulk.tensor boxes with SWIZZLE_128B feed a
- * 4-stage ring, two TMEM accumulators overlap epilogue and MMA.  A (M,K) bf16, W (N,K) bf16, C fp32 (0) / bf16 (1). */
+ * 4-stage ring consumed by two wgmma warpgroups.  A (M,K) bf16, W (N,K) bf16, C fp32 (0) / bf16 (1). */
 int sam6d_gemm_tma(const void* A, const void* W, const float* bias, const void* R, void* C, int c_dtype, int M, int N, int K,
                    long long lda, long long ldw, long long ldc, long long ldr, float alpha, int act, void* stream);
 /* `batch` independent problems stacked along the rows of A and W (problem z: rows [z*a_rpb, +M) of A, [z*w_rpb, +N) of W,
@@ -126,7 +126,7 @@ int sam6d_geo_indices(const float* pts, int b, int S, float sigma_d, float facto
 int sam6d_geo_embed_f32(const float* T, long long npairs, const float* div_term, const float* WaT, const float* WdT,
                         const float* bias, float* E, void* stream);
 
-/* tensor-core version (tcgen05, bf16 operands, fp32 accumulate): Wa/Wd are the (out,in) weights in bf16, E fp32 (0) or bf16 (1) */
+/* tensor-core version (wgmma, bf16 operands, fp32 accumulate): Wa/Wd are the (out,in) weights in bf16, E fp32 (0) or bf16 (1) */
 int sam6d_geo_embed_tc(const float* T, long long npairs, const float* div_term, const void* Wa_bf16, const void* Wd_bf16,
                        const float* bias, void* E, int e_is_bf16, void* stream);
 /* the distance projection of sam6d_geo_embed_tc alone: T (npairs,4) f32 -> E (npairs,256) bf16 = proj_d(emb(T[:,3])) + bias */
@@ -227,7 +227,7 @@ int sam6d_sam_nms(const float* boxes, int N, float thr, unsigned char* keep, voi
 
 /* out = LN2(y + relu(y We^T + be) Ws^T + bs),  y = LN1(hid Wo^T + bo + x): AttentionLayer / RPEAttentionLayer tail and
  * AttentionOutput of PEM/model/transformer.py:176-197, 435-438 (and LinearAttentionLayer / LinearTransformerLayer :575-608)
- * as one persistent TMA + tcgen05 kernel.  hid, x, out (M,256) bf16 with row strides ld_* (multiples of 8); Wo (256,256),
+ * as one persistent TMA + wgmma kernel.  hid, x, out (M,256) bf16 with row strides ld_* (multiples of 8); Wo (256,256),
  * We (512,256), Ws (256,512) bf16 row-major; bo, g1, b1, bs, g2, b2 (256) and be (512) f32; 16-byte aligned pointers. */
 int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const void* x, long long ld_x, const void* Wo, const float* bo,
                                 const float* g1, const float* b1, const void* We, const float* be, const void* Ws, const float* bs,
@@ -238,7 +238,7 @@ int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const void* x
 /* relative-position score term of RPEMultiHeadAttention (PEM/model/transformer.py:389-394) with proj_p folded into
  * the query: E (B,S,S,256) f32 or bf16, U (B*S rows of 4x256, row stride u_ld) = W_p,h^T q_h  ->  SP (B,4,S,S) */
 int sam6d_rpe_scores(const void* E, int e_is_bf16, const float* U, long long u_ld, int B, int S, float* SP, void* stream);
-/* the same term on TMA + tcgen05 (bf16 path, the HBM-bound stream over E): E (B,S,S,256) bf16, U (B*S, 4*256) bf16
+/* the same term on TMA + wgmma (bf16 path, the HBM-bound stream over E): E (B,S,S,256) bf16, U (B*S, 4*256) bf16
  * contiguous, S <= 200  ->  SP (B,4,S,S) f32 */
 int sam6d_rpe_scores_tc(const void* E, const void* U, int B, int S, float* SP, void* stream);
 /* the same with padded score rows: SP (B,4,S,sp_ld), sp_ld >= S; with sp_ld a multiple of 4 sam6d_attn_tc_bias_ld streams it */
@@ -247,16 +247,16 @@ int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, float* SP
 int sam6d_mha(const float* Q, long long q_ld, long long q_bs, const float* K, long long k_ld, long long k_bs, const float* V,
               long long v_ld, long long v_bs, const float* bias, int B, int H, int Sq, int Sk, float scale, float* O,
               long long o_ld, long long o_bs, void* stream);
-/* Tensor-core attention for <= 256 keys (tcgen05 QK^T and PV, TMA-fed, whole score row in TMEM; csrc/attn_tc.cu):
+/* Tensor-core attention for <= 256 keys (wgmma QK^T and PV, TMA-fed, whole score row in registers; csrc/attn_tc.cu):
  * Q / K bf16 column slices of row-major matrices, Vt = V^T per (batch, head) as bf16 (B*H*D, vt_ld) rows; bias_mode 0 none,
  * 1 dense fp32 (B,H,Sq,Sk) [PEM rel-pos scores], 2 decomposed rel-pos [SAM windows; rel_h = both tables pre-packed as bf16
- * UMMA slabs, see ops.pack_rel_pos]; bv value bias (H*D) or NULL. */
+ * wgmma slabs, see ops.pack_rel_pos]; bv value bias (H*D) or NULL. */
 int sam6d_attn_tc(const void* Q, long long q_ld, int q_col0, const void* K, long long k_ld, int k_col0, const void* Vt,
                   long long vt_ld, int B, int H, int Sq, int Sk, int head_dim, int bias_mode, const float* bias,
                   const void* rel_h, const float* rel_w, int Hs, int Ws, const float* bv, float scale, void* out,
                   int out_is_bf16, long long out_ld, void* stream);
 /* sam6d_attn_tc (head dim 64) with a dense fp32 bias in padded planes (B,H,Sq,bias_ld), bias_ld >= Sk a multiple of 4 floats,
- * 16-byte aligned base: the bias tiles stream through cp.async four chunks ahead of the softmax (RPEMultiHeadAttention,
+ * 16-byte aligned base: the bias is read as aligned column pairs (RPEMultiHeadAttention,
  * PEM/model/transformer.py:395-399) */
 int sam6d_attn_tc_bias_ld(const void* Q, long long q_ld, int q_col0, const void* K, long long k_ld, int k_col0, const void* Vt,
                           long long vt_ld, int B, int H, int Sq, int Sk, int head_dim, const float* bias, long long bias_ld,
@@ -278,8 +278,8 @@ int sam6d_linattn_kv(const float* Kf, long long k_ld, long long k_bs, const floa
                      int H, int J, float* KV, float* KS, void* stream);
 int sam6d_linattn_apply(const float* Qf, long long q_rpb, long long q_bs, long long q_ld, const float* KV, const float* KS,
                         int B, int H, float* X, long long x_bs, long long x_ld, void* stream);
-/* The same branch for the dense tokens on tcgen05 (bf16 tokens).  linattn_kv_pack: focused keys Kf and values V ((B,J,256)
- * fp32 views) -> blob = per cloud the bf16 UMMA image of KV_h^T (4 x [64][64], 128-byte swizzle; B x 32 KB) and KS (B,4,64).
+/* The same branch for the dense tokens on wgmma (bf16 tokens).  linattn_kv_pack: focused keys Kf and values V ((B,J,256)
+ * fp32 views) -> blob = per cloud the bf16 wgmma image of KV_h^T (4 x [64][64], 128-byte swizzle; B x 32 KB) and KS (B,4,64).
  * linattn_tc: Q = B clouds x rpb rows x 256 bf16 (row stride q_ld, cloud stride q_bs), the raw query projection; applies the focusing feature map (transformer.py:541-550),
  * X[b,i,h] = (q'_h KV_h) / (q'_h . KS_h + 1e-6), bf16. */
 int sam6d_linattn_kv_pack(const float* Kf, long long k_ld, long long k_bs, const float* V, long long v_ld, long long v_bs, int B,
@@ -302,7 +302,7 @@ int sam6d_coarse_select(const float* Rt, const int* top, int B, int n1, int n2, 
 int sam6d_pe_mlp_max(const float* pts, const int* idx, const int* cnt, int B, int N, int ns, const float* W1,
                      const float* B1, const float* W2, const float* B2, const float* W3, const float* B3, float* out,
                      int out_ld, int out_off, void* stream);
-/* tensor-core version: layers 2 and 3 on tcgen05 (W2 (64,32), W3 (128,64) bf16), max-pool in the TMEM epilogue */
+/* tensor-core version: layers 2 and 3 on wgmma (W2 (64,32), W3 (128,64) bf16), max-pool in the register epilogue */
 int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, int ns, const float* W1, const float* B1,
                         const void* W2_bf16, const float* B2, const void* W3_bf16, const float* B3, void* out, int out_is_bf16,
                         int out_ld, int out_off, void* stream);
@@ -310,8 +310,8 @@ int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, int ns, 
  * ld % 4 == 0, 16-byte aligned rows, S >= 97; scratch rsum/csum (B,ld), cpart/cpi (B,ceil(S/32),ld). */
 int sam6d_fine_assign(const float* A, int B, int S, int ld, float shift, const float* pts2, float* rsum, float* csum, float* cpart,
                       int* cpi, int* lab1, int* lab2, float* wts, float* pred, void* stream);
-/* The same assignment without the (B,S,S) score matrix (bf16 path): every pass recomputes its score tiles on tcgen05 from the
- * L2-normalised bf16 tokens Fa (rows) and Fb (columns), both (B*S, 256), and reduces them in TMEM.
+/* The same assignment without the (B,S,S) score matrix (bf16 path): every pass recomputes its score tiles on wgmma from the
+ * L2-normalised bf16 tokens Fa (rows) and Fb (columns), both (B*S, 256), and reduces them in registers.
  * mode 0: out_inv (B,ld_f) = 1 / sum_j exp(alpha <a_i,b_j> - shift);  mode 1: lab (B,S) = argmax_j (e*row_f_i)*(e*col_f_j);
  * mode 2: mode 1 plus wts (B,S-1), pred (B,S-1,3) for rows >= 1 from q4 (B,ld_f) float4 (sam6d_fine_masked_points).
  * compute_fine_Rt = mode 0 on (F1,F2) and (F2,F1), mode 1 on (F2,F1) [column labels], masked points, mode 2 on (F1,F2). */
@@ -336,9 +336,9 @@ int sam6d_bilinear_gather(const void* up, int up_is_bf16, const long long* choos
 int sam6d_attn_relpos(const float* qkv, long long tok_ld, int nW, int Hs, int Ws, int nH, int head_dim, const float* rel_h,
                       const float* rel_w, float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
 
-/* Global-attention blocks (64 x 64 token grid, 4096 keys, head_dim 80) on tcgen05 with an online softmax: qkv bf16
+/* Global-attention blocks (64 x 64 token grid, 4096 keys, head_dim 80) on wgmma with an online softmax: qkv bf16
  * (B*4096, ld) rows [q|k|v]; Vt = V^T per (image, head) from sam6d_transpose_tokens_bf16 (B*H*80 rows, vt_ld >= 4096);
- * rel_blob = rel_pos_h, rel_pos_w ((127,80) each) packed as bf16 UMMA slabs of 128 rows (ops.pack_rel_pos(.., slab_rows=128));
+ * rel_blob = rel_pos_h, rel_pos_w ((127,80) each) packed as bf16 wgmma slabs of 128 rows (ops.pack_rel_pos(.., slab_rows=128));
  * out (B*4096, H*80) fp32 / bf16.  image_encoder.py:224-240 (attention), 325-361 (add_decomposed_rel_pos). */
 int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H, int grid,
                          float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
@@ -348,7 +348,7 @@ int sam6d_template_score(const float* Qn, const float* Rn, int P, int O, int T, 
                          int* best_obj, float* best_score, int* best_tmpl, void* stream);
 
 /* ---- library info ------------------------------------------------------------------------------------------------- */
-/* "sam6d_b200 <version> sm_100a" */
+/* "sam6d_b200 <version> sm_90a" */
 const char* sam6d_version(void);
 
 #ifdef __cplusplus

@@ -1,12 +1,13 @@
 """oracle/build_ref_ext.py -- TEST INFRASTRUCTURE ONLY.
 
 Compiles the REFERENCE's own PointNet++ CUDA extension (pointnet2._ext) from the sources where they lie under
-/root/reference, into oracle/_ref/ (git-ignored; travels to the GPU box with the snapshot).  No reference source is copied
-into this repository.  tests/test_gpu_pn2_ref.py loads the resulting module on the GPU box and uses it to pin both the C
-restatement (oracle/pn2_oracle.c) and the sam6d_b200 kernels against the reference kernels' actual outputs.
+/root/reference, into oracle/_ref/ (git-ignored).  No reference source is copied into this repository.
+tools/make_golden_pn2.py runs the resulting module on a GPU and stores the reference kernels' outputs in tests/golden/pn2_ref.pt,
+against which tests/test_gpu_pn2_ref.py pins both the C restatement (oracle/pn2_oracle.c) and the sam6d_b200 kernels; bench.py
+times it next to ours when it is present.
 
 The reference's setup.py does not build as shipped (relative include_dirs, PEM/model/pointnet2/setup.py:23), so this is our
-own recipe: torch.utils.cpp_extension.load with an absolute include path and an sm_100 target.
+own recipe: torch.utils.cpp_extension.load with an absolute include path and an sm_90 target.
 """
 import glob
 import os
@@ -28,7 +29,7 @@ def build():
     if not os.path.isdir(SRC):
         raise RuntimeError("reference sources not present (this only builds in the dev container)")
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     from torch.utils.cpp_extension import load
     srcs = sorted(glob.glob(os.path.join(SRC, "src", "*.cpp")) + glob.glob(os.path.join(SRC, "src", "*.cu")))
     load(name=NAME, sources=srcs, extra_include_paths=[os.path.join(SRC, "include")], build_directory=OUT,

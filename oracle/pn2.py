@@ -41,9 +41,9 @@ _ref_mod = None
 
 
 def _ref():
-    """CUDA tensors go to the REFERENCE's own kernels (oracle/_ref/pointnet2_ref_ext.so, built from /root/reference by
-    oracle/build_ref_ext.py): the oracle port then runs on the GPU exactly as the reference would ("reference on the same
-    B200" line of bench.py)."""
+    """CUDA tensors go to the REFERENCE's own kernels (oracle/_ref/pointnet2_ref_ext.so, built from the reference sources by
+    oracle/build_ref_ext.py): the oracle port then runs on the GPU exactly as the reference would (the same-box reference
+    line of bench.py)."""
     global _ref_mod
     if _ref_mod is None:
         from . import build_ref_ext

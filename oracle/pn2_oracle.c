@@ -7,7 +7,7 @@
  * supported")), so this file restates the *algorithm* of each kernel in plain
  * C, including the floating-point expression order the reference compiles to
  * (nvcc -fmad=true contracts  a*a + b*b + c*c  into  fma(c,c, fma(b,b, a*a));
- * verified in the sm_100a SASS of the reference kernel: FMUL, FFMA, FFMA).
+ * the contraction nvcc applies to the reference kernel: FMUL, FFMA, FFMA).
  *
  * Reference (paths relative to SAM-6D/Pose_Estimation_Model/model/pointnet2):
  *   fps          : _ext_src/src/sampling_gpu.cu:75-178  (+ host temp init 1e10, sampling.cpp:78-80)

@@ -1,4 +1,4 @@
-"""sam6d_b200 -- B200-native (sm_100a) implementation of SAM-6D's data-parallel hot path.
+"""sam6d_b200 -- H100-native (sm_90a) implementation of SAM-6D's data-parallel hot path.
 
     from sam6d_b200.pem import Net                       # drop-in for Pose_Estimation_Model `Net`
     import sam6d_b200.pointnet2_ext as _ext              # drop-in for pointnet2._ext (forward ops)

@@ -1,4 +1,4 @@
-"""Build libsam6d_b200.so in-tree with nvcc for sm_100a (one translation unit per .cu, linked into one C-ABI library)."""
+"""Build libsam6d_b200.so in-tree with nvcc for sm_90a (one translation unit per .cu, linked into one C-ABI library)."""
 import hashlib
 import os
 import subprocess
@@ -11,8 +11,9 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libsam6d_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + [
+    "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 
@@ -55,7 +56,7 @@ def build(verbose: bool = False) -> str:
         res = list(ex.map(_compile, _sources()))
     objs = [o for o, _ in res]
     if any(changed for _, changed in res) or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH + ["-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

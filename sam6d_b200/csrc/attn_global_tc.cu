@@ -1,17 +1,17 @@
 // attn_global_tc.cu -- SAM ViT global attention (64 x 64 = 4096 tokens per image, head dim 80, decomposed relative-position
-// bias) on tcgen05 with an online softmax (ISM/segment_anything/modeling/image_encoder.py:224-240, 325-361).
+// bias) on wgmma with an online softmax (ISM/segment_anything/modeling/image_encoder.py:224-240, 325-361).
 //
 //     O = softmax(scale * Q K^T + Rh[q, kh] + Rw[q, kw]) V,     Rh[q, kh] = q . rel_h[qh - kh + 63], Rw likewise (unscaled q)
 //
 // One CTA per (128-query tile = two rows of the token grid, head, image); it walks the 32 key tiles of 128 keys:
-//   warp 5  TMA      : Q once; K tiles and V^T tiles into two independent 2-deep rings (K is released by the score MMA, V by the
-//                      value MMA, so the next K tile arrives a whole tile early)
-//   warp 4  MMA      : G_w = Q rel_w^T, G_h = Q rel_h^T (once), then per key tile S_j = Q K_j^T into one of two 128-column TMEM
-//                      accumulators and O_j = P_j V_j into a third; S_{j+2} is issued as soon as P_j is published
-//   warps 0-3 softmax: thread = query row.  The bias tables come out of G_w / G_h once per CTA (the row's 64 Rw values stay in
-//                      registers, Rh in shared memory); per tile: max pass, exp2 pass writing P_j as bf16 straight into the
-//                      swizzled A slabs, and o = o * alpha + O_{j-1} in registers (no accumulator rescaling in TMEM)
-// The reference materialises a (16 x 4096 x 4096) fp32 score tensor per image and block; here scores never leave TMEM.
+//   warp 8     TMA      : (one thread of warpgroup 2) Q and the rel tables once; then K tiles and V^T tiles into two independent 2-deep rings (the rel
+//                         tables occupy the K ring and the bias scratch the V ring / P slabs until the bias tables are built)
+//   warps 0-7  two warpgroups, warpgroup g owns queries [64 g, 64 g + 64) (one row of the token grid):
+//                G_w = Q rel_w^T, G_h = Q rel_h^T (once) -> the row's 32 Rw values of its key columns in registers, Rh in
+//                shared memory; per key tile: S_j = Q K_j^T (wgmma m64n128k16, 64 registers), row max / exp2 in registers
+//                (rows live in quads), o = o * alpha in registers, P_j as bf16 into the swizzled A slabs, o += P_j V_j
+//                (wgmma m64n80k16, 40 registers)
+// The reference materialises a (16 x 4096 x 4096) fp32 score tensor per image and block; here scores never leave registers.
 #include <cuda.h>
 
 #include "epilogue.cuh"
@@ -20,14 +20,15 @@
 namespace {
 
 constexpr int QT = 128, KT = 128, D = 80, GRID = 64;
-constexpr int NUM_THREADS = 192;
+constexpr int CONSUMERS = 256, NUM_THREADS = CONSUMERS + 128;
 constexpr int Q_SLAB = QT * 128, K_SLAB = KT * 128, V_SLAB = D * 128, P_SLAB = QT * 128, REL_SLAB = 128 * 128;
-constexpr int OFF_Q = 0, OFF_K0 = OFF_Q + 2 * Q_SLAB, OFF_V0 = OFF_K0 + 2 * K_SLAB, OFF_K1 = OFF_V0 + 2 * V_SLAB,
-              OFF_V1 = OFF_K1 + 2 * K_SLAB, OFF_P = OFF_V1 + 2 * V_SLAB, OFF_TABH = OFF_P + 2 * P_SLAB;
-constexpr int TABH_LD = 65, SCR_LD = 129;
+constexpr int OFF_Q = 0, OFF_K0 = OFF_Q + 2 * Q_SLAB, OFF_K1 = OFF_K0 + 2 * K_SLAB, OFF_V0 = OFF_K1 + 2 * K_SLAB,
+              OFF_V1 = OFF_V0 + 2 * V_SLAB, OFF_P = OFF_V1 + 2 * V_SLAB, OFF_TABH = OFF_P + 2 * P_SLAB;
+constexpr int TABH_LD = 64, SCR_LD = 128;
 constexpr int SMEM_BYTES = OFF_TABH + QT * TABH_LD * 4 + 1024;
-static_assert(OFF_K1 % 1024 == 0 && OFF_V1 % 1024 == 0 && OFF_P % 1024 == 0, "UMMA slabs must be 1024-byte aligned");
-static_assert(OFF_TABH - OFF_K1 >= QT * SCR_LD * 4 && OFF_TABH - OFF_K1 >= 4 * REL_SLAB, "scratch / rel tables alias K1..P");
+static_assert(OFF_K1 % 1024 == 0 && OFF_V0 % 1024 == 0 && OFF_V1 % 1024 == 0 && OFF_P % 1024 == 0, "slabs must be 1024-byte aligned");
+static_assert(OFF_K1 + 2 * K_SLAB - OFF_K0 >= 4 * REL_SLAB, "the rel tables occupy the K ring");
+static_assert(OFF_TABH - OFF_V0 >= QT * SCR_LD * 4, "the bias scratch occupies the V ring and the P slabs");
 constexpr float LOG2E = 1.4426950408889634f;
 
 __device__ __forceinline__ float ex2(float x) {
@@ -37,24 +38,23 @@ __device__ __forceinline__ float ex2(float x) {
 }
 
 struct GArgs {
-  const void* rel_blob;   // rel_h, rel_w as bf16 UMMA B slabs: 2 tables x 2 slabs x [128 rows][64 ch], SWIZZLE_128B
+  const void* rel_blob;   // rel_h, rel_w as bf16 wgmma B slabs: 2 tables x 2 slabs x [128 rows][64 ch], SWIZZLE_128B
   void* out; long long out_ld;
   int H;
   float scale;
 };
 
 template <typename OT>
-__global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __grid_constant__ CUtensorMap tmQK,
-                                                                        const __grid_constant__ CUtensorMap tmVt, GArgs a) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt,
+                                                       GArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* q_s = smem + OFF_Q;
   uint8_t* p_s = smem + OFF_P;
-  uint8_t* rel_s = smem + OFF_K1;                                   // before the key loop: rel tables, then the gather scratch
-  float* scratch = reinterpret_cast<float*>(smem + OFF_K1);
+  uint8_t* rel_s = smem + OFF_K0;                                   // before the key loop: rel tables in the K ring
+  float* scratch = reinterpret_cast<float*>(smem + OFF_V0);         // ... and the G_w / G_h rows over the V ring and P
   float* tab_h = reinterpret_cast<float*>(smem + OFF_TABH);
-  __shared__ __align__(8) uint64_t q_bar, g_full, tab_done, k_full[2], k_empty[2], v_full[2], v_empty[2], s_full[2], p_full, o_full;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t q_bar, tab_done, k_full[2], k_empty[2], v_full[2], v_empty[2];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tq = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
@@ -62,30 +62,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __
   const int C = a.H * D;
 
   if (tid == 0) {
-    tc::mbar_init(&q_bar, 1); tc::mbar_init(&g_full, 1); tc::mbar_init(&tab_done, 128);
-    tc::mbar_init(&p_full, 128); tc::mbar_init(&o_full, 1);
+    tc::mbar_init(&q_bar, 1); tc::mbar_init(&tab_done, CONSUMERS / 32);
     for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(&k_full[s], 1); tc::mbar_init(&k_empty[s], 1); tc::mbar_init(&v_full[s], 1); tc::mbar_init(&v_empty[s], 1);
-      tc::mbar_init(&s_full[s], 1);
+      tc::mbar_init(&k_full[s], 1); tc::mbar_init(&k_empty[s], CONSUMERS / 32);
+      tc::mbar_init(&v_full[s], 1); tc::mbar_init(&v_empty[s], CONSUMERS / 32);
     }
     tc::mbar_fence_init();
   }
-  if (warp == 4) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t TM_S = 0, TM_O = 256;                          // S_0 / S_1 at columns 0 / 128 (G_w / G_h before the loop)
 
-  if (warp == 5) {
+  if (warp >= CONSUMERS / 32) {
     // -------------------------------------------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    tc::producer_regs();
+    if (tid == CONSUMERS) {
       tc::mbar_arrive_expect_tx(&q_bar, 2 * Q_SLAB + 4 * REL_SLAB);
       tc::bulk_load_1d(rel_s, a.rel_blob, 4 * REL_SLAB, &q_bar);
       for (int s = 0; s < 2; ++s) tc::tma_load_2d(&tmQK, &q_bar, q_s + s * Q_SLAB, h * D + s * 64, b * L + tq * QT);
+      tc::mbar_wait(&tab_done, 0);                                  // the rings hold the rel tables / bias scratch until then
       for (int j = 0; j < NT; ++j) {
         const int st = j & 1, use = j >> 1;
-        if (j == 1) tc::mbar_wait(&tab_done, 0);                    // ring slot 1 doubles as rel tables / gather scratch until then
         uint8_t* k_s = smem + (st ? OFF_K1 : OFF_K0);
         uint8_t* v_s = smem + (st ? OFF_V1 : OFF_V0);
         tc::mbar_wait(&k_empty[st], (uint32_t)((use & 1) ^ 1));
@@ -96,164 +91,123 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __
         for (int s = 0; s < 2; ++s) tc::tma_load_2d(&tmVt, &v_full[st], v_s + s * V_SLAB, j * KT + s * 64, (b * a.H + h) * D);
       }
     }
-  } else if (warp == 4) {
-    // -------------------------------------------------------------------------------------------------- MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = tc::umma_idesc_bf16(QT, KT), idesc_o = tc::umma_idesc_bf16(QT, D);
-      const uint32_t q_addr = tc::smem_u32(q_s), p_addr = tc::smem_u32(p_s), rel_addr = tc::smem_u32(rel_s);
-      tc::mbar_wait(&q_bar, 0);
-      tc::tc_fence_after_sync();
+    return;
+  }
+  // -------------------------------------------------------------------------------------------------- warpgroups
+  tc::consumer_regs();
+  const int wg = warp >> 2, w = warp & 3;
+  const uint32_t q_addr = tc::smem_u32(q_s) + wg * (64 * 128), p_addr = tc::smem_u32(p_s) + wg * (64 * 128);
+  const int qh = 2 * tq + wg;                                       // this warpgroup's row of the token grid
+  float tw[2][32];                                                  // Rw * log2(e) of the thread's 32 key columns (kw), per row half
+  tc::mbar_wait(&q_bar, 0);
+  // G_w (blob table 1) -> tw,  G_h (blob table 0) -> tab_h, through this warpgroup's rows of the scratch
+#pragma unroll 1
+  for (int t = 0; t < 2; ++t) {
+    float g[KT / 2];
+    tc::wg_fence();
 #pragma unroll
-      for (int t = 0; t < 2; ++t)                                   // t = 0: G_w (blob table 1), t = 1: G_h (blob table 0)
+    for (int k = 0; k < D / 16; ++k)
+      tc::wgmma_bf16<KT>(g, tc::wg_desc(q_addr + (k >> 2) * Q_SLAB + (k & 3) * 32),
+                         tc::wg_desc(tc::smem_u32(rel_s) + ((1 - t) * 2 + (k >> 2)) * REL_SLAB + (k & 3) * 32), k ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
 #pragma unroll
-        for (int k = 0; k < D / 16; ++k)
-          tc::umma_bf16(tmem_base + TM_S + t * 128, tc::umma_desc_sw128(q_addr + (k >> 2) * Q_SLAB + (k & 3) * 32),
-                        tc::umma_desc_sw128(rel_addr + ((1 - t) * 2 + (k >> 2)) * REL_SLAB + (k & 3) * 32), idesc_s, k ? 1u : 0u);
-      tc::umma_commit(&g_full);
-      tc::mbar_wait(&tab_done, 0);
-      tc::tc_fence_after_sync();
-      auto issue_scores = [&](int j) {
-        const int st = j & 1;
-        tc::mbar_wait(&k_full[st], (uint32_t)((j >> 1) & 1));
-        tc::tc_fence_after_sync();
-        const uint32_t k_addr = tc::smem_u32(smem + (st ? OFF_K1 : OFF_K0));
+    for (int e = 0; e < KT / 2; ++e) scratch[(wg * 64 + tc::frag_row(e, w, lane)) * SCR_LD + tc::frag_col(e, lane)] = g[e] * LOG2E;
+    tc::named_bar(1 + wg, 128);
 #pragma unroll
-        for (int k = 0; k < D / 16; ++k)
-          tc::umma_bf16(tmem_base + TM_S + st * 128, tc::umma_desc_sw128(q_addr + (k >> 2) * Q_SLAB + (k & 3) * 32),
-                        tc::umma_desc_sw128(k_addr + (k >> 2) * K_SLAB + (k & 3) * 32), idesc_s, k ? 1u : 0u);
-        tc::umma_commit(&s_full[st]);
-        tc::umma_commit(&k_empty[st]);
-      };
-      issue_scores(0);
-      issue_scores(1);
-      for (int j = 0; j < NT; ++j) {
-        const int st = j & 1;
-        tc::mbar_wait(&p_full, (uint32_t)(j & 1));
-        tc::mbar_wait(&v_full[st], (uint32_t)((j >> 1) & 1));
-        tc::tc_fence_after_sync();
-        const uint32_t v_addr = tc::smem_u32(smem + (st ? OFF_V1 : OFF_V0));
+    for (int hr = 0; hr < 2; ++hr) {
+      const int rl = tc::frag_row(2 * hr, w, lane), r = wg * 64 + rl;   // query column qw = rl
+      const float* srow = scratch + r * SCR_LD;
+      if (t == 0) {
 #pragma unroll
-        for (int k = 0; k < KT / 16; ++k)
-          tc::umma_bf16(tmem_base + TM_O, tc::umma_desc_sw128(p_addr + (k >> 2) * P_SLAB + (k & 3) * 32),
-                        tc::umma_desc_sw128(v_addr + (k >> 2) * V_SLAB + (k & 3) * 32), idesc_o, k ? 1u : 0u);
-        tc::umma_commit(&o_full);
-        tc::umma_commit(&v_empty[st]);
-        if (j + 2 < NT) issue_scores(j + 2);
+        for (int i = 0; i < 32; ++i) tw[hr][i] = srow[rl + (GRID - 1) - tc::frag_col(4 * (i >> 1) + (i & 1), lane)];
+      } else if ((lane & 3) == 0) {
+        for (int kh = 0; kh < GRID; ++kh) tab_h[r * TABH_LD + kh] = srow[qh + (GRID - 1) - kh];
       }
     }
-  } else {
-    // -------------------------------------------------------------------------------------------------- softmax: thread = query row
-    const int r = tid;
-    const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    float tw[GRID];
-    tc::mbar_wait(&g_full, 0);
-    tc::tc_fence_after_sync();
-    {
-      float* srow = scratch + r * SCR_LD;
-      const int qw = r & (GRID - 1), qh = 2 * tq + (r >> 6);
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        tc::tmem_ld32(t_addr + TM_S + c * 32, v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) srow[c * 32 + i] = v[i] * LOG2E;
-      }
-#pragma unroll
-      for (int kw = 0; kw < GRID; ++kw) tw[kw] = srow[qw + (GRID - 1) - kw];
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        tc::tmem_ld32(t_addr + TM_S + 128 + c * 32, v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) srow[c * 32 + i] = v[i] * LOG2E;
-      }
-      for (int kh = 0; kh < GRID; ++kh) tab_h[r * TABH_LD + kh] = srow[qh + (GRID - 1) - kh];
-    }
-    tc::tc_fence_before_sync();
-    tc::mbar_arrive(&tab_done);
+    tc::named_bar(1 + wg, 128);                                     // the scratch rows are read before they are rewritten
+  }
+  if (lane == 0) tc::mbar_arrive(&tab_done);                        // rel tables and scratch are dead: the rings may fill
+  tc::mbar_wait(&tab_done, 0);                                      // ... and P (over the other warpgroup's scratch rows) be written
 
-    const float sl2 = a.scale * LOG2E;
-    float m = -INFINITY, l = 0.f, alpha_prev = 0.f;
-    float o[D];
+  const float sl2 = a.scale * LOG2E;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[D / 2];
 #pragma unroll
-    for (int i = 0; i < D; ++i) o[i] = 0.f;
-
-    auto fold_output = [&](int jprev) {                             // o = o * alpha + O_jprev
-      tc::mbar_wait(&o_full, (uint32_t)(jprev & 1));
-      tc::tc_fence_after_sync();
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float v[32];
-        tc::tmem_ld32(t_addr + TM_O + c * 32, v);                   // the last chunk reads 16 columns past D: ignored
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (c * 32 + i < D) o[c * 32 + i] = fmaf(o[c * 32 + i], alpha_prev, v[i]);
-      }
-    };
-
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
 #pragma unroll 1
-    for (int j = 0; j < NT; ++j) {
-      const int st = j & 1;
-      const float th0 = tab_h[r * TABH_LD + 2 * j], th1 = tab_h[r * TABH_LD + 2 * j + 1];
-      tc::mbar_wait(&s_full[st], (uint32_t)((j >> 1) & 1));
-      tc::tc_fence_after_sync();
-      const uint32_t s_addr = t_addr + TM_S + st * 128;
+  for (int j = 0; j < NT; ++j) {
+    const int st = j & 1;
+    float sacc[KT / 2];
+    tc::mbar_wait(&k_full[st], (uint32_t)((j >> 1) & 1));
+    const uint32_t k_addr = tc::smem_u32(smem + (st ? OFF_K1 : OFF_K0));
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k)
+      tc::wgmma_bf16<KT>(sacc, tc::wg_desc(q_addr + (k >> 2) * Q_SLAB + (k & 3) * 32), tc::wg_desc(k_addr + (k >> 2) * K_SLAB + (k & 3) * 32),
+                         k ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&k_empty[st]);
+    float alpha[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r = wg * 64 + tc::frag_row(2 * hr, w, lane);
+      const float th0 = tab_h[r * TABH_LD + 2 * j], th1 = tab_h[r * TABH_LD + 2 * j + 1];   // key rows 2j, 2j+1 of the grid
       float mt = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        tc::tmem_ld32(s_addr + c * 32, v);
-        const float th = (c < 2) ? th0 : th1;
+      for (int jj = 0; jj < KT / 8; ++jj)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) mt = fmaxf(mt, fmaf(v[i], sl2, th + tw[(c & 1) * 32 + i]));
-      }
-      const float m_new = fmaxf(m, mt);
-      const float alpha = ex2(m - m_new);
-      if (j > 0) fold_output(j - 1);                                // also: P_{j-1} and O_{j-1} have been consumed
+        for (int e = 0; e < 2; ++e) {
+          const int i = 4 * jj + 2 * hr + e;
+          const float x = fmaf(sacc[i], sl2, (jj < 8 ? th0 : th1) + tw[hr][2 * (jj & 7) + e]);
+          sacc[i] = x;
+          mt = fmaxf(mt, x);
+        }
+      const float m_new = fmaxf(m[hr], tc::quad_max(mt));
+      alpha[hr] = ex2(m[hr] - m_new);
+      m[hr] = m_new;
       float sum = 0.f;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        tc::tmem_ld32(s_addr + c * 32, v);
-        const float th = ((c < 2) ? th0 : th1) - m_new;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          v[i] = ex2(fmaf(v[i], sl2, th + tw[(c & 1) * 32 + i]));
-          sum += v[i];
-        }
-        uint8_t* prow = p_s + (c >> 1) * P_SLAB + r * 128;
-#pragma unroll
-        for (int q8 = 0; q8 < 4; ++q8) {
-          const int chunk = (c & 1) * 4 + q8;
-          *reinterpret_cast<uint4*>(prow + ((chunk ^ (r & 7)) << 4)) =
-              make_uint4(tc::pack_bf16(v[q8 * 8], v[q8 * 8 + 1]), tc::pack_bf16(v[q8 * 8 + 2], v[q8 * 8 + 3]),
-                         tc::pack_bf16(v[q8 * 8 + 4], v[q8 * 8 + 5]), tc::pack_bf16(v[q8 * 8 + 6], v[q8 * 8 + 7]));
-        }
+      for (int jj = 0; jj < KT / 8; ++jj) {
+        const int i = 4 * jj + 2 * hr;
+        const float p0 = ex2(sacc[i] - m_new), p1 = ex2(sacc[i + 1] - m_new);
+        sum += p0 + p1;
+        sacc[i] = p0; sacc[i + 1] = p1;
       }
-      l = fmaf(l, alpha, sum);
-      m = m_new;
-      alpha_prev = alpha;
-      tc::tc_fence_before_sync();
-      tc::fence_proxy_async_smem();
-      tc::mbar_arrive(&p_full);
+      l[hr] = fmaf(l[hr], alpha[hr], sum);
     }
-    fold_output(NT - 1);                                            // o now covers every key tile, relative to the final maximum
-    const float inv = 1.f / l;
-    float* stage = reinterpret_cast<float*>(p_s) + warp * epi::WARP_STAGE_FLOATS;   // P is free: the last value MMA has completed
-    const int row0 = b * L + tq * QT + warp * 32;
-    OT* outp = reinterpret_cast<OT*>(a.out);
+    if (j > 0) tc::named_bar(1 + wg, 128);                          // every warp's P_{j-1} V_{j-1} has completed: P may be rewritten
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float v[32];
+    for (int i = 0; i < KT / 2; i += 2) {
+      const int r = wg * 64 + tc::frag_row(i, w, lane), col = tc::frag_col(i, lane);
+      *reinterpret_cast<uint32_t*>(p_s + (col >> 6) * P_SLAB + tc::sw128_offset(r, col & 63)) = tc::pack_bf16(sacc[i], sacc[i + 1]);
+    }
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = (c * 32 + i < D) ? o[c * 32 + i] * inv : 0.f;
-      epi::process_chunk<OT, 0, false, false>(v, stage, lane, row0, b * L + L, h * D + c * 32, h * D + D, 1.f, nullptr, nullptr, 0, outp,
-                                              a.out_ld);
+    for (int i = 0; i < D / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    tc::fence_proxy_async_smem();
+    tc::named_bar(1 + wg, 128);                                     // this warpgroup's P_j rows are complete
+    tc::mbar_wait(&v_full[st], (uint32_t)((j >> 1) & 1));
+    const uint32_t v_addr = tc::smem_u32(smem + (st ? OFF_V1 : OFF_V0));
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < KT / 16; ++k)
+      tc::wgmma_bf16<D>(o, tc::wg_desc(p_addr + (k >> 2) * P_SLAB + (k & 3) * 32), tc::wg_desc(v_addr + (k >> 2) * V_SLAB + (k & 3) * 32), 1u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&v_empty[st]);
+  }
+  OT* outp = reinterpret_cast<OT*>(a.out);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const float inv = 1.f / tc::quad_sum(l[hr]);
+    const int row = b * L + tq * QT + wg * 64 + tc::frag_row(2 * hr, w, lane);
+#pragma unroll
+    for (int jj = 0; jj < D / 8; ++jj) {
+      const int i = 4 * jj + 2 * hr;
+      epi::st2(outp + (size_t)row * a.out_ld + h * D + tc::frag_col(i, lane), o[i] * inv, o[i + 1] * inv);
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace
@@ -290,7 +244,7 @@ int g_make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols
 }  // namespace
 
 // qkv: bf16 (B*4096 rows, ld >= 2*H*80) rows [q | k (| v)], head h at columns h*80 of q and H*80 + h*80 of k; Vt: bf16 (B*H*80 rows, vt_ld >= 4096)
-// = V^T per (image, head) (sam6d_transpose_tokens_bf16); rel_blob: rel_pos_h / rel_pos_w ((127, 80) each) packed as bf16 UMMA
+// = V^T per (image, head) (sam6d_transpose_tokens_bf16); rel_blob: rel_pos_h / rel_pos_w ((127, 80) each) packed as bf16 wgmma
 // slabs with 128-row slabs (ops.pack_rel_pos(..., slab_rows=128)); out (B*4096, H*80) fp32 or bf16.  64 x 64 token grid only.
 S6_API int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H,
                                 int grid, float scale, void* out, int out_is_bf16, long long out_ld, void* stream) {

@@ -1,18 +1,19 @@
-// attn_tc.cu -- multi-head attention on the 5th-gen tensor cores for up to 256 keys per (batch, head):
+// attn_tc.cu -- multi-head attention on the tensor cores (wgmma) for up to 256 keys per (batch, head):
 //     O = softmax((Q K^T + bias) * scale) V (+ b_v)
 // covering PEM's geometric-transformer self / cross attention (197 tokens, head dim 64, dense relative-position bias from
 // rpe_scores; PEM/model/transformer.py:109-148, 369-406) and SAM's windowed attention (196 tokens, head dim 80, decomposed
 // rel-pos bias; ISM/segment_anything/modeling/image_encoder.py:224-240, 325-361).
 //
-// One CTA per (128-query tile, head, batch):
+// One CTA per (128-query tile, head, batch); one thread of warpgroup 2 issues the TMA loads, warpgroup g (warps 4g..4g+3) owns queries
+// [64 g, 64 g + 64) of the tile:
 //   TMA      : Q tile, K tile (boxes of 64 channels x rows, SWIZZLE_128B) and V^T tiles (64 keys x D channels) land in
-//              UMMA K-major slabs; V^T (channels x keys) is produced by a GEMM upstream so that P V is a K-major MMA
-//   MMA 1    : S = Q K^T          tcgen05.mma M128 N(keys, mult. of 16) K16 x D/16       -> TMEM columns [0, 256)
-//   softmax  : 4 warps, thread = query row: the whole score row sits in TMEM (<= 256 keys), so it is a plain two-pass softmax
-//              (no online rescaling): pass 1 max of (s + bias) * scale, pass 2 exp / sum, P written as bf16 straight into the
-//              A-operand slabs
-//   MMA 2    : O = P V            tcgen05.mma M128 N(D) K16 x keys/16                    -> TMEM columns [256, 256 + D)
-//   epilogue : O / rowsum (+ b_v; rows of P sum to 1, so the value bias moves out of the MMA), coalesced stores
+//              K-major slabs; V^T (channels x keys) is produced by a GEMM upstream so that P V is a K-major MMA
+//   MMA 1    : S = Q K^T          wgmma m64n256k16 x D/16 into 128 registers per thread (columns past the keys are ignored)
+//   softmax  : the whole score row sits in the registers of one quad (<= 256 keys), so it is a plain two-pass softmax (no online
+//              rescaling): x = (s + bias) * scale, row max and sum by quad shuffles, P written as bf16 into the A-operand slabs
+//              (they alias Q / K, dead once both warpgroups are past MMA 1)
+//   MMA 2    : O = P V            wgmma m64nDk16 x keys/16
+//   epilogue : O / rowsum (+ b_v; rows of P sum to 1, so the value bias moves out of the MMA), stored from the registers
 // Rows of a tile that run past the batch (197 is not a multiple of 128) are computed on whatever the TMA box fetched (the
 // next batch's finite rows or zero fill) and never stored; keys past Sk are masked to probability 0.
 #include <cuda.h>
@@ -23,11 +24,13 @@
 namespace {
 
 constexpr int QT = 128, MAXK = 256;
-constexpr int NUM_THREADS = 160;   // warps 0-3 softmax/epilogue, warp 4 TMA + MMA
+constexpr int CONSUMERS = 256, NUM_THREADS = CONSUMERS + 128;   // warps 0-7 two MMA warpgroups, warp 8 TMA
+constexpr int REL_SLAB = 32 * 128;                              // BIAS_MODE 2: [32 rows][64 ch] bf16 slab of a rel-pos table
+constexpr int SCR_LD = 64;                                      // BIAS_MODE 2: per query row, Q rel_h^T (0..31) and Q rel_w^T (32..63)
 
 struct AttnArgs {
   const float* bias;     // BIAS_MODE 1: (B,H,Sq,Sk) fp32
-  const void* rel_blob;  // BIAS_MODE 2: rel_h, rel_w pre-packed on the host as bf16 UMMA slabs (2 x DS x [32][64], SWIZZLE_128B)
+  const void* rel_blob;  // BIAS_MODE 2: rel_h, rel_w pre-packed on the host as bf16 wgmma slabs (2 x DS x [32][64], SWIZZLE_128B)
   const float* rel_unused;
   const void* q_rows;    // BIAS_MODE 2: the bf16 matrix Q is a column slice of (for the unscaled-q bias tables)
   long long q_ld;
@@ -47,58 +50,43 @@ struct AttnArgs {
   long long bias_ld;     // BIAS_MODE 4: row stride of the bias planes (B,H,Sq,bias_ld), a multiple of 4 floats, >= Sk
 };
 
-// COMPACT (head dim 64, no / dense bias: the PEM layers): P and the bias staging alias the Q / K slabs (dead once the score MMA
-// has completed) and O aliases the first columns of S in TMEM (dead once P is published), so a CTA needs 97 KB of shared memory
-// and 256 TMEM columns and two CTAs share an SM -- one CTA's serial load -> MMA -> softmax -> MMA -> store chain hides behind
-// the other's.
-template <int D, int BIAS_MODE>
-constexpr bool kCompact = (D == 64) && (BIAS_MODE == 0 || BIAS_MODE == 1 || BIAS_MODE == 4);
+// shared memory: [Q][K] (P aliases them once the score MMAs are done) [V^T: 4 slabs] (BIAS_MODE 2: [rel tables][T scratch])
+template <int D>
+__host__ __device__ constexpr int qkp_bytes(int N1) {
+  return ((((D + 63) / 64) * (QT + N1) * 128 > 4 * QT * 128 ? ((D + 63) / 64) * (QT + N1) * 128 : 4 * QT * 128) + 1023) & ~1023;
+}
 
 template <int D, int BIAS_MODE, typename OT>
-__global__ void __launch_bounds__(NUM_THREADS, kCompact<D, BIAS_MODE> ? 2 : 1) attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ,
-                                                                                             const __grid_constant__ CUtensorMap tmK,
-                                                                                             const __grid_constant__ CUtensorMap tmVt,
-                                                                                             AttnArgs a) {
-  constexpr bool COMPACT = kCompact<D, BIAS_MODE>;
-  constexpr uint32_t TM_O = COMPACT ? 0u : 256u, TM_COLS = COMPACT ? 256u : 512u;
+__global__ void __launch_bounds__(NUM_THREADS, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                                const __grid_constant__ CUtensorMap tmVt, AttnArgs a) {
   constexpr int DS = (D + 63) / 64;                 // 64-channel slabs of Q / K
   constexpr int Q_SLAB = QT * 128, V_SLAB = D * 128, P_SLAB = QT * 128;
-  constexpr int Q_BYTES = DS * Q_SLAB, V_BYTES = 4 * V_SLAB;
   const int K_SLAB = a.N1 * 128;                    // N1 is a multiple of 16 -> multiple of 2048 bytes: slabs stay 1024-aligned
-  const int K_BYTES = DS * K_SLAB;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  // default layout: [Q][K][V^T][P][bias stage | rel tables];  COMPACT: [V^T][Q, K -> bias stage -> P]
-  uint8_t* q_s = COMPACT ? smem + V_BYTES : smem;
-  uint8_t* k_s = q_s + Q_BYTES;
-  uint8_t* v_s = COMPACT ? smem : k_s + K_BYTES;    // 4 slabs [D rows][64 keys]; V_SLAB is a multiple of 1024 for D = 64, 80
-  uint8_t* p_s = COMPACT ? q_s : v_s + ((V_BYTES + 1023) & ~1023);        // 4 slabs [128 rows][64 keys]
-  float* bstage = reinterpret_cast<float*>(p_s + 4 * P_SLAB);             // BIAS_MODE 1/3: 4 warps x [32][33] bias tiles
-  uint8_t* rel_s = p_s + 4 * P_SLAB;                                       // BIAS_MODE 2: rel_h, rel_w as UMMA B operands:
-  constexpr int REL_SLAB = 32 * 128;                                       //   2 tables x DS slabs of [32 rows][64 ch] bf16
-  float* tab = reinterpret_cast<float*>(rel_s + 2 * DS * REL_SLAB);        // BIAS_MODE 2: [128][Hs + Ws] bias tables
-  __shared__ __align__(8) uint64_t load_bar, s_full, p_full, o_full, rel_ready;
-  __shared__ uint32_t tmem_slot;
+  uint8_t* q_s = smem;
+  uint8_t* k_s = q_s + DS * Q_SLAB;
+  uint8_t* p_s = smem;                              // 4 slabs [128 rows][64 keys]
+  uint8_t* v_s = smem + qkp_bytes<D>(a.N1);         // 4 slabs [D rows][64 keys]
+  uint8_t* rel_s = v_s + 4 * V_SLAB;                // BIAS_MODE 2: 2 tables x DS slabs [32 rows][64 ch]
+  float* scr = reinterpret_cast<float*>(rel_s + 2 * DS * REL_SLAB);   // BIAS_MODE 2: [128][SCR_LD]
+  __shared__ __align__(8) uint64_t load_bar;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n0 = blockIdx.x * QT, h = blockIdx.y, b = blockIdx.z;
   const int nslab = (a.N1 + 63) / 64;
 
   if (tid == 0) {
-    tc::mbar_init(&load_bar, 1); tc::mbar_init(&s_full, 1); tc::mbar_init(&p_full, 128); tc::mbar_init(&o_full, 1);
-    tc::mbar_init(&rel_ready, 128);
+    tc::mbar_init(&load_bar, 1);
     tc::mbar_fence_init();
   }
   s6_pdl_trigger();
-  if (warp == 4) tc::tmem_alloc(&tmem_slot, TM_COLS);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   s6_pdl_wait();                                   // Q / K / V^T / bias come from the kernels before us
 
-  if (warp == 4) {
-    if (lane == 0) {
+  if (warp >= CONSUMERS / 32) {
+    tc::producer_regs();
+    if (tid == CONSUMERS) {
       // ---------------------------------------------------------------- TMA loads (one transaction barrier)
       uint32_t bytes = (uint32_t)(DS * (QT * 128) + DS * (a.N1 * 128) + nslab * V_SLAB);
       if (BIAS_MODE == 2) bytes += 2 * DS * REL_SLAB;
@@ -110,238 +98,124 @@ __global__ void __launch_bounds__(NUM_THREADS, kCompact<D, BIAS_MODE> ? 2 : 1) a
         tc::tma_load_2d(&tmK, &load_bar, k_s + s * K_SLAB, a.k_col0 + h * D + s * 64, b * a.k_brows + a.k_row0);
       }
       for (int s = 0; s < nslab; ++s) tc::tma_load_2d(&tmVt, &load_bar, v_s + s * V_SLAB, a.v_col0 + s * 64, (b * a.H + h) * D);
-      tc::mbar_wait(&load_bar, 0);
-      tc::tc_fence_after_sync();
-      // ---------------------------------------------------------------- S = Q K^T
-      const uint32_t idesc1 = tc::umma_idesc_bf16(QT, a.N1);
-#pragma unroll
-      for (int k = 0; k < D / 16; ++k) {
-        const int s = k >> 2, kk = k & 3;
-        tc::umma_bf16(tmem_base, tc::umma_desc_sw128(tc::smem_u32(q_s + s * Q_SLAB) + kk * 32),
-                      tc::umma_desc_sw128(tc::smem_u32(k_s + s * K_SLAB) + kk * 32), idesc1, k ? 1u : 0u);
-      }
-      if (BIAS_MODE == 2) {
-        // decomposed rel-pos: T_h = Q rel_h^T, T_w = Q rel_w^T (128 x 32 each) -> TMEM columns [384,416) and [416,448);
-        // the softmax warps turn them into the per-query bias tables (Hs + Ws dot products per query, on the tensor pipe)
-        constexpr uint32_t idesc_r = tc::umma_idesc_bf16(QT, 32);
-#pragma unroll
-        for (int t = 0; t < 2; ++t)
-#pragma unroll
-          for (int k = 0; k < D / 16; ++k) {
-            const int sl = k >> 2, kk = k & 3;
-            tc::umma_bf16(tmem_base + 384 + t * 32, tc::umma_desc_sw128(tc::smem_u32(q_s + sl * Q_SLAB) + kk * 32),
-                          tc::umma_desc_sw128(tc::smem_u32(rel_s + (t * DS + sl) * REL_SLAB) + kk * 32), idesc_r, k ? 1u : 0u);
-          }
-      }
-      tc::umma_commit(&s_full);
-      // ---------------------------------------------------------------- O = P V
-      tc::mbar_wait(&p_full, 0);
-      tc::tc_fence_after_sync();
-      constexpr uint32_t idesc2 = tc::umma_idesc_bf16(QT, D);
-      const int ksteps = a.N1 / 16;
-      for (int k = 0; k < ksteps; ++k) {
-        const int s = k >> 2, kk = k & 3;
-        tc::umma_bf16(tmem_base + TM_O, tc::umma_desc_sw128(tc::smem_u32(p_s + s * P_SLAB) + kk * 32),
-                      tc::umma_desc_sw128(tc::smem_u32(v_s + s * V_SLAB) + kk * 32), idesc2, k ? 1u : 0u);
-      }
-      tc::umma_commit(&o_full);
     }
-  } else {
-    // ------------------------------------------------------------------ softmax + epilogue: thread <-> query row
-    const int r = tid, n = n0 + r;
-    const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    const int Sk = a.Sk;
-    float* my_tab = nullptr;
-    (void)my_tab;
-    const int nchunk = (a.N1 + 31) / 32;
-    // dense bias tile of a chunk: 32 independent 128-byte requests per warp (for each of the warp's 32 rows the lanes read 32
-    // consecutive columns), transposed through shared memory
-    float bl[32];
-    // warp-uniform 64-bit base + 32-bit per-lane offsets: the 32 row loads need no per-thread 64-bit address arithmetic
-    // (with it the register allocator serialised them into a few dependent batches, see profiles/r01_attn_bias_notes.md)
-    const int wrow0 = min(n0 + warp * 32, a.Sq - 1), rows_ok = max(1, min(32, a.Sq - (n0 + warp * 32)));
-    const float* wbase = a.bias + (((size_t)b * a.H + h) * a.Sq + wrow0) * Sk;
-    auto fetch_bias = [&](int c) {
-      const int col = c * 32 + lane;
-#pragma unroll
-      for (int rr = 0; rr < 32; ++rr) {
-        const int off = min(rr, rows_ok - 1) * Sk + col;
-        bl[rr] = (col < Sk) ? __ldg(wbase + off) : 0.f;
-      }
-    };
-    tc::mbar_wait(&s_full, 0);
-    tc::tc_fence_after_sync();
-    if (BIAS_MODE == 2) {
-      // T_h[r][j] = q_r . rel_h[j]  ->  tab[r][kh] = T_h[r][qh - kh + Hs - 1]; likewise the w table (unscaled q, as the reference)
-      const int TW = a.Hs + a.Ws;
-      my_tab = tab + r * TW;
-      float* scratch = reinterpret_cast<float*>(p_s) + r * 65;            // P slabs are unused until pass 2
-      const int nq = min(n, a.Sq - 1), qh = nq / a.Ws, qw = nq % a.Ws;
-      float v[32];
-      tc::tmem_ld32(t_addr + 384, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) scratch[j] = v[j];
-      tc::tmem_ld32(t_addr + 416, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) scratch[32 + j] = v[j];
-      for (int kh = 0; kh < a.Hs; ++kh) my_tab[kh] = scratch[qh - kh + a.Hs - 1];
-      for (int kw = 0; kw < a.Ws; ++kw) my_tab[a.Hs + kw] = scratch[32 + qw - kw + a.Ws - 1];
-    }
-    // pass 1: x = (s + bias) * scale (+ rel-pos), row max; x is written back over S so pass 2 needs no bias
-    float mx = -INFINITY;
-    // COMPACT: the warp's 32 x 32 tile lives in the rows of P slab 0 only this warp will write (XOR-swizzled, 4 KB exactly)
-    float* my_stage = COMPACT ? reinterpret_cast<float*>(p_s + warp * 32 * 128) : bstage + warp * (32 * 33);
-    auto st_w = [&](int rr, int col) { return COMPACT ? rr * 32 + (col ^ rr) : rr * 33 + col; };
-    int kh_run = 0, kw_run = 0;                                            // (kh, kw) of the running key column, no div / mod
-    if constexpr (BIAS_MODE == 4) {
-      // Padded bias planes (row stride a multiple of 16 bytes): the warp's 32 x 32 tile of a chunk is copied with 8 cp.async of 16
-      // bytes per lane straight into shared memory -- no registers, so FOUR chunks are in flight while one is consumed (a register
-      // prefetch of one chunk spilled; fetching chunk by chunk left a full L2 round trip in front of each of the 7 chunks).
-      // Buffer i = this warp's 32 rows of P slab i (only this warp ever writes them); 16-byte pieces XOR-swizzled by row so that
-      // the thread-per-row read-back is conflict-free per quarter warp.
-      const long long ld = a.bias_ld;
-      const float* wb4 = a.bias + (((size_t)b * a.H + h) * a.Sq + wrow0) * ld;
-      auto issue = [&](int c) {
-        if (c < nchunk) {
-          const uint32_t dst0 = tc::smem_u32(p_s + (c & 3) * P_SLAB + warp * 4096);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int id = i * 32 + lane, rr = id >> 3, pc = id & 7;
-            const int col = c * 32 + pc * 4;
-            if (col < ld) {
-              const float* src = wb4 + (long long)min(rr, rows_ok - 1) * ld + col;
-              asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst0 + rr * 128 + ((pc ^ (rr & 7)) << 4)), "l"(src) : "memory");
-            }
-          }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-      };
-#pragma unroll
-      for (int c = 0; c < 4; ++c) issue(c);
-      for (int c = 0; c < nchunk; ++c) {
-        float v[32];
-        tc::tmem_ld32(t_addr + c * 32, v);
-        asm volatile("cp.async.wait_group 3;" ::: "memory");
-        __syncwarp();
-        const uint8_t* rowp = p_s + (c & 3) * P_SLAB + warp * 4096 + lane * 128;
-#pragma unroll
-        for (int pc = 0; pc < 8; ++pc) {
-          const float4 b4 = *reinterpret_cast<const float4*>(rowp + ((pc ^ (lane & 7)) << 4));
-          const float bq[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int j = pc * 4 + e, col = c * 32 + j;
-            float x = -INFINITY;
-            if (col < Sk) { x = (v[j] + bq[e]) * a.scale; mx = fmaxf(mx, x); }
-            v[j] = x;
-          }
-        }
-        tc::tmem_st32(t_addr + c * 32, v);
-        __syncwarp();                                     // every lane has read the buffer before it is refilled
-        issue(c + 4);
-      }
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-    } else
-    for (int c = 0; c < nchunk; ++c) {
-      float v[32];
-      tc::tmem_ld32(t_addr + c * 32, v);
-      if (BIAS_MODE == 1 || BIAS_MODE == 3) {
-        // (requesting chunk c+1 here, one chunk ahead, was measured: the 32 extra live registers spill at the 168-register cap of
-        //  the two-CTAs-per-SM layout and the launch got slower, 54 -> 72 us)
-        fetch_bias(c);
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) my_stage[st_w(rr, lane)] = bl[rr];
-        __syncwarp();
-      }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = c * 32 + j;
-        float x = -INFINITY;
-        if (col < Sk) {
-          x = v[j];
-          if (BIAS_MODE == 1 || BIAS_MODE == 3) x += my_stage[st_w(lane, j)];
-          x *= a.scale;
-          if (BIAS_MODE == 2) {
-            x += my_tab[kh_run] + my_tab[a.Hs + kw_run];
-            if (++kw_run == a.Ws) { kw_run = 0; ++kh_run; }
-          }
-          mx = fmaxf(mx, x);
-        }
-        v[j] = x;
-      }
-      if (BIAS_MODE == 1 || BIAS_MODE == 2) tc::tmem_st32(t_addr + c * 32, v);
-      if (BIAS_MODE == 1 || BIAS_MODE == 3) __syncwarp();
-    }
-    float sum = 0.f;
-    for (int c = 0; c < nchunk; ++c) {
-      float v[32];
-      tc::tmem_ld32(t_addr + c * 32, v);
-      if (BIAS_MODE == 3) {
-        const int col = c * 32 + lane;
-        const size_t rowbase = ((size_t)b * a.H + h) * a.Sq;
-        float bl[32];
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) {                      // 32 independent 128-byte requests in flight per warp
-          const int nn = min(n0 + warp * 32 + rr, a.Sq - 1);
-          bl[rr] = (col < Sk) ? __ldg(a.bias + (rowbase + nn) * Sk + col) : 0.f;
-        }
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) my_stage[st_w(rr, lane)] = bl[rr];
-        __syncwarp();
-      }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = c * 32 + j;
-        float p = 0.f;
-        if (col < Sk) {
-          float x = v[j];
-          if (BIAS_MODE == 0) x *= a.scale;
-          if (BIAS_MODE == 3) x = (x + my_stage[st_w(lane, j)]) * a.scale;
-          p = __expf(x - mx);
-        }
-        sum += p;
-        v[j] = p;
-      }
-      if (BIAS_MODE == 3) __syncwarp();
-      // 32 probabilities -> 4 x 16-byte chunks of the swizzled P slab (slab = 64 keys)
-      uint8_t* prow = p_s + (c >> 1) * P_SLAB + r * 128;
-#pragma unroll
-      for (int q8 = 0; q8 < 4; ++q8) {
-        const int chunk = (c & 1) * 4 + q8;
-        *reinterpret_cast<uint4*>(prow + ((chunk ^ (r & 7)) << 4)) =
-            make_uint4(tc::pack_bf16(v[q8 * 8], v[q8 * 8 + 1]), tc::pack_bf16(v[q8 * 8 + 2], v[q8 * 8 + 3]),
-                       tc::pack_bf16(v[q8 * 8 + 4], v[q8 * 8 + 5]), tc::pack_bf16(v[q8 * 8 + 6], v[q8 * 8 + 7]));
-      }
-    }
-    tc::tc_fence_before_sync();
-    tc::fence_proxy_async_smem();
-    tc::mbar_arrive(&p_full);
-    // ------------------------------------------------------------------ epilogue
-    tc::mbar_wait(&o_full, 0);
-    tc::tc_fence_after_sync();
-    const float inv = 1.f / sum;
-    if (a.lse && n < a.Sq) a.lse[((size_t)b * a.H + h) * a.Sq + n] = mx + __logf(sum);
-    float* stage = reinterpret_cast<float*>(p_s) + warp * epi::WARP_STAGE_FLOATS;   // P slabs are free once O is complete
-    const int HD = a.H * D;
-    const int row0 = b * a.Sq + n0 + warp * 32;
-    const int m_lim = b * a.Sq + a.Sq;                                               // rows of the next batch are not ours
-#pragma unroll 1
-    for (int c = 0; c < (D + 31) / 32; ++c) {
-      float v[32];
-      tc::tmem_ld32(t_addr + TM_O + c * 32, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] *= inv;
-      const int col0 = h * D + c * 32;
-      const int ncols_lim = h * D + D;                                               // chunk may overhang the head (D = 80)
-      OT* outp = reinterpret_cast<OT*>(a.out);
-      if (a.bv) epi::process_chunk<OT, 0, true, false>(v, stage, lane, row0, m_lim, col0, ncols_lim, 1.f, a.bv, nullptr, 0, outp, a.out_ld);
-      else epi::process_chunk<OT, 0, false, false>(v, stage, lane, row0, m_lim, col0, ncols_lim, 1.f, nullptr, nullptr, 0, outp, a.out_ld);
-    }
-    (void)HD;
+    return;
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc(tmem_base, TM_COLS);
+  // ------------------------------------------------------------------ warpgroup wg <-> queries [64 wg, 64 wg + 64) of the tile
+  tc::consumer_regs();
+  const int wg = warp >> 2, w = warp & 3;
+  const int Sk = a.Sk;
+  tc::mbar_wait(&load_bar, 0);
+  // ---------------------------------------------------------------- S = Q K^T (columns >= N1 read past the K slab: ignored)
+  float sacc[MAXK / 2];
+  {
+    const uint32_t q_addr = tc::smem_u32(q_s) + wg * (64 * 128), k_addr = tc::smem_u32(k_s);
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) {
+      const int sl = k >> 2, kk = k & 3;
+      tc::wgmma_bf16<MAXK>(sacc, tc::wg_desc(q_addr + sl * Q_SLAB + kk * 32), tc::wg_desc(k_addr + sl * K_SLAB + kk * 32), k ? 1u : 0u);
+    }
+    tc::wg_commit();
+    if (BIAS_MODE == 2) {
+      // decomposed rel-pos: T_h = Q rel_h^T, T_w = Q rel_w^T (64 x 32 each per warpgroup) -> scr[row][0..31], [32..63]
+      float tacc[2][16];
+#pragma unroll
+      for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int k = 0; k < D / 16; ++k) {
+          const int sl = k >> 2, kk = k & 3;
+          tc::wgmma_bf16<32>(tacc[t], tc::wg_desc(q_addr + sl * Q_SLAB + kk * 32),
+                             tc::wg_desc(tc::smem_u32(rel_s + (t * DS + sl) * REL_SLAB) + kk * 32), k ? 1u : 0u);
+        }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+#pragma unroll
+      for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int e = 0; e < 16; ++e) scr[(wg * 64 + tc::frag_row(e, w, lane)) * SCR_LD + t * 32 + tc::frag_col(e, lane)] = tacc[t][e];
+      tc::named_bar(1 + wg, 128);
+    } else {
+      tc::wg_wait<0>();
+    }
+  }
+  // ---------------------------------------------------------------- softmax over the thread's two rows
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int r = wg * 64 + tc::frag_row(2 * hr, w, lane), n = n0 + r, nq = min(n, a.Sq - 1);
+    const float* brow = nullptr;
+    if (BIAS_MODE == 1 || BIAS_MODE == 3) brow = a.bias + (((size_t)b * a.H + h) * a.Sq + nq) * Sk;
+    if (BIAS_MODE == 4) brow = a.bias + (((size_t)b * a.H + h) * a.Sq + nq) * a.bias_ld;
+    const float* trow = (BIAS_MODE == 2) ? scr + r * SCR_LD : nullptr;
+    const int qh = (BIAS_MODE == 2) ? nq / a.Ws : 0, qw = (BIAS_MODE == 2) ? nq % a.Ws : 0;
+#pragma unroll
+    for (int j = 0; j < MAXK / 8; ++j) {
+      const int col = tc::frag_col(4 * j, lane);
+      float bb[2] = {0.f, 0.f};
+      if (BIAS_MODE == 4 && col < Sk) { const float2 t = __ldg(reinterpret_cast<const float2*>(brow + col)); bb[0] = t.x; bb[1] = t.y; }
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = col + e;
+        float x = -INFINITY;
+        if (c < Sk) {
+          x = sacc[4 * j + 2 * hr + e];
+          if (BIAS_MODE == 1 || BIAS_MODE == 3) x += __ldg(brow + c);
+          if (BIAS_MODE == 4) x += bb[e];
+          x *= a.scale;
+          if (BIAS_MODE == 2) { const int kh = c / a.Ws, kw = c - kh * a.Ws; x += trow[qh - kh + a.Hs - 1] + trow[32 + qw - kw + a.Ws - 1]; }
+          mx[hr] = fmaxf(mx[hr], x);
+        }
+        sacc[4 * j + 2 * hr + e] = x;
+      }
+    }
+    mx[hr] = tc::quad_max(mx[hr]);
+  }
+  tc::named_bar(3, CONSUMERS);                     // both warpgroups are past MMA 1: Q / K may be overwritten by P (ids 1, 2: per warpgroup)
+  float sum[2] = {0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < MAXK / 8; ++j) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r = wg * 64 + tc::frag_row(2 * hr, w, lane), col = tc::frag_col(4 * j, lane);
+      const float p0 = (col < Sk) ? __expf(sacc[4 * j + 2 * hr] - mx[hr]) : 0.f;
+      const float p1 = (col + 1 < Sk) ? __expf(sacc[4 * j + 2 * hr + 1] - mx[hr]) : 0.f;
+      sum[hr] += p0 + p1;
+      *reinterpret_cast<uint32_t*>(p_s + (col >> 6) * P_SLAB + tc::sw128_offset(r, col & 63)) = tc::pack_bf16(p0, p1);
+    }
+  }
+  tc::fence_proxy_async_smem();
+  tc::named_bar(1 + wg, 128);                      // this warpgroup's P rows are complete
+  // ---------------------------------------------------------------- O = P V
+  float oacc[D / 2];
+  {
+    const uint32_t p_addr = tc::smem_u32(p_s) + wg * (64 * 128), v_addr = tc::smem_u32(v_s);
+    tc::wg_fence();
+    const int ksteps = a.N1 / 16;
+    for (int k = 0; k < ksteps; ++k) {
+      const int sl = k >> 2, kk = k & 3;
+      tc::wgmma_bf16<D>(oacc, tc::wg_desc(p_addr + sl * P_SLAB + kk * 32), tc::wg_desc(v_addr + sl * V_SLAB + kk * 32), k ? 1u : 0u);
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+  }
+  // ---------------------------------------------------------------- epilogue
+  const int m_lim = b * a.Sq + a.Sq;                                   // rows of the next batch are not ours
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const float t = tc::quad_sum(sum[hr]), inv = 1.f / t;
+    const int n = n0 + wg * 64 + tc::frag_row(2 * hr, w, lane), row = b * a.Sq + n;
+    if (a.lse && n < a.Sq && (lane & 3) == 0) a.lse[((size_t)b * a.H + h) * a.Sq + n] = mx[hr] + __logf(t);
+    if (row >= m_lim) continue;
+    OT* orow = reinterpret_cast<OT*>(a.out) + (size_t)row * a.out_ld + h * D;
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j) {
+      const int col = tc::frag_col(4 * j, lane);
+      float o0 = oacc[4 * j + 2 * hr] * inv, o1 = oacc[4 * j + 2 * hr + 1] * inv;
+      if (a.bv) { o0 += __ldg(a.bv + h * D + col); o1 += __ldg(a.bv + h * D + col + 1); }
+      epi::st2(orow + col, o0, o1);
+    }
+  }
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -374,19 +248,11 @@ int make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols, 
 template <int D, int BM, typename OT>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnArgs& a, int B, cudaStream_t st) {
   constexpr int DS = (D + 63) / 64;
-  const int TW = a.Hs + a.Ws;
-  size_t smem = (size_t)DS * QT * 128 + (size_t)DS * a.N1 * 128 + (((size_t)4 * D * 128 + 1023) & ~(size_t)1023) + 4 * QT * 128 + 1024;
-  if (BM == 2) smem += (size_t)QT * TW * sizeof(float) + (size_t)2 * DS * 32 * 128;
-  if (BM == 1 || BM == 3) smem += (size_t)4 * 32 * 33 * sizeof(float);
-  if (kCompact<D, BM>) {                              // [V^T][max(Q + K, P)]
-    const size_t qk = (size_t)DS * QT * 128 + (size_t)DS * a.N1 * 128, pp = (size_t)4 * QT * 128;
-    smem = (size_t)4 * D * 128 + (qk > pp ? qk : pp) + 1024;
-  }
+  size_t smem = (size_t)qkp_bytes<D>(a.N1) + (size_t)4 * D * 128 + 1024;
+  if (BM == 2) smem += (size_t)2 * DS * REL_SLAB + (size_t)QT * SCR_LD * sizeof(float);
   if (smem > 227 * 1024) return S6_EINVAL;
   auto kern = attn_tc_kernel<D, BM, OT>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return (int)e;
-  e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);   // two 97 KB CTAs per SM need the full carve-out
   if (e != cudaSuccess) return (int)e;
   dim3 grid(s6_cdiv(a.Sq, QT), a.H, B);
   cudaError_t le = s6_launch_pdl(kern, grid, dim3(NUM_THREADS), smem, st, tq, tk, tv, a);
@@ -432,7 +298,7 @@ namespace {
 // Q: bf16 matrix (B*Sq rows, q_ld) with head h at columns [q_col0 + h*D, +D); K likewise in (B*Sk rows, k_ld) at k_col0;
 // Vt: bf16 (B*H*D rows, vt_ld >= N1) = V^T per (batch, head): row (b*H + h)*D + c holds channel c over the keys;
 // bias_mode 0 none | 1 dense fp32 (B,H,Sq,Sk) | 2 decomposed rel-pos, Sq = Sk = Hs*Ws, rel_h = the two tables pre-packed as
-// bf16 UMMA slabs (sam6d_b200.ops.pack_rel_pos: 2 x ceil(D/64) x [32 rows][64 ch], 128-byte swizzle), rel_w unused;
+// bf16 wgmma slabs (sam6d_b200.ops.pack_rel_pos: 2 x ceil(D/64) x [32 rows][64 ch], 128-byte swizzle), rel_w unused;
 // bv (H*D) fp32 or NULL; out (B*Sq, H*D) fp32 or bf16 with row stride out_ld.  head_dim 64 or 80, Sk <= 256.
 namespace {
 int attn_tc_launch(const void* Q, long long q_ld, int q_col0, const void* K, long long k_ld, int k_col0, const void* Vt,
@@ -515,8 +381,7 @@ S6_API int sam6d_attn_tc(const void* Q, long long q_ld, int q_col0, const void* 
 }
 
 // sam6d_attn_tc with a dense fp32 bias whose planes are PADDED: (B,H,Sq,bias_ld), bias_ld >= Sk a multiple of 4 floats, base
-// 16-byte aligned (what sam6d_rpe_scores_tc_ld writes).  Head dim 64.  The bias tiles then stream through cp.async, four chunks
-// ahead of the softmax.
+// 16-byte aligned (what sam6d_rpe_scores_tc_ld writes).  Head dim 64.  The bias is then read as aligned column pairs.
 S6_API int sam6d_attn_tc_bias_ld(const void* Q, long long q_ld, int q_col0, const void* K, long long k_ld, int k_col0, const void* Vt,
                                  long long vt_ld, int B, int H, int Sq, int Sk, int head_dim, const float* bias, long long bias_ld,
                                  float scale, void* out, int out_is_bf16, long long out_ld, void* stream) {

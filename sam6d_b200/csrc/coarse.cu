@@ -234,15 +234,11 @@ __global__ void __launch_bounds__(1024) topk_smallest_kernel(const float* __rest
 // (x, y, z, |m|^2) quadruples, so the inner loop is one 16-byte broadcast load and 4 instructions per (hypothesis, point, sample):
 // min_m (|x|^2 - 2 x.m + |m|^2) = |x|^2 + min_m (|m|^2 - 2 x.m), the clamp at 0 commutes with the minimum
 // (pairwise_distance, model_utils.py:98-111).
-// (Measured alternatives: a packed-fp32 FFMA2 variant with 8 hypotheses per CTA, 550 us against 362 us for this one -- FFMA2 issues at
-// half rate; a uniform 8^3 grid over the CAD samples walked shell by shell per thread, bit-identical scores but 3.9 ms -- the
-// walks of a warp's 32 points diverge, and at 1024 samples the regular scan below is only ~110 warp instructions per point.)
+// (Alternatives that lose: a packed-fp32 FFMA2 variant -- FFMA2 issues at half rate; a uniform 8^3 grid over the CAD samples walked
+// shell by shell per thread -- the walks of a warp's 32 points diverge, and at 1024 samples the regular scan below is only ~110 warp
+// instructions per point.)
 constexpr int SEL_PP = 4, SEL_THREADS = 224;
-__device__ __forceinline__ float min3f(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float min3f(float a, float b, float c) { return fminf(fminf(a, b), c); }
 __global__ void __launch_bounds__(SEL_THREADS) coarse_select_kernel(const float* __restrict__ Rt, const int* __restrict__ top, int n1,
                                                                     int n2, const float* __restrict__ pts1, const float* __restrict__ w1,
                                                                     int n, const float* __restrict__ model, int nm,

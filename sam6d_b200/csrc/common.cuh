@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sam6d_b200 kernels (sm_100a only).
+// common.cuh -- shared helpers for the sam6d_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -30,7 +30,7 @@ static inline cudaStream_t s6_stream(void* s) { return reinterpret_cast<cudaStre
 
 // Programmatic dependent launch (PDL).  A step is ~280 launches, many of them 10-us kernels on 12608 token rows: with the
 // launch attribute below the next grid is scheduled as soon as every CTA of the current one has started (s6_pdl_trigger at
-// the top of the kernel), runs its prologue (barrier init, TMEM allocation, descriptor prefetch) on free SMs and blocks in
+// the top of the kernel), runs its prologue (barrier init, shared-memory set-up, descriptor prefetch) on free SMs and blocks in
 // s6_pdl_wait until the predecessor has completed and flushed.  Every kernel launched this way calls s6_pdl_wait before its
 // first global access that may depend on an earlier kernel; kernels launched the ordinary way are unaffected on either side.
 __device__ __forceinline__ void s6_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

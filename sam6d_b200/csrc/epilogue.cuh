@@ -1,19 +1,15 @@
-// epilogue.cuh -- shared TMEM epilogue of the tcgen05 GEMMs.
+// epilogue.cuh -- shared register epilogue of the wgmma GEMMs.
 //
-// A warp owns 32 accumulator rows (its TMEM lane quadrant); per 32-column chunk:
-//   tcgen05.ld (thread = row, 32 columns) -> alpha * acc (+ bias) (activation) (+ residual) -> OT
-// Residual loads and output stores go through a per-warp shared-memory transpose (32 x 32 tile, padded rows) so that every
-// global access is a fully used 128-byte line: with thread-per-row stores each warp instruction touched 32 different lines
-// 16 bytes at a time and the epilogue, not the MMA pipe, set the tile time (1.7 ms vs 0.54 ms on 65536x3840x1280).
+// Input: one 64 x N accumulator fragment of a warpgroup (tc.cuh layout: a thread holds column pairs of four rows).  Per
+// element: alpha * acc (+ bias) (activation) (+ residual) -> OT.  A thread writes its two adjacent columns with one 8-byte
+// (fp32) or 4-byte (bf16) store, so the four lanes of a quad fill 8 adjacent columns of a row and every 32-byte sector of
+// an fp32 output is written whole.
 // Everything that can be decided at compile time is (activation, bias / residual presence): a runtime activation switch
 // if-converts into ~50 predicated erff instructions per element.
 #pragma once
 #include "tc.cuh"
 
 namespace epi {
-
-constexpr int TILE_LD = 36;                       // floats per staged row: 16-byte aligned, conflict-free for LDS/STS.128
-constexpr int WARP_STAGE_FLOATS = 32 * TILE_LD;   // 4.5 KB per warp
 
 template <int ACT>
 __device__ __forceinline__ float act_fn(float x) {
@@ -22,128 +18,47 @@ __device__ __forceinline__ float act_fn(float x) {
   return x;
 }
 
-// v[32]: this thread's row of the chunk.  stage: this warp's WARP_STAGE_FLOATS floats of shared memory.
-// row0: global row of lane 0; col0: first global column of the chunk.  Partial chunks (col0 + 32 > N) take a scalar path.
 template <typename T>
 struct ident { using type = T; };   // keeps RT out of template argument deduction (callers pass nullptr)
 __device__ __forceinline__ float ld_res(const float* p) { return *p; }
 __device__ __forceinline__ float ld_res(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ float2 ld_res2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+__device__ __forceinline__ float2 ld_res2(const __nv_bfloat16* p) { return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p)); }
+__device__ __forceinline__ void st1(float* p, float a) { *p = a; }
+__device__ __forceinline__ void st1(__nv_bfloat16* p, float a) { *p = __float2bfloat16(a); }
+__device__ __forceinline__ void st2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+__device__ __forceinline__ void st2(__nv_bfloat16* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = tc::pack_bf16(a, b); }
 
-template <typename OT, typename RT, bool HAS_RES>
-__device__ __forceinline__ bool chunk_vec_ok(int col0, int N, long long ldc, long long ldr) {
-  return (col0 + 32 <= N) && ((ldc & (sizeof(OT) == 4 ? 3 : 7)) == 0) && (!HAS_RES || (ldr & (sizeof(RT) == 4 ? 3 : 7)) == 0);
-}
-
-// bf16 residual tile of one 32 x 32 chunk in its coalesced register layout: lane l holds 16 B of row (i*8 + l/4), piece l%4.
-// Issued before the accumulator is ready, the loads overlap the tile's TMA and MMA time instead of stalling every chunk.
-__device__ __forceinline__ void prefetch_res_bf16(const __nv_bfloat16* __restrict__ R, long long ldr, int row0, int M, int col0, int lane,
-                                                  uint4 pre[4]) {
+// d: this thread's fragment of a 64 x N accumulator whose row 0 is global row `row0` and column 0 global column `col0`;
+// w: warp index inside the warpgroup.  Only the 8-column groups j in [j_lo, j_hi) are written; rows >= M and columns >= N_lim
+// are skipped.  RT: residual element type.  C, R and bias must allow 2-element accesses at even columns (even ldc / ldr).
+template <typename OT, int ACT, bool HAS_BIAS, bool HAS_RES, typename RT = float, int N>
+__device__ __forceinline__ void store_frag(const float (&d)[N / 2], int w, int lane, int row0, int M, int col0, int N_lim, float alpha,
+                                           const float* __restrict__ bias, const typename ident<RT>::type* __restrict__ R, long long ldr,
+                                           OT* __restrict__ C, long long ldc, int j_lo = 0, int j_hi = N / 8) {
+  const bool pairs = ((ldc & 1) == 0) && (!HAS_RES || (ldr & 1) == 0);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = i * 8 + (lane >> 2), q = lane & 3;
-    pre[i] = make_uint4(0u, 0u, 0u, 0u);
-    if (row0 + r < M) pre[i] = *reinterpret_cast<const uint4*>(R + (size_t)(row0 + r) * ldr + col0 + q * 8);
-  }
-}
-
-// RT: residual element type (fp32, or bf16 for the all-bf16 activation flow).  pre: the chunk's residual from
-// prefetch_res_bf16 (bf16 residual, vector path only) or nullptr.
-template <typename OT, int ACT, bool HAS_BIAS, bool HAS_RES, typename RT = float>
-__device__ __forceinline__ void process_chunk(float v[32], float* stage, int lane, int row0, int M, int col0, int N, float alpha,
-                                              const float* __restrict__ bias, const typename ident<RT>::type* __restrict__ R, long long ldr,
-                                              OT* __restrict__ C, long long ldc, const uint4* pre = nullptr) {
-  const bool vec_ok = chunk_vec_ok<OT, RT, HAS_RES>(col0, N, ldc, ldr);
-  if (vec_ok) {
-    if constexpr (HAS_RES && sizeof(RT) == 2) {
-      // bf16 residual tile: a row of the chunk is 64 bytes; lane l reads 16 B of row (i*8 + l/4), piece l%4
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = col0 + tc::frag_col(4 * j, lane);
+    if (j < j_lo || j >= j_hi || col >= N_lim) continue;
+    const bool two = col + 1 < N_lim;
+    float b0 = 0.f, b1 = 0.f;
+    if constexpr (HAS_BIAS) { b0 = __ldg(bias + col); if (two) b1 = __ldg(bias + col + 1); }
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = i * 8 + (lane >> 2), q = lane & 3;
-        uint4 t = make_uint4(0u, 0u, 0u, 0u);
-        if (pre) t = pre[i];
-        else if (row0 + r < M) t = *reinterpret_cast<const uint4*>(R + (size_t)(row0 + r) * ldr + col0 + q * 8);
-        *reinterpret_cast<uint4*>(stage + r * TILE_LD + q * 4) = t;
-      }
-      __syncwarp();
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint4 t = *reinterpret_cast<const uint4*>(stage + lane * TILE_LD + q * 4);
-        const uint32_t w[4] = {t.x, t.y, t.z, t.w};
-        float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
-        if constexpr (HAS_BIAS) { b0 = __ldg(reinterpret_cast<const float4*>(bias + col0) + 2 * q); b1 = __ldg(reinterpret_cast<const float4*>(bias + col0) + 2 * q + 1); }
-        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          v[q * 8 + 2 * e] = act_fn<ACT>(fmaf(v[q * 8 + 2 * e], alpha, bb[2 * e])) + __uint_as_float(w[e] << 16);
-          v[q * 8 + 2 * e + 1] = act_fn<ACT>(fmaf(v[q * 8 + 2 * e + 1], alpha, bb[2 * e + 1])) + __uint_as_float(w[e] & 0xffff0000u);
-        }
-      }
-      __syncwarp();
-    } else {
-    if constexpr (HAS_RES) {
-      // coalesced residual tile -> smem: lane l reads 16 B of row (i*4 + l/8), float4 column l%8
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3), q = lane & 7;
-        float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < M) t = *reinterpret_cast<const float4*>(R + (size_t)(row0 + r) * ldr + col0 + q * 4);
-        *reinterpret_cast<float4*>(stage + r * TILE_LD + q * 4) = t;
-      }
-      __syncwarp();
-    }
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if constexpr (HAS_BIAS) b4 = __ldg(reinterpret_cast<const float4*>(bias + col0) + q);
-      if constexpr (HAS_RES) r4 = *reinterpret_cast<const float4*>(stage + lane * TILE_LD + q * 4);
-      v[q * 4 + 0] = act_fn<ACT>(fmaf(v[q * 4 + 0], alpha, b4.x)) + r4.x;
-      v[q * 4 + 1] = act_fn<ACT>(fmaf(v[q * 4 + 1], alpha, b4.y)) + r4.y;
-      v[q * 4 + 2] = act_fn<ACT>(fmaf(v[q * 4 + 2], alpha, b4.z)) + r4.z;
-      v[q * 4 + 3] = act_fn<ACT>(fmaf(v[q * 4 + 3], alpha, b4.w)) + r4.w;
-    }
-    if constexpr (HAS_RES) __syncwarp();
-    }
-    if constexpr (sizeof(OT) == 4) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<float4*>(stage + lane * TILE_LD + q * 4) = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3), q = lane & 7;
-        if (row0 + r < M)
-          *reinterpret_cast<float4*>(reinterpret_cast<float*>(C) + (size_t)(row0 + r) * ldc + col0 + q * 4) =
-              *reinterpret_cast<const float4*>(stage + r * TILE_LD + q * 4);
-      }
-    } else {
-      // bf16: a staged row is 64 bytes = 16 words
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(stage + lane * TILE_LD + q * 4) =
-            make_uint4(tc::pack_bf16(v[q * 8], v[q * 8 + 1]), tc::pack_bf16(v[q * 8 + 2], v[q * 8 + 3]),
-                       tc::pack_bf16(v[q * 8 + 4], v[q * 8 + 5]), tc::pack_bf16(v[q * 8 + 6], v[q * 8 + 7]));
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = i * 8 + (lane >> 2), q = lane & 3;
-        if (row0 + r < M)
-          *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(C) + (size_t)(row0 + r) * ldc + col0 + q * 8) =
-              *reinterpret_cast<const uint4*>(stage + r * TILE_LD + q * 4);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int row = row0 + lane;
-    if (row < M) {
-      for (int j = 0; j < 32; ++j) {
-        const int col = col0 + j;
-        if (col < N) {
-          float x = v[j] * alpha;
-          if constexpr (HAS_BIAS) x += bias[col];
-          x = act_fn<ACT>(x);
-          if constexpr (HAS_RES) x += ld_res(R + (size_t)row * ldr + col);
-          if constexpr (sizeof(OT) == 4) reinterpret_cast<float*>(C)[(size_t)row * ldc + col] = x;
-          else reinterpret_cast<__nv_bfloat16*>(C)[(size_t)row * ldc + col] = __float2bfloat16(x);
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + tc::frag_row(2 * h, w, lane);
+      if (row >= M) continue;
+      float x0 = act_fn<ACT>(fmaf(d[4 * j + 2 * h], alpha, b0)), x1 = act_fn<ACT>(fmaf(d[4 * j + 2 * h + 1], alpha, b1));
+      const size_t rc = (size_t)row * ldc + col;
+      if (two && pairs) {
+        if constexpr (HAS_RES) { const float2 r = ld_res2(R + (size_t)row * ldr + col); x0 += r.x; x1 += r.y; }
+        st2(C + rc, x0, x1);
+      } else {
+        if constexpr (HAS_RES) x0 += ld_res(R + (size_t)row * ldr + col);
+        st1(C + rc, x0);
+        if (two) {
+          if constexpr (HAS_RES) x1 += ld_res(R + (size_t)row * ldr + col + 1);
+          st1(C + rc + 1, x1);
         }
       }
     }

@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(256) weighted_procrustes_kernel(const float* _
 }
 
 // pose score (model_utils.py:275-281) and rescaled translation (fine_point_matching.py:80).
-// One thread-block CLUSTER of PS_CS CTAs per proposal (one CTA per proposal left 116 of the 148 SMs idle for the longest
+// One thread-block CLUSTER of PS_CS CTAs per proposal (one CTA per proposal leaves 100 of the 132 SMs idle at 32 proposals for the longest
 // kernel of the tail): each CTA scores a slice of the points against the CAD samples in its shared memory and publishes its
 // two counts (hits, valid points -- integers, so any summation order gives the same result) into CTA 0's distributed
 // shared memory; one cluster barrier later CTA 0 writes the score.

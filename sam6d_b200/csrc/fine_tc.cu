@@ -1,8 +1,8 @@
 // fine_tc.cu -- the dual-softmax assignment of compute_fine_Rt (PEM/utils/model_utils.py:250-283) without the score matrix.
 //
 // The reference forms A = F1 F2^T / temp ((B, 2049, 2049) fp32, 538 MB at B = 32) and walks it about a dozen times.  Here the
-// normalised bf16 tokens are the only inputs and every pass recomputes its score tile on the tensor cores (69 GFLOP per pass,
-// ~40 us of tcgen05 time) and reduces it while it is still in TMEM; nothing of size S x S ever reaches HBM.
+// normalised bf16 tokens are the only inputs and every pass recomputes its score tile on the tensor cores (69 GFLOP per pass)
+// and reduces it while it is still in registers; nothing of size S x S ever reaches HBM.
 //
 //   pass ROWSUM (mode 0)   inv[b,i] = 1 / sum_j e_ij,  e_ij = exp(alpha * <a_i, b_j> - shift)     (shift = 1/temp >= any score)
 //   pass ARGMAX (mode 1)   lab[b,i] = argmax_j P_ij (first maximum),  P_ij = (e_ij * rowf_i) * (e_ij * colf_j)
@@ -12,9 +12,9 @@
 // is the transpose), so compute_fine_Rt is: ROWSUM(F1,F2), ROWSUM(F2,F1), ARGMAX(F2,F1), masked points, ASSIGN(F1,F2).
 //
 // One persistent CTA per SM walks work items (cloud b, 128-row tile); the row tile (4 k-blocks of A, 64 KB) stays in shared
-// memory while the 256-column tiles of B stream through a 4-stage TMA ring; tcgen05.mma M128 N256 K16 into two TMEM
-// accumulators; 8 epilogue warps (two per TMEM lane quadrant, 128 columns each) keep the per-row state in registers across the
-// column tiles and merge their halves through shared memory at the end of the item.
+// memory while the 256-column tiles of B stream through a 4-stage TMA ring fed by one thread of warpgroup 2.  Warpgroup g (warps 4g..4g+3) owns
+// rows [64 g, 64 g + 64) of the item: wgmma m64n256k16 into 128 registers per thread, reduced in place; a thread keeps the state
+// of its two rows across the column tiles, and the four threads of a row merge theirs with quad shuffles at the end of the item.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -24,7 +24,7 @@ namespace {
 
 constexpr int BM = 128, BN = 256, BK = 64, KB = 4, STAGES = 4;       // K = 256 channels
 constexpr int A_KB = BM * BK * 2, B_KB = BN * BK * 2;
-constexpr int NUM_THREADS = 64 + 256;
+constexpr int CONSUMERS = 256, NUM_THREADS = CONSUMERS + 128;
 constexpr int SMEM_BYTES = KB * A_KB + STAGES * B_KB + 1024;
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -44,18 +44,14 @@ __device__ __forceinline__ float ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 template <int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                   const __grid_constant__ CUtensorMap tmB, FArgs g) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, FArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* a_res = smem;                       // 4 k-block slabs [128][64] of the row tile
   uint8_t* ring = smem + KB * A_KB;            // stages of [256][64]
-  __shared__ __align__(8) uint64_t a_full, a_empty, full_bar[STAGES], empty_bar[STAGES], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
-  __shared__ float comb[2][BM][6];             // upper-half partial state of each row, double-buffered over items
+  __shared__ __align__(8) uint64_t a_full, a_empty, full_bar[STAGES], empty_bar[STAGES];
   __shared__ float sc[2][BN];                  // column factors of the current / next column tile (modes 1, 2)
   __shared__ __align__(16) float4 sq[2][BN];   // masked template points of the tile (mode 2)
 
@@ -64,22 +60,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_
   const int items = g.B * m_tiles;
 
   if (tid == 0) {
-    tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, 1);
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tmem_full_bar[a], 1); tc::mbar_init(&tmem_empty_bar[a], 256); }
+    tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, CONSUMERS / 32);
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], CONSUMERS / 32); }
     tc::mbar_fence_init();
     tc::tma_prefetch_desc(&tmA);
     tc::tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (warp >= CONSUMERS / 32) {
+    // ------------------------------------------------------------------ TMA producer (one thread of the third warpgroup)
+    tc::producer_regs();
+    if (tid == CONSUMERS) {
       long long gk = 0;
       int it = 0;
       for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
@@ -96,112 +88,96 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_
           }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(BM, BN);
-      const uint32_t a_addr = tc::smem_u32(a_res);
-      long long gk = 0, tcount = 0;
-      int it = 0;
-      for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
-        tc::mbar_wait(&a_full, (uint32_t)(it & 1));
-        tc::tc_fence_after_sync();
-        for (int nt = 0; nt < n_tiles; ++nt, ++tcount) {
-          const int acc = (int)(tcount & 1);
-          tc::mbar_wait(&tmem_empty_bar[acc], (uint32_t)(((tcount >> 1) & 1) ^ 1));
-          tc::tc_fence_after_sync();
-          const uint32_t d_addr = tmem_base + (uint32_t)(acc * BN);
-          for (int kb = 0; kb < KB; ++kb, ++gk) {
-            const int s = (int)(gk % STAGES);
-            tc::mbar_wait(&full_bar[s], (uint32_t)((gk / STAGES) & 1));
-            tc::tc_fence_after_sync();
-            const uint32_t b_addr = tc::smem_u32(ring + s * B_KB);
+    return;
+  }
+  // ------------------------------------------------------------------ consumers: thread = (two rows of the item, column pairs)
+  tc::consumer_regs();
+  const int wg = warp >> 2, w = warp & 3;
+  const uint32_t a_addr = tc::smem_u32(a_res) + wg * (64 * 128);
+  long long gk = 0, tcount = 0;
+  int it = 0;
+  for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
+    const int b = item / m_tiles, mt = item - b * m_tiles;
+    float rf[2] = {0.f, 0.f};
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              tc::umma_bf16(d_addr, tc::umma_desc_sw128(a_addr + kb * A_KB + k * 32), tc::umma_desc_sw128(b_addr + k * 32), idesc,
-                            (kb | k) ? 1u : 0u);
-            tc::umma_commit(&empty_bar[s]);
-          }
-          tc::umma_commit(&tmem_full_bar[acc]);
+    for (int hr = 0; hr < 2; ++hr) {
+      const int i = mt * BM + wg * 64 + tc::frag_row(2 * hr, w, lane);      // row index inside the cloud
+      if (MODE != 0 && i < g.S) rf[hr] = g.row_f[(size_t)b * g.ld_f + i];
+    }
+    const float* cf = (MODE != 0) ? g.col_f + (size_t)b * g.ld_f : nullptr;
+    const float4* q4 = (MODE == 2) ? g.q4 + (size_t)b * g.ld_f : nullptr;
+    float sum[2] = {0.f, 0.f}, bv[2] = {-INFINITY, -INFINITY}, ws[2] = {0.f, 0.f}, px[2] = {0.f, 0.f}, py[2] = {0.f, 0.f}, pz[2] = {0.f, 0.f};
+    int bi[2] = {0x7fffffff, 0x7fffffff};
+    tc::mbar_wait(&a_full, (uint32_t)(it & 1));
+    for (int nt = 0; nt < n_tiles; ++nt, ++tcount) {
+      const int buf = (int)(tcount & 1);
+      if (MODE != 0) {
+        // stage the tile's 256 column factors (and masked points) once per CTA; the element loop then reads them as
+        // shared-memory broadcasts instead of two dependent global loads per element
+        const int j = nt * BN + tid;
+        sc[buf][tid] = (j < g.S) ? cf[j] : 0.f;
+        if (MODE == 2) sq[buf][tid] = (j < g.S) ? q4[j] : make_float4(0.f, 0.f, 0.f, 0.f);
+        tc::named_bar(1, CONSUMERS);
+      }
+      float acc[BN / 2];
+      int prev = -1;
+      for (int kb = 0; kb < KB; ++kb, ++gk) {
+        const int s = (int)(gk % STAGES);
+        tc::mbar_wait(&full_bar[s], (uint32_t)((gk / STAGES) & 1));
+        const uint32_t b_addr = tc::smem_u32(ring + s * B_KB);
+        tc::wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          tc::wgmma_bf16<BN>(acc, tc::wg_desc(a_addr + kb * A_KB + k * 32), tc::wg_desc(b_addr + k * 32), (kb | k) ? 1u : 0u);
+        tc::wg_commit();
+        if (prev >= 0) {
+          tc::wg_wait<1>();
+          if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
         }
-        tc::umma_commit(&a_empty);
+        prev = s;
+      }
+      tc::wg_wait<0>();
+      if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+      if (nt == n_tiles - 1 && lane == 0) tc::mbar_arrive(&a_empty);   // the row tile is no longer read
+#pragma unroll
+      for (int e = 0; e < BN / 2; ++e) {
+        const int hr = (e >> 1) & 1, cl = tc::frag_col(e, lane), j = nt * BN + cl;
+        const float ev = (j < g.S) ? ex2(fmaf(acc[e], g.a2, -g.s2)) : 0.f;
+        if (MODE == 0) {
+          sum[hr] += ev;
+        } else {
+          const float p = (ev * rf[hr]) * (ev * sc[buf][cl]);         // column factor 0 past the last column
+          if (p > bv[hr]) { bv[hr] = p; bi[hr] = j; }                 // ascending j inside this thread: first maximum
+          if (MODE == 2) {
+            const float4 q = sq[buf][cl];
+            const float pm = p * q.w;
+            ws[hr] += pm; px[hr] = fmaf(pm, q.x, px[hr]); py[hr] = fmaf(pm, q.y, py[hr]); pz[hr] = fmaf(pm, q.z, pz[hr]);
+          }
+        }
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue: thread = (row of the tile, column half)
-    const int quad = warp & 3, half = (warp - 2) >> 2;               // warps 2..9: quadrants 2,3,0,1,2,3,0,1
-    const int row = quad * 32 + lane;
-    long long tcount = 0;
-    int it = 0;
-    for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
-      const int b = item / m_tiles, mt = item - b * m_tiles;
-      const int i = mt * BM + row;                                   // row index inside the cloud
-      float rf = 0.f;
-      if (MODE != 0 && i < g.S) rf = g.row_f[(size_t)b * g.ld_f + i];
-      const float* cf = (MODE != 0) ? g.col_f + (size_t)b * g.ld_f : nullptr;
-      const float4* q4 = (MODE == 2) ? g.q4 + (size_t)b * g.ld_f : nullptr;
-      float sum = 0.f, bv = -INFINITY, w = 0.f, px = 0.f, py = 0.f, pz = 0.f;
-      int bi = 0x7fffffff;
-      for (int nt = 0; nt < n_tiles; ++nt, ++tcount) {
-        const int acc = (int)(tcount & 1);
-        if (MODE != 0) {
-          // stage the tile's 256 column factors (and masked points) once per CTA while the MMAs of the tile run; the
-          // element loop then reads them as shared-memory broadcasts instead of two dependent global loads per element
-          const int et = tid - 64, j = nt * BN + et;
-          sc[acc][et] = (j < g.S) ? cf[j] : 0.f;
-          if (MODE == 2) sq[acc][et] = (j < g.S) ? q4[j] : make_float4(0.f, 0.f, 0.f, 0.f);
-          epi_bar();
-        }
-        tc::mbar_wait(&tmem_full_bar[acc], (uint32_t)((tcount >> 1) & 1));
-        tc::tc_fence_after_sync();
-        const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + half * 128);
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          const int j0 = nt * BN + half * 128 + c * 32;
-          if (j0 >= g.S) break;                                       // uniform: whole chunk past the last column
-          float v[32];
-          tc::tmem_ld32(t_addr + c * 32, v);
+    // ---- merge the four threads of every row (they hold interleaved columns: compare indices so that the first maximum wins)
 #pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const int j = j0 + k;
-            const float e = (j < g.S) ? ex2(fmaf(v[k], g.a2, -g.s2)) : 0.f;
-            if (MODE == 0) {
-              sum += e;
-            } else {
-              const float cj = sc[acc][half * 128 + c * 32 + k];      // 0 past the last column
-              const float p = (e * rf) * (e * cj);
-              if (p > bv) { bv = p; bi = j; }                         // ascending j inside this thread: first maximum
-              if (MODE == 2) {
-                const float4 q = sq[acc][half * 128 + c * 32 + k];
-                const float pm = p * q.w;
-                w += pm; px = fmaf(pm, q.x, px); py = fmaf(pm, q.y, py); pz = fmaf(pm, q.z, pz);
-              }
-            }
-          }
+    for (int hr = 0; hr < 2; ++hr) {
+      const int i = mt * BM + wg * 64 + tc::frag_row(2 * hr, w, lane);
+      if (MODE == 0) {
+        const float t = tc::quad_sum(sum[hr]);
+        if ((lane & 3) == 0 && i < g.S) g.out_inv[(size_t)b * g.ld_f + i] = 1.f / t;
+      } else {
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, bv[hr], o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi[hr], o);
+          if (ov > bv[hr] || (ov == bv[hr] && oi < bi[hr])) { bv[hr] = ov; bi[hr] = oi; }
         }
-        tc::tc_fence_before_sync();
-        tc::mbar_arrive(&tmem_empty_bar[acc]);
-      }
-      // ---- merge the two column halves of every row (the lower half scanned the lower columns of each tile, but tiles
-      // interleave: compare indices explicitly so that the first maximum wins)
-      float* cb = comb[it & 1][row];
-      if (half == 1) {
-        if (MODE == 0) cb[0] = sum;
-        else { cb[0] = bv; cb[1] = __int_as_float(bi); if (MODE == 2) { cb[2] = w; cb[3] = px; cb[4] = py; cb[5] = pz; } }
-      }
-      epi_bar();
-      if (half == 0 && i < g.S) {
-        if (MODE == 0) {
-          g.out_inv[(size_t)b * g.ld_f + i] = 1.f / (sum + cb[0]);
-        } else {
-          const float ov = cb[0];
-          const int oi = __float_as_int(cb[1]);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-          if (bi == 0x7fffffff) bi = 0;
-          g.lab[(size_t)b * g.S + i] = bi;
+        float ww = 0.f, qx = 0.f, qy = 0.f, qz = 0.f;
+        if (MODE == 2) { ww = tc::quad_sum(ws[hr]); qx = tc::quad_sum(px[hr]); qy = tc::quad_sum(py[hr]); qz = tc::quad_sum(pz[hr]); }
+        if ((lane & 3) == 0 && i < g.S) {
+          int lb = bi[hr];
+          if (lb == 0x7fffffff) lb = 0;
+          g.lab[(size_t)b * g.S + i] = lb;
           if (MODE == 2 && i >= 1) {
-            float ww = w + cb[2], qx = px + cb[3], qy = py + cb[4], qz = pz + cb[5];
-            if (bi == 0) { ww = 0.f; qx = 0.f; qy = 0.f; qz = 0.f; }    // background label: the row carries no weight
+            if (lb == 0) { ww = 0.f; qx = 0.f; qy = 0.f; qz = 0.f; }    // background label: the row carries no weight
             const size_t o = (size_t)b * (g.S - 1) + (i - 1);
             const float d = ww + 1e-6f;
             g.wts[o] = ww;
@@ -211,9 +187,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_
       }
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

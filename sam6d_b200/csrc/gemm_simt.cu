@@ -1,6 +1,6 @@
 // gemm_simt.cu -- fp32 CUDA-core GEMM  C = act(A W^T + bias) (+ R)  with strided batches.
 //
-// This is the exact-precision path (and the comparator for the tcgen05 bf16 path): every Linear /
+// This is the exact-precision path (and the comparator for the wgmma bf16 path): every Linear /
 // 1x1-conv of the matching stage maps onto it.  A is (M,K) row-major with row stride lda, W is
 // (N,K) row-major (nn.Linear layout) with row stride ldw, C is (M,N) with row stride ldc.  A batch
 // index z = blockIdx.z offsets A, W, C, R by their batch strides (0 = shared operand).

@@ -1,13 +1,12 @@
-// gemm_tc.cu -- bf16 tensor-core GEMM on tcgen05 (UMMA) with fp32 accumulation in TMEM:
+// gemm_tc.cu -- bf16 tensor-core GEMM on wgmma with fp32 accumulation in registers:
 //     C[z] = alpha * A[z] W[z]^T (+ bias) (ReLU) (+ R[z])
 // Same contract as sam6d_gemm_f32 (gemm_simt.cu); A and W may be fp32 (converted to bf16 while staging) or bf16, C fp32 or bf16.
 //
-// CTA = one 128 x 256 output tile, 9 warps, warp-specialised:
-//   warps 4-7  producers : coalesced 16-byte global loads -> bf16 -> st.shared into K-major, 128B-swizzled [rows][64] slabs
-//                          (the canonical UMMA layout a TMA SWIZZLE_128B box would produce), 2-stage mbarrier ring
-//   warp  8    MMA issuer: one thread issues 4 x tcgen05.mma (M128 N256 K16) per 64-wide k-block, tcgen05.commit frees the stage
-//   warps 0-3  epilogue  : tcgen05.ld 32 lanes x 32 columns -> bias / ReLU / residual -> global
-// Two CTAs fit per SM (2 x 98 KB smem, 2 x 256 TMEM columns) so one tile's epilogue overlaps the other's loads and MMAs.
+// CTA = one 128 x 256 output tile, 12 warps, warp-specialised:
+//   warps 8-11 producers : coalesced 16-byte global loads -> bf16 -> st.shared into K-major, 128B-swizzled [rows][64] slabs
+//                          (the layout a TMA SWIZZLE_128B box would produce), 2-stage mbarrier ring
+//   warps 0-7  consumers : warpgroup g owns rows [64 g, 64 g + 64): 4 x wgmma m64n256k16 per 64-wide k-block, then
+//                          bias / ReLU / residual -> global straight from the accumulator registers (epilogue.cuh)
 #include "epilogue.cuh"
 #include "tc.cuh"
 
@@ -15,7 +14,7 @@ namespace {
 
 constexpr int BM = 128, BN = 256, BK = 64, STAGES = 2;
 constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int NUM_THREADS = 288;
+constexpr int CONSUMERS = 256, NUM_THREADS = CONSUMERS + 128;
 
 struct TcArgs {
   const void* A; const void* W; const float* bias; const float* R; void* C;
@@ -26,8 +25,8 @@ struct TcArgs {
 };
 
 // stage `rows` x 64 of a row-major (rows_total, K) operand into a swizzled slab; zero-fill out-of-range rows / columns.
-// All global loads of a batch are issued before the first use (16 x 16-byte loads in flight per thread) -- with the loads
-// interleaved with the conversion the kernel was latency-bound at ~8 GB/s per CTA.
+// All global loads of a batch are issued before the first use (16 x 16-byte loads in flight per thread): with the loads
+// interleaved with the conversion every load's latency is exposed.
 template <typename T, int ROWS>
 __device__ __forceinline__ void stage_tile(const T* __restrict__ base, long long ld, int row0, int rows_total, int k0, int K,
                                            uint8_t* __restrict__ slab, int ptid) {
@@ -73,11 +72,10 @@ __device__ __forceinline__ void stage_tile(const T* __restrict__ base, long long
 }
 
 template <typename AT, typename WT, typename OT, int ACT, bool HAS_BIAS, bool HAS_RES>
-__global__ void __launch_bounds__(NUM_THREADS, 2) gemm_tc_kernel(TcArgs g) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(TcArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int z = blockIdx.z, m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
@@ -86,19 +84,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 2) gemm_tc_kernel(TcArgs g) {
   const int nkb = (g.K + BK - 1) / BK;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 128); tc::mbar_init(&empty_bar[s], 1); }
-    tc::mbar_init(&tmem_full_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 128); tc::mbar_init(&empty_bar[s], CONSUMERS / 32); }
     tc::mbar_fence_init();
   }
-  if (warp == 8) tc::tmem_alloc(&tmem_slot, BN);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp >= 4 && warp < 8) {
+  if (tid >= CONSUMERS) {
     // ------------------------------------------------------------------ producers
-    const int ptid = tid - 128;
+    const int ptid = tid - CONSUMERS;
     for (int kb = 0; kb < nkb; ++kb) {
       const int s = kb % STAGES;
       tc::mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
@@ -109,44 +102,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 2) gemm_tc_kernel(TcArgs g) {
       tc::fence_proxy_async_smem();
       tc::mbar_arrive(&full_bar[s]);
     }
-  } else if (warp == 8) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(BM, BN);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % STAGES;
-        tc::mbar_wait(&full_bar[s], (kb / STAGES) & 1);
-        tc::tc_fence_after_sync();
-        const uint32_t a_addr = tc::smem_u32(smem + s * STAGE_BYTES), b_addr = a_addr + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          tc::umma_bf16(tmem_base, tc::umma_desc_sw128(a_addr + k * 32), tc::umma_desc_sw128(b_addr + k * 32), idesc,
-                        (kb | k) ? 1u : 0u);
-        }
-        tc::umma_commit(&empty_bar[s]);
-      }
-      tc::umma_commit(&tmem_full_bar);
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 0-3 <-> TMEM lanes 32w..32w+31)
-    tc::mbar_wait(&tmem_full_bar, 0);
-    tc::tc_fence_after_sync();
-    // all MMAs of this (single) tile have completed, so the operand ring is free: reuse it as the store-transpose staging
-    float* stage = reinterpret_cast<float*>(smem) + warp * epi::WARP_STAGE_FLOATS;
-    OT* Cz = reinterpret_cast<OT*>(g.C) + (size_t)z * g.sC;
-    const float* Rz = g.R ? g.R + (size_t)z * g.sR : nullptr;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      const int col0 = n0 + c * 32;
-      if (col0 >= g.N) break;
-      float v[32];
-      tc::tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(c * 32), v);
-      epi::process_chunk<OT, ACT, HAS_BIAS, HAS_RES>(v, stage, lane, m0 + warp * 32, g.M, col0, g.N, g.alpha, g.bias, Rz, g.ldr, Cz, g.ldc);
-    }
+    return;
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc(tmem_base, BN);
+  // ------------------------------------------------------------------ consumers: warpgroup wg <-> rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, w = warp & 3;
+  float acc[BN / 2];
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb % STAGES;
+    tc::mbar_wait(&full_bar[s], (kb / STAGES) & 1);
+    const uint32_t a_addr = tc::smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128), b_addr = tc::smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) tc::wgmma_bf16<BN>(acc, tc::wg_desc(a_addr + k * 32), tc::wg_desc(b_addr + k * 32), (kb | k) ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&empty_bar[s]);
+  }
+  OT* Cz = reinterpret_cast<OT*>(g.C) + (size_t)z * g.sC;
+  const float* Rz = g.R ? g.R + (size_t)z * g.sR : nullptr;
+  epi::store_frag<OT, ACT, HAS_BIAS, HAS_RES, float, BN>(acc, w, lane, m0 + wg * 64, g.M, n0, g.N, g.alpha, g.bias, Rz, g.ldr, Cz, g.ldc);
 }
 
 template <typename AT, typename WT, typename OT>

@@ -1,16 +1,13 @@
-// gemm_tma.cu -- persistent, TMA-fed bf16 GEMM on tcgen05:   C = act(A W^T + bias) (+ R),   A (M,K) bf16, W (N,K) bf16.
+// gemm_tma.cu -- persistent, TMA-fed bf16 GEMM on wgmma:   C = act(A W^T + bias) (+ R),   A (M,K) bf16, W (N,K) bf16.
 //
 // One CTA per SM loops over 128 x 256 output tiles (m fastest, so CTAs running together share the same W tile in L2):
-//   warp 0   TMA producer : cp.async.bulk.tensor 2-D boxes {64 k, 128 rows} of A and {64 k, 256 rows} of W, SWIZZLE_128B,
-//                           straight into the UMMA K-major slabs of a 4-stage ring (48 KB per stage); out-of-range rows /
-//                           columns are zero-filled by the TMA unit
-//   warp 1   MMA issuer   : 4 x tcgen05.mma M128 N256 K16 per stage into one of two 256-column TMEM accumulators,
-//                           tcgen05.commit releases the stage / publishes the accumulator
-//   warps 2..  epilogue   : tcgen05.ld -> alpha, bias, activation, residual -> fp32 or bf16, transposed through shared memory
-//                           into full-line global stores (epilogue.cuh); overlaps the next tile's loads and MMAs through
-//                           the second accumulator
-// No register staging and no LSU traffic for the operands: the CUDA-core staged kernel (gemm_tc.cu) tops out near 8 GB/s per
-// CTA of operand traffic, this one is bounded by L2 -> SM bandwidth and the tensor pipe.
+//   warp 8      TMA producer : (one thread; its warpgroup hands its registers to the two below) cp.async.bulk.tensor 2-D boxes {64 k, 128 rows} of A and {64 k, 256 rows} of W, SWIZZLE_128B,
+//                              straight into the K-major slabs of a 4-stage ring (48 KB per stage); out-of-range rows /
+//                              columns are zero-filled by the TMA unit
+//   warps 0..7  two consumer warpgroups: warpgroup g owns rows [64 g, 64 g + 64) of the tile, 4 x wgmma m64n256k16 per stage
+//                              into 128 fp32 registers per thread; one wgmma group stays in flight while the stage before it is
+//                              released; then alpha, bias, activation, residual -> fp32 or bf16 straight from the registers
+//                              (epilogue.cuh) while the producer already fills the ring with the next tile
 #include <cuda.h>
 
 #include "epilogue.cuh"
@@ -18,18 +15,10 @@
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 64;
+constexpr int BM = 128, BN = 256, BK = 64, STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
-// Two shapes of the same kernel (227 KB of shared memory decide the split):
-//   deep K  (K >= 1024, the ViT-H Linears): 4-stage ring, 4 epilogue warps -- the MMAs of a tile outlast its epilogue
-//   short K (the 256/512-wide PEM Linears): a tile is 4-8 k-blocks, the epilogue sets the pace -> 8 epilogue warps (two per
-//           TMEM lane quadrant, 4 column chunks each), 3-stage ring
-template <int STAGES, int EW>
-struct Cfg {
-  static constexpr int kThreads = 64 + EW * 32;
-  static constexpr int kEpiBytes = EW * epi::WARP_STAGE_FLOATS * 4;
-  static constexpr int kSmem = STAGES * STAGE_BYTES + kEpiBytes + 1024;
-};
+constexpr int CONSUMERS = 256, THREADS = CONSUMERS + 128;
+constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
 
 struct Args {
   const float* bias; const void* R; void* C;   // R has the element type of C
@@ -48,13 +37,12 @@ struct Args {
   int vt_col1; void* c2; long long ldc2;
 };
 
-template <typename OT, int ACT, bool HAS_BIAS, bool HAS_RES, int STAGES, int EW, bool VT = false>
-__global__ void __launch_bounds__(64 + EW * 32, 1) gemm_tma_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                   const __grid_constant__ CUtensorMap tmW, Args g) {
+template <typename OT, int ACT, bool HAS_BIAS, bool HAS_RES, bool VT = false>
+__global__ void __launch_bounds__(THREADS, 1) gemm_tma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                              const __grid_constant__ CUtensorMap tmW, Args g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
@@ -62,23 +50,19 @@ __global__ void __launch_bounds__(64 + EW * 32, 1) gemm_tma_kernel(const __grid_
   const int nkb = (g.K + BK - 1) / BK;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tmem_full_bar[a], 1); tc::mbar_init(&tmem_empty_bar[a], EW * 32); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], CONSUMERS / 32); }
     tc::mbar_fence_init();
     tc::tma_prefetch_desc(&tmA);
     tc::tma_prefetch_desc(&tmW);
   }
   s6_pdl_trigger();
-  if (warp == 1) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   s6_pdl_wait();                                   // operands / residual may come from the kernel before us
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (warp >= CONSUMERS / 32) {
+    // ------------------------------------------------------------------ TMA producer (one thread of the third warpgroup)
+    tc::producer_regs();
+    if (tid == CONSUMERS) {
       long long gk = 0;
       for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long long bz = tile / tpb, t = tile - bz * tpb;
@@ -94,109 +78,67 @@ __global__ void __launch_bounds__(64 + EW * 32, 1) gemm_tma_kernel(const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(BM, BN);
-      long long gk = 0, it = 0;
-      for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int acc = (int)(it & 1);
-        tc::mbar_wait(&tmem_empty_bar[acc], (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc::tc_fence_after_sync();
-        const uint32_t d_addr = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < nkb; ++kb, ++gk) {
-          const int s = (int)(gk % STAGES);
-          tc::mbar_wait(&full_bar[s], (uint32_t)((gk / STAGES) & 1));
-          tc::tc_fence_after_sync();
-          const uint32_t a_addr = tc::smem_u32(smem + s * STAGE_BYTES), b_addr = a_addr + A_BYTES;
+    return;
+  }
+  // ------------------------------------------------------------------ consumers: warpgroup wg <-> rows [64 wg, 64 wg + 64)
+  tc::consumer_regs();
+  const int wg = warp >> 2, w = warp & 3;
+  float acc[BN / 2];
+  long long gk = 0;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long bz = tile / tpb, t = tile - bz * tpb;
+    const int m0 = (int)(t % m_tiles) * BM, n0 = (int)(t / m_tiles) * BN;
+    int prev = -1;
+    for (int kb = 0; kb < nkb; ++kb, ++gk) {
+      const int s = (int)(gk % STAGES);
+      tc::mbar_wait(&full_bar[s], (uint32_t)((gk / STAGES) & 1));
+      const uint32_t a_addr = tc::smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128), b_addr = tc::smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+      tc::wg_fence();
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            tc::umma_bf16(d_addr, tc::umma_desc_sw128(a_addr + k * 32), tc::umma_desc_sw128(b_addr + k * 32), idesc, (kb | k) ? 1u : 0u);
-          tc::umma_commit(&empty_bar[s]);
-        }
-        tc::umma_commit(&tmem_full_bar[acc]);
+      for (int k = 0; k < BK / 16; ++k) tc::wgmma_bf16<BN>(acc, tc::wg_desc(a_addr + k * 32), tc::wg_desc(b_addr + k * 32), (kb | k) ? 1u : 0u);
+      tc::wg_commit();
+      if (prev >= 0) {
+        tc::wg_wait<1>();                          // the previous stage's MMAs are complete: hand it back to the producer
+        if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
       }
+      prev = s;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue: warp w -> TMEM lanes 32*(w%4) ..
-    const int quad = warp & 3;
-    const int c_lo = (EW == 8) ? ((warp - 2) >> 2) * (BN / 64) : 0, c_hi = (EW == 8) ? c_lo + BN / 64 : BN / 32;
-    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES) + (warp - 2) * epi::WARP_STAGE_FLOATS;
-    long long it = 0;
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = (int)(it & 1);
-      const long long bz = tile / tpb, t = tile - bz * tpb;
-      const int m0 = (int)(t % m_tiles) * BM, n0 = (int)(t / m_tiles) * BN;
-      OT* Cb = reinterpret_cast<OT*>(g.C) + bz * g.c_bs;
-      const OT* Rb = reinterpret_cast<const OT*>(g.R) + bz * g.r_bs;
-      constexpr bool PRE = HAS_RES && (sizeof(OT) == 2) && (EW == 8);   // short-K tiles with a bf16 residual stream
-      uint4 pre[PRE ? 4 : 1][4];
-      if constexpr (PRE) {
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+
+    const int row0 = m0 + wg * 64;
+    OT* Cb = reinterpret_cast<OT*>(g.C) + bz * g.c_bs;
+    const OT* Rb = reinterpret_cast<const OT*>(g.R) + bz * g.r_bs;
+    if constexpr (VT) {
+      // 8-column groups below vt_col0 -> C, [vt_col0, vt_col1) -> V^T (transposed per cloud), from vt_col1 -> c2; the group
+      // boundaries are multiples of 32 columns, so no group straddles two outputs
+      const int jv = min(max((g.vt_col0 - n0) / 8, 0), BN / 8), ju = min(max((g.vt_col1 - n0) / 8, 0), BN / 8);
+      epi::store_frag<OT, ACT, HAS_BIAS, false, OT, BN>(acc, w, lane, row0, g.M, n0, g.N, g.alpha, g.bias, nullptr, 0, Cb, g.ldc, 0, jv);
+      epi::store_frag<OT, ACT, HAS_BIAS, false, OT, BN>(acc, w, lane, row0, g.M, n0 - g.vt_col1, g.N - g.vt_col1, g.alpha,
+                                                        g.bias ? g.bias + g.vt_col1 : nullptr, nullptr, 0, reinterpret_cast<OT*>(g.c2),
+                                                        g.ldc2, ju, BN / 8);
 #pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          const int col0 = n0 + (c_lo + cc) * 32;
-          if (epi::chunk_vec_ok<OT, OT, true>(col0, g.N, g.ldc, g.ldr))
-            epi::prefetch_res_bf16(reinterpret_cast<const __nv_bfloat16*>(Rb), g.ldr, m0 + quad * 32, g.M, col0, lane, pre[cc]);
+      for (int j = 0; j < BN / 8; ++j) {
+        if (j < jv || j >= ju) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + tc::frag_row(2 * h, w, lane);
+          if (row >= g.M) continue;
+          const int cloud = row / g.vt_S, tok = row - cloud * g.vt_S;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = n0 + tc::frag_col(4 * j + e, lane);
+            float x = acc[4 * j + 2 * h + e] * g.alpha;
+            if constexpr (HAS_BIAS) x += __ldg(g.bias + col);
+            reinterpret_cast<__nv_bfloat16*>(g.vt)[((size_t)cloud * g.vt_C + (col - g.vt_col0)) * g.vt_N1 + tok] =
+                __float2bfloat16(epi::act_fn<ACT>(x));
+          }
         }
       }
-      tc::mbar_wait(&tmem_full_bar[acc], (uint32_t)((it >> 1) & 1));
-      tc::tc_fence_after_sync();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      if constexpr (PRE) {
-#pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          const int c = c_lo + cc, col0 = n0 + c * 32;
-          if (col0 < g.N) {
-            float v[32];
-            tc::tmem_ld32(t_addr + c * 32, v);
-            if (epi::chunk_vec_ok<OT, OT, true>(col0, g.N, g.ldc, g.ldr))   // two call sites: `pre` stays in registers
-              epi::process_chunk<OT, ACT, HAS_BIAS, HAS_RES, OT>(v, stage, lane, m0 + quad * 32, g.M, col0, g.N, g.alpha, g.bias,
-                                                                 Rb, g.ldr, Cb,
-                                                                 g.ldc, pre[cc]);
-            else
-              epi::process_chunk<OT, ACT, HAS_BIAS, HAS_RES, OT>(v, stage, lane, m0 + quad * 32, g.M, col0, g.N, g.alpha, g.bias,
-                                                                 Rb, g.ldr, Cb,
-                                                                 g.ldc);
-          }
-        }
-      } else {
-        [[maybe_unused]] const int vrow = m0 + quad * 32 + lane, vcloud = VT ? vrow / g.vt_S : 0, vtok = VT ? vrow - vcloud * g.vt_S : 0;
-#pragma unroll 1
-        for (int c = c_lo; c < c_hi; ++c) {
-          const int col0 = n0 + c * 32;
-          if (col0 >= g.N) break;
-          float v[32];
-          tc::tmem_ld32(t_addr + c * 32, v);
-          if (VT && col0 >= g.vt_col1) {
-            epi::process_chunk<OT, ACT, HAS_BIAS, HAS_RES, OT>(v, stage, lane, m0 + quad * 32, g.M, col0, g.N, g.alpha, g.bias, Rb, g.ldr,
-                                                               reinterpret_cast<OT*>(g.c2) - g.vt_col1, g.ldc2);
-            continue;
-          }
-          if (VT && col0 >= g.vt_col0) {
-            // lane = token: 32 lanes write 32 adjacent tokens of one channel row (64 bytes) per store
-            if (vrow < g.M) {
-              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.vt) + ((size_t)vcloud * g.vt_C + (col0 - g.vt_col0)) * g.vt_N1 + vtok;
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < g.vt_col1) {
-                  float x = v[i] * g.alpha;
-                  if constexpr (HAS_BIAS) x += __ldg(g.bias + col0 + i);
-                  dst[(size_t)i * g.vt_N1] = __float2bfloat16(epi::act_fn<ACT>(x));
-                }
-            }
-            continue;
-          }
-          epi::process_chunk<OT, ACT, HAS_BIAS, HAS_RES, OT>(v, stage, lane, m0 + quad * 32, g.M, col0, g.N, g.alpha, g.bias,
-                                                             Rb, g.ldr, Cb, g.ldc);
-        }
-      }
-      tc::tc_fence_before_sync();
-      tc::mbar_arrive(&tmem_empty_bar[acc]);
+    } else {
+      epi::store_frag<OT, ACT, HAS_BIAS, HAS_RES, OT, BN>(acc, w, lane, row0, g.M, n0, g.N, g.alpha, g.bias, Rb, g.ldr, Cb, g.ldc);
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -256,20 +198,15 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
   Args g{bias, R, C, M, N, K, ldc, ldr, alpha, act, batch, a_rpb, w_rpb, c_bs, r_bs, vt, vt_col0, vt_S, vt_N1, vt_col1 - vt_col0,
          vt_col1, c2, ldc2};
   cudaStream_t st = s6_stream(stream);
-  const bool deep_k = K >= 1024;
-#define LAUNCH_ONE(OT, ACT, HB, HR, ST, EWN)                                                                           \
+#define LAUNCH_ONE(OT, ACT, HB, HR, VTK)                                                                               \
   do {                                                                                                                 \
-    auto k = gemm_tma_kernel<OT, ACT, HB, HR, ST, EWN>;                                                                \
-    S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<ST, EWN>::kSmem));               \
-    S6_CHECK(s6_launch_pdl(k, dim3(grid), dim3(Cfg<ST, EWN>::kThreads), Cfg<ST, EWN>::kSmem, st, tmA, tmW, g));        \
+    auto k = gemm_tma_kernel<OT, ACT, HB, HR, VTK>;                                                                    \
+    S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));                              \
+    S6_CHECK(s6_launch_pdl(k, dim3(grid), dim3(THREADS), SMEM, st, tmA, tmW, g));                                      \
   } while (0)
 #define LAUNCH_TMA(ACT, HB, HR)                                                                                        \
   do {                                                                                                                 \
-    if (c_dtype) {                                                                                                     \
-      if (deep_k) LAUNCH_ONE(__nv_bfloat16, ACT, HB, HR, 4, 4); else LAUNCH_ONE(__nv_bfloat16, ACT, HB, HR, 3, 8);    \
-    } else {                                                                                                           \
-      if (deep_k) LAUNCH_ONE(float, ACT, HB, HR, 4, 4); else LAUNCH_ONE(float, ACT, HB, HR, 3, 8);                    \
-    }                                                                                                                  \
+    if (c_dtype) LAUNCH_ONE(__nv_bfloat16, ACT, HB, HR, false); else LAUNCH_ONE(float, ACT, HB, HR, false);           \
   } while (0)
   if (vt) {
     // V^T epilogue: bf16 output, bias, no activation / residual (the QKV and KV projections)
@@ -277,15 +214,7 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
                vt_N1 >= vt_S);
     S6_REQUIRE(vt_col1 > vt_col0 && vt_col1 <= N && (vt_col1 % 32) == 0 &&
                (vt_col1 == N || (c2 && (ldc2 % 8) == 0 && ldc2 >= N - vt_col1 && (reinterpret_cast<uintptr_t>(c2) & 15) == 0)));
-    if (deep_k) {
-      auto k = gemm_tma_kernel<__nv_bfloat16, 0, true, false, 4, 4, true>;
-      S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<4, 4>::kSmem));
-      S6_CHECK(s6_launch_pdl(k, dim3(grid), dim3(Cfg<4, 4>::kThreads), Cfg<4, 4>::kSmem, st, tmA, tmW, g));
-    } else {
-      auto k = gemm_tma_kernel<__nv_bfloat16, 0, true, false, 3, 8, true>;
-      S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3, 8>::kSmem));
-      S6_CHECK(s6_launch_pdl(k, dim3(grid), dim3(Cfg<3, 8>::kThreads), Cfg<3, 8>::kSmem, st, tmA, tmW, g));
-    }
+    LAUNCH_ONE(__nv_bfloat16, 0, true, false, true);
     S6_LAUNCH_CHECK();
     return 0;
   }

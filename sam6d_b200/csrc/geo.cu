@@ -6,7 +6,7 @@
 // anchor, the three triplet angles and the distance index -> T[b,i,j,4] = {a0, a1, a2, d}.
 // Stage 2 (geo_embed_f32): the two 256x256 projections applied to sinusoidal embeddings that are generated
 // on the fly (never materialised), max over the three angle rows fused in the epilogue.  This file holds the
-// exact fp32 CUDA-core version; geo_tc.cu holds the tcgen05 bf16 version.
+// exact fp32 CUDA-core version; geo_tc.cu holds the wgmma bf16 version.
 #include "common.cuh"
 
 namespace {

@@ -5,12 +5,11 @@
 // emb(x) is the 256-entry sinusoidal embedding of ONE scalar, so g_a and g_d are smooth vector-valued functions of a scalar:
 // frequencies <= 1 rad per index unit, angle indices in [0, 12] (angles in [0, pi] / sigma_a), distance indices of points in
 // normalised clouds below 12 (the table spans [0, 32): 6.4 object radii).  The reference evaluates them with 4 x 256 sin/cos and two 256 x 256 products PER PAIR (651 GFLOP
-// per cloud batch; the tensor-core version of this repo, geo_tc.cu, still spent 1.3 ms per step on it, bound by MUFU, MMA issue and
+// per cloud batch; the tensor-core version of this repo, geo_tc.cu, still runs those products, bound by MUFU, MMA issue and
 // its epilogue together).  Here both functions are tabulated once per weight set on a grid of step 1/8 (host side, float64,
 // from the fp32 weights: 97 + 257 rows of 256 bf16 = 181 KB) and a pair costs four linear interpolations out of shared memory:
 // no sin/cos, no MMA, E written exactly once.  Interpolation error at step 1/8 is < 1e-4 of |E| -- below the bf16 rounding of
-// the table and of E itself; measured against the float64 embedding the result is closer than the bf16-operand tensor-core
-// product was (rms 1.6e-3 vs 1.8e-3 at |E| ~ 0.56, tools/geo_lut_error.py).
+// the table and of E itself (tools/geo_lut_error.py compares it with the float64 embedding).
 //
 // Kernel: persistent, 16 warps per CTA (two pairs in flight per warp), both tables resident in shared memory.  A warp takes 32 consecutive pairs: lane l loads
 // the indices of pair l (one coalesced 512-byte read), then for each pair the four indices are broadcast by shuffles and lane l
@@ -22,9 +21,9 @@
 // Distance indices outside the table (>= 32): pairs of row 0 / column 0 -- the background point of SAM-6D sits at (100,100,100),
 // ~870 index units from everything -- read g_d from `far` (clouds, 2, S, 256), computed exactly (tensor-core distance pass of
 // geo_tc.cu) from the 2 S distances of that row and column; any other out-of-range pair takes a slow exact path (sin/cos + a
-// 256 x 256 product per pair on CUDA cores, ~5000 warp instructions against ~100 for a table pair: measured on the bench's
-// synthetic clouds, whose 20 % gaussian outliers put 3 % of the pairs beyond index 16, a [0, 16) table spent most of its 1.5 ms
-// there -- hence the [0, 32) span), so the kernel is correct for any input and fast for the clouds the model produces.
+// 256 x 256 product per pair on CUDA cores, ~5000 warp instructions against ~100 for a table pair: the bench's synthetic clouds,
+// whose 20 % gaussian outliers put 3 % of the pairs beyond index 16, would spend most of the time there with a [0, 16) table --
+// hence the [0, 32) span), so the kernel is correct for any input and fast for the clouds the model produces.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -124,8 +123,8 @@ __device__ __noinline__ uint4 slow_distance(float x, const float* __restrict__ d
 
 // PRECISE: interpolation, maximum and sum in fp32, ONE rounding to bf16 at the store (rms error 1.2e-3 against 1.6e-3 for the packed
 // bf16x2 arithmetic, at about twice the instructions per pair)
-// LUT_THREADS / UNROLL: warps per CTA against pairs in flight per warp (the kernel is bound by the shared-memory pipe: ncu shows it
-// 60-68 % busy with 32 warps and one pair per iteration, warps waiting on their LDS results)
+// LUT_THREADS / UNROLL: warps per CTA against pairs in flight per warp (the kernel is bound by the shared-memory pipe, warps waiting
+// on their LDS results)
 template <bool PRECISE, int LUT_THREADS, int UNROLL>
 __global__ void __launch_bounds__(LUT_THREADS, 1) geo_embed_lut_kernel(const float4* __restrict__ T, long long npairs, int S,
                                                                       const uint4* __restrict__ tabA_g, int na, float inv_ha,
@@ -224,8 +223,8 @@ S6_API int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const vo
   S6_CHECK(cudaGetDevice(&dev));
   S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int smem = (na + nd) * 512;
-  // launch shape (SAM6D_GEO_LUT_CFG): 1 = 16 warps x 2 pairs in flight per warp (default: 0.615 ms per 64 clouds); 0 = 32 warps x 1
-  // pair (0.666 ms); 2 = 24 warps x 2 pairs (0.671 ms) -- profiles/r02_bench_bf16_v8.json and its cfg lines
+  // launch shape (SAM6D_GEO_LUT_CFG): 1 = 16 warps x 2 pairs in flight per warp (default); 0 = 32 warps x 1 pair; 2 = 24 warps x
+  // 2 pairs
   static const int cfg = [] { const char* e = getenv("SAM6D_GEO_LUT_CFG"); return e ? atoi(e) : 1; }();
   const long long nblocks = (npairs + 31) / 32;
   cudaStream_t st = s6_stream(stream);

@@ -1,24 +1,19 @@
-// geo_tc.cu -- GeometricStructureEmbedding projections on the 5th-gen tensor cores (PEM/model/transformer.py:334-349).
+// geo_tc.cu -- GeometricStructureEmbedding projections on the tensor cores (wgmma; PEM/model/transformer.py:334-349).
 //
 //   E[p,:] = proj_d(sin_emb(d_p)) + max_{k<3} proj_a(sin_emb(a_{p,k})) + (b_a + b_d)           p = (b,i,j) pair
 //
 // The reference materialises sin_emb for 4 scalars per pair (3.8 GB at B=32) and runs two 256x256 Linears over them
 // (651 GFLOP per cloud).  Here one persistent, warp-specialised kernel per projection keeps the 256x256 bf16 weight
-// resident in shared memory (128 KB, UMMA K-major SWIZZLE_128B slabs) and never materialises the embeddings:
-//   producers (warps 4-11): a thread owns one 16-byte chunk column (4 frequencies, kept in registers) of 3-4 token rows:
+// resident in shared memory (128 KB, K-major SWIZZLE_128B slabs) and never materialises the embeddings:
+//   producers (warps 8-11): a thread owns one 16-byte chunk column (4 frequencies, kept in registers) of 6-8 token rows:
 //                           x*omega_f -> __sincosf -> bf16 (sin,cos) pairs written straight into the swizzled A slab of a
-//                           4-deep k-block ring (16 KB per 128x64 slab).  Two producer warps per scheduler: one warp alone
-//                           issued an instruction every ~7 cycles (dependent-latency bound), a third of the MUFU rate.
-//                           The angle pass skips the unused 4th row of every pair (the slab rows stay zero).
-//   MMA issuer (warp 12)  : 4 x tcgen05.mma M128 N256 K16 per k-block into one of two 256-column TMEM accumulators
-//   epilogue (warps 0-3)  : tcgen05.ld; pass ANGLE: rows are (pair, k) quadruples (k = 3 unused), max over k by a 24-shuffle
-//                           transpose-reduce, each lane adds its 8-column share into E ; pass DIST (runs first): rows are
-//                           pairs, E = acc + bias with full-line stores (epilogue.cuh).
+//                           4-deep k-block ring (16 KB per 128x64 slab).  The angle pass skips the unused 4th row of every
+//                           pair (it repeats the 3rd).
+//   consumers (warps 0-7) : warpgroup g owns rows [64 g, 64 g + 64) of the tile: 4 x wgmma m64n256k16 per k-block into 128
+//                           registers per thread; pass ANGLE: rows are (pair, k) quadruples, the max over k is two shuffles
+//                           (the four rows of a pair sit in lanes 4 apart) and each of the four lanes adds a quarter of the
+//                           columns into E; pass DIST (runs first): rows are pairs, E = acc + bias.
 // E is fp32 or bf16.  Accuracy: operands rounded to bf16 (sin/cos via MUFU), fp32 accumulation.
-#include <cuda.h>
-
-#include <cstring>
-
 #include "epilogue.cuh"
 #include "tc.cuh"
 
@@ -27,57 +22,16 @@ namespace {
 constexpr int BM = 128, BN = 256, BK = 64, KBLOCKS = 4;
 constexpr int A_SLAB = BM * BK * 2;          // 16 KB
 constexpr int W_SLAB = BN * BK * 2;          // 32 KB
-constexpr int NUM_PRODUCERS = 256;                  // warps 4-11
-constexpr int MMA_WARP = 12;
-constexpr int NUM_THREADS = 128 + NUM_PRODUCERS + 32 + 128;   // epilogue warps 0-3 and 13-16 (two per TMEM lane quadrant)
-// the distance pass stages its full-line stores through shared memory (8 warps x 4.5 KB) and runs a 3-deep A ring to fit
-// A ring stage holds kKps k-blocks (slabs).  Measured (profiles/r02_geo_notes.md): two k-blocks per stage (half the
-// fence.proxy.async + barrier round trips of the producers) made the angle pass 5 % SLOWER than one per stage with a 4-deep ring,
-// so the synchronisation count is not what bounds it; one k-block per stage stays.
-template <int MODE>
-struct Cfg {
-  static constexpr int kKps = 1;
-  static constexpr int kStages = (MODE == 0) ? 4 : 3;
-  static constexpr int kEpiBytes = (MODE == 0) ? 0 : 8 * epi::WARP_STAGE_FLOATS * 4;
-  static constexpr int kSmem = KBLOCKS * W_SLAB + kStages * kKps * A_SLAB + kEpiBytes + 1024;
-};
+constexpr int CONSUMERS = 256;                      // warps 0-7
+constexpr int NUM_PRODUCERS = 128;                  // warps 8-11
+constexpr int NUM_THREADS = CONSUMERS + NUM_PRODUCERS;
+constexpr int ASTAGES = 4;
+constexpr int SMEM = KBLOCKS * W_SLAB + ASTAGES * A_SLAB + 1024;
 
-__device__ __forceinline__ uint32_t bf16x2_max(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("max.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
 __device__ __forceinline__ uint32_t bf16x2_add(uint32_t a, uint32_t b) {
   uint32_t d;
   asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
   return d;
-}
-
-template <typename ET>
-__device__ __forceinline__ void store8(ET* p, const float v[8]);
-template <>
-__device__ __forceinline__ void store8<float>(float* p, const float v[8]) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
-}
-template <>
-__device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* p, const float v[8]) {
-  *reinterpret_cast<uint4*>(p) = make_uint4(tc::pack_bf16(v[0], v[1]), tc::pack_bf16(v[2], v[3]), tc::pack_bf16(v[4], v[5]),
-                                            tc::pack_bf16(v[6], v[7]));
-}
-template <typename ET>
-__device__ __forceinline__ void load8(const ET* p, float v[8]);
-template <>
-__device__ __forceinline__ void load8<float>(const float* p, float v[8]) {
-  float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
-template <>
-__device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* p, float v[8]) {
-  uint4 a = *reinterpret_cast<const uint4*>(p);
-  const uint32_t w[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { v[2 * i] = __uint_as_float(w[i] << 16); v[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u); }
 }
 
 // MODE 0: angle pass (rows = pair*4 + k), MODE 1: distance pass (rows = pairs)
@@ -85,15 +39,12 @@ template <int MODE, typename ET>
 __global__ void __launch_bounds__(NUM_THREADS, 1) geo_embed_tc_kernel(const float* __restrict__ T, long long npairs,
                                                                       const float* __restrict__ div_term,
                                                                       const __nv_bfloat16* __restrict__ Wb,   // (256 out, 256 in) bf16
-                                                                      const float* __restrict__ bias, ET* __restrict__ E,
-                                                                      const __grid_constant__ CUtensorMap tmE) {
-  constexpr int ASTAGES = Cfg<MODE>::kStages, KPS = Cfg<MODE>::kKps, STAGE_BYTES = KPS * A_SLAB;
+                                                                      const float* __restrict__ bias, ET* __restrict__ E) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* w_smem = smem;                              // 4 slabs [256][64] bf16
   uint8_t* a_smem = smem + KBLOCKS * W_SLAB;           // ring of [128][64] bf16
-  __shared__ __align__(8) uint64_t full_bar[ASTAGES], empty_bar[ASTAGES], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[ASTAGES], empty_bar[ASTAGES];
   __shared__ float omega[128];
   __shared__ __align__(16) float sbias[256];
 
@@ -102,8 +53,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) geo_embed_tc_kernel(const floa
   const long long ntiles = (npairs + PAIRS_PER_TILE - 1) / PAIRS_PER_TILE;
 
   if (tid == 0) {
-    for (int s = 0; s < ASTAGES; ++s) { tc::mbar_init(&full_bar[s], NUM_PRODUCERS / 32); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tmem_full_bar[a], 1); tc::mbar_init(&tmem_empty_bar[a], 8); }
+    for (int s = 0; s < ASTAGES; ++s) { tc::mbar_init(&full_bar[s], NUM_PRODUCERS / 32); tc::mbar_init(&empty_bar[s], CONSUMERS / 32); }
     tc::mbar_fence_init();
   }
   if (tid < 128) omega[tid] = div_term[tid];
@@ -114,20 +64,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) geo_embed_tc_kernel(const floa
     const uint4 v = *reinterpret_cast<const uint4*>(Wb + (size_t)n * 256 + c);
     *reinterpret_cast<uint4*>(w_smem + (c >> 6) * W_SLAB + tc::sw128_offset(n, c & 63)) = v;
   }
-  for (int u = tid; u < ASTAGES * STAGE_BYTES / 16; u += NUM_THREADS)   // rows the angle pass never writes must be finite
+  for (int u = tid; u < ASTAGES * A_SLAB / 16; u += NUM_THREADS)   // rows the angle pass never writes must be finite
     reinterpret_cast<uint4*>(a_smem)[u] = make_uint4(0u, 0u, 0u, 0u);
   tc::fence_proxy_async_smem();
-  if (warp == MMA_WARP) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp >= 4 && warp < MMA_WARP) {
+  if (tid >= CONSUMERS) {
     // ------------------------------------------------------------------ producers: thread <-> (chunk column, NT token rows)
-    const int pt = tid - 128;
+    const int pt = tid - CONSUMERS;
     const int c = pt & 7;                               // 16-byte chunk of the 128-byte slab row: frequencies 32 kb + 4c .. + 3
-    constexpr int NT = (MODE == 0) ? 3 : 4;             // tasks per thread per k-block
+    constexpr int NT = (MODE == 0) ? 96 * 8 / NUM_PRODUCERS : 128 * 8 / NUM_PRODUCERS;   // tasks per thread per k-block
     int row[NT];
 #pragma unroll
     for (int j = 0; j < NT; ++j) {
@@ -162,260 +108,111 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) geo_embed_tc_kernel(const floa
 #pragma unroll
       for (int j = 0; j < NT; ++j) x[j] = xn[j];
 #pragma unroll
-      for (int kb0 = 0; kb0 < KBLOCKS; kb0 += KPS, ++g) {
+      for (int kb = 0; kb < KBLOCKS; ++kb, ++g) {
         const int s = (int)(g % ASTAGES);
         tc::mbar_wait(&empty_bar[s], (uint32_t)(((g / ASTAGES) & 1) ^ 1));
 #pragma unroll
-        for (int kk = 0; kk < KPS; ++kk) {
-          const int kb = kb0 + kk;
+        for (int j = 0; j < NT; ++j) {
+          uint32_t w[4];
 #pragma unroll
-          for (int j = 0; j < NT; ++j) {
-            uint32_t w[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              float sv, cv;
-              __sincosf(x[j] * om[kb][q], &sv, &cv);
-              w[q] = tc::pack_bf16(sv, cv);
-            }
-            const uint32_t addr = a_base + s * STAGE_BYTES + kk * A_SLAB + row[j] * 128 + ((c ^ (row[j] & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-            if (MODE == 0 && (row[j] & 3) == 2) {
-              // the pair's 4th (padding) row repeats its 3rd neighbour: a maximum ignores duplicates, so the epilogue needs no mask
-              const uint32_t addr2 = a_base + s * STAGE_BYTES + kk * A_SLAB + (row[j] + 1) * 128 + ((c ^ ((row[j] + 1) & 7)) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr2), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-            }
+          for (int q = 0; q < 4; ++q) {
+            float sv, cv;
+            __sincosf(x[j] * om[kb][q], &sv, &cv);
+            w[q] = tc::pack_bf16(sv, cv);
+          }
+          const uint32_t addr = a_base + s * A_SLAB + row[j] * 128 + ((c ^ (row[j] & 7)) << 4);
+          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
+          if (MODE == 0 && (row[j] & 3) == 2) {
+            // the pair's 4th (padding) row repeats its 3rd neighbour: a maximum ignores duplicates, so the epilogue needs no mask
+            const uint32_t addr2 = a_base + s * A_SLAB + (row[j] + 1) * 128 + ((c ^ ((row[j] + 1) & 7)) << 4);
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr2), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
           }
         }
         tc::fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) tc::mbar_arrive(&full_bar[s]);
         // next tile's indices: issued behind the first fence (a fence waits for the thread's outstanding loads, so a prefetch
-        // issued before it stalls the first k-block by the full load latency -- ncu r02_geo_v2); k-block 1 covers the latency
-        if (kb0 == 0) fetch(tile + gridDim.x, xn);
+        // issued before it would stall the first k-block by the full load latency); k-block 1 covers the latency
+        if (kb == 0) fetch(tile + gridDim.x, xn);
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(BM, BN);
-      const uint32_t w_addr = tc::smem_u32(w_smem), a_addr0 = tc::smem_u32(a_smem);
-      long long g = 0, it = 0;
-      for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int acc = (int)(it & 1);
-        tc::mbar_wait_suspend(&tmem_empty_bar[acc], (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc::tc_fence_after_sync();
-        const uint32_t d_addr = tmem_base + (uint32_t)(acc * BN);
-        for (int kb0 = 0; kb0 < KBLOCKS; kb0 += KPS, ++g) {
-          const int s = (int)(g % ASTAGES);
-          tc::mbar_wait_suspend(&full_bar[s], (uint32_t)((g / ASTAGES) & 1));
-          tc::tc_fence_after_sync();
-#pragma unroll
-          for (int kk = 0; kk < KPS; ++kk)
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              tc::umma_bf16(d_addr, tc::umma_desc_sw128(a_addr0 + s * STAGE_BYTES + kk * A_SLAB + k * 32),
-                            tc::umma_desc_sw128(w_addr + (kb0 + kk) * W_SLAB + k * 32), idesc, (kb0 | kk | k) ? 1u : 0u);
-          tc::umma_commit(&empty_bar[s]);
-        }
-        tc::umma_commit(&tmem_full_bar[acc]);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: warp w <-> TMEM lanes 32w .. 32w+31
-    long long it = 0;
-    const int quad = warp & 3, c0 = (warp < 4) ? 0 : 4;        // this warp's TMEM lane quadrant and its 4 column chunks
-    const int r = quad * 32 + lane;
-    // angle pass: E already holds proj_d(...) + biases from the distance pass.  This lane's 4 x 8 columns of the NEXT tile are
-    // fetched while the current tile is processed: issued only one accumulator wait ahead, the add stalled on DRAM latency
-    constexpr int RAW = (MODE == 0) ? 4 : 1;
-    constexpr int RU = sizeof(ET) == 4 ? 2 : 1;
-    uint4 raw[RAW][RU], rawn[RAW][RU];
-    auto fetch_e = [&](long long tile, uint4 (&dst)[RAW][RU]) {
-      if (MODE == 0) {
-        const long long pair = tile * 32 + (r >> 2);
-        if (tile < ntiles && pair < npairs) {
-          const uint4* src = reinterpret_cast<const uint4*>(E + pair * 256 + (r & 3) * 8);
-#pragma unroll
-          for (int c = 0; c < RAW; ++c)
-#pragma unroll
-            for (int u = 0; u < RU; ++u) dst[c][u] = src[(c0 + c) * (sizeof(ET) == 4 ? 8 : 4) + u];
-        }
-      }
-    };
-    fetch_e(blockIdx.x, rawn);
-    uint32_t st_pending = 0;
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = (int)(it & 1);
-#pragma unroll
-      for (int c = 0; c < RAW; ++c)
-#pragma unroll
-        for (int u = 0; u < RU; ++u) raw[c][u] = rawn[c][u];
-      fetch_e(tile + gridDim.x, rawn);
-      tc::mbar_wait_suspend(&tmem_full_bar[acc], (uint32_t)((it >> 1) & 1));
-      tc::tc_fence_after_sync();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      if (MODE == 0) {
-        const long long pair = tile * 32 + (r >> 2);
-        const int q = r & 3;
-        const bool up2 = (lane & 2) != 0, up1 = (lane & 1) != 0;
-#pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          const int c = c0 + cc;
-          float v[32];
-          tc::tmem_ld32(t_addr + c * 32, v);
-          // max over the 4 rows of the pair (row 3 repeats row 2), transposed so that lane q ends with columns [8q, 8q+8)
-          if constexpr (sizeof(ET) == 2) {
-            // packed: rounding to bf16 is monotone, so max(bf16(a), bf16(b)) = bf16(max(a, b)); half the selects / shuffles / maxima
-            uint32_t w[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) w[i] = tc::pack_bf16(v[2 * i], v[2 * i + 1]);
-            uint32_t m[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const uint32_t keep = up2 ? w[8 + i] : w[i], send = up2 ? w[i] : w[8 + i];
-              m[i] = bf16x2_max(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-            }
-            uint32_t o[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const uint32_t keep = up1 ? m[4 + i] : m[i], send = up1 ? m[i] : m[4 + i];
-              o[i] = bf16x2_max(keep, __shfl_xor_sync(0xffffffffu, send, 1));
-            }
-            if (pair < npairs) {
-              const uint4 e = raw[cc][0];
-              *reinterpret_cast<uint4*>(E + pair * 256 + c * 32 + q * 8) =
-                  make_uint4(bf16x2_add(e.x, o[0]), bf16x2_add(e.y, o[1]), bf16x2_add(e.z, o[2]), bf16x2_add(e.w, o[3]));
-            }
-          } else {
-            float m[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float keep = up2 ? v[16 + i] : v[i], send = up2 ? v[i] : v[16 + i];
-              m[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-            }
-            float o[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float keep = up1 ? m[8 + i] : m[i], send = up1 ? m[i] : m[8 + i];
-              o[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 1));
-            }
-            if (pair < npairs) {
-              float e[8];
-              load8<ET>(reinterpret_cast<const ET*>(&raw[cc][0]), e);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) e[i] += o[i];
-              store8<ET>(E + pair * 256 + c * 32 + q * 8, e);
-            }
-          }
-        }
-      } else {
-        uint8_t* stage_b = smem + KBLOCKS * W_SLAB + ASTAGES * STAGE_BYTES;
-        const long long row0 = tile * 128 + quad * 32;
-        (void)raw;
-        if constexpr (sizeof(ET) == 2) {
-          // rows = pairs: E = acc + (b_a + b_d).  The warp packs two chunks (64 columns) of its 32 rows into a SWIZZLE_128B
-          // 4 KB stage and one lane hands it to the TMA unit: no read-back, no per-lane global stores, rows past npairs are
-          // clipped by the tensor map.  The stage is reused once the previous store has been read out of it.
-          uint8_t* stage = stage_b + (quad + c0) * 4096;
-#pragma unroll 1
-          for (int h = 0; h < 2; ++h) {
-#pragma unroll 1
-            for (int cc = 0; cc < 2; ++cc) {
-              const int c = c0 + 2 * h + cc;
-              float v[32];
-              tc::tmem_ld32(t_addr + c * 32, v);
-              uint32_t w[16];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 b4 = *reinterpret_cast<const float4*>(&sbias[c * 32 + i * 4]);
-                w[2 * i] = tc::pack_bf16(v[4 * i] + b4.x, v[4 * i + 1] + b4.y);
-                w[2 * i + 1] = tc::pack_bf16(v[4 * i + 2] + b4.z, v[4 * i + 3] + b4.w);
-              }
-              if (cc == 0 && st_pending) {
-                if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                __syncwarp();
-              }
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                *reinterpret_cast<uint4*>(stage + lane * 128 + (((cc * 4 + j) ^ (lane & 7)) << 4)) =
-                    make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-            }
-            tc::fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                               reinterpret_cast<uint64_t>(&tmE)),
-                           "r"(tc::smem_u32(stage)), "r"((c0 + 2 * h) * 32), "r"((int)row0)
-                           : "memory");
-              asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-            st_pending = 1;
-          }
-        } else {
-          float* stage = reinterpret_cast<float*>(stage_b) + (quad + c0) * epi::WARP_STAGE_FLOATS;
-#pragma unroll 1
-          for (int c = c0; c < c0 + 4; ++c) {
-            float v[32];
-            tc::tmem_ld32(t_addr + c * 32, v);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 b4 = *reinterpret_cast<const float4*>(&sbias[c * 32 + i * 4]);
-              v[4 * i] += b4.x; v[4 * i + 1] += b4.y; v[4 * i + 2] += b4.z; v[4 * i + 3] += b4.w;
-            }
-            epi::process_chunk<ET, 0, false, false>(v, stage, lane, (int)row0, (int)npairs, c * 32, 256, 1.f, nullptr, nullptr, 0, E, 256);
-          }
-        }
-      }
-      tc::tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tmem_empty_bar[acc]);      // one arrival per warp: 256 arrivals on one word serialise
-    }
-    if (st_pending && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    return;
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tc::tmem_dealloc(tmem_base, 512);
-}
-
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// E (npairs, 256) bf16 as a 2-D tensor, box = 64 columns x 32 rows, SWIZZLE_128B (the epilogue's stage layout)
-int make_e_map(CUtensorMap* map, const void* E, long long npairs) {
-  static EncodeFn enc = nullptr;
-  if (!enc) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return 999;
-    enc = reinterpret_cast<EncodeFn>(p);
+  // ------------------------------------------------------------------ consumers: warpgroup wg <-> rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, w = warp & 3;
+  const uint32_t w_addr = tc::smem_u32(w_smem), a_addr0 = tc::smem_u32(a_smem) + wg * (64 * 128);
+  long long g = 0;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    float acc[BN / 2];
+    int prev = -1;
+    for (int kb = 0; kb < KBLOCKS; ++kb, ++g) {
+      const int s = (int)(g % ASTAGES);
+      tc::mbar_wait(&full_bar[s], (uint32_t)((g / ASTAGES) & 1));
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        tc::wgmma_bf16<BN>(acc, tc::wg_desc(a_addr0 + s * A_SLAB + k * 32), tc::wg_desc(w_addr + kb * W_SLAB + k * 32), (kb | k) ? 1u : 0u);
+      tc::wg_commit();
+      if (prev >= 0) {
+        tc::wg_wait<1>();
+        if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+      }
+      prev = s;
+    }
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+    if (MODE == 0) {
+      // rows 4p .. 4p+3 of a pair are held by lanes l, l^4, l^8, l^12: max over them, then lane quarter q = (l >> 2) & 3
+      // adds the 8-column groups j with j % 4 == q into E (E already holds proj_d(...) + biases from the distance pass)
+      const int q = (lane >> 2) & 3;
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const long long pair = tile * 32 + (wg * 64 + 16 * w + 8 * hr + (lane >> 2)) / 4;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          float m0 = acc[4 * j + 2 * hr], m1 = acc[4 * j + 2 * hr + 1];
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 4)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 4));
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 8)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 8));
+          if ((j & 3) == q && pair < npairs) {
+            ET* e = E + pair * 256 + tc::frag_col(4 * j, lane);
+            if constexpr (sizeof(ET) == 2) {
+              // rounding to bf16 is monotone, so bf16(max) = max of the bf16 values; the sum is a packed bf16 add
+              uint32_t* e2 = reinterpret_cast<uint32_t*>(e);
+              *e2 = bf16x2_add(*e2, tc::pack_bf16(m0, m1));
+            } else {
+              float2* e2 = reinterpret_cast<float2*>(e);
+              const float2 v = *e2;
+              *e2 = make_float2(v.x + m0, v.y + m1);
+            }
+          }
+        }
+      }
+    } else {
+      // rows = pairs: E = acc + (b_a + b_d)
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const long long pair = tile * 128 + wg * 64 + tc::frag_row(2 * hr, w, lane);
+        if (pair >= npairs) continue;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = tc::frag_col(4 * j, lane);
+          epi::st2(E + pair * 256 + col, acc[4 * j + 2 * hr] + sbias[col], acc[4 * j + 2 * hr + 1] + sbias[col + 1]);
+        }
+      }
+    }
   }
-  cuuint64_t gdim[2] = {256, (cuuint64_t)npairs};
-  cuuint64_t gstride[1] = {512};
-  cuuint32_t box[2] = {64, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(E), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
 }
 
 template <int MODE, typename ET>
 int launch_pass(const float* T, long long npairs, const float* div_term, const __nv_bfloat16* W, const float* bias, ET* E, int sms,
                 cudaStream_t st) {
   auto kern = geo_embed_tc_kernel<MODE, ET>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<MODE>::kSmem);
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
   if (e != cudaSuccess) return (int)e;
   const long long per = (MODE == 0) ? 32 : 128;
   const long long ntiles = (npairs + per - 1) / per;
   const int grid = (int)(ntiles < sms ? ntiles : sms);
-  CUtensorMap tmE;
-  memset(&tmE, 0, sizeof(tmE));
-  if (MODE == 1 && sizeof(ET) == 2) {
-    const int rc = make_e_map(&tmE, E, npairs);
-    if (rc) return rc;
-  }
-  kern<<<grid, NUM_THREADS, Cfg<MODE>::kSmem, st>>>(T, npairs, div_term, W, bias, E, tmE);
+  kern<<<grid, NUM_THREADS, SMEM, st>>>(T, npairs, div_term, W, bias, E);
   return (int)cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// linattn_tc.cu -- the dense side of the focused linear attention (PEM/model/transformer.py:541-559) on tcgen05:
+// linattn_tc.cu -- the dense side of the focused linear attention (PEM/model/transformer.py:541-559) on wgmma:
 //
 //   q' = focus(q)                       q = relu(x)+1e-6; q /= softplus(scale); n = ||q||; q = q^3; q = q/||q|| * n
 //   x_h = (q'_h KV_h) / (q'_h . ksum_h + 1e-6)       per head h (4 heads x 64 channels), KV_h = sum_j k'_j v_j^T
@@ -7,13 +7,13 @@
 // mat-vecs.  One CTA handles 128 token rows of one cloud:
 //   * all 8 warps: read the bf16 q rows (lane = 8 channels), apply the feature map in fp32 (two warp reductions), compute the
 //     normaliser q'_h . ksum_h in fp32 (3-step reduction inside the 8 lanes of a head), and write q' as bf16 straight into the
-//     swizzled UMMA A slabs (one [128][64] slab per head)
-//   * KV_h^T arrives as a ready-made bf16 UMMA B image (4 x [64][64], SWIZZLE_128B) written by linattn_kv_pack_kernel,
+//     swizzled wgmma A slabs (one [128][64] slab per head)
+//   * KV_h^T arrives as a ready-made bf16 wgmma B image (4 x [64][64], SWIZZLE_128B) written by linattn_kv_pack_kernel,
 //     pulled with one cp.async.bulk
-//   * 16 x tcgen05.mma M128 N64 K16 -> 4 x 64 TMEM columns; the epilogue scales by 1/normaliser and stores bf16 full lines.
-// 99 KB of shared memory and 256 TMEM columns per CTA: two CTAs per SM overlap the feature-map phase of one with the MMA/epilogue
-// of the other.  HBM traffic: q in, x out (2 x rows x 512 B).
-#include "epilogue.cuh"
+//   * per head, each of the two warpgroups runs 4 x wgmma m64n64k16 on its 64 rows; the result is scaled by 1/normaliser and
+//     stored as bf16 straight from the registers.
+// 99 KB of shared memory per CTA: two CTAs per SM overlap the feature-map phase of one with the MMA/epilogue of the other.
+// HBM traffic: q in, x out (2 x rows x 512 B).
 #include "tc.cuh"
 
 namespace {
@@ -27,7 +27,7 @@ constexpr int LT_SMEM = H * A_SLAB + H * B_SLAB + 128 * H * 4 + 1024;
 
 // grid = B*H, 1024 threads.  Kf: focused keys, V: values, both (B, J, ld) fp32 views.  Writes the bf16 B-operand image of KV_h^T
 // and ksum.  Thread (d, e0..e0+3) walks the J sparse tokens: a 196-step chain of 4 FMAs (a 256-thread version with 16
-// accumulators per thread took 65 us for 256 CTAs -- pure dependent-issue latency).
+// accumulators per thread is bound by dependent-issue latency).
 __global__ void __launch_bounds__(1024) linattn_kv_pack_kernel(const float* __restrict__ Kf, long long k_ld, long long k_bs,
                                                                const float* __restrict__ V, long long v_ld, long long v_bs, int J,
                                                                uint8_t* __restrict__ blob, float* __restrict__ KS) {
@@ -69,22 +69,19 @@ struct LtArgs {
 __global__ void __launch_bounds__(LT_THREADS, 2) linattn_tc_kernel(LtArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* a_s = smem;                                  // 4 head slabs; re-used as the epilogue staging once the MMAs are done
+  uint8_t* a_s = smem;                                  // 4 head slabs [128 rows][64 ch]
   uint8_t* b_s = smem + H * A_SLAB;
   float* zs = reinterpret_cast<float*>(b_s + H * B_SLAB);   // [128][4] reciprocal normalisers
-  __shared__ __align__(8) uint64_t blob_bar, mma_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t blob_bar;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x / a.tiles_per_cloud, tile = blockIdx.x - b * a.tiles_per_cloud;
   if (tid == 0) {
     tc::mbar_init(&blob_bar, 1);
-    tc::mbar_init(&mma_bar, 1);
     tc::mbar_fence_init();
     tc::mbar_arrive_expect_tx(&blob_bar, BLOB_BYTES);
     tc::bulk_load_1d(b_s, a.blob + (size_t)b * BLOB_BYTES, BLOB_BYTES, &blob_bar);
   }
-  if (warp == 0) tc::tmem_alloc(&tmem_slot, 256);
 
   // ---------------------------------------------------------------- feature map: warp <-> rows warp, warp+8, ...
   float rs[8], ksv[8];
@@ -142,45 +139,37 @@ __global__ void __launch_bounds__(LT_THREADS, 2) linattn_tc_kernel(LtArgs a) {
     }
   }
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (tid == 0) {
-    tc::mbar_wait(&blob_bar, 0);
-    constexpr uint32_t idesc = tc::umma_idesc_bf16(128, D);
-#pragma unroll
-    for (int h = 0; h < H; ++h)
-#pragma unroll
-      for (int k = 0; k < D / 16; ++k)
-        tc::umma_bf16(tmem_base + h * D, tc::umma_desc_sw128(tc::smem_u32(a_s + h * A_SLAB) + k * 32),
-                      tc::umma_desc_sw128(tc::smem_u32(b_s + h * B_SLAB) + k * 32), idesc, k ? 1u : 0u);
-    tc::umma_commit(&mma_bar);
-  }
-  if (warp < 4) {
-    tc::mbar_wait(&mma_bar, 0);
-    tc::tc_fence_after_sync();
-    float* stage = reinterpret_cast<float*>(a_s) + warp * epi::WARP_STAGE_FLOATS;
-    const int row = warp * 32 + lane;
-    __nv_bfloat16* xb = a.X + (size_t)b * a.x_bs;       // rows of this cloud
-    const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
+  // ---------------------------------------------------------------- x = q' KV / z: warpgroup wg <-> rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, w = warp & 3;
+  tc::mbar_wait(&blob_bar, 0);
+  __nv_bfloat16* xb = a.X + (size_t)b * a.x_bs;         // rows of this cloud
 #pragma unroll 1
-    for (int c = 0; c < C / 32; ++c) {
-      float v[32];
-      tc::tmem_ld32(t_addr + c * 32, v);
-      const float z = zs[row * H + (c >> 1)];
-      epi::process_chunk<__nv_bfloat16, 0, false, false>(v, stage, lane, tile * 128 + warp * 32, a.rpb, c * 32, C, z, nullptr, nullptr, 0, xb, a.x_ld);
+  for (int h = 0; h < H; ++h) {
+    float acc[D / 2];
+    const uint32_t a_addr = tc::smem_u32(a_s + h * A_SLAB) + wg * (64 * 128), b_addr = tc::smem_u32(b_s + h * B_SLAB);
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) tc::wgmma_bf16<D>(acc, tc::wg_desc(a_addr + k * 32), tc::wg_desc(b_addr + k * 32), k ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r = wg * 64 + tc::frag_row(2 * hr, w, lane), row = tile * 128 + r;
+      if (row >= a.rpb) continue;
+      const float z = zs[r * H + h];
+#pragma unroll
+      for (int j = 0; j < D / 8; ++j)
+        *reinterpret_cast<uint32_t*>(xb + (size_t)row * a.x_ld + h * D + tc::frag_col(4 * j, lane)) =
+            tc::pack_bf16(acc[4 * j + 2 * hr] * z, acc[4 * j + 2 * hr + 1] * z);
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace
 
-// Kf, V: (B,J,4*64) fp32 views (row stride ld, cloud stride bs) -> blob (B x 32 KB bf16 UMMA image of KV_h^T), KS (B,4,64) fp32
+// Kf, V: (B,J,4*64) fp32 views (row stride ld, cloud stride bs) -> blob (B x 32 KB bf16 wgmma image of KV_h^T), KS (B,4,64) fp32
 S6_API int sam6d_linattn_kv_pack(const float* Kf, long long k_ld, long long k_bs, const float* V, long long v_ld, long long v_bs,
                                  int B, int J, void* blob, float* KS, void* stream) {
   S6_REQUIRE(Kf && V && blob && KS && B >= 0 && J > 0);

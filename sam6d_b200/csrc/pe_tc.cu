@@ -1,16 +1,16 @@
 // pe_tc.cu -- PositionalEncoding shared MLP on the tensor cores (PEM/model/fine_point_matching.py:101-121).
 //
 // Rows are (point, sample) pairs of the ball-query groups, 128 rows per tile (4 points at nsample 32, 2 at nsample 64).
-// Per tile, in one CTA of 128 worker threads (thread <-> row) + 1 MMA warp:
+// Per tile, in one CTA of one warpgroup (layer 1: thread <-> row):
 //   layer 1 (6 -> 32)   CUDA cores, fp32: x = [p_j - p_i, p_j]; h1 = relu(W1 x + b1) -> bf16 row of the A1 slab
-//   layer 2 (32 -> 64)  tcgen05.mma M128 N64 (2 x K16) into TMEM; workers read it back, + b2, ReLU, bf16 -> A2 slab
-//   layer 3 (64 -> 128) tcgen05.mma M128 N128 (4 x K16) with the operands swapped: D^T = W3 A2^T, so a TMEM lane is an output
-//                       channel and the columns are the tile's rows (both slabs are K-major, either can be the A operand)
-//   max-pool            thread = channel: the samples of a point are 32 / 64 adjacent columns of its lane -> tcgen05.ld + a
-//                       register max, no shuffles; + b3, ReLU (monotone, commutes with max); a warp stores 32 adjacent channels
+//   layer 2 (32 -> 64)  2 x (2 x wgmma m64n64k16), one per 64-row half; + b2, ReLU, bf16 -> A2 slab straight from the registers
+//   layer 3 (64 -> 128) wgmma with the operands swapped: D^T = W3 A2^T (M = output channel, N = the tile's 128 rows; both slabs are
+//                       K-major, either can be the A operand), one 64-channel half at a time
+//   max-pool            the samples of a point are 32 / 64 adjacent columns: a register max over the thread's columns, then over
+//                       the quad; + b3, ReLU (monotone, commutes with max)
 // BatchNorm is folded into the 1x1 convs on the host.  The (B,6,N,ns) grouped tensor and the (B,128,N,ns) activations of the
 // reference are never materialised; padded duplicate samples are simply recomputed (they cannot change a max).
-// Four CTAs share an SM (56 KB smem, 128 TMEM columns each), so one tile's serial chain hides behind the others'.
+// Four CTAs share an SM (49 KB smem each), so one tile's serial chain hides behind the others'.
 #include <cstdlib>
 
 #include "tc.cuh"
@@ -22,11 +22,9 @@ constexpr int SLAB = ROWS * 128;            // [128 rows][64 bf16]
 constexpr int W2_SLAB = 64 * 128;           // [64 out][64 k] (k >= 32 unused)
 constexpr int W3_SLAB = 128 * 128;          // [128 out][64 k]
 // W2 (64 x 32) lives in the UNUSED K columns 32..63 of the first 64 rows of the A1 slab (layer 1 has 32 channels, so A1 fills only
-// K 0..31 of its 128-byte rows): with a slab of its own a CTA took 57 KB + static and only THREE fitted an SM while the grid was
-// sized for four (ncu r02_pe_sel: a second, quarter-filled wave).  (Letting A2 alias A1 instead was measured: 1.23 ms against
-// 0.86 ms for both radii, at any occupancy.)
+// K 0..31 of its 128-byte rows): with a slab of its own a CTA takes 57 KB + static and only three fit an SM.
 constexpr int SMEM_BYTES = 2 * SLAB + W3_SLAB + 1024;
-constexpr int NUM_THREADS = 160;
+constexpr int NUM_THREADS = 128;
 
 __device__ __forceinline__ void worker_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
@@ -47,8 +45,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 4) pe_tc_kernel(const float* __re
   uint8_t* w3s = a2 + SLAB;
   __shared__ __align__(16) float w1s[32 * 8];
   __shared__ __align__(16) float b1s[32], b2s[64], b3s[128];
-  __shared__ __align__(8) uint64_t a1_full, d2_full, a2_full, d3_full;
-  __shared__ uint32_t tmem_slot;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int PPT = ROWS / NS;                                  // points per tile
@@ -67,44 +63,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 4) pe_tc_kernel(const float* __re
     const int n = u >> 3, c = (u & 7) << 3;
     *reinterpret_cast<uint4*>(w3s + tc::sw128_offset(n, c)) = *reinterpret_cast<const uint4*>(W3 + n * 64 + c);
   }
-  if (tid == 0) {
-    tc::mbar_init(&a1_full, 4); tc::mbar_init(&a2_full, 4);   // one arrival per worker warp (128 arrivals on one word serialise)
-    tc::mbar_init(&d2_full, 1); tc::mbar_init(&d3_full, 1);
-    tc::mbar_fence_init();
-  }
   tc::fence_proxy_async_smem();
-  if (warp == 4) tc::tmem_alloc(&tmem_slot, 128);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 4) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc2 = tc::umma_idesc_bf16(128, 64), idesc3 = tc::umma_idesc_bf16(128, 128);
-      const uint32_t a1_addr = tc::smem_u32(a1), a2_addr = tc::smem_u32(a2), w2_addr = tc::smem_u32(a1) + 64, w3_addr = tc::smem_u32(w3s);
-      uint32_t ph = 0;
-      for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ph ^= 1) {
-        tc::mbar_wait_suspend(&a1_full, ph);
-        tc::tc_fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 2; ++k)
-          tc::umma_bf16(tmem_base, tc::umma_desc_sw128(a1_addr + k * 32), tc::umma_desc_sw128(w2_addr + k * 32), idesc2, k ? 1u : 0u);
-        tc::umma_commit(&d2_full);
-        tc::mbar_wait_suspend(&a2_full, ph);
-        tc::tc_fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc::umma_bf16(tmem_base, tc::umma_desc_sw128(w3_addr + k * 32), tc::umma_desc_sw128(a2_addr + k * 32), idesc3, k ? 1u : 0u);
-        tc::umma_commit(&d3_full);
-      }
-    }
-  } else {
+  {
     // ------------------------------------------------------------------ workers: thread <-> row of the tile
     const int r = tid;
-    const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    uint32_t ph = 0;
+    const uint32_t a1_addr = tc::smem_u32(a1), a2_addr = tc::smem_u32(a2), w2_addr = tc::smem_u32(a1) + 64, w3_addr = tc::smem_u32(w3s);
     // gather pipeline: the neighbour index of tile t+2 and the coordinates of tile t+1 are in flight while tile t is computed.
     // They are issued behind the tile's LAST fence.proxy.async (a fence waits for the thread's outstanding loads).
     auto load_idx = [&](long long tile) -> int {
@@ -127,7 +92,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 4) pe_tc_kernel(const float* __re
     float xn[6];
     load_x(blockIdx.x, load_idx(blockIdx.x), xn);
     int jn = load_idx((long long)blockIdx.x + gridDim.x);
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ph ^= 1) {
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       // ---- layer 1
       {
         float x[6];
@@ -155,64 +120,57 @@ __global__ void __launch_bounds__(NUM_THREADS, 4) pe_tc_kernel(const float* __re
           *reinterpret_cast<uint4*>(row_ptr + ((c ^ (r & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
         }
         tc::fence_proxy_async_smem();
-        __syncwarp();
-        if ((tid & 31) == 0) tc::mbar_arrive(&a1_full);
+        worker_bar();
       }
-      // ---- layer 2 epilogue -> A2
-      tc::mbar_wait_suspend(&d2_full, ph);
-      tc::tc_fence_after_sync();
-      {
-        uint8_t* row_ptr = a2 + r * 128;
+      // ---- layer 2 -> A2
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          float v[32];
-          tc::tmem_ld32(t_addr + half * 32, v);
+      for (int blk = 0; blk < 2; ++blk) {
+        float acc[32];
+        tc::wg_fence();
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t w[4];
-            const float4 ba = *reinterpret_cast<const float4*>(&b2s[half * 32 + c * 8]);
-            const float4 bb = *reinterpret_cast<const float4*>(&b2s[half * 32 + c * 8 + 4]);
-            const float bq[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
+        for (int k = 0; k < 2; ++k)
+          tc::wgmma_bf16<64>(acc, tc::wg_desc(a1_addr + blk * (64 * 128) + k * 32), tc::wg_desc(w2_addr + k * 32), k ? 1u : 0u);
+        tc::wg_commit();
+        tc::wg_wait<0>();
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int o = c * 8 + q * 2;
-              w[q] = tc::pack_bf16(fmaxf(v[o] + bq[q * 2], 0.f), fmaxf(v[o + 1] + bq[q * 2 + 1], 0.f));
-            }
-            *reinterpret_cast<uint4*>(row_ptr + (((half * 4 + c) ^ (r & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-          }
+        for (int i = 0; i < 32; i += 2) {
+          const int row = blk * 64 + tc::frag_row(i, warp, lane), col = tc::frag_col(i, lane);
+          *reinterpret_cast<uint32_t*>(a2 + tc::sw128_offset(row, col)) =
+              tc::pack_bf16(fmaxf(acc[i] + b2s[col], 0.f), fmaxf(acc[i + 1] + b2s[col + 1], 0.f));
         }
-        tc::tc_fence_before_sync();          // our TMEM reads are done before the issuer overwrites the columns
-        tc::fence_proxy_async_smem();
-        __syncwarp();
-        if ((tid & 31) == 0) tc::mbar_arrive(&a2_full);
       }
+      tc::fence_proxy_async_smem();
+      worker_bar();                                         // A2 complete; every thread is past its layer-2 reads of A1
       load_x(tile + gridDim.x, jn, xn);
       jn = load_idx(tile + 2LL * gridDim.x);
-      // ---- layer 3 epilogue: this thread is output channel `tid`; columns [32 c, 32 c + 32) are rows of the tile
-      tc::mbar_wait_suspend(&d3_full, ph);
-      tc::tc_fence_after_sync();
-      {
-        const float bias = b3s[tid];
-        float m = -INFINITY;
+      // ---- layer 3: rows of the accumulator are output channels, columns the tile's rows
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          float v[32];
-          tc::tmem_ld32(t_addr + c * 32, v);
+      for (int blk = 0; blk < 2; ++blk) {
+        float acc[64];
+        tc::wg_fence();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) m = fmaxf(m, v[i]);
-          if (NS == 32 || (c & 1)) {                                // a point's samples are complete
-            const long long p_out = tile * PPT + (NS == 32 ? c : (c >> 1));
-            if (p_out < total_points) st_feat(out + p_out * out_ld + out_off + tid, fmaxf(m + bias, 0.f));
-            m = -INFINITY;
+        for (int k = 0; k < 4; ++k)
+          tc::wgmma_bf16<128>(acc, tc::wg_desc(w3_addr + blk * (64 * 128) + k * 32), tc::wg_desc(a2_addr + k * 32), k ? 1u : 0u);
+        tc::wg_commit();
+        tc::wg_wait<0>();
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int ch = blk * 64 + tc::frag_row(2 * hr, warp, lane);
+          const float bias = b3s[ch];
+#pragma unroll
+          for (int p = 0; p < PPT; ++p) {
+            constexpr int JG = NS / 8;                        // 8-column groups per point
+            float m = -INFINITY;
+#pragma unroll
+            for (int j = p * JG; j < (p + 1) * JG; ++j) m = fmaxf(m, fmaxf(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1]));
+            m = tc::quad_max(m);
+            const long long p_out = tile * PPT + p;
+            if ((lane & 3) == 0 && p_out < total_points) st_feat(out + p_out * out_ld + out_off + ch, fmaxf(m + bias, 0.f));
           }
         }
       }
-      tc::tc_fence_before_sync();
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc(tmem_base, 128);
 }
 
 }  // namespace
@@ -238,8 +196,8 @@ S6_API int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, i
     S6_CHECK(cudaFuncSetAttribute(pe_tc_kernel<NSV, OT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));                 \
     /* ask for the largest shared-memory carve-out: with the default the driver sizes it for fewer resident CTAs */                   \
     S6_CHECK(cudaFuncSetAttribute(pe_tc_kernel<NSV, OT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));                     \
-    /* four CTAs per SM: 4 x 128 TMEM columns, 4 x (49 KB + static) shared memory, 4 x 160 x 96 registers.  (The occupancy    */   \
-    /* API is not used: with the default carve-out it answered fewer and the grid shrank -- measured 1.23 ms instead of 0.86.) */   \
+    /* four CTAs per SM: 4 x (49 KB + static) shared memory, 4 x 128 x 128 registers.  (The occupancy API is not used: with   */   \
+    /* the default carve-out it answers fewer and the grid shrinks.)                                                             */   \
     int per_sm = 4;                                                                                                                 \
     if (const char* ev = getenv("SAM6D_PE_CTAS")) per_sm = atoi(ev) > 0 && atoi(ev) < per_sm ? atoi(ev) : per_sm;                   \
     const int grid = (int)(ntiles < (long long)sms * per_sm ? ntiles : (long long)sms * per_sm);                                    \

@@ -447,8 +447,7 @@ S6_API int sam6d_ball_query(const float* new_xyz, const float* xyz, int b, int n
 // Two concentric ball queries over the same clouds in one sweep (PositionalEncoding groups every point at r1/ns1 and r2/ns2,
 // fine_point_matching.py:104-109).  THREAD per query, candidates broadcast from shared memory as (x, y, z, -) quadruples: one
 // LDS.128 serves 32 queries and a candidate costs ~9 issue slots per warp (3 subtractions, the reference's mul/fma/fma chain,
-// two compares) against ~25 per 32 candidates for the warp-per-query ballot scan it replaces (ncu: that one was issue-bound at
-// 0.47 ms for 131 072 queries x 2048 candidates).  Hits are rare (a few per cent), so the list bookkeeping sits behind a branch.
+// two compares) against ~25 per 32 candidates for the warp-per-query ballot scan it replaces (that one is issue-bound).  Hits are rare (a few per cent), so the list bookkeeping sits behind a branch.
 // The order of a list is the scan order, i.e. ascending index, as in ball_query_gpu.cu:17-49.
 constexpr int BQP_THREADS = 256, BQP_TILE = 2048;
 __global__ void __launch_bounds__(BQP_THREADS) ball_query_pair_kernel(const float* __restrict__ new_xyz, const float* __restrict__ xyz, int n,

@@ -1,20 +1,18 @@
-// rpe_tc.cu -- the relative-position score term of RPEMultiHeadAttention on TMA + tcgen05 (bf16 path).
+// rpe_tc.cu -- the relative-position score term of RPEMultiHeadAttention on TMA + wgmma (bf16 path).
 //
 //   s_p[b,h,n,m] = q_h[b,n,:] . proj_p(E[b,n,m,:])_h = u_h[b,n,:] . E[b,n,m,:],   u_h = W_p,h^T q_h      (PEM/model/transformer.py:369-399)
 //
 // E (clouds, S, S, 256) bf16 is the 1.27 GB pair embedding: this kernel is the one streaming pass over it per self-attention
-// layer -- the HBM-bound "PEM attention" kernel of the roofline report.  The CUDA-core version (attn.cu: rpe_scores_kernel) spends
-// one LDG.128 + 4 unpack + 32 FMA + a 16-value shuffle transpose per 8 channels and is issue-bound at ~0.8 of the HBM peak.
-// Here no CUDA core touches E:
-//   * a query row (b, n) owns the contiguous 197 x 256 bf16 block E[b, n, :, :] (100 KB).  The TMA unit drops it into shared
-//     memory as four K-major SWIZZLE_128B slabs [keys][64 channels] -- exactly the A operand of a tcgen05.mma with M = keys;
+// layer, bound by HBM bandwidth.  The CUDA-core version (attn.cu: rpe_scores_kernel) spends one LDG.128 + 4 unpack + 32 FMA +
+// a 16-value shuffle transpose per 8 channels.  Here no CUDA core touches E:
+//   * a query row (b, n) owns the contiguous S x 256 bf16 block E[b, n, :, :] (100 KB).  The TMA unit drops it into shared
+//     memory as four K-major SWIZZLE_128B slabs [keys][64 channels] -- exactly the A operand of a wgmma with M = keys;
 //   * the four per-head folded queries u_h[b,n,:] (4 x 256 bf16 = 2 KB, contiguous in the projection GEMM's output) arrive by TMA
 //     as rows 0..3 of a 16-row B operand whose other rows stay zero;
-//   * D^T[m, h] = sum_c E[n,m,c] u_h[c]: 2 key tiles x 16 MMAs (M128 N16 K16) per query row into 16 TMEM columns; the tensor
-//     pipe is ~15 % busy, shared memory reads ~20 %, the kernel runs at the speed the 2-stage TMA ring pulls E from HBM;
-//   * 8 epilogue warps read 4 columns per (key tile, query row) with tcgen05.ld: lane = key, so each store instruction writes
-//     32 consecutive fp32 of s_p[b, h, n, :].
-// Persistent: one CTA per SM walks a contiguous range of the clouds*S query rows (rows are independent).
+//   * D^T[m, h] = sum_c E[n,m,c] u_h[c]: per 64-key block 16 x wgmma m64n16k16 into 8 registers per thread; lane = key, so the
+//     threads holding a head's column write adjacent keys of s_p[b, h, n, :].
+// Persistent: one CTA per SM walks a contiguous range of the clouds*S query rows (rows are independent); warp 4 feeds a 2-stage
+// TMA ring, warps 0-3 (one warpgroup) run the MMAs and the stores.
 #include <cuda.h>
 
 #include "tc.cuh"
@@ -29,9 +27,7 @@ constexpr int NB = 16;                                // MMA N: 4 heads + 12 zer
 constexpr int U_SLAB = NB * 128, U_BYTES = KSLABS * U_SLAB;   // 8192
 constexpr int STAGE_BYTES = E_BYTES + U_BYTES;        // 110592
 constexpr int STAGES = 2;
-constexpr int GROUP = 8;                              // query rows per TMEM buffer: 2 key tiles x 8 x 16 = 256 columns
-constexpr int EPI_WARPS = 8;
-constexpr int THREADS = 64 + EPI_WARPS * 32;
+constexpr int THREADS = 128 + 32;
 constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
 
 __global__ void __launch_bounds__(THREADS, 1) rpe_scores_tc_kernel(const __grid_constant__ CUtensorMap tmE,
@@ -39,18 +35,16 @@ __global__ void __launch_bounds__(THREADS, 1) rpe_scores_tc_kernel(const __grid_
                                                                    float* __restrict__ SP, int sp_ld) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // contiguous, balanced row range of this CTA
   const int per = total_rows / gridDim.x, rem = total_rows % gridDim.x;
   const int r0 = blockIdx.x * per + min((int)blockIdx.x, rem), nrows = per + ((int)blockIdx.x < rem ? 1 : 0);
-  const int ntile = (S + 127) >> 7;                   // key tiles of 128 (M of the MMA)
+  const int nblk = (S + 63) >> 6;                     // 64-key blocks (M of the MMA)
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tmem_full_bar[a], 1); tc::mbar_init(&tmem_empty_bar[a], EPI_WARPS * 32); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 4); }
     tc::mbar_fence_init();
     tc::tma_prefetch_desc(&tmE);
     tc::tma_prefetch_desc(&tmU);
@@ -62,14 +56,10 @@ __global__ void __launch_bounds__(THREADS, 1) rpe_scores_tc_kernel(const __grid_
     *reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + E_BYTES + o * 16) = make_uint4(0, 0, 0, 0);
   }
   tc::fence_proxy_async_smem();
-  if (warp == 1) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   s6_pdl_wait();                                      // u comes from the projection GEMM right before us
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------------------------------------------ TMA producer: one query row per stage
     if (lane == 0) {
       const uint32_t tx = (uint32_t)(KSLABS * S * 128 + KSLABS * 4 * 128);
@@ -84,81 +74,45 @@ __global__ void __launch_bounds__(THREADS, 1) rpe_scores_tc_kernel(const __grid_
         for (int kb = 0; kb < KSLABS; ++kb) tc::tma_load_2d(&tmU, &full_bar[s], st + E_BYTES + kb * U_SLAB, kb * 64, row * 4);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(128, NB);
-      int g = 0;
-      for (int i = 0; i < nrows; ++i) {
-        const int s = i % STAGES, j = i % GROUP, buf = g & 1;
-        if (j == 0) {
-          tc::mbar_wait(&tmem_empty_bar[buf], (uint32_t)(((g >> 1) & 1) ^ 1));
-          tc::tc_fence_after_sync();
-        }
-        tc::mbar_wait(&full_bar[s], (uint32_t)((i / STAGES) & 1));
-        tc::tc_fence_after_sync();
-        const uint32_t e_addr = tc::smem_u32(smem + s * STAGE_BYTES), u_addr = e_addr + E_BYTES;
-        for (int t = 0; t < ntile; ++t) {
-          const uint32_t d_addr = tmem_base + (uint32_t)(buf * 256 + t * 128 + j * NB);
+    return;
+  }
+  // ------------------------------------------------------------------ warpgroup: MMAs and stores
+  const size_t SS = (size_t)S * sp_ld;
+  const int w = warp;
+  for (int i = 0; i < nrows; ++i) {
+    const int s = i % STAGES, row = r0 + i;
+    tc::mbar_wait(&full_bar[s], (uint32_t)((i / STAGES) & 1));
+    const uint32_t e_addr = tc::smem_u32(smem + s * STAGE_BYTES), u_addr = e_addr + E_BYTES;
+    float acc[4][NB / 2];
+    tc::wg_fence();
 #pragma unroll
-          for (int kb = 0; kb < KSLABS; ++kb)
+    for (int t = 0; t < 4; ++t) {
+      if (t < nblk) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              tc::umma_bf16(d_addr, tc::umma_desc_sw128(e_addr + kb * SLAB_BYTES + t * (128 * 128) + k * 32),
-                            tc::umma_desc_sw128(u_addr + kb * U_SLAB + k * 32), idesc, (kb | k) ? 1u : 0u);
-        }
-        tc::umma_commit(&empty_bar[s]);
-        if (j == GROUP - 1 || i == nrows - 1) {
-          tc::umma_commit(&tmem_full_bar[buf]);
-          ++g;
-        }
+        for (int kb = 0; kb < KSLABS; ++kb)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            tc::wgmma_bf16<NB>(acc[t], tc::wg_desc(e_addr + kb * SLAB_BYTES + t * (64 * 128) + k * 32), tc::wg_desc(u_addr + kb * U_SLAB + k * 32),
+                               (kb | k) ? 1u : 0u);
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue: warp -> (key tile, TMEM lane quarter)
-    const int ew = warp - 2, quad = warp & 3, t = ew >> 2;
-    const int m = t * 128 + quad * 32 + lane;
-    const bool tile_on = t < ntile;
-    const size_t SS = (size_t)S * sp_ld;
-    int g = 0;
-    for (int i0 = 0; i0 < nrows; i0 += GROUP, ++g) {
-      const int buf = g & 1, cnt = min(GROUP, nrows - i0);
-      tc::mbar_wait(&tmem_full_bar[buf], (uint32_t)((g >> 1) & 1));
-      tc::tc_fence_after_sync();
-      if (tile_on) {
-        uint32_t v[GROUP][4];
-        const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * 256 + t * 128);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&empty_bar[s]);  // values are in registers: the producer may refill the stage
+    // heads 0..3 are columns 0..3 of the fragment: elements 0..3 of the lanes with (lane & 3) < 2
+    if ((lane & 3) < 2) {
+      const int b = row / S, n = row - b * S;
+      float* o = SP + ((size_t)b * 4 * S + n) * sp_ld;
 #pragma unroll
-        for (int j = 0; j < GROUP; ++j)
-          if (j < cnt)
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                         : "=r"(v[j][0]), "=r"(v[j][1]), "=r"(v[j][2]), "=r"(v[j][3])
-                         : "r"(t_addr + j * NB));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tc::tc_fence_before_sync();
-        tc::mbar_arrive(&tmem_empty_bar[buf]);        // values are in registers: the MMA warp may refill the buffer
-        if (m < S) {
-          int row = r0 + i0;
-          int b = row / S, n = row - b * S;
+      for (int t = 0; t < 4; ++t) {
 #pragma unroll
-          for (int j = 0; j < GROUP; ++j) {
-            if (j < cnt) {
-              float* o = SP + ((size_t)b * 4 * S + n) * sp_ld + m;
-#pragma unroll
-              for (int h = 0; h < 4; ++h) o[h * SS] = __uint_as_float(v[j][h]);
-              if (++n == S) { n = 0; ++b; }
-            }
-          }
+        for (int e = 0; e < 4; ++e) {
+          const int m = t * 64 + tc::frag_row(e, w, lane), h = tc::frag_col(e, lane);
+          if (t < nblk && m < S) o[h * SS + m] = acc[t][e];
         }
-      } else {
-        tc::tc_fence_before_sync();
-        tc::mbar_arrive(&tmem_empty_bar[buf]);
       }
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -194,7 +148,7 @@ int make_map(CUtensorMap* map, const void* ptr, long long rows, int box_rows) {
 }  // namespace
 
 // E (B,S,S,256) bf16 contiguous, U (B*S, 4*256) bf16 contiguous (row = the four folded per-head queries of a token)
-// -> SP (B,4,S,S) fp32.  S <= 200.  The tcgen05 / TMA form of sam6d_rpe_scores (PEM/model/transformer.py:369-399).
+// -> SP (B,4,S,S) fp32.  S <= 200.  The wgmma / TMA form of sam6d_rpe_scores (PEM/model/transformer.py:369-399).
 namespace {
 int rpe_scores_tc_launch(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream) {
   S6_REQUIRE(E && U && SP && B >= 0 && S > 0 && S <= SLAB_ROWS && sp_ld >= S);

@@ -1,6 +1,6 @@
 // sam_dec.cu -- the small kernels of the SAM prompt encoder / mask decoder / automatic mask generator (SURVEY.md 8f row N4;
 // ISM/segment_anything/modeling/{prompt_encoder,mask_decoder,transformer}.py, automatic_mask_generator.py, utils/amg.py).
-// The Linears of the decoder (token and image side, the two transposed convolutions written as GEMMs) run on the tcgen05 GEMMs
+// The Linears of the decoder (token and image side, the two transposed convolutions written as GEMMs) run on the wgmma GEMMs
 // (sam6d_gemm_tma / sam6d_gemm_bf16); this file holds what is not a GEMM:
 //   sam_pe_encode          random-Fourier positional encoding of point prompts / of the dense 64 x 64 grid
 //   sam_self_attn          7-token self-attention of the prompt tokens (8 heads x 32)

@@ -6,27 +6,19 @@
 // hid, x, out: (M, 256) bf16;  W_o (256,256), W_e (512,256), W_s (256,512) bf16;  fp32 biases and LayerNorm parameters.
 // The five launches this replaces (GEMM+residual, LayerNorm, GEMM+ReLU, GEMM+residual, LayerNorm) moved each 128-row tile through
 // HBM/L2 nine times; here the tile stays on chip from the attention output to the layer output:
-//   warp 0     TMA: hid tile and x tile (SWIZZLE_128B slabs), then the 20 weight k-blocks {64 k, 256 rows} of the tile through a
-//              3-stage ring (weights come from L2: 640 KB per tile)
-//   warp 1     MMA issuer, tcgen05.mma M128 N256 K16 into two 256-column TMEM accumulators A = [0,256), B = [256,512):
-//                G1 : hid W_o^T                -> A
-//                G2a: y W_e[0:256]^T           -> B          G2b: y W_e[256:512]^T -> A   (A is free once LN1 has read it)
-//                G3 : h[:,0:256] W_s[:,0:256]^T (+) h[:,256:512] W_s[:,256:512]^T -> B     (B is free once h[:,0:256] is written)
-//   warps 2-17 epilogues, thread = (row, 64-column quarter) (eight warps with 128 columns per thread left the four epilogue
-//              phases of a tile as 17 of its 22 us: each is a dependent tcgen05.ld -> math -> st chain per thread, so the phase
-//              time is set by the columns per thread, not by issue slots):
-//                E1 : acc + b_o + x -> LayerNorm1 -> y (bf16) written over the hid slabs as the next A operand
-//                E2a/E2b: relu(acc + b_e) -> h half (bf16) into the slabs the x tile occupied
-//                E3 : acc + b_s + y -> LayerNorm2 -> bf16 tile staged in shared memory -> TMA store
-//              LayerNorm statistics: sum and sum of squares per thread, exchanged between the four warps of a TMEM lane quadrant;
-//              pass 1 writes the pre-norm values back to TMEM so pass 2 is a load + affine.
-// Shared memory: 64 KB (hid -> y) + 64 KB (x -> h half -> output stage) + 96 KB weight ring.
-// Measured and not kept: CTA pairs sharing the weight stream (each CTA loads half of every k-block and TMA-multicasts it into
-// both rings, stages released by multicast tcgen05.commit) -- 0.997 ms per step for the 21 launches against 0.977 ms: the weight
-// reads from L2 are not what bounds a tile, its serial GEMM -> epilogue chain is (22 us per tile, 5 us of it MMA time).
+//   warp 8      TMA (one thread; its warpgroup hands its registers to warps 0-7): hid tile and x tile (SWIZZLE_128B slabs), then the 20 weight k-blocks {64 k, 256 rows} of the tile through a
+//               3-stage ring (weights come from L2: 640 KB per tile)
+//   warps 0-7   two warpgroups; warpgroup g owns rows [64 g, 64 g + 64) of the tile and runs, with one m64n256 fp32 accumulator
+//               in registers (128 per thread):
+//                 G1 : hid W_o^T        E1 : + b_o + x -> LayerNorm1 -> y: bf16 over the hid rows (next A operand) and into the
+//                                            tile's rows of out, where the same thread reads it back as the residual of E3
+//                 G2a: y W_e[0:256]^T   E2a: relu(+ b_e) -> h[:, 0:256] over the x rows
+//                 G2b: y W_e[256:512]^T E2b: relu(+ b_e) -> h[:, 256:512] over the y rows
+//                 G3 : h W_s^T (8 k-blocks from both buffers)   E3 : + b_s + y -> LayerNorm2 -> bf16 rows of out
+//               A row lives in the four threads of a quad: the LayerNorm statistics are two shuffles.  The warpgroups share the
+//               weight stream and nothing else.
+// Shared memory: 64 KB (hid -> y -> h half 1) + 64 KB (x -> h half 0) + 96 KB weight ring.
 #include <cuda.h>
-
-#include <cstdlib>
 
 #include "tc.cuh"
 
@@ -38,8 +30,7 @@ constexpr int T_BYTES = 4 * T_SLAB;              // 64 KB token tile
 constexpr int W_STAGE = 256 * 128;               // 32 KB: [256 rows][64 k] bf16
 constexpr int W_STAGES = 3;
 constexpr int W_PER_TILE = 20;                   // weight k-blocks per tile: 4 (W_o) + 8 (W_e) + 8 (W_s)
-// EPI_WARPS (template parameter): 16 = four column parts per row (default), 8 = two (the first cut, kept as the comparator:
-// SAM6D_TAIL_EPI_WARPS=8)
+constexpr int CONSUMERS = 256, THREADS = CONSUMERS + 128;
 constexpr int SMEM = 2 * T_BYTES + W_STAGES * W_STAGE + 1024;
 
 struct TailArgs {
@@ -49,80 +40,50 @@ struct TailArgs {
   float eps;
 };
 
-__device__ __forceinline__ void named_bar(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// bf16 pair (row r, columns col, col + 1; col even) of a token tile stored as 4 SWIZZLE_128B slabs
+__device__ __forceinline__ uint32_t* tile_pair(uint8_t* tile, int r, int col) {
+  return reinterpret_cast<uint32_t*>(tile + (col >> 6) * T_SLAB + r * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4) + (col & 7) * 2);
+}
+__device__ __forceinline__ float2 unpack2(uint32_t w) { return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u)); }
 
-__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int crd0, int crd1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
-               "r"(tc::smem_u32(smem_src)), "r"(crd0), "r"(crd1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit_wait() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-}
-
-// 8 bf16 of row r, columns [col, col+8) of a token tile stored as 4 SWIZZLE_128B slabs
-__device__ __forceinline__ uint8_t* tile_ptr(uint8_t* tile, int r, int col) {
-  return tile + (col >> 6) * T_SLAB + r * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4);
-}
-__device__ __forceinline__ void unpack8(const uint4& t, float f[8]) {
-  const uint32_t w[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { f[2 * i] = __uint_as_float(w[i] << 16); f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u); }
-}
-
-template <int EPI_WARPS>
-__global__ void __launch_bounds__(64 + EPI_WARPS * 32, 1) tail_tc_kernel(const __grid_constant__ CUtensorMap tmHid, const __grid_constant__ CUtensorMap tmX,
-                                                             const __grid_constant__ CUtensorMap tmWo, const __grid_constant__ CUtensorMap tmWe,
-                                                             const __grid_constant__ CUtensorMap tmWs, const __grid_constant__ CUtensorMap tmOut,
-                                                             TailArgs a) {
-  constexpr int PARTS = EPI_WARPS / 4;             // column parts per row (one warp per TMEM lane quadrant and part)
-  constexpr int CPT = C / PARTS;                   // columns per epilogue thread
-  constexpr int CHUNKS = CPT / 32;
+__global__ void __launch_bounds__(THREADS, 1) tail_tc_kernel(const __grid_constant__ CUtensorMap tmHid, const __grid_constant__ CUtensorMap tmX,
+                                                const __grid_constant__ CUtensorMap tmWo, const __grid_constant__ CUtensorMap tmWe,
+                                                const __grid_constant__ CUtensorMap tmWs, TailArgs a, __nv_bfloat16* __restrict__ out,
+                                                long long ld_out) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* a_buf = smem;                      // hid -> y
-  uint8_t* x_buf = smem + T_BYTES;            // x -> h half 0 -> h half 1 -> output stage
+  uint8_t* a_buf = smem;                      // hid -> y -> h half 1
+  uint8_t* x_buf = smem + T_BYTES;            // x -> h half 0
   uint8_t* w_ring = smem + 2 * T_BYTES;
-  __shared__ __align__(8) uint64_t in_full, w_full[W_STAGES], w_empty[W_STAGES];
-  __shared__ __align__(8) uint64_t acc_full[5];      // G1, G2a, G2b, G3 (and [4]: G3 part 0 complete = h buffer reusable)
-  __shared__ __align__(8) uint64_t y_ready, h0_ready, h1_ready, tile_done;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t in_full, in_empty, w_full[W_STAGES], w_empty[W_STAGES];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntiles = (a.M + BM - 1) / BM;
 
   if (tid == 0) {
-    tc::mbar_init(&in_full, 1);
-    for (int s = 0; s < W_STAGES; ++s) { tc::mbar_init(&w_full[s], 1); tc::mbar_init(&w_empty[s], 1); }
-    for (int i = 0; i < 5; ++i) tc::mbar_init(&acc_full[i], 1);
-    tc::mbar_init(&y_ready, EPI_WARPS); tc::mbar_init(&h0_ready, EPI_WARPS); tc::mbar_init(&h1_ready, EPI_WARPS);   // one arrival per warp
-    tc::mbar_init(&tile_done, 1);
+    tc::mbar_init(&in_full, 1); tc::mbar_init(&in_empty, CONSUMERS / 32);
+    for (int s = 0; s < W_STAGES; ++s) { tc::mbar_init(&w_full[s], 1); tc::mbar_init(&w_empty[s], CONSUMERS / 32); }
     tc::mbar_fence_init();
     tc::tma_prefetch_desc(&tmHid); tc::tma_prefetch_desc(&tmX); tc::tma_prefetch_desc(&tmWo);
-    tc::tma_prefetch_desc(&tmWe); tc::tma_prefetch_desc(&tmWs); tc::tma_prefetch_desc(&tmOut);
+    tc::tma_prefetch_desc(&tmWe); tc::tma_prefetch_desc(&tmWs);
   }
   s6_pdl_trigger();
-  if (warp >= 2) {
-    // the 2048 bias / LayerNorm parameters (8 KB) are read with __ldg inside the four epilogue phases, i.e. on the tile's serial
-    // GEMM -> epilogue chain: a first touch costs an L2 round trip per 32-column chunk (ncu: the epilogue warps' top stall is the
-    // long scoreboard).  They do not depend on the previous kernel, so they are pulled into L1 here, in front of the dependency wait
-    for (int i = tid - 64; i < 512; i += EPI_WARPS * 32) {
+  if (tid < CONSUMERS) {
+    // the 2048 bias / LayerNorm parameters (8 KB) do not depend on the previous kernel: pull them into L1 in front of the
+    // dependency wait instead of paying an L2 round trip inside the first epilogue
+    for (int i = tid; i < 512; i += CONSUMERS) {
       const float* p = i < 64 ? a.bo + i * 4 : i < 128 ? a.g1 + (i - 64) * 4 : i < 192 ? a.b1 + (i - 128) * 4 : i < 320 ? a.be + (i - 192) * 4
                      : i < 384 ? a.bs + (i - 320) * 4 : i < 448 ? a.g2 + (i - 384) * 4 : a.b2 + (i - 448) * 4;
       asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
     }
   }
-  if (warp == 1) tc::tmem_alloc(&tmem_slot, 512);
-  tc::tc_fence_before_sync();
   __syncthreads();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   s6_pdl_wait();                                     // hid / x come from the kernels before us
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (warp >= CONSUMERS / 32) {
+    // ------------------------------------------------------------------ TMA producer (one thread of the third warpgroup)
+    tc::producer_regs();
+    if (tid == CONSUMERS) {
       long long gw = 0;
       int it = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
@@ -138,8 +99,8 @@ __global__ void __launch_bounds__(64 + EPI_WARPS * 32, 1) tail_tc_kernel(const _
           ++gw;
         };
         int j = 0;
-        for (; j < W_STAGES; ++j) load_w(j);         // the ring refills while the previous tile is still in its last epilogue
-        if (it > 0) tc::mbar_wait(&tile_done, (uint32_t)((it - 1) & 1));   // previous tile: y / output stage no longer read
+        for (; j < W_STAGES; ++j) load_w(j);         // the ring refills while the previous tile is still in its last GEMM
+        tc::mbar_wait(&in_empty, (uint32_t)((it & 1) ^ 1));   // previous tile: its G3 no longer reads the h halves
         tc::mbar_arrive_expect_tx(&in_full, 2 * T_BYTES);
 #pragma unroll
         for (int kb = 0; kb < 4; ++kb) {
@@ -149,174 +110,106 @@ __global__ void __launch_bounds__(64 + EPI_WARPS * 32, 1) tail_tc_kernel(const _
         for (; j < W_PER_TILE; ++j) load_w(j);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(BM, 256);
-      const uint32_t a_addr = tc::smem_u32(a_buf), h_addr = tc::smem_u32(x_buf), w_addr0 = tc::smem_u32(w_ring);
-      long long gw = 0;
-      int it = 0;
-      auto gemm4 = [&](uint32_t d_addr, uint32_t op_addr, bool first_acc) {   // 4 weight k-blocks against the 4 slabs of an operand tile
-        for (int kb = 0; kb < 4; ++kb, ++gw) {
-          const int s = (int)(gw % W_STAGES);
-          tc::mbar_wait(&w_full[s], (uint32_t)((gw / W_STAGES) & 1));
-          tc::tc_fence_after_sync();
+    return;
+  }
+  // ------------------------------------------------------------------ warpgroups
+  tc::consumer_regs();
+  const int wg = warp >> 2, w = warp & 3;
+  const uint32_t a_addr = tc::smem_u32(a_buf) + wg * (64 * 128), x_addr = tc::smem_u32(x_buf) + wg * (64 * 128), w_addr0 = tc::smem_u32(w_ring);
+  long long gw = 0;
+  float acc[C / 2];
+  // nkb weight k-blocks against the slabs of an operand tile (k-block kb reads slab kb & 3 of op_addr, or of op_addr2 from kb 4 on)
+  auto gemm = [&](uint32_t op_addr, uint32_t op_addr2, int nkb) {
+    int prev = -1;
+    for (int kb = 0; kb < nkb; ++kb, ++gw) {
+      const int s = (int)(gw % W_STAGES);
+      tc::mbar_wait(&w_full[s], (uint32_t)((gw / W_STAGES) & 1));
+      const uint32_t op = (kb < 4 ? op_addr : op_addr2) + (kb & 3) * T_SLAB;
+      tc::wg_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc::umma_bf16(d_addr, tc::umma_desc_sw128(op_addr + kb * T_SLAB + k * 32), tc::umma_desc_sw128(w_addr0 + s * W_STAGE + k * 32),
-                          idesc, (first_acc && kb == 0 && k == 0) ? 0u : 1u);
-          tc::umma_commit(&w_empty[s]);
-        }
-      };
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const uint32_t ph = (uint32_t)(it & 1);
-        const uint32_t accA = tmem_base, accB = tmem_base + 256;
-        tc::mbar_wait(&in_full, ph);
-        tc::tc_fence_after_sync();
-        gemm4(accA, a_addr, true);                   // G1
-        tc::umma_commit(&acc_full[0]);
-        tc::mbar_wait(&y_ready, ph);                 // y is in a_buf, accumulator A has been read
-        tc::tc_fence_after_sync();
-        gemm4(accB, a_addr, true);                   // G2a
-        tc::umma_commit(&acc_full[1]);
-        gemm4(accA, a_addr, true);                   // G2b
-        tc::umma_commit(&acc_full[2]);
-        tc::mbar_wait(&h0_ready, ph);                // h[:, 0:256] is in x_buf, accumulator B has been read
-        tc::tc_fence_after_sync();
-        gemm4(accB, h_addr, true);                   // G3, k-blocks 0..3
-        tc::umma_commit(&acc_full[4]);
-        tc::mbar_wait(&h1_ready, ph);                // h[:, 256:512] is in x_buf
-        tc::tc_fence_after_sync();
-        gemm4(accB, h_addr, false);                  // G3, k-blocks 4..7
-        tc::umma_commit(&acc_full[3]);
+      for (int k = 0; k < 4; ++k)
+        tc::wgmma_bf16<C>(acc, tc::wg_desc(op + k * 32), tc::wg_desc(w_addr0 + s * W_STAGE + k * 32), (kb | k) ? 1u : 0u);
+      tc::wg_commit();
+      if (prev >= 0) {
+        tc::wg_wait<1>();
+        if (lane == 0) tc::mbar_arrive(&w_empty[prev]);
       }
+      prev = s;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogues: thread = (row, column part)
-    const int ew = warp - 2, quad = warp & 3, part = ew >> 2;
-    const int r = quad * 32 + lane;
-    const int col_h = part * CPT;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const int etid = tid - 64;
-    int it = 0;
-    // LayerNorm over acc + bias + residual tile; result as bf16 into dst tile (SWIZZLE_128B slabs)
-    auto layernorm_epilogue = [&](uint32_t acc, const float* __restrict__ bias, uint8_t* res_tile, const float* __restrict__ g,
-                                  const float* __restrict__ b, uint8_t* dst_tile) {
-      float s = 0.f, q = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < CHUNKS; ++c) {
-        const int col0 = col_h + c * 32;
-        float v[32];
-        tc::tmem_ld32(lane_addr + acc + col0, v);
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(&w_empty[prev]);
+  };
+  // acc <- LayerNorm(acc + bias + residual) * g + b, the residual given per element pair
+  auto layernorm = [&](const float* __restrict__ bias, const float* __restrict__ g, const float* __restrict__ b, auto&& residual) {
+    float s[2] = {0.f, 0.f}, q[2] = {0.f, 0.f};
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float f[8];
-          unpack8(*reinterpret_cast<const uint4*>(tile_ptr(res_tile, r, col0 + j * 8)), f);
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col0 + j * 8)), b1 = __ldg(reinterpret_cast<const float4*>(bias + col0 + j * 8) + 1);
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+    for (int e = 0; e < C / 2; e += 2) {
+      const int hr = (e >> 1) & 1, col = tc::frag_col(e, lane);
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col)), rr = residual(e, hr, col);
+      acc[e] += bb.x + rr.x; acc[e + 1] += bb.y + rr.y;
+      s[hr] += acc[e] + acc[e + 1];
+      q[hr] = fmaf(acc[e], acc[e], fmaf(acc[e + 1], acc[e + 1], q[hr]));
+    }
+    float mean[2], rstd[2];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float x = v[j * 8 + e] + bb[e] + f[e];
-            v[j * 8 + e] = x;
-            s += x;
-            q = fmaf(x, x, q);
-          }
-        }
-        tc::tmem_st32(lane_addr + acc + col0, v);
-      }
-      // statistics of the column parts meet in the first 8 * PARTS bytes of the row's slot in the destination tile: only this
-      // row's threads ever touch those bytes, and pass 2 overwrites them after all of them have read
-      float* stat = reinterpret_cast<float*>(dst_tile + r * 128);
-      stat[part * 2] = s;
-      stat[part * 2 + 1] = q;
-      named_bar(1 + quad, PARTS * 32);               // the warps that share this TMEM lane quadrant
-      float ts = 0.f, tq = 0.f;
+    for (int hr = 0; hr < 2; ++hr) {
+      mean[hr] = tc::quad_sum(s[hr]) * (1.f / C);
+      rstd[hr] = rsqrtf(fmaxf(tc::quad_sum(q[hr]) * (1.f / C) - mean[hr] * mean[hr], 0.f) + a.eps);
+    }
 #pragma unroll
-      for (int p = 0; p < PARTS; ++p) { ts += stat[2 * p]; tq += stat[2 * p + 1]; }
-      const float mean = ts * (1.f / C);
-      const float rstd = rsqrtf(fmaxf(tq * (1.f / C) - mean * mean, 0.f) + a.eps);
-      named_bar(1 + quad, PARTS * 32);               // stat[] may be rewritten by the next LayerNorm only after all have read
-#pragma unroll 1
-      for (int c = 0; c < CHUNKS; ++c) {
-        const int col0 = col_h + c * 32;
-        float v[32];
-        tc::tmem_ld32(lane_addr + acc + col0, v);
+    for (int e = 0; e < C / 2; e += 2) {
+      const int hr = (e >> 1) & 1, col = tc::frag_col(e, lane);
+      const float2 gg = __ldg(reinterpret_cast<const float2*>(g + col)), bb = __ldg(reinterpret_cast<const float2*>(b + col));
+      acc[e] = fmaf((acc[e] - mean[hr]) * rstd[hr], gg.x, bb.x);
+      acc[e + 1] = fmaf((acc[e + 1] - mean[hr]) * rstd[hr], gg.y, bb.y);
+    }
+  };
+  // h half = relu(acc + b_e[...]) -> dst rows of this warpgroup
+  auto relu_store = [&](const float* __restrict__ bias, uint8_t* dst) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 g0 = __ldg(reinterpret_cast<const float4*>(g + col0 + j * 8)), g1 = __ldg(reinterpret_cast<const float4*>(g + col0 + j * 8) + 1);
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(b + col0 + j * 8)), b1 = __ldg(reinterpret_cast<const float4*>(b + col0 + j * 8) + 1);
-          const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w}, bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          float o[8];
+    for (int e = 0; e < C / 2; e += 2) {
+      const int col = tc::frag_col(e, lane), r = wg * 64 + tc::frag_row(e, w, lane);
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+      *tile_pair(dst, r, col) = tc::pack_bf16(fmaxf(acc[e] + bb.x, 0.f), fmaxf(acc[e + 1] + bb.y, 0.f));
+    }
+  };
+  auto publish = [&]() {                             // generic-proxy tile writes -> the warpgroup's next wgmma
+    tc::fence_proxy_async_smem();
+    tc::named_bar(1 + wg, 128);
+  };
+  int it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    tc::mbar_wait(&in_full, (uint32_t)(it & 1));
+    gemm(a_addr, a_addr, 4);                         // G1
+    layernorm(a.bo, a.g1, a.b1, [&](int e, int hr, int col) {
+      return unpack2(*tile_pair(x_buf, wg * 64 + tc::frag_row(e, w, lane), col));
+    });
 #pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] = fmaf((v[j * 8 + e] - mean) * rstd, gg[e], bb[e]);
-          *reinterpret_cast<uint4*>(tile_ptr(dst_tile, r, col0 + j * 8)) =
-              make_uint4(tc::pack_bf16(o[0], o[1]), tc::pack_bf16(o[2], o[3]), tc::pack_bf16(o[4], o[5]), tc::pack_bf16(o[6], o[7]));
-        }
-      }
-    };
-    auto relu_epilogue = [&](uint32_t acc, const float* __restrict__ bias) {   // h half = relu(acc + b_e[...]) -> x_buf
-#pragma unroll 1
-      for (int c = 0; c < CHUNKS; ++c) {
-        const int col0 = col_h + c * 32;
-        float v[32];
-        tc::tmem_ld32(lane_addr + acc + col0, v);
+    for (int e = 0; e < C / 2; e += 2) {             // E1: y -> over the hid rows (G1 has completed) and into out
+      const int r = wg * 64 + tc::frag_row(e, w, lane), col = tc::frag_col(e, lane), row = tile * BM + r;
+      const uint32_t y2 = tc::pack_bf16(acc[e], acc[e + 1]);
+      *tile_pair(a_buf, r, col) = y2;
+      if (row < a.M) *reinterpret_cast<uint32_t*>(out + (size_t)row * ld_out + col) = y2;
+    }
+    publish();                                       // also: every thread has read its x before h half 0 goes there
+    gemm(a_addr, a_addr, 4);                         // G2a
+    relu_store(a.be, x_buf);
+    gemm(a_addr, a_addr, 4);                         // G2b
+    tc::named_bar(1 + wg, 128);                      // all of G2b has read y before h half 1 overwrites it
+    relu_store(a.be + 256, a_buf);
+    publish();
+    gemm(x_addr, a_addr, 8);                         // G3
+    if (lane == 0) tc::mbar_arrive(&in_empty);       // the tile buffers are free for the next tile's hid / x
+    layernorm(a.bs, a.g2, a.b2, [&](int e, int, int col) {
+      const int row = tile * BM + wg * 64 + tc::frag_row(e, w, lane);
+      return row < a.M ? unpack2(*reinterpret_cast<const uint32_t*>(out + (size_t)row * ld_out + col)) : make_float2(0.f, 0.f);
+    });
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col0 + j * 8)), b1 = __ldg(reinterpret_cast<const float4*>(bias + col0 + j * 8) + 1);
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          float o[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] = fmaxf(v[j * 8 + e] + bb[e], 0.f);
-          *reinterpret_cast<uint4*>(tile_ptr(x_buf, r, col0 + j * 8)) =
-              make_uint4(tc::pack_bf16(o[0], o[1]), tc::pack_bf16(o[2], o[3]), tc::pack_bf16(o[4], o[5]), tc::pack_bf16(o[6], o[7]));
-        }
-      }
-    };
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const uint32_t ph = (uint32_t)(it & 1);
-      // E1: y = LN1(acc A + b_o + x) -> a_buf (the hid slabs: G1 has completed)
-      tc::mbar_wait_suspend(&acc_full[0], ph);
-      tc::tc_fence_after_sync();
-      layernorm_epilogue(0u, a.bo, x_buf, a.g1, a.b1, a_buf);
-      tc::tc_fence_before_sync();
-      tc::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&y_ready);          // per warp: 512 arrivals on one barrier word serialise
-      // E2a: h[:, 0:256] = relu(acc B + b_e[0:256]) -> x_buf (the x tile is dead: every thread passed y_ready before G2a ran)
-      tc::mbar_wait_suspend(&acc_full[1], ph);
-      tc::tc_fence_after_sync();
-      relu_epilogue(256u, a.be);
-      tc::tc_fence_before_sync();
-      tc::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&h0_ready);          // per warp: 512 arrivals on one barrier word serialise
-      // E2b: h[:, 256:512] = relu(acc A + b_e[256:512]) -> x_buf once G3's first half has consumed h[:, 0:256]
-      tc::mbar_wait_suspend(&acc_full[2], ph);
-      tc::mbar_wait_suspend(&acc_full[4], ph);
-      tc::tc_fence_after_sync();
-      relu_epilogue(0u, a.be + 256);
-      tc::tc_fence_before_sync();
-      tc::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&h1_ready);          // per warp: 512 arrivals on one barrier word serialise
-      // E3: out = LN2(acc B + b_s + y) -> staged in x_buf (G3 has completed) -> TMA store
-      tc::mbar_wait_suspend(&acc_full[3], ph);
-      tc::tc_fence_after_sync();
-      layernorm_epilogue(256u, a.bs, a_buf, a.g2, a.b2, x_buf);
-      tc::tc_fence_before_sync();
-      tc::fence_proxy_async_smem();
-      named_bar(5, EPI_WARPS * 32);
-      if (etid == 0) {
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) tma_store_2d(&tmOut, x_buf + kb * T_SLAB, kb * BK, tile * BM);
-        tma_store_commit_wait();                     // the stage has been read: the next tile's x may land in it
-        tc::mbar_arrive(&tile_done);
-      }
+    for (int e = 0; e < C / 2; e += 2) {
+      const int row = tile * BM + wg * 64 + tc::frag_row(e, w, lane);
+      if (row < a.M) *reinterpret_cast<uint32_t*>(out + (size_t)row * ld_out + tc::frag_col(e, lane)) = tc::pack_bf16(acc[e], acc[e + 1]);
     }
   }
-  tc::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -352,7 +245,8 @@ int make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols, 
 
 // out = LN2(y + relu(y We^T + be) Ws^T + bs),  y = LN1(hid Wo^T + bo + x)   (PEM/model/transformer.py:176-197, 435-438)
 // hid, x, out: (M,256) bf16 with row strides ld_* (multiples of 8 elements); Wo (256,256), We (512,256), Ws (256,512) bf16
-// row-major contiguous; fp32 vectors bo, g1, b1 (256), be (512), bs, g2, b2 (256).  out may not overlap hid or x of other rows.
+// row-major contiguous; fp32 vectors bo, g1, b1 (256), be (512), bs, g2, b2 (256).  out may not overlap hid or x of other rows
+// (it is the scratch of the intermediate y of its own rows).
 S6_API int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const void* x, long long ld_x, const void* Wo, const float* bo,
                                        const float* g1, const float* b1, const void* We, const float* be, const void* Ws, const float* bs,
                                        const float* g2, const float* b2, void* out, long long ld_out, int M, float eps, void* stream) {
@@ -363,11 +257,10 @@ S6_API int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const 
                reinterpret_cast<uintptr_t>(bs) | reinterpret_cast<uintptr_t>(g1) | reinterpret_cast<uintptr_t>(b1) | reinterpret_cast<uintptr_t>(g2) |
                reinterpret_cast<uintptr_t>(b2)) & 15) == 0);
   if (M == 0) return 0;
-  CUtensorMap tmHid, tmX, tmWo, tmWe, tmWs, tmOut;
+  CUtensorMap tmHid, tmX, tmWo, tmWe, tmWs;
   int rc;
   if ((rc = make_map(&tmHid, hid, M, C, ld_hid, BM))) return rc;
   if ((rc = make_map(&tmX, x, M, C, ld_x, BM))) return rc;
-  if ((rc = make_map(&tmOut, out, M, C, ld_out, BM))) return rc;
   if ((rc = make_map(&tmWo, Wo, C, C, C, 256))) return rc;
   if ((rc = make_map(&tmWe, We, HID, C, C, 256))) return rc;
   if ((rc = make_map(&tmWs, Ws, C, HID, HID, 256))) return rc;
@@ -376,14 +269,9 @@ S6_API int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const 
   S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int ntiles = s6_cdiv(M, BM), grid = ntiles < sms ? ntiles : sms;
   TailArgs a{bo, g1, b1, be, bs, g2, b2, M, eps};
-  static const int epi_warps = [] { const char* e = getenv("SAM6D_TAIL_EPI_WARPS"); return (e && atoi(e) == 8) ? 8 : 16; }();
-  if (epi_warps == 8) {
-    S6_CHECK(cudaFuncSetAttribute(tail_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    S6_CHECK(s6_launch_pdl(tail_tc_kernel<8>, dim3(grid), dim3(64 + 8 * 32), SMEM, s6_stream(stream), tmHid, tmX, tmWo, tmWe, tmWs, tmOut, a));
-  } else {
-    S6_CHECK(cudaFuncSetAttribute(tail_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    S6_CHECK(s6_launch_pdl(tail_tc_kernel<16>, dim3(grid), dim3(64 + 16 * 32), SMEM, s6_stream(stream), tmHid, tmX, tmWo, tmWe, tmWs, tmOut, a));
-  }
+  S6_CHECK(cudaFuncSetAttribute(tail_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  S6_CHECK(s6_launch_pdl(tail_tc_kernel, dim3(grid), dim3(THREADS), SMEM, s6_stream(stream), tmHid, tmX, tmWo, tmWe, tmWs, a,
+                         reinterpret_cast<__nv_bfloat16*>(out), ld_out));
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -1,5 +1,9 @@
-// tc.cuh -- sm_100a tensor-core plumbing: mbarrier, TMEM allocation, UMMA (tcgen05.mma) descriptors for K-major
-// 128-byte-swizzled bf16 operands, tcgen05.ld epilogue loads, proxy fences and TMA 2-D tile loads.  Inline PTX only.
+// tc.cuh -- sm_90a tensor-core plumbing: mbarrier, TMA 2-D tile loads, proxy fences and warpgroup MMA (wgmma) on K-major
+// 128-byte-swizzled bf16 operands with fp32 accumulators in registers.  Inline PTX only.
+//
+// Accumulator fragment of one m64nN wgmma (the layout every kernel here reads its results in): thread t of the warpgroup
+// (warp w = t / 32, lane l) holds d[i], i < N/2, at row 16 w + l/4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1)
+// (frag_row / frag_col).  A row of the tile lives in the four lanes of a quad, so row reductions are two xor-shuffles.
 #pragma once
 #include "common.cuh"
 
@@ -38,112 +42,101 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
-// the same wait with a suspend-time hint: the warp sleeps in the barrier unit instead of re-issuing try_wait every ~25 cycles
-// (a lone MMA-issuer thread spinning took 22 % of its sub-partition's issue slots in the geometric embedding, ncu r02_geo)
-__device__ __forceinline__ void mbar_wait_suspend(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity), "r"(0x989680u)
-      : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------------------- fences
-// generic-proxy smem writes (st.shared) -> visible to the async proxy (tcgen05.mma / TMA reads)
+// generic-proxy smem writes (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// ---------------------------------------------------------------------------------------------------------- TMEM
-// whole warp; writes the base address (lane 0, column base) into *slot (shared memory)
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float v[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 32 lanes x 32 consecutive fp32 columns, registers -> TMEM (same mapping as tmem_ld32)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float v[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-      "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-      "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-      "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-      "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------- UMMA
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 64 bf16 (128 bytes) with the 128-byte
-// swizzle (16-byte chunk index XOR (row % 8)); 8-row groups are 1024 bytes apart (SBO), tile base 1024-byte aligned.
-// Fields (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// layout_type [61,64) = 2 (SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// ---------------------------------------------------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 64 bf16 (128 bytes) with the 128-byte swizzle
+// (16-byte chunk index XOR (row % 8)); 8-row groups are 1024 bytes apart (SBO), tile base 1024-byte aligned.  The k-th 16-wide
+// K step of a slab starts 32 k bytes further.  Fields: start>>4 [0,14), LBO>>4 [16,30) (unused when swizzled), SBO>>4 [32,46),
+// layout [62,64) = 1 (SWIZZLE_128B).
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                    // LBO (ignored for swizzled K-major), canonical value 1
-  d |= (uint64_t)(1024 >> 4) << 32;          // SBO = 1024 B between 8-row groups
-  d |= (uint64_t)1 << 46;                    // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                    // SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
+// before the first wgmma that reads or writes accumulator registers the warpgroup has touched
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed groups of this warpgroup are still running
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Instruction descriptor (InstrDescriptor): D fp32, A/B bf16, both K-major, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4)        // c_format = F32
-         | (1u << 7)      // a_format = BF16
-         | (1u << 10)     // b_format = BF16
-         | (0u << 15)     // a_major = K
-         | (0u << 16)     // b_major = K
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D (64 x N, fp32 fragment) (+)= A (64 x 16, K-major smem) * B (N x 16, K-major smem)^T; all 128 threads of the warpgroup
+template <int N>
+struct Wgmma;
+// the specialisations: register lists "%0, ..." in chunks of eight, "+f" operand lists of the fragment
+#define S6_R0 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define S6_R1 "%8, %9, %10, %11, %12, %13, %14, %15"
+#define S6_R2 "%16, %17, %18, %19, %20, %21, %22, %23"
+#define S6_R3 "%24, %25, %26, %27, %28, %29, %30, %31"
+#define S6_R4 "%32, %33, %34, %35, %36, %37, %38, %39"
+#define S6_R5 "%40, %41, %42, %43, %44, %45, %46, %47"
+#define S6_R6 "%48, %49, %50, %51, %52, %53, %54, %55"
+#define S6_R7 "%56, %57, %58, %59, %60, %61, %62, %63"
+#define S6_R8 "%64, %65, %66, %67, %68, %69, %70, %71"
+#define S6_R9 "%72, %73, %74, %75, %76, %77, %78, %79"
+#define S6_R10 "%80, %81, %82, %83, %84, %85, %86, %87"
+#define S6_R11 "%88, %89, %90, %91, %92, %93, %94, %95"
+#define S6_R12 "%96, %97, %98, %99, %100, %101, %102, %103"
+#define S6_R13 "%104, %105, %106, %107, %108, %109, %110, %111"
+#define S6_R14 "%112, %113, %114, %115, %116, %117, %118, %119"
+#define S6_R15 "%120, %121, %122, %123, %124, %125, %126, %127"
+#define S6_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define S6_F8(i) S6_F4(i), S6_F4(i + 4)
+#define S6_F16(i) S6_F8(i), S6_F8(i + 8)
+#define S6_F32(i) S6_F16(i), S6_F16(i + 16)
+#define S6_F64(i) S6_F32(i), S6_F32(i + 32)
+// DA, DB, ACC: the operand numbers that follow the N/2 accumulator registers
+#define S6_WGMMA(N, REGS, DA, DB, ACC, ...)                                                                                     \
+  template <>                                                                                                                \
+  struct Wgmma<N> {                                                                                                          \
+    __device__ __forceinline__ static void mma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {                 \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " ACC ", 0;\n\twgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" \
+                   REGS "}, " DA ", " DB ", p, 1, 1, 0, 0;\n\t}"                                                             \
+                   : __VA_ARGS__                                                                                             \
+                   : "l"(da), "l"(db), "r"(acc));                                                                            \
+    }                                                                                                                        \
+  };
+S6_WGMMA(16, S6_R0, "%8", "%9", "%10", S6_F8(0))
+S6_WGMMA(32, S6_R0 ", " S6_R1, "%16", "%17", "%18", S6_F16(0))
+S6_WGMMA(64, S6_R0 ", " S6_R1 ", " S6_R2 ", " S6_R3, "%32", "%33", "%34", S6_F32(0))
+S6_WGMMA(80, S6_R0 ", " S6_R1 ", " S6_R2 ", " S6_R3 ", " S6_R4, "%40", "%41", "%42", S6_F32(0), S6_F8(32))
+S6_WGMMA(128, S6_R0 ", " S6_R1 ", " S6_R2 ", " S6_R3 ", " S6_R4 ", " S6_R5 ", " S6_R6 ", " S6_R7, "%64", "%65", "%66", S6_F64(0))
+S6_WGMMA(256, S6_R0 ", " S6_R1 ", " S6_R2 ", " S6_R3 ", " S6_R4 ", " S6_R5 ", " S6_R6 ", " S6_R7 ", " S6_R8 ", " S6_R9 ", " S6_R10
+         ", " S6_R11 ", " S6_R12 ", " S6_R13 ", " S6_R14 ", " S6_R15, "%128", "%129", "%130", S6_F64(0), S6_F64(64))
+
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  Wgmma<N>::mma(d, da, db, accumulate);
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// position of fragment element i inside the 64-row tile of warpgroup thread (warp w of the group, lane l)
+__host__ __device__ constexpr int frag_row(int i, int w, int l) { return 16 * w + (l >> 2) + 8 * ((i >> 1) & 1); }
+__host__ __device__ constexpr int frag_col(int i, int l) { return 8 * (i >> 2) + 2 * (l & 3) + (i & 1); }
+
+// sum / max over the four lanes of a quad (the four threads that hold one accumulator row)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
+
+// warp-specialised kernels of three warpgroups (one TMA thread + two MMA warpgroups): the TMA warpgroup hands its registers
+// to the MMA warpgroups (40 + 2 x 232 per thread of a warpgroup fill the register file at 384 threads)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs)); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs)); }
+
+__device__ __forceinline__ void named_bar(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // byte offset of element (row, col) inside a [rows][64] bf16 tile with the 128-byte swizzle
 __device__ __forceinline__ uint32_t sw128_offset(int row, int col) {

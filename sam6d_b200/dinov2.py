@@ -1,4 +1,4 @@
-"""ISM descriptor branch on B200 kernels (SURVEY.md 8f row N2): drop-ins for
+"""ISM descriptor branch on H100 kernels (SURVEY.md 8f row N2): drop-ins for
     DinoVisionTransformer (ViT-L/14 = dinov2_vitl14)   ISM/model/vision_transformer.py:43-375
     CustomDINOv2                                        ISM/model/dinov2.py:92-258
     MaskedPatch_MatrixSimilarity (compute_straight / compute_visible_ratio)   ISM/model/loss.py:46-77
@@ -7,7 +7,7 @@
 The trunk is a pre-norm ViT with LayerScale: parameter names are the reference's (`cls_token`, `pos_embed` (1, 1370, C),
 `mask_token`, `patch_embed.proj`, `blocks.N.{norm1, attn.{qkv,proj}, ls1.gamma, norm2, mlp.{fc1,fc2}, ls2.gamma}`, `norm`), so
 `dinov2_vitl14_pretrain.pth` loads unchanged.  Every forward runs through the C ABI:
-    patch embedding, qkv / proj / fc1 / fc2                -> sam6d_gemm_tma / sam6d_gemm_tc (tcgen05; bias, GELU, residual epilogues;
+    patch embedding, qkv / proj / fc1 / fc2                -> sam6d_gemm_tma / sam6d_gemm_tc (wgmma; bias, GELU, residual epilogues;
                                                               LayerScale folded into proj / fc2 when the weights are packed)
     LayerNorm                                              -> sam6d_layernorm_bf16
     attention over 257 tokens (16 heads x 64)              -> sam6d_attn_tc_ex on keys 0..255 (tensor cores, log-sum-exp out)

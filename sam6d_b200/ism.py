@@ -3,7 +3,7 @@
 Mirrors  PairwiseSimilarity                         ISM/model/loss.py:21-44
          Instance_Segmentation_Model.compute_semantic_score / best_template_pose
                                                     ISM/model/detector.py:198-207, 260-296
-with the same call signatures and return values.  One fused sm_100a kernel (csrc/ism.cu) computes the clamped cosine
+with the same call signatures and return values.  One fused sm_90a kernel (csrc/ism.cu) computes the clamped cosine
 matrix, the avg-5 aggregation, the object argmax and the best-template argmax; the reference's P-fold replication of the
 reference descriptors is never formed.
 

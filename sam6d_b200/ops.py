@@ -158,7 +158,7 @@ _DT = {torch.float32: 0, torch.bfloat16: 1}
 
 def gemm_tc_raw(A_ptr, a_dt, W_ptr, w_dt, bias, R_ptr, C_ptr, c_dt, M, N, K, lda, ldw, ldc, ldr, batch=1, sA=0, sW=0, sC=0, sR=0,
                 alpha=1.0, relu=False):
-    """tcgen05 bf16 GEMM over raw device addresses; *_dt: 0 = fp32, 1 = bf16"""
+    """wgmma bf16 GEMM over raw device addresses; *_dt: 0 = fp32, 1 = bf16"""
     _lib.call("sam6d_gemm_bf16", ctypes.c_void_p(A_ptr), int(a_dt), ctypes.c_void_p(W_ptr), int(w_dt), _p(bias),
               ctypes.c_void_p(R_ptr or 0), ctypes.c_void_p(C_ptr), int(c_dt), int(M), int(N), int(K), _ll(lda), _ll(ldw), _ll(ldc),
               _ll(ldr), int(batch), _ll(sA), _ll(sW), _ll(sC), _ll(sR), _f(alpha), int(relu), _s())
@@ -184,7 +184,7 @@ def gemm_tc(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optio
 
 def gemm_tma(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optional[Tensor] = None, out: Optional[Tensor] = None,
              act: int = 0, alpha: float = 1.0, out_dtype=torch.float32) -> Tensor:
-    """persistent TMA-fed tcgen05 GEMM: A (M,K) bf16, W (N,K) bf16 -> (M,N) fp32|bf16"""
+    """persistent TMA-fed wgmma GEMM: A (M,K) bf16, W (N,K) bf16 -> (M,N) fp32|bf16"""
     _check(A, torch.bfloat16, "A", 2)
     _check(W, torch.bfloat16, "W", 2)
     M, K = A.shape
@@ -293,7 +293,7 @@ def layernorm_bf16io(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5, 
 def transformer_tail_bf16(hid: Tensor, x: Tensor, wo: Tensor, bo: Tensor, g1: Tensor, b1: Tensor, we: Tensor, be: Tensor, ws: Tensor,
                           bs: Tensor, g2: Tensor, b2: Tensor, out: Optional[Tensor] = None, eps: float = 1e-5) -> Tensor:
     """LN2(y + relu(y We^T + be) Ws^T + bs) with y = LN1(hid Wo^T + bo + x): the attention-layer tail + AttentionOutput of
-    transformer.py:176-197 as one persistent TMA / tcgen05 kernel (csrc/tail_tc.cu).  hid, x (M,256) bf16 -> (M,256) bf16."""
+    transformer.py:176-197 as one persistent TMA / wgmma kernel (csrc/tail_tc.cu).  hid, x (M,256) bf16 -> (M,256) bf16."""
     _check(hid, torch.bfloat16, "hid", 2)
     _check(x, torch.bfloat16, "x", 2)
     M = hid.shape[0]
@@ -418,7 +418,7 @@ def geo_embed_f32(T: Tensor, div_term: Tensor, WaT: Tensor, WdT: Tensor, bias: T
 
 
 def geo_embed_tc(T: Tensor, div_term: Tensor, Wa_bf16: Tensor, Wd_bf16: Tensor, bias: Tensor, out_dtype=torch.bfloat16) -> Tensor:
-    """tcgen05 version: weights (out,in) bf16, E (B,S,S,256) fp32 or bf16"""
+    """wgmma version: weights (out,in) bf16, E (B,S,S,256) fp32 or bf16"""
     _check(T, torch.float32, "T", 4)
     _check(Wa_bf16, torch.bfloat16, "Wa", 2)
     _check(Wd_bf16, torch.bfloat16, "Wd", 2)
@@ -430,7 +430,7 @@ def geo_embed_tc(T: Tensor, div_term: Tensor, Wa_bf16: Tensor, Wd_bf16: Tensor, 
 
 
 def geo_embed_dist_tc(T: Tensor, div_term: Tensor, Wd_bf16: Tensor, bias: Tensor) -> Tensor:
-    """distance projection only: T (..., 4) f32 -> (..., 256) bf16 = proj_d(emb(T[..., 3])) + bias (tcgen05)"""
+    """distance projection only: T (..., 4) f32 -> (..., 256) bf16 = proj_d(emb(T[..., 3])) + bias (wgmma)"""
     if T.dtype != torch.float32 or not T.is_cuda or not T.is_contiguous() or T.shape[-1] != 4:
         raise RuntimeError("T must be a contiguous CUDA float32 tensor (..., 4)")
     _check(Wd_bf16, torch.bfloat16, "Wd", 2)
@@ -475,7 +475,7 @@ def rpe_scores(E: Tensor, U: Tensor, u_ptr: Optional[int] = None, u_ld: int = 10
 
 def rpe_scores_tc(E: Tensor, U: Tensor) -> Tensor:
     """E (B,S,S,256) bf16, U (B*S, 1024) bf16 = the four folded per-head queries of every token -> (B,4,S,S) f32.
-    TMA + tcgen05 stream over E (csrc/rpe_tc.cu); S <= 200."""
+    TMA + wgmma stream over E (csrc/rpe_tc.cu); S <= 200."""
     _check(E, torch.bfloat16, "E", 4)
     _check(U, torch.bfloat16, "U", 2)
     B, S = E.shape[0], E.shape[1]
@@ -543,7 +543,7 @@ def pack_rel_pos(rel_h: Tensor, rel_w: Tensor, slab_rows: int = 32) -> Tensor:
 
 
 def attn_global_tc(qkv: Tensor, vt: Tensor, rel_blob: Tensor, B: int, H: int, grid: int, scale: float, out_dtype=torch.bfloat16) -> Tensor:
-    """SAM global attention (grid x grid = 4096 tokens, head_dim 80) on tcgen05: qkv (B*L, 3*H*80) bf16, vt from
+    """SAM global attention (grid x grid = 4096 tokens, head_dim 80) on wgmma: qkv (B*L, 3*H*80) bf16, vt from
     transpose_tokens, rel_blob from pack_rel_pos(rel_h, rel_w, slab_rows=128) -> (B*L, H*80)"""
     _check(qkv, torch.bfloat16, "qkv", 2)
     _check(vt, torch.bfloat16, "vt", 2)
@@ -624,7 +624,7 @@ def linattn_apply_raw(q_ptr, q_rpb, q_bs, q_ld, KV: Tensor, KS: Tensor, B, H, x_
 
 # ---------------------------------------------------------------------------------------------- coarse pose
 def linattn_kv_pack_raw(k_ptr, k_ld, k_bs, v_ptr, v_ld, v_bs, B, J, device):
-    """focused keys / values ((B,J,256) fp32 views) -> (blob: B x 32 KB bf16 UMMA image of KV_h^T, KS (B,4,64) fp32)"""
+    """focused keys / values ((B,J,256) fp32 views) -> (blob: B x 32 KB bf16 wgmma image of KV_h^T, KS (B,4,64) fp32)"""
     blob = torch.empty(B, 4 * 64 * 64, dtype=torch.bfloat16, device=device)
     KS = torch.empty(B, 4, 64, dtype=torch.float32, device=device)
     _lib.call("sam6d_linattn_kv_pack", ctypes.c_void_p(k_ptr), _ll(k_ld), _ll(k_bs), ctypes.c_void_p(v_ptr), _ll(v_ld), _ll(v_bs),
@@ -633,7 +633,7 @@ def linattn_kv_pack_raw(k_ptr, k_ld, k_bs, v_ptr, v_ld, v_bs, B, J, device):
 
 
 def linattn_tc_raw(q_ptr, q_ld, q_bs, blob: Tensor, KS: Tensor, sp_scale: Tensor, B, rpb, x_ptr, x_ld, x_bs):
-    """dense tokens (bf16): focusing feature map + per-head (q' KV) / (q' . ksum) on tcgen05"""
+    """dense tokens (bf16): focusing feature map + per-head (q' KV) / (q' . ksum) on wgmma"""
     _lib.call("sam6d_linattn_tc", ctypes.c_void_p(q_ptr), _ll(q_ld), _ll(q_bs), _p(blob), _p(KS), _p(sp_scale), int(B), int(rpb),
               ctypes.c_void_p(x_ptr), _ll(x_ld), _ll(x_bs), _s())
 
@@ -752,7 +752,7 @@ def fine_assign(A: Tensor, pts2: Tensor, shift: float):
 
 def fine_assign_tc(f1n: Tensor, f2n: Tensor, pts2: Tensor, alpha: float):
     """the assignment of compute_fine_Rt from the normalised bf16 tokens f1n (B,S,256) [scene, rows] and f2n (B,S,256) [template,
-    columns] without forming the (B,S,S) score matrix: 4 tcgen05 passes (row sums, column sums, column labels, row labels +
+    columns] without forming the (B,S,S) score matrix: 4 wgmma passes (row sums, column sums, column labels, row labels +
     weighted correspondences).  alpha = 1/temp (also the softmax shift: cosine <= 1).  -> lab1 (B,S), lab2 (B,S), wts, pred"""
     _check(f1n, torch.bfloat16, "f1n", 3)
     _check(f2n, torch.bfloat16, "f2n", 3)

@@ -1,4 +1,4 @@
-"""Pose Estimation Model matching path on B200 kernels -- drop-in for the reference's model classes.
+"""Pose Estimation Model matching path on H100 kernels -- drop-in for the reference's model classes.
 
 Class names, constructor arguments, sub-module / parameter names (hence `state_dict` keys) and the `forward` contracts
 mirror the reference:
@@ -9,7 +9,7 @@ mirror the reference:
     CoarsePointMatching         PEM/model/coarse_point_matching.py:14-81
     FinePointMatching           PEM/model/fine_point_matching.py:12-126
 so `sam-6d-pem-base.pth` loads unchanged.  The torch modules here are parameter containers only: every forward runs
-hand-written sm_100a kernels through the C ABI (sam6d_b200/ops.py); inference only (the reference's training branches --
+hand-written sm_90a kernels through the C ABI (sam6d_b200/ops.py); inference only (the reference's training branches --
 losses, pose-noise augmentation -- are out of scope), and there is no CPU path.
 """
 import math
@@ -25,16 +25,16 @@ from . import ops
 NUM_HEADS = 4  # hard-coded in the reference (coarse_point_matching.py:31, fine_point_matching.py:29)
 
 # Arithmetic of the dense projections.  "fp32": CUDA-core kernels, fp32 storage (exact path, parity reference).
-# "bf16": tcgen05 tensor-core kernels -- operands rounded to bf16, fp32 accumulation in TMEM, geometric embedding stored
+# "bf16": wgmma tensor-core kernels -- operands rounded to bf16, fp32 accumulation in registers, geometric embedding stored
 # in bf16.  Index-valued results (FPS, ball query, labels) and the pose solvers are identical in both modes.
 PRECISIONS = ("fp32", "bf16")
 # bf16 path: linear + residual + LayerNorm + FFN + LayerNorm of every transformer layer as one kernel (csrc/tail_tc.cu);
 # False = the five-launch form (GEMM, LayerNorm, GEMM, GEMM, LayerNorm) kept as its comparator
 FUSED_TAIL = os.environ.get("SAM6D_FUSED_TAIL", "1") != "0"
-# the relative-position score stream over E on TMA + tcgen05 (csrc/rpe_tc.cu); False = the CUDA-core kernel (csrc/attn.cu)
+# the relative-position score stream over E on TMA + wgmma (csrc/rpe_tc.cu); False = the CUDA-core kernel (csrc/attn.cu)
 PADDED_BIAS = os.environ.get("SAM6D_PADDED_BIAS", "1") != "0"
 RPE_TC = os.environ.get("SAM6D_RPE_TC", "1") != "0"
-# bf16 path: the geometric embedding by table interpolation (csrc/geo_lut.cu); False = the tcgen05 projections (csrc/geo_tc.cu)
+# bf16 path: the geometric embedding by table interpolation (csrc/geo_lut.cu); False = the wgmma projections (csrc/geo_tc.cu)
 GEO_LUT = os.environ.get("SAM6D_GEO_LUT", "1") != "0"
 GEO_LUT_PRECISE = os.environ.get("SAM6D_GEO_LUT_PRECISE", "1") != "0"   # fp32 interpolation, one rounding at the store
 GEO_LUT_INV_H = 8.0            # table step 1/8 index unit
@@ -266,7 +266,7 @@ class GeometricTransformer(nn.Module):
         x2d = x.view(B * S, C)
         if RPE_TC and S <= 200 and emb.dtype == torch.bfloat16:
             # ONE projection launch: (q | k) rows, V^T, and the folded rel-pos queries u as bf16 rows = the B operand of the TMA /
-            # tcgen05 stream over E (csrc/rpe_tc.cu)
+            # wgmma stream over E (csrc/rpe_tc.cu)
             qk, vt, u = ops.gemm_tma_vt2(x2d, w["w_self"].bf16, w["b_self"], 2 * C, 3 * C, S)
             if PADDED_BIAS:
                 # score planes with 16-key padded rows: the attention kernel streams them with 16-byte cp.async copies
@@ -707,7 +707,7 @@ class SparseToDenseTransformer(nn.Module):
     def _dense_layer_bf16(self, dense, sparse, w):
         """_dense_layer for the bf16 token stream: dense (B,N+1,C) bf16, sparse (B,J+1,C) fp32.  Every GEMM is the persistent
         TMA kernel over all B*(N+1) rows (the bg row rides along and is overwritten at the end), the feature map and the
-        per-head (q' KV) / (q' . ksum) run in one tcgen05 kernel, LayerNorms read and write bf16."""
+        per-head (q' KV) / (q' . ksum) run in one wgmma kernel, LayerNorms read and write bf16."""
         B, N1, C = dense.shape
         N, J = N1 - 1, sparse.shape[1] - 1
         dev = dense.device
@@ -944,7 +944,7 @@ class Net(nn.Module):
         return self
 
     def set_precision(self, precision: str):
-        """'fp32' (CUDA-core kernels, exact path) or 'bf16' (tcgen05 tensor-core kernels, bf16 operands / fp32 accumulate)"""
+        """'fp32' (CUDA-core kernels, exact path) or 'bf16' (wgmma tensor-core kernels, bf16 operands / fp32 accumulate)"""
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {PRECISIONS}")
         self.precision = precision

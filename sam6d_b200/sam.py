@@ -1,16 +1,16 @@
-"""SAM ViT image encoder on B200 kernels -- drop-in for `segment_anything.modeling.image_encoder.ImageEncoderViT`
+"""SAM ViT image encoder on H100 kernels -- drop-in for `segment_anything.modeling.image_encoder.ImageEncoderViT`
 (ISM/segment_anything/modeling/image_encoder.py:17-116; built by ISM/segment_anything/build_sam.py:55-80 and reached through
 `SamPredictor.set_image -> model.image_encoder(x)`, ISM/segment_anything/predictor.py:89).
 
 Same constructor signature, same parameter names (so `sam_vit_h_4b8939.pth: image_encoder.*` loads unchanged), same
 forward contract: (B,3,1024,1024) normalised image -> (B,256,64,64).  The torch sub-modules are parameter containers; the
-forward runs sm_100a kernels through the C ABI.  precision="bf16" (default):
-    every Linear (qkv, proj, MLP)        -> sam6d_gemm_tma (persistent TMA-fed tcgen05 GEMM; GELU / bias / fp32 residual in the
+forward runs sm_90a kernels through the C ABI.  precision="bf16" (default):
+    every Linear (qkv, proj, MLP)        -> sam6d_gemm_tma (persistent TMA-fed wgmma GEMM; GELU / bias / fp32 residual in the
                                             epilogue; the qkv projection writes V^T itself, sam6d_gemm_tma_vt)
     LayerNorm                            -> sam6d_layernorm_bf16 (fp32 residual stream -> bf16 GEMM operand)
     window partition (pad 64 -> 70 AFTER norm1) / unpartition -> sam6d_gather_rows with a static index map (-1 = zero pad row)
     windowed attention (14 x 14 tokens)  -> sam6d_attn_tc with the decomposed rel-pos bias (tables from two extra MMAs)
-    global attention (64 x 64 tokens)    -> sam6d_attn_global_tc (online softmax, scores never leave TMEM)
+    global attention (64 x 64 tokens)    -> sam6d_attn_global_tc (online softmax, scores never leave registers)
     patch embed 16x16/16, neck 1x1 and 3x3 (9 shifted GEMMs) -> sam6d_gemm_bf16 / sam6d_gemm_tma, LayerNorm2d -> sam6d_layernorm
 precision="fp32" keeps everything on the CUDA-core kernels (sam6d_gemm_f32, sam6d_attn_relpos: flash-style, no HW x HW score
 tensor) and is the exact-parity comparator (max error 8e-6 against the reference module).
@@ -227,12 +227,12 @@ def _block_bf16(self, blk, bw, tok, B, L, C, G, maps):
     else:
         xw, nW, Hs = xn, B, G
     if Hs * Hs <= 256:
-        # windowed blocks: tensor-core attention (QK^T and PV on tcgen05, decomposed rel-pos bias in the softmax warps)
+        # windowed blocks: tensor-core attention (QK^T and PV on wgmma, decomposed rel-pos bias in the softmax warps)
         qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs)                   # [q|k] rows and V^T per window
         att = ops.attn_tc(qk, 0, qk, C, vt, nW, self.num_heads, Hs * Hs, Hs * Hs, C // self.num_heads, blk.attn.scale,
                           rel=(bw["rel_blob"], Hs, Hs), out_dtype=torch.bfloat16)
     elif Hs == 64 and C // self.num_heads == 80 and bw["rel_blob"] is not None:
-        # global blocks of the 64 x 64 grid (4096 keys): tcgen05 attention with an online softmax, scores never leave TMEM
+        # global blocks of the 64 x 64 grid (4096 keys): wgmma attention with an online softmax, scores never leave registers
         qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs, slot=2)
         att = ops.attn_global_tc(qk, vt, bw["rel_blob"], nW, self.num_heads, Hs, blk.attn.scale)
     else:

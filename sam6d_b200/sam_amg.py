@@ -1,4 +1,4 @@
-"""SAM prompt encoder, mask decoder and automatic mask generator on B200 kernels (SURVEY.md 8f row N4): drop-ins for
+"""SAM prompt encoder, mask decoder and automatic mask generator on H100 kernels (SURVEY.md 8f row N4): drop-ins for
     PromptEncoder (point prompts)        ISM/segment_anything/modeling/prompt_encoder.py:16-214
     MaskDecoder / TwoWayTransformer      ISM/segment_anything/modeling/{mask_decoder,transformer}.py
     Sam (preprocess / postprocess)       ISM/segment_anything/modeling/sam.py
@@ -7,7 +7,7 @@ with the reference's module and parameter names (`sam_vit_h_4b8939.pth` loads un
 `mask_decoder.*`).
 
 Work split.  Every Linear of the decoder -- token side and image side, and the two transposed convolutions written as GEMMs over
-pixel rows -- runs on the tcgen05 GEMMs (`sam6d_gemm_tma(_batched)` for the 262 144-row image side of a 64-prompt batch,
+pixel rows -- runs on the wgmma GEMMs (`sam6d_gemm_tma(_batched)` for the 262 144-row image side of a 64-prompt batch,
 `sam6d_gemm_f32` for the 448-row token side); csrc/sam_dec.cu holds the attention cores (7 tokens <-> 4096 pixels, head dims 16 /
 32), LayerNorm2d + GELU, the hypernetwork product with both pixel shuffles folded into its output index, and the mask
 post-processing.  Three algebraic savings over the reference's formulation, all exact:

@@ -1,11 +1,11 @@
-"""PEM RGB branch on B200 kernels (SURVEY.md 8f, row N1): drop-in for `ViT`, `ViT_AE` and `ViTEncoder` of
+"""PEM RGB branch on H100 kernels (SURVEY.md 8f, row N1): drop-in for `ViT`, `ViT_AE` and `ViTEncoder` of
 PEM/model/feature_extraction.py:17-181.
 
 The reference subclasses timm's VisionTransformer (ViT-B/16, 224 x 224, cls token, learned 197-position embedding, pre-norm
 blocks, LayerNorm eps 1e-6, GELU MLP x4), takes the normalised outputs of blocks 2/5/8/11, concatenates them (3072 channels),
 applies `output_upscaling` Linear(3072 -> 16*256), reshapes to a (B,256,56,56) map, F.interpolate's it to (B,256,224,224)
 and gathers the 2048 chosen pixels per image.  Here:
-    patch embedding, qkv / proj / fc1 / fc2 / output_upscaling  -> sam6d_gemm_tma (tcgen05; GELU, bias, residual in the epilogue;
+    patch embedding, qkv / proj / fc1 / fc2 / output_upscaling  -> sam6d_gemm_tma (wgmma; GELU, bias, residual in the epilogue;
                                                                    V^T of every attention layer written by the qkv epilogue)
     LayerNorm                                                   -> sam6d_layernorm_bf16 (fp32 residual stream -> bf16 operand)
     attention (197 tokens, 12 heads x 64)                       -> sam6d_attn_tc

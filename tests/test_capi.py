@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds (nvcc cross-compiles sm_100a without a GPU), loads, and exports every symbol that
+"""CPU: the C-ABI library builds (nvcc cross-compiles sm_90a without a GPU), loads, and exports every symbol that
 include/sam6d_b200.h declares; the host-side drop-in classes keep the reference's state_dict layout.  No compute calls."""
 import ctypes
 import os
@@ -29,9 +29,9 @@ def test_header_symbols_exported(libpath):
     assert set(protos) <= exported
 
 
-def test_library_is_sm100a(libpath):
+def test_library_is_sm90a(libpath):
     out = subprocess.run(["cuobjdump", "-lelf", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_version_and_loader():

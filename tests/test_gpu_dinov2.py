@@ -43,7 +43,7 @@ def test_crop_resize_pad_bit_exact(gold, desc):
 
 
 def test_vit_l14_descriptors_match_reference(gold, desc):
-    """cls tokens and masked, normalised patch tokens of the 24-block ViT-L/14 (257-token attention = 256 keys on tcgen05 + the
+    """cls tokens and masked, normalised patch tokens of the 24-block ViT-L/14 (257-token attention = 256 keys on wgmma + the
     class token merged by log-sum-exp); bf16 operands, so the bound is the measured drift plus margin, stated relative to the
     descriptor scale; the patch-validity pattern is exact"""
     image, masks, boxes = do.make_proposals(P=gold["meta"]["P"], seed=gold["meta"]["seed"])

@@ -209,8 +209,8 @@ def test_rpe_scores_and_mha(ops):
 
 @pytest.mark.parametrize("B,S", [(2, 197), (3, 65), (5, 129), (1, 200), (64, 197)])
 def test_rpe_scores_tensor_core(ops, B, S):
-    """TMA + tcgen05 stream over E (csrc/rpe_tc.cu) against the einsum on the same bf16 operands; B = 64, S = 197 is the
-    launch shape of the bench step (more query rows than SMs: every CTA walks a range, both TMEM buffers and ring stages wrap)"""
+    """TMA + wgmma stream over E (csrc/rpe_tc.cu) against the einsum on the same bf16 operands; B = 64, S = 197 is the
+    launch shape of the bench step (more query rows than SMs: every CTA walks a range and the ring stages wrap)"""
     E = (torch.randn(B, S, S, 256, generator=G(1)) * 0.7).bfloat16()
     U = torch.randn(B * S, 1024, generator=G(2)).bfloat16()
     got = ops.rpe_scores_tc(E.cuda(), U.cuda())
@@ -298,7 +298,7 @@ def test_linear_attention(ops):
 
 @pytest.mark.parametrize("B,N,J", [(2, 300, 50), (3, 2048, 196), (1, 129, 7)])
 def test_linear_attention_tensor_core(ops, B, N, J):
-    """bf16 dense tokens: feature map + per-head (q' KV)/(q' . ksum) in one tcgen05 kernel, against fp64 math on the same
+    """bf16 dense tokens: feature map + per-head (q' KV)/(q' . ksum) in one wgmma kernel, against fp64 math on the same
     bf16-rounded query projection.  The token rows sit behind a bg row (the (B,N+1,C) layout of the fine stage)."""
     C = 256
     sp = (torch.rand(C, generator=G(5)) + 0.5)
@@ -538,7 +538,7 @@ def test_template_score_matches_reference_golden(ops, golden_dir, case):
     torch.testing.assert_close(sim, c["sim"], atol=2e-6, rtol=1e-5)
 
 
-# ------------------------------------------------------------------------------------------------- tcgen05 GEMM
+# ------------------------------------------------------------------------------------------------- wgmma GEMM
 @pytest.mark.parametrize("M,N,K", [(197 * 3, 1792, 256), (1000, 512, 256), (4096, 256, 512), (130, 40, 64), (2049, 2049, 256)])
 @pytest.mark.parametrize("adt,wdt,odt", [(torch.float32, torch.bfloat16, torch.float32), (torch.float32, torch.float32, torch.float32),
                                          (torch.bfloat16, torch.bfloat16, torch.bfloat16)])
@@ -569,7 +569,7 @@ def test_gemm_tc_batched_strided(ops):
 
 @pytest.mark.parametrize("S,edt", [(64, torch.float32), (197, torch.bfloat16), (197, torch.float32), (33, torch.bfloat16)])
 def test_geo_embed_tc(ops, S, edt):
-    """tcgen05 geometric embedding: bf16 operands (sin/cos and weights), fp32 accumulation, E in fp32 or bf16"""
+    """wgmma geometric embedding: bf16 operands (sin/cos and weights), fp32 accumulation, E in fp32 or bf16"""
     sd = po.make_state_dict(seed=2)
     pts = _sparse_cloud(3, S, 9)
     ref = exact_geo_embedding(sd, pts)
@@ -634,7 +634,7 @@ def test_geo_embed_lut(ops, S, far_point, precise, monkeypatch):
 
 
 def test_positional_encoding_tensor_core(ops):
-    """layers 2/3 of the PE shared MLP on tcgen05 (bf16 operands) against the fp32 oracle"""
+    """layers 2/3 of the PE shared MLP on wgmma (bf16 operands) against the fp32 oracle"""
     from sam6d_b200.pem import PositionalEncoding
     sd = po.make_state_dict(seed=5)
     pe = PositionalEncoding(256).cuda().eval()
@@ -695,7 +695,7 @@ def _dense_attention(q, k, v, H, scale, bias=None):
 @pytest.mark.parametrize("B,Sq,Sk,H,D,with_bias", [(3, 197, 197, 4, 64, True), (2, 197, 150, 4, 64, False), (5, 196, 196, 2, 80, False),
                                                     (1, 33, 256, 1, 64, True)])
 def test_attn_tc_dense(ops, B, Sq, Sk, H, D, with_bias):
-    """tcgen05 attention against fp64 softmax attention on the bf16-rounded operands"""
+    """wgmma attention against fp64 softmax attention on the bf16-rounded operands"""
     g = G(Sq + Sk)
     q = torch.randn(B, Sq, H * D, generator=g)
     k = torch.randn(B, Sk, H * D, generator=g)
@@ -744,7 +744,7 @@ def test_attn_tc_sam_window(ops):
 
 
 def test_attn_global_tensor_core(ops):
-    """SAM global attention (64 x 64 tokens, online softmax on tcgen05) against the reference formula
+    """SAM global attention (64 x 64 tokens, online softmax on wgmma) against the reference formula
     (image_encoder.py:224-240, 325-361) evaluated in fp32 on the same bf16-rounded q, k, v."""
     from oracle import sam_oracle as so
     B, S, H, D = 2, 64, 2, 80
@@ -820,7 +820,7 @@ def test_gemm_tma_vt2_three_column_ranges(ops, nB, S):
 
 @pytest.mark.parametrize("B,S", [(2, 513), (3, 2049), (1, 130)])
 def test_fine_assign_tensor_core_fused(ops, B, S):
-    """compute_fine_Rt's assignment recomputed tile by tile on tcgen05 (no (B,S,S) matrix) against fp64 math on the same
+    """compute_fine_Rt's assignment recomputed tile by tile on wgmma (no (B,S,S) matrix) against fp64 math on the same
     bf16-rounded normalised tokens: labels exact (planted matches make them decisive), weights / correspondences to 1e-3"""
     g = G(31)
     C, temp = 256, 0.1

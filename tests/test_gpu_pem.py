@@ -227,7 +227,7 @@ def _bf16_checks(net, gold, tag, min_match_frac):
 
 
 def test_config2_b32_matches_oracle_bf16(golden_dir):
-    """BASELINE config #2 in the bench precision (tcgen05 kernels, bf16 operands, fp32 accumulation): see _bf16_checks"""
+    """BASELINE config #2 in the bench precision (wgmma kernels, bf16 operands, fp32 accumulation): see _bf16_checks"""
     from sam6d_b200.pem import Net
     gold = torch.load(os.path.join(golden_dir, "pem_b32.pt"), weights_only=False)
     m = gold["meta"]
@@ -278,7 +278,7 @@ def test_batch_32_properties():
 
 
 def test_bf16_tensor_core_mode_matches_reference_golden(golden_dir):
-    """precision='bf16' (tcgen05 kernels: bf16 operands, fp32 accumulation, bf16 geometric embedding): same poses within the
+    """precision='bf16' (wgmma kernels: bf16 operands, fp32 accumulation, bf16 geometric embedding): same poses within the
     north-star tolerance on every proposal."""
     from sam6d_b200.pem import Net
     gold = torch.load(os.path.join(golden_dir, "pem_full.pt"), weights_only=False)

@@ -1,4 +1,4 @@
-"""micro-benchmark: tcgen05 GEMM vs CUDA-core GEMM on the shapes of the matching path (GPU box)"""
+"""micro-benchmark: wgmma GEMM vs CUDA-core GEMM on the shapes of the matching path (GPU box)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from sam6d_b200 import ops
@@ -28,7 +28,7 @@ t1 = timeit(lambda: ops.gemm_tc_raw(f1.data_ptr(), 0, f2.data_ptr(), 0, None, 0,
 fl = 2.0 * B * S * S * C
 print(f"fine score 32x2049x2049x256: simt {t0:.3f} ms ({fl/t0/1e9:.1f} TF)  tc {t1:.3f} ms ({fl/t1/1e9:.1f} TF; output write {B*S*S*4/t1/1e6:.0f} GB/s)")
 
-print("--- persistent TMA GEMM (bf16 in, bf16 out) vs staged tcgen05 GEMM")
+print("--- persistent TMA GEMM (bf16 in, bf16 out) vs staged wgmma GEMM")
 for (M, N, K) in [(65536, 3840, 1280), (65536, 1280, 1280), (65536, 5120, 1280), (65536, 1280, 5120), (78400, 3840, 1280), (65536, 256, 256), (6304, 1792, 256), (65536, 512, 256)]:
     Ab = torch.randn(M, K, device="cuda").bfloat16(); Wb = torch.randn(N, K, device="cuda").bfloat16(); b = torch.randn(N, device="cuda")
     t1 = timeit(lambda: ops.gemm_tc(Ab, Wb, b, out_dtype=torch.bfloat16), n=5)
