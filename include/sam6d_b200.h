@@ -347,6 +347,23 @@ int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long lon
 int sam6d_template_score(const float* Qn, const float* Rn, int P, int O, int T, int C, float* sim_out, float* obj_score,
                          int* best_obj, float* best_score, int* best_tmpl, void* stream);
 
+/* ---- CAD template rendering (the stage SAM-6D/Render/render_{custom,bop}_templates.py runs in BlenderProc; csrc/render.cu) */
+
+/* O meshes x T views, one pinhole K (fx, fy, cx, cy) and H x W.  verts (n_verts,3) f32 and faces (n_faces,3) i32 of all meshes
+ * packed in order; faces index their own mesh's vertices.  mesh_info (O,8) i32 on the device = first vertex, vertex count,
+ * first face, face count, colour mode (0 base_color (O,3) f32 in [0,1]; 1 vcol (n_verts,3) u8; 2 uv (n_verts,2) f32 sampling
+ * the RGB u8 texture at tex + tex_off[o] bilinearly), texture height, texture width, 0.  poses (O,T,4,4) f32 object -> camera
+ * (OpenCV axes).  Caller-owned scratch: vrec (T*n_verts,4) i32, vis (O*T*H*W) u64, big (big_cap,2) i32, counters (O+1) i32
+ * (counters[1+o] = triangle-view pairs of mesh o dropped for a vertex at z <= znear or beyond the +-2^14 px guard band).
+ * Outputs per (object, view, pixel): rgb u8 x3, mask u8 (255 = object), xyz f16 x3 (object coordinates, 0 off the mask),
+ * tri i32 (face index within its mesh, -1 = empty), depth f32 (camera z, 0 = empty).  Shading: albedo x (ambient +
+ * (1 - ambient) max(0, n.l)), point light at -1.5 t in the camera frame.  Exact visibility rules: csrc/render.cu. */
+int sam6d_render_meshes(const float* verts, const int* faces, const int* mesh_info, int O, int n_verts, int n_faces,
+                        const unsigned char* vcol, const float* uv, const unsigned char* tex, const long long* tex_off,
+                        const float* base_color, const float* poses, int T, float fx, float fy, float cx, float cy, int H, int W,
+                        float znear, float ambient, int* vrec, unsigned long long* vis, int* big, int big_cap, int* counters,
+                        unsigned char* rgb, unsigned char* mask, void* xyz, int* tri, float* depth, void* stream);
+
 /* ---- library info ------------------------------------------------------------------------------------------------- */
 /* "sam6d_b200 <version> sm_90a" */
 const char* sam6d_version(void);

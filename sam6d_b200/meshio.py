@@ -1,16 +1,21 @@
 """CAD input of the CLIs: PLY reading and area-weighted surface sampling -- what the reference gets from
 `trimesh.load_mesh(cad_path).sample(n)` (PEM/run_inference_custom.py:182-183; trimesh is not a dependency here).
-Host-side numpy; ASCII and binary_little_endian PLY with `vertex` (x, y, z first) and `face` (vertex_indices list) elements."""
+Host-side numpy; ASCII and binary_little_endian PLY with `vertex` (x, y, z first) and `face` (vertex_indices list) elements.
+load_ply_mesh() also reads per-vertex texture coordinates and the `comment TextureFile` image of BOP's textured models."""
+import os
+from dataclasses import dataclass
+from typing import Optional
+
 import numpy as np
 
 _PLY_TYPES = {"char": "i1", "uchar": "u1", "short": "i2", "ushort": "u2", "int": "i4", "uint": "u4", "float": "f4", "double": "f8",
               "int8": "i1", "uint8": "u1", "int16": "i2", "uint16": "u2", "int32": "i4", "uint32": "u4", "float32": "f4", "float64": "f8"}
 
 
-def load_ply(path):
-    """-> (vertices (V,3) float32, faces (F,3) int64 or empty, vertex colours (V,3) uint8 or None)"""
+def _read_ply(path):
+    """-> (vertex columns {name: array}, faces (F,3) int64 or empty, header comments)"""
     with open(path, "rb") as fh:
-        fmt, elements = None, []
+        fmt, elements, comments = None, [], []
         while True:
             line = fh.readline()
             if not line:
@@ -20,13 +25,15 @@ def load_ply(path):
                 continue
             if tok[0] == "format":
                 fmt = tok[1]
+            elif tok[0] == "comment":
+                comments.append(tok[1:])
             elif tok[0] == "element":
                 elements.append(dict(name=tok[1], count=int(tok[2]), props=[]))
             elif tok[0] == "property":
                 elements[-1]["props"].append(tok[1:])
             elif tok[0] == "end_header":
                 break
-        verts, faces, colors = None, np.zeros((0, 3), np.int64), None
+        vcols, faces = None, np.zeros((0, 3), np.int64)
         for el in elements:
             names = [p[-1] for p in el["props"]]
             if el["name"] == "vertex":
@@ -37,9 +44,7 @@ def load_ply(path):
                     dt = np.dtype([(p[-1], ("<" if fmt == "binary_little_endian" else ">") + _PLY_TYPES[p[0]]) for p in el["props"]])
                     rec = np.frombuffer(fh.read(dt.itemsize * el["count"]), dtype=dt)
                     cols = {n: rec[n] for n in names}
-                verts = np.stack([cols["x"], cols["y"], cols["z"]], axis=1).astype(np.float32)
-                if all(c in cols for c in ("red", "green", "blue")):
-                    colors = np.stack([cols["red"], cols["green"], cols["blue"]], axis=1).astype(np.uint8)
+                vcols = cols
             elif el["name"] == "face":
                 if fmt == "ascii":
                     rows = [fh.readline().split() for _ in range(el["count"])]
@@ -64,9 +69,57 @@ def load_ply(path):
                         fh.readline()
                 else:
                     raise ValueError(f"binary PLY element {el['name']} is not supported")
-    if verts is None:
+    if vcols is None:
         raise ValueError("PLY without a vertex element")
-    return verts, faces, colors
+    return vcols, faces, comments
+
+
+def _colors(cols):
+    if all(c in cols for c in ("red", "green", "blue")):
+        return np.stack([cols["red"], cols["green"], cols["blue"]], axis=1).astype(np.uint8)
+    return None
+
+
+def load_ply(path):
+    """-> (vertices (V,3) float32, faces (F,3) int64 or empty, vertex colours (V,3) uint8 or None)"""
+    cols, faces, _ = _read_ply(path)
+    return np.stack([cols["x"], cols["y"], cols["z"]], axis=1).astype(np.float32), faces, _colors(cols)
+
+
+@dataclass
+class Mesh:
+    """A triangle mesh with its appearance: numpy arrays from load_ply_mesh, CUDA tensors after sam6d_b200.render.upload.
+    vertices (V,3) float32 in model units, faces (F,3) int, colors (V,3) uint8, uv (V,2) float32 (v = 0 is the bottom row
+    of the texture), texture (Ht,Wt,3) uint8 RGB; any of the last three may be None."""
+    vertices: object
+    faces: object
+    colors: Optional[object] = None
+    uv: Optional[object] = None
+    texture: Optional[object] = None
+    texture_file: Optional[str] = None
+
+
+def load_ply_mesh(path, read_texture: bool = True) -> Mesh:
+    """load_ply plus texture coordinates (vertex properties texture_u/texture_v or s/t) and the image named by
+    `comment TextureFile <png>` (relative to the PLY's folder), as in BOP's YCB-V models"""
+    cols, faces, comments = _read_ply(path)
+    verts = np.stack([cols["x"], cols["y"], cols["z"]], axis=1).astype(np.float32)
+    uv = None
+    for u, v in (("texture_u", "texture_v"), ("s", "t")):
+        if u in cols and v in cols:
+            uv = np.stack([cols[u], cols[v]], axis=1).astype(np.float32)
+            break
+    tex_file = next((" ".join(c[1:]) for c in comments if len(c) > 1 and c[0] == "TextureFile"), None)
+    if tex_file is not None:
+        tex_file = os.path.join(os.path.dirname(os.path.abspath(path)), tex_file)
+    texture = None
+    if read_texture and uv is not None and tex_file is not None:
+        import cv2
+        img = cv2.imread(tex_file, cv2.IMREAD_COLOR)
+        if img is None:
+            raise FileNotFoundError(f"texture {tex_file} named by {path} cannot be read")
+        texture = np.ascontiguousarray(img[:, :, ::-1])
+    return Mesh(verts, faces, _colors(cols), uv, texture, tex_file)
 
 
 def sample_surface(verts, faces, n, rng=None):
