@@ -364,6 +364,33 @@ int sam6d_render_meshes(const float* verts, const int* faces, const int* mesh_in
                         float znear, float ambient, int* vrec, unsigned long long* vis, int* big, int big_cap, int* counters,
                         unsigned char* rgb, unsigned char* mask, void* xyz, int* tri, float* depth, void* stream);
 
+/* ---- FastSAM segmentor: YOLOv8x-seg (ultralytics SegmentationModel behind ISM/model/fast_sam.py; csrc/conv_tc.cu, csrc/yolo.cu) */
+
+/* Implicit-GEMM convolution on wgmma, NHWC bf16: x (B,Hi,Wi,ldx) channels [0,Cin) (a channel slice: offset the pointer),
+ * w (Cout,k,k,Cin) bf16, k in {1,3} with padding k/2, stride 1 or 2, bias (Cout) f32 (folded BatchNorm), silu 0/1, r bf16
+ * residual or NULL -> y bf16 (y_is_f32 0) or f32 (1, no residual) at
+ * y[n*y_bs + ((sy*oy_pix + oy)*Wy + sx*ox_pix + ox)*ldy + c] (r addressed the same way with ldr, r_bs).  Cin % 8 == 0,
+ * ldx % 8 == 0, 16-byte aligned x and w. */
+int sam6d_conv2d_tc(const void* x, long long ldx, int B, int Hi, int Wi, int Cin, const void* w, int k, int stride, int Cout,
+                    const float* bias, int silu, const void* r, long long ldr, long long r_bs, void* y, int y_is_f32, long long ldy,
+                    long long y_bs, int Wy, int sy, int sx, int oy, int ox, void* stream);
+/* stem: img (B,H,W,3) u8 letterboxed, channel-flipped and /255 on the fly; w (80,3,3,3) f32 (out,ky,kx,in), bias (80) f32 ->
+ * out (B,ceil(H/2),ceil(W/2),80) bf16 = SiLU(3x3 stride-2 conv) */
+int sam6d_yolo_stem(const unsigned char* img, int B, int H, int W, const float* w, const float* bias, void* out, void* stream);
+/* SPPF pools: buf (B,H,W,ld) bf16, channels [0,C) -> [C,2C), [2C,3C), [3C,4C) = 5x5, 9x9, 13x13 max (-inf padding) */
+int sam6d_yolo_sppf(void* buf, long long ld, int B, int H, int W, int C, void* stream);
+/* nearest x2: x (B,H,W,ldx) channels [0,C) -> y (B,2H,2W,ldy) channels [0,C); C, ldx, ldy % 8 == 0 */
+int sam6d_yolo_upsample2x(const void* x, long long ldx, int B, int H, int W, int C, void* y, long long ldy, void* stream);
+/* Segment head decode: head (B,A,ld) f32 rows [64 DFL logits | class logit | 32 coefficients], frame stride bs, anchors of the
+ * h0 x w0 (stride 8), h1 x w1 (16), h2 x w2 (32) grids -> cand (B,A,38) f32 rows (x1,y1,x2,y2,conf,cls,32 coefficients) with
+ * conf > conf_thr in anchor order, count (B) i32 */
+int sam6d_yolo_decode(const float* head, long long ld, long long bs, int B, int h0, int w0, int h1, int w1, int h2, int w2, float conf_thr,
+                      float* cand, int* count, void* stream);
+/* process_mask(upsample=True) of one frame: proto (mh,mw,32) f32, rows (N,row_ld) candidate rows, kx = mw/iw, ky = mh/ih, low
+ * (N,mh,mw) f32 scratch -> out (N,ih,iw) u8 = bilinear(crop(sigmoid(coeffs . proto))) > 0.5 */
+int sam6d_yolo_masks(const float* proto, int mh, int mw, const float* rows, long long row_ld, int N, int ih, int iw, float kx, float ky,
+                     float* low, unsigned char* out, void* stream);
+
 /* ---- library info ------------------------------------------------------------------------------------------------- */
 /* "sam6d_b200 <version> sm_90a" */
 const char* sam6d_version(void);

@@ -12,7 +12,10 @@ automatic mask generation (ViT-H encoder, prompt encoder, mask decoder, filters,
 All model compute runs through the C ABI (sam6d_b200/{sam,sam_amg,dinov2,ism}.py).  The geometric score needs the camera pose of
 every template view: `templates/template_poses.npy` (42 x 4 x 4, written by render_point_templates; for BlenderProc renders pass the
 reference's predefined level-0 poses with --template_poses); without it the final score is (semantic + appearance) / 2.
-FastSAM (`--segmentor_model fastsam`) is out of scope."""
+
+`--segmentor_model fastsam` (ISM_fastsam.yaml) replaces SAM by FastSAM (sam6d_b200/fast_sam.py: YOLOv8x-seg, conf 0.25, iou 0.9,
+max_det 200) built from `{checkpoint_dir}/FastSAM/FastSAM-x.pt` or the reference's `./checkpoints/FastSAM/FastSAM-x.pt`; it needs
+only the DINOv2 checkpoint besides.  The rest of the pipeline and the output files are the same."""
 import argparse
 import glob
 import json
@@ -39,7 +42,8 @@ def get_parser():
     ap.add_argument("--cam_path", nargs="?", help="Path to camera information")
     ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
     # not in the reference: where weights / template poses come from
-    ap.add_argument("--checkpoint_dir", default=None, help="directory with sam_vit_h_4b8939.pth and dinov2_vitl14_pretrain.pth")
+    ap.add_argument("--checkpoint_dir", default=None,
+                    help="directory with segment-anything/sam_vit_h_4b8939.pth (or FastSAM/FastSAM-x.pt) and dinov2/dinov2_vitl14_pretrain.pth")
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
     ap.add_argument("--template_poses", default=None, help="(T,4,4) .npy of the template camera poses (default: templates/template_poses.npy)")
     ap.add_argument("--points_per_side", default=32, type=int)
@@ -75,9 +79,35 @@ def mask_to_rle(binary_mask: np.ndarray):
     return {"counts": counts, "size": list(binary_mask.shape)}
 
 
+def build_fastsam(args, device):
+    """FastSAM (ISM/configs/model/segmentor_model/fast_sam.yaml) + DINOv2"""
+    from ..dinov2 import CustomDINOv2
+    from ..fast_sam import FastSAM
+    desc = CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+    ck = args.checkpoint_dir
+    cands = ([os.path.join(ck, "FastSAM", "FastSAM-x.pt")] if ck else []) + [os.path.join(".", "checkpoints", "FastSAM", "FastSAM-x.pt")]
+    fs_ck = next((c for c in cands if os.path.exists(c)), None)
+    dino_ck = os.path.join(ck, "dinov2", "dinov2_vitl14_pretrain.pth") if ck else None
+    cfg = dict(iou_threshold=0.9, conf_threshold=0.05, max_det=200)
+    if fs_ck and dino_ck and os.path.exists(dino_ck):
+        seg = FastSAM(fs_ck, cfg, segmentor_width_size=640, device=device)
+        desc.model.load_state_dict(torch.load(dino_ck, map_location="cpu"), strict=True)
+    elif args.random_weights:
+        from .. import synth
+        print("=> WARNING: no checkpoints, seeded random weights (detections are meaningless; plumbing run)", file=sys.stderr)
+        seg = FastSAM(None, cfg, segmentor_width_size=640, device=device)
+        seg.model.load_state_dict(synth.make_fastsam_state_dict(seed=1), strict=True)
+        desc.model.load_state_dict(synth.make_dinov2_state_dict(seed=1), strict=True)
+    else:
+        raise FileNotFoundError("FastSAM / DINOv2 checkpoints not found (pass --checkpoint_dir, or --random_weights for a plumbing run)")
+    return seg, desc
+
+
 def build_models(args, device):
     from ..dinov2 import CustomDINOv2
     from ..sam_amg import CustomSamAutomaticMaskGenerator, build_sam_vit_h
+    if args.segmentor_model == "fastsam":
+        return build_fastsam(args, device)
     sam = build_sam_vit_h("bf16").to(device).eval()
     desc = CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
     ck = args.checkpoint_dir
@@ -102,8 +132,8 @@ def build_models(args, device):
 
 def main(argv=None):
     args = get_parser().parse_args(argv)
-    if args.segmentor_model != "sam":
-        raise ValueError(f"The segmentor_model {args.segmentor_model} is not supported (FastSAM is out of scope)")
+    if args.segmentor_model not in ("sam", "fastsam"):
+        raise ValueError(f"The segmentor_model {args.segmentor_model} is not supported")
     from PIL import Image
     from .. import ism, meshio
     from ..dinov2 import MaskedPatch_MatrixSimilarity

@@ -150,6 +150,18 @@ __device__ __forceinline__ void tma_load_2d(const void* tmap, uint64_t* bar, voi
                "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(crd0), "r"(crd1)
                : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(const void* tmap, uint64_t* bar, void* smem_dst, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+                   smem_u32(smem_dst)),
+               "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(const void* tmap, uint64_t* bar, void* smem_dst, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
+                   smem_u32(smem_dst)),
+               "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
 // 1-D bulk copy global -> shared (size multiple of 16 bytes), completion counted on an mbarrier
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),

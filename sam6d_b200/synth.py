@@ -372,3 +372,58 @@ def make_image_embedding(seed=1, size=64) -> torch.Tensor:
         blob = torch.exp(-((yy - cy) ** 2 + (xx - cx) ** 2) / (2 * (0.05 + 0.15 * r) ** 2))
         emb += d[:, None, None] * blob[None]
     return emb.unsqueeze(0)
+
+
+def make_fastsam_state_dict(seed: int = 1) -> SD:
+    """Seeded YOLOv8x-seg (nc=1) weights under ultralytics' keys (the layout of FastSAM-x.pt).  Convolutions are drawn at
+    1/sqrt(fan_in) and BatchNorm statistics are randomised, so activations stay O(1) through the 23 layers and folding is
+    exercised.  The heads' last layers are scaled so decoded boxes vary, masks are crisp (few pixels near the 0.5 threshold) and,
+    on the test frames, several hundred anchors pass conf 0.25 and more than max_det = 200 survive NMS, so the max_det cut is
+    exercised."""
+    from .fast_sam import YOLOv8Seg
+    g = torch.Generator().manual_seed(seed)
+    sd: SD = {}
+    for k, v in YOLOv8Seg().state_dict().items():
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.zeros((), dtype=torch.long)
+        elif k.endswith("dfl.conv.weight"):
+            sd[k] = torch.arange(16, dtype=torch.float32).view(1, 16, 1, 1)
+        elif k.endswith("bn.weight"):
+            sd[k] = 0.8 + 0.4 * torch.rand(v.shape, generator=g)
+        elif k.endswith("bn.bias") or k.endswith("bn.running_mean"):
+            sd[k] = 0.1 * torch.randn(v.shape, generator=g)
+        elif k.endswith("bn.running_var"):
+            sd[k] = 0.5 + torch.rand(v.shape, generator=g)
+        elif k.endswith("weight"):
+            fan_in = v.shape[0] * v.shape[2] * v.shape[3] if "upsample" in k else v[0].numel()
+            sd[k] = torch.randn(v.shape, generator=g) * (1.25 if k.endswith("conv.weight") else 1.0) / math.sqrt(fan_in)
+        else:
+            sd[k] = 0.05 * torch.randn(v.shape, generator=g)
+    # the heads' last 1x1 convolutions: zero-sum rows (the SiLU features have a positive mean, which would otherwise give every
+    # anchor the same offset), scaled so DFL logits have std ~2.4 and class logits ~N(-2.5, 1.5) (~18 % of anchors pass 0.25);
+    # the mask coefficients are scaled and biased so that coeffs . proto is ~0 on average over anchors with std ~1.6 within a mask
+    for i in range(3):
+        for name, scale in (("cv2", 20.0), ("cv3", 35.0), ("cv4", 300.0)):
+            w = sd[f"model.22.{name}.{i}.2.weight"]
+            sd[f"model.22.{name}.{i}.2.weight"] = (w - w.mean(dim=1, keepdim=True)) * scale
+        sd[f"model.22.cv3.{i}.2.bias"].zero_()
+        sd[f"model.22.cv4.{i}.2.bias"].fill_(0.065)
+    return sd
+
+
+def make_fastsam_frame(H: int = 480, W: int = 640, seed: int = 0):
+    """(H,W,3) uint8 RGB test frame: smooth background and a few filled rectangles and discs"""
+    import numpy as np
+    rs = np.random.RandomState(seed)
+    yy, xx = np.mgrid[0:H, 0:W].astype(np.float32)
+    img = np.stack([80 + 60 * np.sin(xx / (37 + 11 * c) + c) * np.cos(yy / (53 - 7 * c)) for c in range(3)], -1)
+    for _ in range(12):
+        col = rs.randint(0, 256, 3)
+        y0, x0 = rs.randint(0, H - 20), rs.randint(0, W - 20)
+        if rs.rand() < 0.5:
+            img[y0:y0 + rs.randint(20, H // 3), x0:x0 + rs.randint(20, W // 3)] = col
+        else:
+            r = rs.randint(10, min(H, W) // 5)
+            img[(yy - y0) ** 2 + (xx - x0) ** 2 < r * r] = col
+    img += rs.randn(H, W, 3) * 8
+    return np.clip(img, 0, 255).astype(np.uint8)
