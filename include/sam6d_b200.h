@@ -331,8 +331,8 @@ int sam6d_bilinear_gather(const void* up, int up_is_bf16, const long long* choos
                           float* out, void* stream);
 
 /* ---- SAM ViT image encoder attention (ISM/segment_anything/modeling/image_encoder.py:224-240,325-361) ---------------- */
-/* softmax((q*scale) k^T + q.Rh + q.Rw) v per window and head (head_dim 80), flash-style.  qkv: (nW*Hs*Ws, 3*nH*80) rows
- * [q|k|v], rel_h (2Hs-1,80), rel_w (2Ws-1,80), out (nW*Hs*Ws, nH*80).  Hs, Ws <= 64. */
+/* softmax((q*scale) k^T + q.Rh + q.Rw) v per window and head (head_dim D = 80 or 64), flash-style.  qkv: (nW*Hs*Ws, 3*nH*D)
+ * rows [q|k|v], rel_h (2Hs-1,D), rel_w (2Ws-1,D), out (nW*Hs*Ws, nH*D).  Hs, Ws <= 64. */
 int sam6d_attn_relpos(const float* qkv, long long tok_ld, int nW, int Hs, int Ws, int nH, int head_dim, const float* rel_h,
                       const float* rel_w, float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
 
@@ -342,6 +342,10 @@ int sam6d_attn_relpos(const float* qkv, long long tok_ld, int nW, int Hs, int Ws
  * out (B*4096, H*80) fp32 / bf16.  image_encoder.py:224-240 (attention), 325-361 (add_decomposed_rel_pos). */
 int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H, int grid,
                          float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
+/* The same at head_dim 64 (SAM ViT-L: 1024 / 16, ViT-B: 768 / 12) or 80 (ViT-H): every "80" above reads head_dim; one rel-pos
+ * slab per table at 64.  sam6d_attn_global_tc is this call with head_dim = 80.  Any other head_dim returns -22. */
+int sam6d_attn_global_tc_ex(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H, int grid,
+                            int head_dim, float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
 
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 int sam6d_template_score(const float* Qn, const float* Rn, int P, int O, int T, int C, float* sim_out, float* obj_score,

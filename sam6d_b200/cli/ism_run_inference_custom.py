@@ -7,11 +7,15 @@ segmentation{counts,size}}`, ISM/model/utils.py:153-216).
         --rgb_path rgb.png --depth_path depth.png --cam_path camera.json [--stability_score_thresh 0.97]
 
 Pipeline (ISM/run_inference_custom.py:97-209): template descriptors (DINOv2 cls + masked patch tokens of the 42 views) -> SAM
-automatic mask generation (ViT-H encoder, prompt encoder, mask decoder, filters, NMS) -> proposal descriptors -> semantic score
+automatic mask generation (ViT-H / -L / -B encoder, prompt encoder, mask decoder, filters, NMS) -> proposal descriptors -> semantic score
 (avg-5 template cosine) -> appearance score -> geometric score (template pose projection IoU x visible ratio) -> final score.
 All model compute runs through the C ABI (sam6d_b200/{sam,sam_amg,dinov2,ism}.py).  The geometric score needs the camera pose of
 every template view: `templates/template_poses.npy` (42 x 4 x 4, written by render_point_templates; for BlenderProc renders pass the
 reference's predefined level-0 poses with --template_poses); without it the final score is (semantic + appearance) / 2.
+
+`--sam_model_type {vit_h,vit_l,vit_b}` picks the SAM backbone (the reference's hydra `model.segmentor_model.sam.model_type`,
+default vit_h) and its checkpoint `{checkpoint_dir}/segment-anything/sam_vit_{h_4b8939,l_0b3195,b_01ec64}.pth` through
+sam_amg.load_sam.
 
 `--segmentor_model fastsam` (ISM_fastsam.yaml) replaces SAM by FastSAM (sam6d_b200/fast_sam.py: YOLOv8x-seg, conf 0.25, iou 0.9,
 max_det 200) built from `{checkpoint_dir}/FastSAM/FastSAM-x.pt` or the reference's `./checkpoints/FastSAM/FastSAM-x.pt`; it needs
@@ -43,7 +47,10 @@ def get_parser():
     ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
     # not in the reference: where weights / template poses come from
     ap.add_argument("--checkpoint_dir", default=None,
-                    help="directory with segment-anything/sam_vit_h_4b8939.pth (or FastSAM/FastSAM-x.pt) and dinov2/dinov2_vitl14_pretrain.pth")
+                    help="directory with segment-anything/sam_vit_h_4b8939.pth (or the --sam_model_type's file, or FastSAM/FastSAM-x.pt) "
+                         "and dinov2/dinov2_vitl14_pretrain.pth")
+    ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"),
+                    help="not in the reference: the hydra `model.segmentor_model.sam.model_type` (SAM backbone)")
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
     ap.add_argument("--template_poses", default=None, help="(T,4,4) .npy of the template camera poses (default: templates/template_poses.npy)")
     ap.add_argument("--points_per_side", default=32, type=int)
@@ -105,21 +112,29 @@ def build_fastsam(args, device):
 
 def build_models(args, device):
     from ..dinov2 import CustomDINOv2
-    from ..sam_amg import CustomSamAutomaticMaskGenerator, build_sam_vit_h
+    from ..sam import VIT_CONFIGS
+    from ..sam_amg import CustomSamAutomaticMaskGenerator, load_sam, pretrained_weight_dict, sam_model_registry
     if args.segmentor_model == "fastsam":
         return build_fastsam(args, device)
-    sam = build_sam_vit_h("bf16").to(device).eval()
-    desc = CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+    mt = args.sam_model_type
+
+    def new_desc():            # built after SAM: module construction keeps drawing torch's global RNG in the same order
+        return CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+
     ck = args.checkpoint_dir
-    sam_ck = os.path.join(ck, "segment-anything", "sam_vit_h_4b8939.pth") if ck else None
+    sam_dir = os.path.join(ck, "segment-anything") if ck else None
+    sam_ck = os.path.join(sam_dir, pretrained_weight_dict[mt]) if ck else None
     dino_ck = os.path.join(ck, "dinov2", "dinov2_vitl14_pretrain.pth") if ck else None
     if sam_ck and os.path.exists(sam_ck) and os.path.exists(dino_ck):
-        sam.load_state_dict(torch.load(sam_ck, map_location="cpu"), strict=True)
+        sam = load_sam(mt, sam_dir, "bf16").to(device).eval()
+        desc = new_desc()
         desc.model.load_state_dict(torch.load(dino_ck, map_location="cpu"), strict=True)
     elif args.random_weights:
         from .. import synth
         print("=> WARNING: no checkpoints, seeded random weights (detections are meaningless; plumbing run)", file=sys.stderr)
-        sd = {"image_encoder." + k: v for k, v in synth.make_sam_state_dict(embed_dim=1280, depth=32, num_heads=16, global_attn_indexes=(7, 15, 23, 31), seed=1).items()}
+        sam = sam_model_registry[mt]("bf16").to(device).eval()
+        desc = new_desc()
+        sd = {"image_encoder." + k: v for k, v in synth.make_sam_state_dict(**VIT_CONFIGS[mt], seed=1).items()}
         sd.update(synth.make_sam_decoder_state_dict(seed=1))
         sam.load_state_dict(sd, strict=True)
         desc.model.load_state_dict(synth.make_dinov2_state_dict(seed=1), strict=True)

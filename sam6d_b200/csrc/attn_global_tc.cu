@@ -1,5 +1,5 @@
-// attn_global_tc.cu -- SAM ViT global attention (64 x 64 = 4096 tokens per image, head dim 80, decomposed relative-position
-// bias) on wgmma with an online softmax (ISM/segment_anything/modeling/image_encoder.py:224-240, 325-361).
+// attn_global_tc.cu -- SAM ViT global attention (64 x 64 = 4096 tokens per image, head dim D = 80 for ViT-H, 64 for ViT-L / ViT-B,
+// decomposed relative-position bias) on wgmma with an online softmax (ISM/segment_anything/modeling/image_encoder.py:224-240, 325-361).
 //
 //     O = softmax(scale * Q K^T + Rh[q, kh] + Rw[q, kw]) V,     Rh[q, kh] = q . rel_h[qh - kh + 63], Rw likewise (unscaled q)
 //
@@ -10,7 +10,9 @@
 //                G_w = Q rel_w^T, G_h = Q rel_h^T (once) -> the row's 32 Rw values of its key columns in registers, Rh in
 //                shared memory; per key tile: S_j = Q K_j^T (wgmma m64n128k16, 64 registers), row max / exp2 in registers
 //                (rows live in quads), o = o * alpha in registers, P_j as bf16 into the swizzled A slabs, o += P_j V_j
-//                (wgmma m64n80k16, 40 registers)
+//                (wgmma m64nDk16, D/2 registers)
+// Q, K and each rel table are DS = ceil(D/64) slabs of 64 channels (two at D = 80, the second one 16 channels deep; one at D = 64);
+// a V^T tile is two [D rows][64 keys] slabs.  Both head dims share the code; only the slab counts and the k-step counts differ.
 // The reference materialises a (16 x 4096 x 4096) fp32 score tensor per image and block; here scores never leave registers.
 #include <cuda.h>
 
@@ -19,16 +21,25 @@
 
 namespace {
 
-constexpr int QT = 128, KT = 128, D = 80, GRID = 64;
+constexpr int QT = 128, KT = 128, GRID = 64;
 constexpr int CONSUMERS = 256, NUM_THREADS = CONSUMERS + 128;
-constexpr int Q_SLAB = QT * 128, K_SLAB = KT * 128, V_SLAB = D * 128, P_SLAB = QT * 128, REL_SLAB = 128 * 128;
-constexpr int OFF_Q = 0, OFF_K0 = OFF_Q + 2 * Q_SLAB, OFF_K1 = OFF_K0 + 2 * K_SLAB, OFF_V0 = OFF_K1 + 2 * K_SLAB,
-              OFF_V1 = OFF_V0 + 2 * V_SLAB, OFF_P = OFF_V1 + 2 * V_SLAB, OFF_TABH = OFF_P + 2 * P_SLAB;
+constexpr int Q_SLAB = QT * 128, K_SLAB = KT * 128, P_SLAB = QT * 128, REL_SLAB = 128 * 128;
 constexpr int TABH_LD = 64, SCR_LD = 128;
-constexpr int SMEM_BYTES = OFF_TABH + QT * TABH_LD * 4 + 1024;
-static_assert(OFF_K1 % 1024 == 0 && OFF_V0 % 1024 == 0 && OFF_V1 % 1024 == 0 && OFF_P % 1024 == 0, "slabs must be 1024-byte aligned");
-static_assert(OFF_K1 + 2 * K_SLAB - OFF_K0 >= 4 * REL_SLAB, "the rel tables occupy the K ring");
-static_assert(OFF_TABH - OFF_V0 >= QT * SCR_LD * 4, "the bias scratch occupies the V ring and the P slabs");
+
+// shared-memory plan of the head-dim-D kernel: [Q: DS slabs][K ring: 2 x DS slabs][V ring: 2 x 2 slabs][P: 2 slabs][tab_h]
+template <int D>
+struct Cfg {
+  static constexpr int DS = (D + 63) / 64, V_SLAB = D * 128;
+  static constexpr int OFF_Q = 0, OFF_K0 = OFF_Q + DS * Q_SLAB, OFF_K1 = OFF_K0 + DS * K_SLAB, OFF_V0 = OFF_K1 + DS * K_SLAB,
+                       OFF_V1 = OFF_V0 + 2 * V_SLAB, OFF_P = OFF_V1 + 2 * V_SLAB, OFF_TABH = OFF_P + 2 * P_SLAB;
+  static constexpr int SMEM_BYTES = OFF_TABH + QT * TABH_LD * 4 + 1024;
+  static_assert(D % 16 == 0 && D <= 128, "head dim: whole k-steps, at most two 64-channel slabs");
+  static_assert(OFF_K0 % 1024 == 0 && OFF_K1 % 1024 == 0 && OFF_V0 % 1024 == 0 && OFF_V1 % 1024 == 0 && OFF_P % 1024 == 0,
+                "slabs must be 1024-byte aligned");
+  static_assert(OFF_K1 + DS * K_SLAB - OFF_K0 >= 2 * DS * REL_SLAB, "the rel tables occupy the K ring");
+  static_assert(OFF_TABH - OFF_V0 >= QT * SCR_LD * 4, "the bias scratch occupies the V ring and the P slabs");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
+};
 constexpr float LOG2E = 1.4426950408889634f;
 
 __device__ __forceinline__ float ex2(float x) {
@@ -38,15 +49,18 @@ __device__ __forceinline__ float ex2(float x) {
 }
 
 struct GArgs {
-  const void* rel_blob;   // rel_h, rel_w as bf16 wgmma B slabs: 2 tables x 2 slabs x [128 rows][64 ch], SWIZZLE_128B
+  const void* rel_blob;   // rel_h, rel_w as bf16 wgmma B slabs: 2 tables x DS slabs x [128 rows][64 ch], SWIZZLE_128B
   void* out; long long out_ld;
   int H;
   float scale;
 };
 
-template <typename OT>
+template <int D, typename OT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt,
                                                        GArgs a) {
+  using CF = Cfg<D>;
+  constexpr int DS = CF::DS, V_SLAB = CF::V_SLAB, OFF_Q = CF::OFF_Q, OFF_K0 = CF::OFF_K0, OFF_K1 = CF::OFF_K1, OFF_V0 = CF::OFF_V0,
+                OFF_V1 = CF::OFF_V1, OFF_P = CF::OFF_P, OFF_TABH = CF::OFF_TABH;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* q_s = smem + OFF_Q;
@@ -75,17 +89,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __
     // -------------------------------------------------------------------------------------------------- TMA producer
     tc::producer_regs();
     if (tid == CONSUMERS) {
-      tc::mbar_arrive_expect_tx(&q_bar, 2 * Q_SLAB + 4 * REL_SLAB);
-      tc::bulk_load_1d(rel_s, a.rel_blob, 4 * REL_SLAB, &q_bar);
-      for (int s = 0; s < 2; ++s) tc::tma_load_2d(&tmQK, &q_bar, q_s + s * Q_SLAB, h * D + s * 64, b * L + tq * QT);
+      tc::mbar_arrive_expect_tx(&q_bar, DS * Q_SLAB + 2 * DS * REL_SLAB);
+      tc::bulk_load_1d(rel_s, a.rel_blob, 2 * DS * REL_SLAB, &q_bar);
+      for (int s = 0; s < DS; ++s) tc::tma_load_2d(&tmQK, &q_bar, q_s + s * Q_SLAB, h * D + s * 64, b * L + tq * QT);
       tc::mbar_wait(&tab_done, 0);                                  // the rings hold the rel tables / bias scratch until then
       for (int j = 0; j < NT; ++j) {
         const int st = j & 1, use = j >> 1;
         uint8_t* k_s = smem + (st ? OFF_K1 : OFF_K0);
         uint8_t* v_s = smem + (st ? OFF_V1 : OFF_V0);
         tc::mbar_wait(&k_empty[st], (uint32_t)((use & 1) ^ 1));
-        tc::mbar_arrive_expect_tx(&k_full[st], 2 * K_SLAB);
-        for (int s = 0; s < 2; ++s) tc::tma_load_2d(&tmQK, &k_full[st], k_s + s * K_SLAB, C + h * D + s * 64, b * L + j * KT);
+        tc::mbar_arrive_expect_tx(&k_full[st], DS * K_SLAB);
+        for (int s = 0; s < DS; ++s) tc::tma_load_2d(&tmQK, &k_full[st], k_s + s * K_SLAB, C + h * D + s * 64, b * L + j * KT);
         tc::mbar_wait(&v_empty[st], (uint32_t)((use & 1) ^ 1));
         tc::mbar_arrive_expect_tx(&v_full[st], 2 * V_SLAB);
         for (int s = 0; s < 2; ++s) tc::tma_load_2d(&tmVt, &v_full[st], v_s + s * V_SLAB, j * KT + s * 64, (b * a.H + h) * D);
@@ -108,7 +122,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __
 #pragma unroll
     for (int k = 0; k < D / 16; ++k)
       tc::wgmma_bf16<KT>(g, tc::wg_desc(q_addr + (k >> 2) * Q_SLAB + (k & 3) * 32),
-                         tc::wg_desc(tc::smem_u32(rel_s) + ((1 - t) * 2 + (k >> 2)) * REL_SLAB + (k & 3) * 32), k ? 1u : 0u);
+                         tc::wg_desc(tc::smem_u32(rel_s) + ((1 - t) * DS + (k >> 2)) * REL_SLAB + (k & 3) * 32), k ? 1u : 0u);
     tc::wg_commit();
     tc::wg_wait<0>();
 #pragma unroll
@@ -243,13 +257,30 @@ int g_make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols
 
 }  // namespace
 
-// qkv: bf16 (B*4096 rows, ld >= 2*H*80) rows [q | k (| v)], head h at columns h*80 of q and H*80 + h*80 of k; Vt: bf16 (B*H*80 rows, vt_ld >= 4096)
-// = V^T per (image, head) (sam6d_transpose_tokens_bf16); rel_blob: rel_pos_h / rel_pos_w ((127, 80) each) packed as bf16 wgmma
-// slabs with 128-row slabs (ops.pack_rel_pos(..., slab_rows=128)); out (B*4096, H*80) fp32 or bf16.  64 x 64 token grid only.
-S6_API int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H,
-                                int grid, float scale, void* out, int out_is_bf16, long long out_ld, void* stream) {
+namespace {
+
+template <int D, typename OT>
+int launch_global(const CUtensorMap& tqk, const CUtensorMap& tv, const GArgs& a, int B, cudaStream_t st) {
+  constexpr int SMEM = Cfg<D>::SMEM_BYTES;
+  auto k = attn_global_tc_kernel<D, OT>;
+  S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  k<<<dim3(GRID * GRID / QT, a.H, B), NUM_THREADS, SMEM, st>>>(tqk, tv, a);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
+// qkv: bf16 (B*4096 rows, ld >= 2*H*D) rows [q | k (| v)], head h at columns h*D of q and H*D + h*D of k; Vt: bf16 (B*H*D rows,
+// vt_ld >= 4096) = V^T per (image, head) (sam6d_transpose_tokens_bf16); rel_blob: rel_pos_h / rel_pos_w ((127, D) each) packed as
+// bf16 wgmma slabs with 128-row slabs (ops.pack_rel_pos(..., slab_rows=128)); out (B*4096, H*D) fp32 or bf16.  64 x 64 token grid
+// only; head_dim D = 80 (ViT-H) or 64 (ViT-L, ViT-B).
+S6_API int sam6d_attn_global_tc_ex(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H,
+                                   int grid, int head_dim, float scale, void* out, int out_is_bf16, long long out_ld, void* stream) {
+  S6_REQUIRE(head_dim == 64 || head_dim == 80);
   S6_REQUIRE(qkv && Vt && rel_blob && out && B >= 0 && H > 0 && grid == GRID);
-  S6_REQUIRE((ld % 8) == 0 && ld >= 2LL * H * D && (vt_ld % 8) == 0 && vt_ld >= GRID * GRID && (out_ld % (out_is_bf16 ? 8 : 4)) == 0);
+  S6_REQUIRE((ld % 8) == 0 && ld >= 2LL * H * head_dim && (vt_ld % 8) == 0 && vt_ld >= GRID * GRID &&
+             (out_ld % (out_is_bf16 ? 8 : 4)) == 0);
   S6_REQUIRE((reinterpret_cast<uintptr_t>(rel_blob) & 15) == 0 && (reinterpret_cast<uintptr_t>(qkv) & 15) == 0 &&
              (reinterpret_cast<uintptr_t>(Vt) & 15) == 0);
   if (B == 0) return 0;
@@ -258,20 +289,17 @@ S6_API int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, l
   CUtensorMap tqk, tv;
   int rc = g_make_map(&tqk, qkv, (long long)B * L, ld, ld, 64, QT);
   if (rc) return rc;
-  rc = g_make_map(&tv, Vt, (long long)B * H * D, vt_ld, vt_ld, 64, D);
+  rc = g_make_map(&tv, Vt, (long long)B * H * head_dim, vt_ld, vt_ld, 64, head_dim);
   if (rc) return rc;
   GArgs a{rel_blob, out, out_ld, H, scale};
-  dim3 gridDim3(L / QT, H, B);
   cudaStream_t st = s6_stream(stream);
-  if (out_is_bf16) {
-    auto k = attn_global_tc_kernel<__nv_bfloat16>;
-    S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    k<<<gridDim3, NUM_THREADS, SMEM_BYTES, st>>>(tqk, tv, a);
-  } else {
-    auto k = attn_global_tc_kernel<float>;
-    S6_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    k<<<gridDim3, NUM_THREADS, SMEM_BYTES, st>>>(tqk, tv, a);
-  }
-  S6_LAUNCH_CHECK();
-  return 0;
+  if (head_dim == 64)
+    return out_is_bf16 ? launch_global<64, __nv_bfloat16>(tqk, tv, a, B, st) : launch_global<64, float>(tqk, tv, a, B, st);
+  return out_is_bf16 ? launch_global<80, __nv_bfloat16>(tqk, tv, a, B, st) : launch_global<80, float>(tqk, tv, a, B, st);
+}
+
+// sam6d_attn_global_tc_ex at head_dim 80 (SAM ViT-H)
+S6_API int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H,
+                                int grid, float scale, void* out, int out_is_bf16, long long out_ld, void* stream) {
+  return sam6d_attn_global_tc_ex(qkv, ld, Vt, vt_ld, rel_blob, B, H, grid, 80, scale, out, out_is_bf16, out_ld, stream);
 }

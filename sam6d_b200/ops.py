@@ -542,16 +542,18 @@ def pack_rel_pos(rel_h: Tensor, rel_w: Tensor, slab_rows: int = 32) -> Tensor:
     return blob
 
 
-def attn_global_tc(qkv: Tensor, vt: Tensor, rel_blob: Tensor, B: int, H: int, grid: int, scale: float, out_dtype=torch.bfloat16) -> Tensor:
-    """SAM global attention (grid x grid = 4096 tokens, head_dim 80) on wgmma: qkv (B*L, 3*H*80) bf16, vt from
-    transpose_tokens, rel_blob from pack_rel_pos(rel_h, rel_w, slab_rows=128) -> (B*L, H*80)"""
+def attn_global_tc(qkv: Tensor, vt: Tensor, rel_blob: Tensor, B: int, H: int, grid: int, scale: float, out_dtype=torch.bfloat16,
+                   D: int = 80) -> Tensor:
+    """SAM global attention (grid x grid = 4096 tokens, head_dim D = 80 for ViT-H or 64 for ViT-L / ViT-B) on wgmma: qkv
+    (B*L, >= 2*H*D) bf16 rows [q|k(|v)], vt from transpose_tokens, rel_blob from pack_rel_pos(rel_h, rel_w, slab_rows=128)
+    -> (B*L, H*D)"""
     _check(qkv, torch.bfloat16, "qkv", 2)
     _check(vt, torch.bfloat16, "vt", 2)
     _check(rel_blob, torch.bfloat16, "rel_blob", 1)
     L = grid * grid
-    out = torch.empty(B * L, H * 80, dtype=out_dtype, device=qkv.device)
-    _lib.call("sam6d_attn_global_tc", _p(qkv), _ll(qkv.shape[1]), _p(vt), _ll(vt.shape[1]), _p(rel_blob), int(B), int(H), int(grid),
-              _f(scale), _p(out), int(out_dtype == torch.bfloat16), _ll(H * 80), _s())
+    out = torch.empty(B * L, H * D, dtype=out_dtype, device=qkv.device)
+    _lib.call("sam6d_attn_global_tc_ex", _p(qkv), _ll(qkv.shape[1]), _p(vt), _ll(vt.shape[1]), _p(rel_blob), int(B), int(H), int(grid),
+              int(D), _f(scale), _p(out), int(out_dtype == torch.bfloat16), _ll(H * D), _s())
     return out
 
 
@@ -804,7 +806,7 @@ def pose_score(pts1: Tensor, lab1: Tensor, R: Tensor, t: Tensor, model: Tensor, 
 # ---------------------------------------------------------------------------------------------- SAM encoder attention
 def attn_relpos(qkv: Tensor, nW: int, Hs: int, Ws: int, nH: int, rel_h: Tensor, rel_w: Tensor, scale: float,
                 out_dtype=torch.float32) -> Tensor:
-    """qkv (nW*Hs*Ws, 3*nH*80) f32 -> (nW*Hs*Ws, nH*80) f32|bf16"""
+    """qkv (nW*Hs*Ws, 3*nH*D) f32 -> (nW*Hs*Ws, nH*D) f32|bf16, head_dim D = 80 or 64"""
     _check(qkv, torch.float32, "qkv", 2)
     _check(rel_h, torch.float32, "rel_pos_h", 2)
     _check(rel_w, torch.float32, "rel_pos_w", 2)

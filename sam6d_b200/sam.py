@@ -2,15 +2,17 @@
 (ISM/segment_anything/modeling/image_encoder.py:17-116; built by ISM/segment_anything/build_sam.py:55-80 and reached through
 `SamPredictor.set_image -> model.image_encoder(x)`, ISM/segment_anything/predictor.py:89).
 
-Same constructor signature, same parameter names (so `sam_vit_h_4b8939.pth: image_encoder.*` loads unchanged), same
-forward contract: (B,3,1024,1024) normalised image -> (B,256,64,64).  The torch sub-modules are parameter containers; the
+All three SAM backbones of build_sam.py:14-46 are covered (VIT_CONFIGS, build_image_encoder): ViT-H (head dim 80), ViT-L and
+ViT-B (head dim 64); the attention kernels are instantiated for exactly these two head dims.  Same constructor signature, same
+parameter names (so `sam_vit_{h,l,b}_*.pth: image_encoder.*` load unchanged), same forward contract: (B,3,1024,1024) normalised
+image -> (B,256,64,64).  The torch sub-modules are parameter containers; the
 forward runs sm_90a kernels through the C ABI.  precision="bf16" (default):
     every Linear (qkv, proj, MLP)        -> sam6d_gemm_tma (persistent TMA-fed wgmma GEMM; GELU / bias / fp32 residual in the
                                             epilogue; the qkv projection writes V^T itself, sam6d_gemm_tma_vt)
     LayerNorm                            -> sam6d_layernorm_bf16 (fp32 residual stream -> bf16 GEMM operand)
     window partition (pad 64 -> 70 AFTER norm1) / unpartition -> sam6d_gather_rows with a static index map (-1 = zero pad row)
     windowed attention (14 x 14 tokens)  -> sam6d_attn_tc with the decomposed rel-pos bias (tables from two extra MMAs)
-    global attention (64 x 64 tokens)    -> sam6d_attn_global_tc (online softmax, scores never leave registers)
+    global attention (64 x 64 tokens)    -> sam6d_attn_global_tc_ex (online softmax, scores never leave registers)
     patch embed 16x16/16, neck 1x1 and 3x3 (9 shifted GEMMs) -> sam6d_gemm_bf16 / sam6d_gemm_tma, LayerNorm2d -> sam6d_layernorm
 precision="fp32" keeps everything on the CUDA-core kernels (sam6d_gemm_f32, sam6d_attn_relpos: flash-style, no HW x HW score
 tensor) and is the exact-parity comparator (max error 8e-6 against the reference module).
@@ -24,6 +26,15 @@ from . import ops
 from .pem import _W, _f32, _Packed, _param_key, _gemm, PRECISIONS
 
 _ACT_GELU = 2
+HEAD_DIMS = (64, 80)            # the head dims sam6d_attn_relpos / sam6d_attn_global_tc_ex / sam6d_attn_tc are built for
+
+# build_sam.py:14-46: embed_dim, depth, num_heads, global_attn_indexes per backbone (the keyword arguments of
+# synth.make_sam_state_dict as well)
+VIT_CONFIGS = {
+    "vit_h": dict(embed_dim=1280, depth=32, num_heads=16, global_attn_indexes=(7, 15, 23, 31)),
+    "vit_l": dict(embed_dim=1024, depth=24, num_heads=16, global_attn_indexes=(5, 11, 17, 23)),
+    "vit_b": dict(embed_dim=768, depth=12, num_heads=12, global_attn_indexes=(2, 5, 8, 11)),
+}
 
 
 class LayerNorm2d(nn.Module):
@@ -91,8 +102,9 @@ class ImageEncoderViT(nn.Module):
         super().__init__()
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {PRECISIONS}")
-        if (embed_dim // num_heads) != 80:
-            raise ValueError("sam6d_attn_relpos is built for head_dim 80 (SAM ViT-H: 1280 / 16)")
+        if embed_dim % num_heads or (embed_dim // num_heads) not in HEAD_DIMS:
+            raise ValueError(f"the SAM attention kernels are built for head dims {HEAD_DIMS} (ViT-B 768 / 12, ViT-L 1024 / 16, "
+                             f"ViT-H 1280 / 16); got embed_dim {embed_dim} / num_heads {num_heads}")
         self.img_size, self.patch_size, self.embed_dim, self.num_heads = img_size, patch_size, embed_dim, num_heads
         self.precision = precision
         self.patch_embed = PatchEmbed(kernel_size=(patch_size, patch_size), stride=(patch_size, patch_size), in_chans=in_chans,
@@ -231,10 +243,10 @@ def _block_bf16(self, blk, bw, tok, B, L, C, G, maps):
         qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs)                   # [q|k] rows and V^T per window
         att = ops.attn_tc(qk, 0, qk, C, vt, nW, self.num_heads, Hs * Hs, Hs * Hs, C // self.num_heads, blk.attn.scale,
                           rel=(bw["rel_blob"], Hs, Hs), out_dtype=torch.bfloat16)
-    elif Hs == 64 and C // self.num_heads == 80 and bw["rel_blob"] is not None:
+    elif Hs == 64 and bw["rel_blob"] is not None:
         # global blocks of the 64 x 64 grid (4096 keys): wgmma attention with an online softmax, scores never leave registers
         qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs, slot=2)
-        att = ops.attn_global_tc(qk, vt, bw["rel_blob"], nW, self.num_heads, Hs, blk.attn.scale)
+        att = ops.attn_global_tc(qk, vt, bw["rel_blob"], nW, self.num_heads, Hs, blk.attn.scale, D=C // self.num_heads)
     else:
         # other grids: flash-style CUDA-core kernel with online softmax
         qkv = ops.gemm_tma(xw, bw["qkv"].bf16, bw["qkv_b"])
@@ -251,13 +263,13 @@ ImageEncoderViT._block_bf16 = _block_bf16
 
 
 def build_image_encoder(name: str = "vit_h", precision: str = "bf16") -> ImageEncoderViT:
-    """the image_encoder argument of ISM/segment_anything/build_sam.py:14-21,55-80 for vit_h -- the variant SAM-6D uses
-    (ISM/configs/model/segmentor_model/sam.yaml); the rel-pos attention kernels are built for its head dim 80, so vit_l / vit_b
-    (head dim 64) are rejected here rather than at the first forward"""
+    """the image_encoder argument of ISM/segment_anything/build_sam.py:14-46,55-80 for `vit_h` (the variant SAM-6D's
+    ISM/configs/model/segmentor_model/sam.yaml selects), `vit_l` or `vit_b`"""
     from functools import partial
-    if name != "vit_h":
-        raise ValueError("sam6d_b200 builds the SAM ViT-H image encoder (head dim 80); vit_l / vit_b are not supported")
-    cfg = {"vit_h": (1280, 32, 16, (7, 15, 23, 31))}[name]
-    return ImageEncoderViT(depth=cfg[1], embed_dim=cfg[0], img_size=1024, mlp_ratio=4, norm_layer=partial(torch.nn.LayerNorm, eps=1e-6),
-                           num_heads=cfg[2], patch_size=16, qkv_bias=True, use_rel_pos=True, global_attn_indexes=cfg[3],
-                           window_size=14, out_chans=256, precision=precision)
+    if name not in VIT_CONFIGS:
+        raise ValueError(f"unknown SAM image encoder {name!r}: expected one of {sorted(VIT_CONFIGS)}")
+    cfg = VIT_CONFIGS[name]
+    return ImageEncoderViT(depth=cfg["depth"], embed_dim=cfg["embed_dim"], img_size=1024, mlp_ratio=4,
+                           norm_layer=partial(torch.nn.LayerNorm, eps=1e-6), num_heads=cfg["num_heads"], patch_size=16, qkv_bias=True,
+                           use_rel_pos=True, global_attn_indexes=cfg["global_attn_indexes"], window_size=14, out_chans=256,
+                           precision=precision)

@@ -3,8 +3,9 @@
     MaskDecoder / TwoWayTransformer      ISM/segment_anything/modeling/{mask_decoder,transformer}.py
     Sam (preprocess / postprocess)       ISM/segment_anything/modeling/sam.py
     CustomSamAutomaticMaskGenerator      ISM/model/sam.py:52-155 over SamAutomaticMaskGenerator (automatic_mask_generator.py)
-with the reference's module and parameter names (`sam_vit_h_4b8939.pth` loads unchanged: `image_encoder.*`, `prompt_encoder.*`,
-`mask_decoder.*`).
+with the reference's module and parameter names (`sam_vit_{h,l,b}_*.pth` load unchanged: `image_encoder.*`, `prompt_encoder.*`,
+`mask_decoder.*`).  `sam_model_registry` and `load_sam` are the reference's entry points for picking the backbone (vit_h, vit_l,
+vit_b); the prompt encoder and mask decoder are the same for all three.
 
 Work split.  Every Linear of the decoder -- token side and image side, and the two transposed convolutions written as GEMMs over
 pixel rows -- runs on the wgmma GEMMs (`sam6d_gemm_tma(_batched)` for the 262 144-row image side of a 64-prompt batch,
@@ -20,6 +21,7 @@ post-processing.  Three algebraic savings over the reference's formulation, all 
 The reference's RLE encode / decode round trip inside `_generate_masks` is the identity and is skipped."""
 import ctypes
 import math
+import os
 from typing import Any, Dict, Optional, Tuple
 
 import numpy as np
@@ -347,6 +349,47 @@ def build_sam_vit_h(precision="bf16") -> Sam:
     """build_sam.py:14-21,55-106 with this package's modules"""
     from .sam import build_image_encoder
     return Sam(build_image_encoder("vit_h", precision=precision), PromptEncoder(), MaskDecoder())
+
+
+def build_sam_vit_l(precision="bf16") -> Sam:
+    """build_sam.py:27-34,55-106 with this package's modules"""
+    from .sam import build_image_encoder
+    return Sam(build_image_encoder("vit_l", precision=precision), PromptEncoder(), MaskDecoder())
+
+
+def build_sam_vit_b(precision="bf16") -> Sam:
+    """build_sam.py:37-44,55-106 with this package's modules"""
+    from .sam import build_image_encoder
+    return Sam(build_image_encoder("vit_b", precision=precision), PromptEncoder(), MaskDecoder())
+
+
+# build_sam.py:47-52
+sam_model_registry = {
+    "default": build_sam_vit_h,
+    "vit_h": build_sam_vit_h,
+    "vit_l": build_sam_vit_l,
+    "vit_b": build_sam_vit_b,
+}
+
+# ISM/model/sam.py:17-21: the checkpoint file of each model type inside checkpoint_dir
+pretrained_weight_dict = {
+    "vit_l": "sam_vit_l_0b3195.pth",
+    "vit_b": "sam_vit_b_01ec64.pth",
+    "vit_h": "sam_vit_h_4b8939.pth",
+}
+
+
+def load_sam(model_type: str, checkpoint_dir: str, precision: str = "bf16") -> Sam:
+    """drop-in for ISM/model/sam.py: load_sam (the hydra `model.segmentor_model.sam` target): builds `model_type` and loads
+    `checkpoint_dir/pretrained_weight_dict[model_type]` strictly.  Returns the model on the CPU, like the reference."""
+    if model_type not in pretrained_weight_dict:
+        raise ValueError(f"unknown SAM model_type {model_type!r}: expected one of {sorted(pretrained_weight_dict)}")
+    path = os.path.join(checkpoint_dir, pretrained_weight_dict[model_type])
+    if not os.path.isfile(path):
+        raise FileNotFoundError(f"SAM {model_type} checkpoint not found: {path} (expected {pretrained_weight_dict[model_type]} in {checkpoint_dir})")
+    sam = sam_model_registry[model_type](precision)
+    sam.load_state_dict(torch.load(path, map_location="cpu"), strict=True)
+    return sam
 
 
 def preprocess_shape(oldh, oldw, long_side=1024) -> Tuple[int, int]:

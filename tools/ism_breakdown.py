@@ -12,7 +12,7 @@ with torch.no_grad():
     enc(img); enc(img)
     torch.cuda.synchronize()
     names = [n for n in dir(_lib.lib()) if n.startswith("sam6d_")] if hasattr(_lib.lib(), "__dir__") else []
-    names = ["sam6d_gemm_tma", "sam6d_gemm_tma_vt", "sam6d_attn_tc", "sam6d_attn_global_tc", "sam6d_layernorm_bf16", "sam6d_layernorm",
+    names = ["sam6d_gemm_tma", "sam6d_gemm_tma_vt", "sam6d_attn_tc", "sam6d_attn_global_tc_ex", "sam6d_layernorm_bf16", "sam6d_layernorm",
              "sam6d_gather_rows", "sam6d_gemm_bf16", "sam6d_transpose_tokens_bf16", "sam6d_gemm_f32", "sam6d_attn_relpos"]
     for n in names:
         _lib.time_kernel(n, True)

@@ -150,7 +150,8 @@ def run_case(mods, tag, B, n, coarse_npoint, seed, out_dir, store_inputs):
 def run_sam_case(out_dir, tag="sam_small", cfg=None, check_oracle=True):
     """SAM image encoder: the vendored reference module against oracle/sam_oracle.py.
     sam_small: 2 blocks of ViT-H width (one windowed, one global), 1024^2 input -- every code path of the 32-block model.
-    sam_vith:  the full 32-block ViT-H of build_sam.py:14-21 on one frame (5.96 TFLOP on the CPU)."""
+    sam_vith:  the full 32-block ViT-H of build_sam.py:14-21 on one frame (5.96 TFLOP on the CPU).
+    sam_vitl / sam_vitb: the full 24-block ViT-L / 12-block ViT-B of build_sam.py:27-44 (head dim 64)."""
     from oracle import sam_oracle as so
     sys.path.insert(0, os.path.join(REF, "Instance_Segmentation_Model"))
     from functools import partial
@@ -177,6 +178,24 @@ def run_sam_case(out_dir, tag="sam_small", cfg=None, check_oracle=True):
     print(f"  wrote {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
+def run_sam_keys_case(out_dir):
+    """the (key, shape) list and parameter count of the reference's sam_model_registry[t]() for vit_h, vit_l and vit_b
+    (build_sam.py:14-52): the checkpoint layout each backbone's drop-in must load strictly"""
+    sys.path.insert(0, os.path.join(REF, "Instance_Segmentation_Model"))
+    from segment_anything.build_sam import sam_model_registry
+    gold = dict(meta=dict(source="segment_anything sam_model_registry imported from /root/reference"), types={})
+    for t in ("vit_h", "vit_l", "vit_b"):
+        torch.manual_seed(0)
+        model = sam_model_registry[t]()
+        keys = [(k, tuple(v.shape)) for k, v in model.state_dict().items()]
+        n = sum(p.numel() for p in model.parameters())
+        gold["types"][t] = dict(keys=keys, n_params=n)
+        print(f"  {t}: {len(keys)} state_dict tensors, {n} parameters")
+    path = os.path.join(out_dir, "sam_keys.pt")
+    torch.save(gold, path)
+    print(f"  wrote {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
+
+
 def main(only=None):
     out_dir = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out_dir, exist_ok=True)
@@ -194,6 +213,12 @@ def main(only=None):
         run_sam_case(out_dir)
     if want("sam_vith"):
         run_sam_case(out_dir, "sam_vith", dict(embed_dim=1280, depth=32, num_heads=16, global_attn_indexes=(7, 15, 23, 31)))
+    if want("sam_vitl"):
+        run_sam_case(out_dir, "sam_vitl", dict(embed_dim=1024, depth=24, num_heads=16, global_attn_indexes=(5, 11, 17, 23)))
+    if want("sam_vitb"):
+        run_sam_case(out_dir, "sam_vitb", dict(embed_dim=768, depth=12, num_heads=12, global_attn_indexes=(2, 5, 8, 11)))
+    if want("sam_keys"):
+        run_sam_keys_case(out_dir)
 
 
 if __name__ == "__main__":
