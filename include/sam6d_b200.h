@@ -70,7 +70,10 @@ int sam6d_gemm_bf16(const void* A, int a_dtype, const void* W, int w_dtype, cons
                     long long sA, long long sW, long long sC, long long sR, float alpha, int relu, void* stream);
 
 /* Persistent TMA-fed version for plain (non-batched) bf16 operands: cp.async.bulk.tensor boxes with SWIZZLE_128B feed a
- * 4-stage ring consumed by two wgmma warpgroups.  A (M,K) bf16, W (N,K) bf16, C fp32 (0) / bf16 (1). */
+ * 4-stage ring consumed by two wgmma warpgroups.  A (M,K) bf16, W (N,K) bf16, C fp32 (0) / bf16 (1).
+ * act: 0 none, 1 ReLU, 2 GELU(erf), 3 SwiGLU -- W holds a w12 whose rows are interleaved in blocks of 128 (gate rows of hidden
+ * units [128t, 128t+128), then their up rows), bias packed alike; C (M, N/2) bf16 = silu(gate) * up; N % 256 == 0, bias, no
+ * residual. */
 int sam6d_gemm_tma(const void* A, const void* W, const float* bias, const void* R, void* C, int c_dtype, int M, int N, int K,
                    long long lda, long long ldw, long long ldc, long long ldr, float alpha, int act, void* stream);
 /* `batch` independent problems stacked along the rows of A and W (problem z: rows [z*a_rpb, +M) of A, [z*w_rpb, +N) of W,

@@ -19,7 +19,11 @@ sam_amg.load_sam.
 
 `--segmentor_model fastsam` (ISM_fastsam.yaml) replaces SAM by FastSAM (sam6d_b200/fast_sam.py: YOLOv8x-seg, conf 0.25, iou 0.9,
 max_det 200) built from `{checkpoint_dir}/FastSAM/FastSAM-x.pt` or the reference's `./checkpoints/FastSAM/FastSAM-x.pt`; it needs
-only the DINOv2 checkpoint besides.  The rest of the pipeline and the output files are the same."""
+only the DINOv2 checkpoint besides.  The rest of the pipeline and the output files are the same.
+
+`--dinov2_model {dinov2_vits14,dinov2_vitb14,dinov2_vitl14,dinov2_vitg14}` picks the descriptor backbone (the reference's hydra
+`model.descriptor_model.model_name`, default dinov2_vitl14) and its checkpoint `{checkpoint_dir}/dinov2/<name>_pretrain.pth`.
+dinov2_vitg14 is built with the SwiGLU FFN its published checkpoint holds (sam6d_b200/dinov2.py: FFN_OF_MODEL)."""
 import argparse
 import glob
 import json
@@ -48,9 +52,11 @@ def get_parser():
     # not in the reference: where weights / template poses come from
     ap.add_argument("--checkpoint_dir", default=None,
                     help="directory with segment-anything/sam_vit_h_4b8939.pth (or the --sam_model_type's file, or FastSAM/FastSAM-x.pt) "
-                         "and dinov2/dinov2_vitl14_pretrain.pth")
+                         "and dinov2/<--dinov2_model>_pretrain.pth")
     ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"),
                     help="not in the reference: the hydra `model.segmentor_model.sam.model_type` (SAM backbone)")
+    ap.add_argument("--dinov2_model", default="dinov2_vitl14", choices=("dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"),
+                    help="not in the reference: the hydra `model.descriptor_model.model_name` (DINOv2 descriptor backbone)")
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
     ap.add_argument("--template_poses", default=None, help="(T,4,4) .npy of the template camera poses (default: templates/template_poses.npy)")
     ap.add_argument("--points_per_side", default=32, type=int)
@@ -86,15 +92,29 @@ def mask_to_rle(binary_mask: np.ndarray):
     return {"counts": counts, "size": list(binary_mask.shape)}
 
 
+def _new_desc(args, device):
+    from ..dinov2 import CustomDINOv2
+    return CustomDINOv2(args.dinov2_model, "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+
+
+def _dino_checkpoint(args):
+    return os.path.join(args.checkpoint_dir, "dinov2", f"{args.dinov2_model}_pretrain.pth") if args.checkpoint_dir else None
+
+
+def _seeded_dino_state_dict(vit):
+    """seed-1 weights for the built backbone (the defaults are ViT-L/14's: the same draw as before the backbone was selectable)"""
+    from .. import synth
+    return synth.make_dinov2_state_dict(embed_dim=vit.embed_dim, depth=vit.depth, num_heads=vit.num_heads, seed=1, ffn_layer=vit.ffn_layer)
+
+
 def build_fastsam(args, device):
     """FastSAM (ISM/configs/model/segmentor_model/fast_sam.yaml) + DINOv2"""
-    from ..dinov2 import CustomDINOv2
     from ..fast_sam import FastSAM
-    desc = CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+    desc = _new_desc(args, device)
     ck = args.checkpoint_dir
     cands = ([os.path.join(ck, "FastSAM", "FastSAM-x.pt")] if ck else []) + [os.path.join(".", "checkpoints", "FastSAM", "FastSAM-x.pt")]
     fs_ck = next((c for c in cands if os.path.exists(c)), None)
-    dino_ck = os.path.join(ck, "dinov2", "dinov2_vitl14_pretrain.pth") if ck else None
+    dino_ck = _dino_checkpoint(args)
     cfg = dict(iou_threshold=0.9, conf_threshold=0.05, max_det=200)
     if fs_ck and dino_ck and os.path.exists(dino_ck):
         seg = FastSAM(fs_ck, cfg, segmentor_width_size=640, device=device)
@@ -104,14 +124,13 @@ def build_fastsam(args, device):
         print("=> WARNING: no checkpoints, seeded random weights (detections are meaningless; plumbing run)", file=sys.stderr)
         seg = FastSAM(None, cfg, segmentor_width_size=640, device=device)
         seg.model.load_state_dict(synth.make_fastsam_state_dict(seed=1), strict=True)
-        desc.model.load_state_dict(synth.make_dinov2_state_dict(seed=1), strict=True)
+        desc.model.load_state_dict(_seeded_dino_state_dict(desc.model), strict=True)
     else:
         raise FileNotFoundError("FastSAM / DINOv2 checkpoints not found (pass --checkpoint_dir, or --random_weights for a plumbing run)")
     return seg, desc
 
 
 def build_models(args, device):
-    from ..dinov2 import CustomDINOv2
     from ..sam import VIT_CONFIGS
     from ..sam_amg import CustomSamAutomaticMaskGenerator, load_sam, pretrained_weight_dict, sam_model_registry
     if args.segmentor_model == "fastsam":
@@ -119,12 +138,12 @@ def build_models(args, device):
     mt = args.sam_model_type
 
     def new_desc():            # built after SAM: module construction keeps drawing torch's global RNG in the same order
-        return CustomDINOv2("dinov2_vitl14", "x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640).to(device).eval()
+        return _new_desc(args, device)
 
     ck = args.checkpoint_dir
     sam_dir = os.path.join(ck, "segment-anything") if ck else None
     sam_ck = os.path.join(sam_dir, pretrained_weight_dict[mt]) if ck else None
-    dino_ck = os.path.join(ck, "dinov2", "dinov2_vitl14_pretrain.pth") if ck else None
+    dino_ck = _dino_checkpoint(args)
     if sam_ck and os.path.exists(sam_ck) and os.path.exists(dino_ck):
         sam = load_sam(mt, sam_dir, "bf16").to(device).eval()
         desc = new_desc()
@@ -137,7 +156,7 @@ def build_models(args, device):
         sd = {"image_encoder." + k: v for k, v in synth.make_sam_state_dict(**VIT_CONFIGS[mt], seed=1).items()}
         sd.update(synth.make_sam_decoder_state_dict(seed=1))
         sam.load_state_dict(sd, strict=True)
-        desc.model.load_state_dict(synth.make_dinov2_state_dict(seed=1), strict=True)
+        desc.model.load_state_dict(_seeded_dino_state_dict(desc.model), strict=True)
     else:
         raise FileNotFoundError("SAM / DINOv2 checkpoints not found (pass --checkpoint_dir, or --random_weights for a plumbing run)")
     seg = CustomSamAutomaticMaskGenerator(sam, points_per_batch=64, stability_score_thresh=args.stability_score_thresh, box_nms_thresh=0.7,

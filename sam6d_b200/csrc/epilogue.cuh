@@ -65,6 +65,30 @@ __device__ __forceinline__ void store_frag(const float (&d)[N / 2], int w, int l
   }
 }
 
+// Gated (SwiGLU) epilogue of a 64 x 256 fragment: columns [0, 128) of the tile are the gate pre-activations x1 of 128 hidden
+// units, columns [128, 256) the matching "up" pre-activations x2 (the W rows are interleaved in blocks of 128 on the host).
+// Column 8j + 2(lane&3) + e and column 8(j+16) + 2(lane&3) + e sit in the same thread (d[4j + 2h + e], d[4(j+16) + 2h + e]),
+// so hidden = silu(x1) * x2 is formed in registers and 128 bf16 columns are written from out_col0 on.  bias: the packed
+// (interleaved) bias, indexed by the tile's column col0.  C must allow 2-element stores at even columns (even ldc).
+__device__ __forceinline__ void store_frag_swiglu(const float (&d)[128], int w, int lane, int row0, int M, int col0, int out_col0,
+                                                  float alpha, const float* __restrict__ bias, __nv_bfloat16* __restrict__ C,
+                                                  long long ldc) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = tc::frag_col(4 * j, lane);
+    const float g0 = __ldg(bias + col0 + c), g1 = __ldg(bias + col0 + c + 1);
+    const float u0 = __ldg(bias + col0 + 128 + c), u1 = __ldg(bias + col0 + 128 + c + 1);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + tc::frag_row(2 * h, w, lane);
+      if (row >= M) continue;
+      const float x0 = fmaf(d[4 * j + 2 * h], alpha, g0), x1 = fmaf(d[4 * j + 2 * h + 1], alpha, g1);
+      const float y0 = fmaf(d[4 * (j + 16) + 2 * h], alpha, u0), y1 = fmaf(d[4 * (j + 16) + 2 * h + 1], alpha, u1);
+      st2(C + (size_t)row * ldc + out_col0 + c, x0 / (1.f + __expf(-x0)) * y0, x1 / (1.f + __expf(-x1)) * y1);
+    }
+  }
+}
+
 // run-time -> compile-time dispatch of (ACT, HAS_BIAS, HAS_RES)
 #define EPI_DISPATCH(ACT_V, BIAS_P, RES_P, ...)                                              \
   do {                                                                                       \

@@ -135,6 +135,9 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tma_kernel(const __grid_const
           }
         }
       }
+    } else if constexpr (ACT == 3) {
+      // SwiGLU: N tile t holds the gate and up rows of hidden units [128 t, 128 t + 128) -> output columns n0 / 2 + [0, 128)
+      epi::store_frag_swiglu(acc, w, lane, row0, g.M, n0, n0 / 2, g.alpha, g.bias, Cb, g.ldc);
     } else {
       epi::store_frag<OT, ACT, HAS_BIAS, HAS_RES, OT, BN>(acc, w, lane, row0, g.M, n0, g.N, g.alpha, g.bias, Rb, g.ldr, Cb, g.ldc);
     }
@@ -179,7 +182,7 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
                     long long lda, long long ldw, long long ldc, long long ldr, int batch, long long a_rpb, long long w_rpb,
                     long long c_bs, long long r_bs, float alpha, int act, void* stream, void* vt = nullptr, int vt_col0 = 0, int vt_S = 1,
                     int vt_N1 = 0, int vt_col1 = -1, void* c2 = nullptr, long long ldc2 = 0) {
-  S6_REQUIRE(A && W && C && M >= 0 && N > 0 && K > 0 && (K % 8) == 0 && (lda % 8) == 0 && (ldw % 8) == 0 && act >= 0 && act <= 2);
+  S6_REQUIRE(A && W && C && M >= 0 && N > 0 && K > 0 && (K % 8) == 0 && (lda % 8) == 0 && (ldw % 8) == 0 && act >= 0 && act <= 3);
   S6_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0 && batch >= 0);
   S6_REQUIRE(a_rpb * (long long)batch < 2000000000LL && w_rpb * (long long)batch < 2000000000LL);
   if (M == 0 || batch == 0) return 0;
@@ -218,6 +221,13 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
     S6_LAUNCH_CHECK();
     return 0;
   }
+  if (act == 3) {
+    // SwiGLU: bf16 output of N / 2 columns, bias, no residual; every N tile holds 128 gate rows then their 128 up rows
+    S6_REQUIRE(c_dtype == 1 && bias && !R && (N % BN) == 0 && (ldc % 2) == 0 && ldc >= N / 2);
+    LAUNCH_ONE(__nv_bfloat16, 3, true, false, false);
+    S6_LAUNCH_CHECK();
+    return 0;
+  }
   EPI_DISPATCH(act, bias, R, LAUNCH_TMA);
 #undef LAUNCH_TMA
 #undef LAUNCH_ONE
@@ -229,7 +239,10 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
 
 // A (M,K) bf16 lda, W (N,K) bf16 ldw, C (M,N) fp32 (c_dtype 0) or bf16 (1), bias (N) fp32 or NULL, R (M,N) or NULL: the
 // residual has the element type of C (fp32 stream with fp32 output, bf16 stream with bf16 output).
-// K % 8 == 0, lda % 8 == 0, ldw % 8 == 0, 16-byte aligned bases.  act: 0 none, 1 ReLU, 2 GELU(erf).
+// K % 8 == 0, lda % 8 == 0, ldw % 8 == 0, 16-byte aligned bases.  act: 0 none, 1 ReLU, 2 GELU(erf), 3 SwiGLU.
+// act 3: W is a SwiGLU w12 with its rows interleaved in blocks of 128 (gate rows of hidden units [128t, 128t + 128), then their
+// up rows), bias packed the same way; C (M, N/2) bf16 = silu(gate) * up with row stride ldc; N % 256 == 0, bias required,
+// no residual, bf16 output only (-22 otherwise).
 S6_API int sam6d_gemm_tma(const void* A, const void* W, const float* bias, const void* R, void* C, int c_dtype, int M, int N, int K,
                           long long lda, long long ldw, long long ldc, long long ldr, float alpha, int act, void* stream) {
   return launch_gemm_tma(A, W, bias, R, C, c_dtype, M, N, K, lda, ldw, ldc, ldr, 1, 0, 0, 0, 0, alpha, act, stream);

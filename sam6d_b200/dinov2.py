@@ -1,20 +1,22 @@
 """ISM descriptor branch on H100 kernels (SURVEY.md 8f row N2): drop-ins for
-    DinoVisionTransformer (ViT-L/14 = dinov2_vitl14)   ISM/model/vision_transformer.py:43-375
+    DinoVisionTransformer (ViT-S/B/L/g 14 = dinov2_vit{s,b,l,g}14)   ISM/model/vision_transformer.py:43-392
     CustomDINOv2                                        ISM/model/dinov2.py:92-258
     MaskedPatch_MatrixSimilarity (compute_straight / compute_visible_ratio)   ISM/model/loss.py:46-77
     compute_appearance_score / compute_geometric_score  ISM/model/detector.py:298-323
 
 The trunk is a pre-norm ViT with LayerScale: parameter names are the reference's (`cls_token`, `pos_embed` (1, 1370, C),
-`mask_token`, `patch_embed.proj`, `blocks.N.{norm1, attn.{qkv,proj}, ls1.gamma, norm2, mlp.{fc1,fc2}, ls2.gamma}`, `norm`), so
-`dinov2_vitl14_pretrain.pth` loads unchanged.  Every forward runs through the C ABI:
+`mask_token`, `patch_embed.proj`, `blocks.N.{norm1, attn.{qkv,proj}, ls1.gamma, norm2, mlp.{fc1,fc2} or mlp.{w12,w3}, ls2.gamma}`, `norm`), so
+`dinov2_vit{s,b,l,g}14_pretrain.pth` load unchanged.  Every forward runs through the C ABI:
     patch embedding, qkv / proj / fc1 / fc2                -> sam6d_gemm_tma / sam6d_gemm_tc (wgmma; bias, GELU, residual epilogues;
                                                               LayerScale folded into proj / fc2 when the weights are packed)
+    ViT-g's SwiGLU FFN w12 / w3                            -> sam6d_gemm_tma act=3 (silu(gate) * up formed in the epilogue registers,
+                                                              w12 rows interleaved in blocks of 128 when packed) / residual epilogue
     LayerNorm                                              -> sam6d_layernorm_bf16
-    attention over 257 tokens (16 heads x 64)              -> sam6d_attn_tc_ex on keys 0..255 (tensor cores, log-sum-exp out)
+    attention over 257 tokens (C / 64 heads x 64)          -> sam6d_attn_tc_ex on keys 0..255 (tensor cores, log-sum-exp out)
                                                               + sam6d_attn_merge_key for the 257th token
     crop / mask / nearest resize / pad of all proposals    -> sam6d_crop_resize_pad
     masked, normalised patch tokens                        -> sam6d_masked_patch_normalize
-    appearance score + visible ratio                       -> sam6d_gemm_tma_batched (256 x 256 x 1024 per proposal) + sam6d_appearance_reduce
+    appearance score + visible ratio                       -> sam6d_gemm_tma_batched (256 x 256 x C per proposal) + sam6d_appearance_reduce
 There is no CPU path.  The positional-embedding interpolation (bicubic, once per input size) is weight preprocessing in torch."""
 import ctypes
 import math
@@ -58,6 +60,19 @@ class _Mlp(nn.Module):
         self.fc2 = nn.Linear(hidden, dim)
 
 
+class _SwiGLUFFNFused(nn.Module):
+    """SwiGLUFFNFused (ISM/model/layers/swiglu_ffn.py:45-63): w12 = [gate; up] rows, hidden = (int(hidden * 2 / 3) + 7) // 8 * 8"""
+
+    def __init__(self, dim, hidden):
+        super().__init__()
+        hidden = (int(hidden * 2 / 3) + 7) // 8 * 8
+        self.w12 = nn.Linear(dim, 2 * hidden)
+        self.w3 = nn.Linear(hidden, dim)
+
+
+FFN_LAYERS = {"mlp": _Mlp, "swiglufused": _SwiGLUFFNFused}
+
+
 class _LayerScale(nn.Module):
     def __init__(self, dim, init_values):
         super().__init__()
@@ -65,13 +80,13 @@ class _LayerScale(nn.Module):
 
 
 class _Block(nn.Module):
-    def __init__(self, dim, mlp_ratio, init_values):
+    def __init__(self, dim, mlp_ratio, init_values, ffn_layer="mlp"):
         super().__init__()
         self.norm1 = nn.LayerNorm(dim, eps=1e-6)
         self.attn = _Attention(dim)
         self.ls1 = _LayerScale(dim, init_values)
         self.norm2 = nn.LayerNorm(dim, eps=1e-6)
-        self.mlp = _Mlp(dim, int(dim * mlp_ratio))
+        self.mlp = FFN_LAYERS[ffn_layer](dim, int(dim * mlp_ratio))
         self.ls2 = _LayerScale(dim, init_values)
 
 
@@ -81,18 +96,21 @@ class DinoVisionTransformer(nn.Module):
     most 256 patches (the 224 x 224 proposal crops of SAM-6D give 16 x 16)."""
 
     def __init__(self, img_size=518, patch_size=14, in_chans=3, embed_dim=1024, depth=24, num_heads=16, mlp_ratio=4.0, init_values=1.0,
-                 interpolate_offset=0.1, interpolate_antialias=False, num_register_tokens=0):
+                 interpolate_offset=0.1, interpolate_antialias=False, num_register_tokens=0, ffn_layer="mlp"):
         super().__init__()
         if embed_dim // num_heads != 64 or num_register_tokens or interpolate_antialias:
-            raise ValueError("sam6d_b200 DinoVisionTransformer: head dim 64, no register tokens (dinov2_vit{s,b,l}14)")
+            raise ValueError("sam6d_b200 DinoVisionTransformer: head dim 64, no register tokens (dinov2_vit{s,b,l,g}14)")
+        if ffn_layer not in FFN_LAYERS:
+            raise NotImplementedError(f"sam6d_b200 DinoVisionTransformer: ffn_layer {ffn_layer!r} (supported: {', '.join(FFN_LAYERS)})")
         self.embed_dim, self.num_heads, self.patch_size, self.depth = embed_dim, num_heads, patch_size, depth
+        self.ffn_layer = ffn_layer
         self.interpolate_offset = interpolate_offset
         self.patch_embed = _PatchEmbed(patch_size, in_chans, embed_dim)
         n = (img_size // patch_size) ** 2
         self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
         self.pos_embed = nn.Parameter(torch.zeros(1, n + 1, embed_dim))
         self.mask_token = nn.Parameter(torch.zeros(1, embed_dim))
-        self.blocks = nn.ModuleList([_Block(embed_dim, mlp_ratio, init_values) for _ in range(depth)])
+        self.blocks = nn.ModuleList([_Block(embed_dim, mlp_ratio, init_values, ffn_layer) for _ in range(depth)])
         self.norm = nn.LayerNorm(embed_dim, eps=1e-6)
         self._packed = _Packed()
         self._pos_cache = {}
@@ -111,11 +129,18 @@ class DinoVisionTransformer(nn.Module):
             for blk in self.blocks:
                 g1, g2 = _f32(blk.ls1.gamma).double(), _f32(blk.ls2.gamma).double()
                 # x + gamma * (W y + b) = x + (diag(gamma) W) y + gamma * b : LayerScale folded into the projection
+                # Mlp: f1 / f2 = fc1 / fc2.  SwiGLU: f1 = w12 with its gate and up rows interleaved for gemm_tma(act=3), f2 = w3
+                if self.ffn_layer == "swiglufused":
+                    f1, f1b = _W(ops.pack_swiglu_rows(_f32(blk.mlp.w12.weight))), ops.pack_swiglu_rows(_f32(blk.mlp.w12.bias))
+                    f2w, f2b = blk.mlp.w3.weight, blk.mlp.w3.bias
+                else:
+                    f1, f1b = _W(blk.mlp.fc1.weight), _f32(blk.mlp.fc1.bias)
+                    f2w, f2b = blk.mlp.fc2.weight, blk.mlp.fc2.bias
                 w["blocks"].append(dict(
                     n1w=_f32(blk.norm1.weight), n1b=_f32(blk.norm1.bias), qkv=_W(blk.attn.qkv.weight), qkv_b=_f32(blk.attn.qkv.bias),
                     proj=_W((_f32(blk.attn.proj.weight).double() * g1[:, None]).float()), proj_b=(_f32(blk.attn.proj.bias).double() * g1).float().contiguous(),
-                    n2w=_f32(blk.norm2.weight), n2b=_f32(blk.norm2.bias), f1=_W(blk.mlp.fc1.weight), f1b=_f32(blk.mlp.fc1.bias),
-                    f2=_W((_f32(blk.mlp.fc2.weight).double() * g2[:, None]).float()), f2b=(_f32(blk.mlp.fc2.bias).double() * g2).float().contiguous()))
+                    n2w=_f32(blk.norm2.weight), n2b=_f32(blk.norm2.bias), f1=f1, f1b=f1b,
+                    f2=_W((_f32(f2w).double() * g2[:, None]).float()), f2b=(_f32(f2b).double() * g2).float().contiguous()))
             self._packed.w, self._packed.key = w, key
             self._pos_cache = {}
         return self._packed.w
@@ -170,13 +195,14 @@ class DinoVisionTransformer(nn.Module):
         ops.gemm_tc_raw(patches.data_ptr(), 0, w["pe_w"].bf16.data_ptr(), 1, w["pe_b"], pos.data_ptr(), tok.data_ptr() + C * 4, 0,
                         L, C, Kp, Kp, Kp, C, C, batch=B, sA=L * Kp, sW=0, sC=S * C, sR=0)
         tok = tok.view(B * S, C)
+        act = ops.ACT_SWIGLU if self.ffn_layer == "swiglufused" else _ACT_GELU
         for bw in w["blocks"]:
             xn = ops.layernorm_bf16(tok, bw["n1w"], bw["n1b"], eps=1e-6)
             qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, S, slot=4)
             att = self._attention(qk, vt, B, S, C)
             tok = ops.gemm_tma(att, bw["proj"].bf16, bw["proj_b"], residual=tok)
             xn = ops.layernorm_bf16(tok, bw["n2w"], bw["n2b"], eps=1e-6)
-            hid = ops.gemm_tma(xn, bw["f1"].bf16, bw["f1b"], act=_ACT_GELU, out_dtype=torch.bfloat16)
+            hid = ops.gemm_tma(xn, bw["f1"].bf16, bw["f1b"], act=act, out_dtype=torch.bfloat16)
             tok = ops.gemm_tma(hid, bw["f2"].bf16, bw["f2b"], residual=tok)
         xn = ops.layernorm(tok, w["nw"], w["nb"], eps=1e-6).view(B, S, C)
         return {"x_norm_clstoken": xn[:, 0], "x_norm_regtokens": xn[:, 1:1], "x_norm_patchtokens": xn[:, 1:], "x_prenorm": tok.view(B, S, C),
@@ -188,11 +214,47 @@ class DinoVisionTransformer(nn.Module):
         return ret if is_training else ret["x_norm_clstoken"]
 
 
-def vit_large(patch_size=14, **kwargs):
-    """dinov2_vitl14 (vision_transformer.py:364-375 with the arguments of _make_dinov2_model, dinov2.py:46-90)"""
-    kw = dict(img_size=518, init_values=1.0, embed_dim=1024, depth=24, num_heads=16, mlp_ratio=4)
+def _vit(patch_size, embed_dim, depth, num_heads, kwargs):
+    """the constructors of vision_transformer.py:336-392 with the arguments of _make_dinov2_model (dinov2.py:46-90)"""
+    kw = dict(img_size=518, init_values=1.0, embed_dim=embed_dim, depth=depth, num_heads=num_heads, mlp_ratio=4)
     kw.update(kwargs)
     return DinoVisionTransformer(patch_size=patch_size, **kw)
+
+
+def vit_small(patch_size=14, **kwargs):
+    """dinov2_vits14 (vision_transformer.py:336-347)"""
+    return _vit(patch_size, 384, 12, 6, kwargs)
+
+
+def vit_base(patch_size=14, **kwargs):
+    """dinov2_vitb14 (vision_transformer.py:350-361)"""
+    return _vit(patch_size, 768, 12, 12, kwargs)
+
+
+def vit_large(patch_size=14, **kwargs):
+    """dinov2_vitl14 (vision_transformer.py:364-375 with the arguments of _make_dinov2_model, dinov2.py:46-90)"""
+    return _vit(patch_size, 1024, 24, 16, kwargs)
+
+
+def vit_giant2(patch_size=14, **kwargs):
+    """vision_transformer.py:378-392 (1536 / 24 heads of 64 / 40 blocks); dinov2_vitg14 passes ffn_layer='swiglufused'"""
+    return _vit(patch_size, 1536, 40, 24, kwargs)
+
+
+# ISM/model/dinov2.py:14-26
+descriptor_size = {"dinov2_vits14": 384, "dinov2_vitb14": 768, "dinov2_vitl14": 1024, "dinov2_vitg14": 1536}
+descriptor_map = {"dinov2_vits14": "vit_small", "dinov2_vitb14": "vit_base", "dinov2_vitl14": "vit_large", "dinov2_vitg14": "vit_giant2"}
+_CONSTRUCTORS = {"vit_small": vit_small, "vit_base": vit_base, "vit_large": vit_large, "vit_giant2": vit_giant2}
+# The reference builds every backbone with the default Mlp FFN, but the published dinov2_vitg14_pretrain.pth holds SwiGLU weights
+# (blocks.N.mlp.w12 / w3), which its strict load_state_dict rejects.  Here ViT-g is built as the checkpoint is: SwiGLUFFNFused.
+FFN_OF_MODEL = {"dinov2_vitg14": "swiglufused"}
+
+
+def build_descriptor_vit(model_name, patch_size=14):
+    """the backbone of CustomDINOv2(model_name): dinov2_vit{s,b,l,g}14 -> DinoVisionTransformer"""
+    if model_name not in descriptor_map:
+        raise NotImplementedError(f"DINOv2 model {model_name!r}: sam6d_b200 supports {', '.join(descriptor_map)} (no register-token variants)")
+    return _CONSTRUCTORS[descriptor_map[model_name]](patch_size, ffn_layer=FFN_OF_MODEL.get(model_name, "mlp"))
 
 
 # =====================================================================================================================
@@ -217,10 +279,8 @@ class CustomDINOv2(nn.Module):
     def __init__(self, model_name="dinov2_vitl14", token_name="x_norm_clstoken", image_size=224, chunk_size=16, descriptor_width_size=640,
                  checkpoint_dir=None, patch_size=14, validpatch_thresh=0.5, model: Optional[nn.Module] = None):
         super().__init__()
-        if model_name != "dinov2_vitl14" and model is None:
-            raise NotImplementedError("SAM-6D configures dinov2_vitl14")
         self.model_name = model_name
-        self.model = model if model is not None else vit_large(patch_size)
+        self.model = model if model is not None else build_descriptor_vit(model_name, patch_size)
         if checkpoint_dir is not None:
             import os.path as osp
             self.model.load_state_dict(torch.load(osp.join(checkpoint_dir, f"{model_name}_pretrain.pth"), map_location="cpu"))

@@ -184,20 +184,35 @@ def gemm_tc(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optio
 
 def gemm_tma(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optional[Tensor] = None, out: Optional[Tensor] = None,
              act: int = 0, alpha: float = 1.0, out_dtype=torch.float32) -> Tensor:
-    """persistent TMA-fed wgmma GEMM: A (M,K) bf16, W (N,K) bf16 -> (M,N) fp32|bf16"""
+    """persistent TMA-fed wgmma GEMM: A (M,K) bf16, W (N,K) bf16 -> (M,N) fp32|bf16.
+    act=3 (SwiGLU): W and bias are a w12 packed by pack_swiglu_rows -> (M, N/2) bf16 silu(x w1^T + b1) * (x w2^T + b2)"""
     _check(A, torch.bfloat16, "A", 2)
     _check(W, torch.bfloat16, "W", 2)
     M, K = A.shape
     N = W.shape[0]
     if W.shape[1] != K:
         raise RuntimeError("gemm: inner dimensions differ")
+    Nout = N // 2 if act == ACT_SWIGLU else N
     if out is None:
-        out = torch.empty(M, N, dtype=out_dtype, device=A.device)
+        out = torch.empty(M, Nout, dtype=torch.bfloat16 if act == ACT_SWIGLU else out_dtype, device=A.device)
     if residual is not None:
         _check(residual, out.dtype, "residual", 2)          # the residual stream has the element type of the output
-    _lib.call("sam6d_gemm_tma", _p(A), _p(W), _p(bias), _p(residual), _p(out), _DT[out.dtype], M, N, K, _ll(K), _ll(K), _ll(N), _ll(N),
+    _lib.call("sam6d_gemm_tma", _p(A), _p(W), _p(bias), _p(residual), _p(out), _DT[out.dtype], M, N, K, _ll(K), _ll(K), _ll(Nout), _ll(N),
               _f(alpha), int(act), _s())
     return out
+
+
+ACT_SWIGLU = 3
+
+
+def pack_swiglu_rows(t: Tensor, block: int = 128) -> Tensor:
+    """w12 (2H, K) or its bias (2H,) in the reference's order (rows [0, H) gate, [H, 2H) up) -> the order gemm_tma(act=3)
+    reads: gate rows [128t, 128t + 128) followed by up rows [128t, 128t + 128), for t = 0 .. H/128 - 1.  H % 128 == 0."""
+    H = t.shape[0] // 2
+    if t.shape[0] != 2 * H or H % block:
+        raise ValueError(f"SwiGLU w12 needs 2H rows with H % {block} == 0, got {t.shape[0]}")
+    rest = t.shape[1:]
+    return t.reshape(2, H // block, block, *rest).transpose(0, 1).reshape(2 * H, *rest).contiguous()
 
 
 _VT_CACHE = {}

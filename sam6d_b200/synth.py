@@ -224,10 +224,12 @@ def make_vit_state_dict(embed_dim=768, depth=12, out_dim=256, n_patches=196, num
     return sd
 
 
-def make_dinov2_state_dict(embed_dim=1024, depth=24, num_heads=16, patch=14, img_size=518, seed=1) -> SD:
-    """seeded weights under the names of `dinov2_vitl14_pretrain.pth` (DinoVisionTransformer, ISM/model/vision_transformer.py):
+def make_dinov2_state_dict(embed_dim=1024, depth=24, num_heads=16, patch=14, img_size=518, seed=1, ffn_layer="mlp") -> SD:
+    """seeded weights under the names of `dinov2_vit{s,b,l,g}14_pretrain.pth` (DinoVisionTransformer, ISM/model/vision_transformer.py):
     linear weights ~ trunc-normal-like N(0, 0.02) as the reference initialises them, but NON-trivial biases, LayerNorm affines and
-    LayerScale gammas (the reference's zero / one initial values would hide those code paths)"""
+    LayerScale gammas (the reference's zero / one initial values would hide those code paths).  ffn_layer "mlp" (fc1 / fc2) or
+    "swiglufused" (w12 / w3, hidden (int(4C * 2/3) + 7) // 8 * 8, ISM/model/layers/swiglu_ffn.py:45-63); the defaults draw the
+    ViT-L/14 tensors of tests/golden/dinov2.pt."""
     g = torch.Generator().manual_seed(seed)
     C = embed_dim
     n = (img_size // patch) ** 2
@@ -253,8 +255,13 @@ def make_dinov2_state_dict(embed_dim=1024, depth=24, num_heads=16, patch=14, img
         lin(p + "attn.proj", C, C)
         sd[p + "ls1.gamma"] = 0.5 + torch.rand(C, generator=g)
         ln(p + "norm2")
-        lin(p + "mlp.fc1", 4 * C, C)
-        lin(p + "mlp.fc2", C, 4 * C)
+        if ffn_layer == "swiglufused":
+            hid = (int(4 * C * 2 / 3) + 7) // 8 * 8
+            lin(p + "mlp.w12", 2 * hid, C)
+            lin(p + "mlp.w3", C, hid)
+        else:
+            lin(p + "mlp.fc1", 4 * C, C)
+            lin(p + "mlp.fc2", C, 4 * C)
         sd[p + "ls2.gamma"] = 0.5 + torch.rand(C, generator=g)
     ln("norm")
     return sd
