@@ -199,6 +199,17 @@ int sam6d_project_template_iou(const float* poses, int T, const float* pointclou
                                const long long* pred_obj, const float* translate, const double* K, int N, int H, int W,
                                const long long* boxes, int* image_vu, int* xyxy, float* iou, unsigned char* ok, void* stream);
 
+/* ---- ISM -> PEM hand-off: proposal masks -> uncompressed COCO RLE (ISM/model/utils.py:25-43 mask_to_rle) ------------- */
+
+/* masks (n,H,W) f32, a pixel set iff value > 0 -> the cumulative run ends of every mask's column-major RLE in the
+ * (rle_cum, rle_off) layout of sam6d_inputs_stage_a: the positions k = x*H + y where the pixel differs from position k-1
+ * (k = 0 when pixel (0,0) is set), then H*W.  Two calls: sam6d_mask_rle_count (2 launches) fills col_cnt (n,W) i32 scratch,
+ * band_off (n, ceil(W/32)) i32 and rle_off (n+1) i32, rle_off[n] = total run ends; the host sizes rle_cum from rle_off[n] and
+ * sam6d_mask_rle_write fills it.  n <= 65535, H*W < 2^31. */
+int sam6d_mask_rle_count(const float* masks, int n, int H, int W, int* col_cnt, int* band_off, int* rle_off, void* stream);
+int sam6d_mask_rle_write(const float* masks, int n, int H, int W, const int* col_cnt, const int* band_off, const int* rle_off,
+                         int* rle_cum, void* stream);
+
 /* ---- SAM prompt encoder / mask decoder / automatic mask generator: everything that is not a GEMM
  *      (ISM/segment_anything/modeling/{prompt_encoder,mask_decoder,transformer}.py, automatic_mask_generator.py:225-321,
  *       utils/amg.py:156-176,303-345, modeling/sam.py:133-162) ------------------------------------------------------------ */

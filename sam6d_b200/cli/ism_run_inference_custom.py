@@ -30,7 +30,6 @@ import json
 import os
 import sys
 import time
-from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -169,8 +168,7 @@ def main(argv=None):
     if args.segmentor_model not in ("sam", "fastsam"):
         raise ValueError(f"The segmentor_model {args.segmentor_model} is not supported")
     from PIL import Image
-    from .. import ism, meshio
-    from ..dinov2 import MaskedPatch_MatrixSimilarity
+    from .. import meshio, pipeline
     device = torch.device("cuda")
     os.makedirs(f"{args.output_dir}/sam6d_results", exist_ok=True)
     t_start = time.time()
@@ -178,63 +176,32 @@ def main(argv=None):
     # ---- templates (run_inference_custom.py:129-165) ---------------------------------------------------------------------
     tdir = os.path.join(args.output_dir, "templates")
     n_t = len(glob.glob(f"{tdir}/*.npy")) - int(os.path.exists(os.path.join(tdir, "template_poses.npy")))
-    boxes, masks, templates = [], [], []
-    for idx in range(n_t):
-        image = Image.open(os.path.join(tdir, f"rgb_{idx}.png"))
-        mask = Image.open(os.path.join(tdir, f"mask_{idx}.png"))
-        boxes.append(mask.getbbox())
-        image = torch.from_numpy(np.array(image.convert("RGB")) / 255).float()
-        mask = torch.from_numpy(np.array(mask.convert("L")) / 255).float()
-        templates.append(image * mask[:, :, None])
-        masks.append(mask.unsqueeze(-1))
-    templates = torch.stack(templates).permute(0, 3, 1, 2)
-    masks_t = torch.stack(masks).permute(0, 3, 1, 2)
-    boxes = torch.tensor(np.array(boxes))
-    templates = crop_resize_pad_images(templates, boxes).to(device)
-    masks_cropped = crop_resize_pad_images(masks_t, boxes).to(device)
-    ref_cls, ref_patch = desc.compute_cls_and_patch_features(templates, masks_cropped[:, 0, :, :].contiguous())
-    ref_data = {"descriptors": ref_cls.unsqueeze(0), "appe_descriptors": ref_patch.unsqueeze(0)}
-    # ---- proposals + descriptors + scores (:167-209) ----------------------------------------------------------------------------
-    rgb = np.array(Image.open(args.rgb_path).convert("RGB"))
-    det = seg.generate_masks(rgb)
-    det = SimpleNamespace(masks=det["masks"], boxes=det["boxes"].long())
-    out_json = f"{args.output_dir}/sam6d_results/detection_ism.json"
-    if det.masks.shape[0] == 0:
-        json.dump([], open(out_json, "w"))
-        print("=> no mask proposal survived the filters")
-        return 0
-    q_cls, q_patch = desc(rgb, det)
-    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_data["descriptors"], "avg_5", args.confidence_thresh)
-    det.masks, det.boxes, q_patch = det.masks[idx_sel], det.boxes[idx_sel], q_patch[idx_sel]
-    if idx_sel.numel() == 0:
-        json.dump([], open(out_json, "w"))
-        print("=> no proposal above the semantic-score threshold")
-        return 0
-    ref_aux = ref_data["appe_descriptors"][pred_obj, best_t, ...]
-    appe, vis = MaskedPatch_MatrixSimilarity().scores(q_patch, ref_aux, VISIBLE_THRED)
+    rgbs = np.stack([np.array(Image.open(os.path.join(tdir, f"rgb_{i}.png")).convert("RGB")) for i in range(n_t)])
+    masks = np.stack([np.array(Image.open(os.path.join(tdir, f"mask_{i}.png")).convert("L")) for i in range(n_t)])
+    ref_cls, ref_patch = pipeline.ism_reference_features(desc, rgbs, masks, device)
     pose_path = args.template_poses or os.path.join(tdir, "template_poses.npy")
+    geometry = None
     if os.path.exists(pose_path):
         cam = json.load(open(args.cam_path))
-        depth = torch.from_numpy(np.array(Image.open(args.depth_path)).astype(np.int32)).to(device)
-        K = torch.tensor(np.array(cam["cam_K"]).reshape(3, 3), device=device)
-        poses = torch.tensor(np.load(pose_path)).float().to(device)
         verts, faces, _ = meshio.load_ply(args.cad_path)
-        pc = torch.from_numpy(meshio.sample_surface(verts, faces, 2048) / 1000.0).float().to(device)
-        geo, _, _ = ism.compute_geometric_iou(poses, pc, best_t, torch.zeros_like(best_t), det.masks, depth, K,
-                                              float(np.array(cam["depth_scale"])), det.boxes)
-        final = (sem + appe + geo * vis) / (1 + 1 + vis)
+        geometry = pipeline.ism_geometry(np.load(pose_path), meshio.sample_surface(verts, faces, pipeline.N_ISM_CLOUD) / 1000.0,
+                                         np.array(Image.open(args.depth_path)), cam["cam_K"], cam["depth_scale"], device)
     else:
         print("=> no template poses: final score = (semantic + appearance) / 2", file=sys.stderr)
-        final = (sem + appe) / 2
+    # ---- proposals + descriptors + scores (:167-209) ----------------------------------------------------------------------------
+    rgb = np.array(Image.open(args.rgb_path).convert("RGB"))
+    det = pipeline.ism_detect(seg, desc, ref_cls, ref_patch, rgb, args.confidence_thresh, geometry)
+    out_json = f"{args.output_dir}/sam6d_results/detection_ism.json"
+    if det.reason is not None:
+        json.dump([], open(out_json, "w"))
+        print(f"=> {det.reason}")
+        return 0
     # ---- BOP-23 records (ISM/model/utils.py:153-216) --------------------------------------------------------------------------
+    results = pipeline.ism_records_from_masks(det, time.time() - t_start)
     b = det.boxes.cpu().numpy()
-    m = det.masks.cpu().numpy()
-    runtime = time.time() - t_start
-    results = [dict(scene_id=0, image_id=0, category_id=1, bbox=[int(b[i, 0]), int(b[i, 1]), int(b[i, 2] - b[i, 0]), int(b[i, 3] - b[i, 1])],
-                    score=float(final[i]), time=float(runtime), segmentation=mask_to_rle(m[i] > 0)) for i in range(len(b))]
     np.savez(f"{args.output_dir}/sam6d_results/detection_ism.npz", scene_id=0, image_id=0, category_id=np.ones(len(b), dtype=np.int64),
-             score=final.cpu().numpy(), bbox=np.stack([b[:, 0], b[:, 1], b[:, 2] - b[:, 0], b[:, 3] - b[:, 1]], axis=1), time=runtime,
-             segmentation=m)
+             score=det.scores.cpu().numpy(), bbox=np.stack([b[:, 0], b[:, 1], b[:, 2] - b[:, 0], b[:, 3] - b[:, 1]], axis=1),
+             time=results[0]["time"], segmentation=det.masks.cpu().numpy())
     json.dump(results, open(out_json, "w"))
     print(f"=> {len(results)} detections written to {out_json}")
     return 0

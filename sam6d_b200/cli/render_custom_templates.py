@@ -73,19 +73,8 @@ def to_metres(poses_mm):
 
 def main(argv=None):
     args = get_parser().parse_args(argv)
-    mesh = meshio.load_ply_mesh(args.cad_path)
-    if args.normalize:
-        r = max(np.linalg.norm(mesh.vertices.max(axis=0)), np.linalg.norm(mesh.vertices.min(axis=0)))
-        distance = 4.0 * float(r)
-    else:
-        distance = 2.0
-    if args.colorize:
-        mesh.colors = mesh.uv = mesh.texture = None
-        grey = float(args.base_color)
-    else:
-        grey = BLENDER_DEFAULT_GREY
-    poses = view_poses(distance, args.poses)
-    out = render_views([render.upload(mesh)], poses[None], args.size, [[grey] * 3])
+    from ..pipeline import render_templates
+    out, poses = render_templates(meshio.load_ply_mesh(args.cad_path), args.size, args.normalize, args.colorize, args.base_color, args.poses)
     dropped = int(out["dropped"][0])
     if dropped:
         print(f"=> WARNING: {dropped} triangle views dropped (vertex behind the camera or outside the guard band)")

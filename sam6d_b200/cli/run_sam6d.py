@@ -1,0 +1,72 @@
+"""SAM-6D's demo.sh in one process: render the CAD templates, segment and score the frame (ISM), estimate the poses (PEM),
+with every model built once and no file between the stages (sam6d_b200/pipeline.py: SAM6D).
+
+    python -m sam6d_b200.cli.run_sam6d --cad_path obj.ply --rgb_path rgb.png --depth_path depth.png --cam_path camera.json \\
+        --output_dir OUT [--segmentor_model sam|fastsam] [--checkpoint_dir checkpoints --checkpoint sam-6d-pem-base.pth]
+
+Writes what the chained CLIs write as results: $OUT/sam6d_results/detection_ism.json, detection_pem.json and vis_pem.png,
+with the same records.  It does not write the template files ($OUT/templates/*) nor detection_ism.npz: the npz is an
+intermediate of the reference that nothing downstream reads, and writing it would copy every dense proposal mask to the
+host, which the device-side RLE hand-off exists to avoid.  Random draws use numpy's global RNG in the chained CLIs' order, so
+`np.random.seed(s)` before this CLI gives what `np.random.seed(s)` before the ISM CLI gives the chain."""
+import argparse
+import json
+import os
+import sys
+
+from . import ism_run_inference_custom as ism_cli
+from . import pem_run_inference_custom as pem_cli
+
+
+def get_parser():
+    ap = argparse.ArgumentParser(description="SAM-6D: templates -> ISM -> PEM in one process")
+    ap.add_argument("--segmentor_model", default="sam", choices=("sam", "fastsam"), help="The segmentor model in ISM")
+    ap.add_argument("--output_dir", required=True, help="Path to root directory of the output")
+    ap.add_argument("--cad_path", required=True, help="Path to CAD(mm)")
+    ap.add_argument("--rgb_path", required=True, help="Path to RGB image")
+    ap.add_argument("--depth_path", required=True, help="Path to Depth image(mm)")
+    ap.add_argument("--cam_path", required=True, help="Path to camera information")
+    ap.add_argument("--template_size", default=512, type=int, help="template width and height in pixels (render_custom_templates --size)")
+    # the ISM CLI's options
+    ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
+    ap.add_argument("--checkpoint_dir", default=None, help="the ISM CLI's --checkpoint_dir (SAM / FastSAM and DINOv2 weights)")
+    ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"))
+    ap.add_argument("--dinov2_model", default="dinov2_vitl14", choices=("dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"))
+    ap.add_argument("--points_per_side", default=32, type=int)
+    ap.add_argument("--pred_iou_thresh", default=0.88, type=float)
+    ap.add_argument("--confidence_thresh", default=ism_cli.CONFIDENCE_THRESH, type=float, help="semantic-score threshold")
+    # the PEM CLI's options
+    ap.add_argument("--det_score_thresh", default=0.2, type=float, help="The score threshold of detection")
+    ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth (default: the PEM CLI's)")
+    ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+    ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
+    return ap
+
+
+def main(argv=None):
+    args = get_parser().parse_args(argv)
+    from ..pipeline import SAM6D
+    sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, dinov2_model=args.dinov2_model,
+                  checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
+                  stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
+                  points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
+                  det_score_thresh=args.det_score_thresh, precision=args.precision)
+    obj = sam6d.onboard(args.cad_path, template_size=args.template_size)
+    cam = json.load(open(args.cam_path))
+    rgb = pem_cli.load_im(args.rgb_path).astype("uint8")
+    res = sam6d(rgb, pem_cli.load_im(args.depth_path), cam["cam_K"], cam["depth_scale"], obj)
+    out_dir = os.path.join(args.output_dir, "sam6d_results")
+    os.makedirs(out_dir, exist_ok=True)
+    json.dump(res.ism, open(os.path.join(out_dir, "detection_ism.json"), "w"))
+    with open(os.path.join(out_dir, "detection_pem.json"), "w") as f:
+        json.dump(res.pem, f)
+    if res.reason is not None:
+        print(f"=> {res.reason}")
+    print(f"=> {len(res.ism)} ISM detections, {len(res.pem)} poses written to {out_dir}")
+    if res.pem:
+        pem_cli.write_vis(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -866,3 +866,20 @@ def template_score(Qn: Tensor, Rn: Tensor, want_sim: bool = True):
     bt = torch.zeros(P, dtype=torch.int32, device=dev)
     _lib.call("sam6d_template_score", _p(Qn), _p(Rn), P, O, T, C, _p(sim), _p(obj), _p(bo), _p(bs), _p(bt), _s())
     return sim, obj, bo, bs, bt
+
+
+# ---------------------------------------------------------------------------------------------- ISM -> PEM hand-off
+def mask_rle(masks: Tensor) -> Tuple[Tensor, Tensor]:
+    """masks (n,H,W) f32 (set iff > 0) -> (rle_cum, rle_off) int32 on the device: the cumulative run ends of every mask's
+    uncompressed COCO RLE (mask_to_rle of the ISM CLI), concatenated, and the (n+1) offsets: the layout inputs.pack_rle builds.
+    One 4-byte device-to-host copy (the total) sizes the output."""
+    _check(masks, torch.float32, "masks", 3)
+    n, H, W = masks.shape
+    dev = masks.device
+    col_cnt = torch.empty(n, W, dtype=torch.int32, device=dev)
+    band_off = torch.empty(n, (W + 31) // 32, dtype=torch.int32, device=dev)
+    rle_off = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    _lib.call("sam6d_mask_rle_count", _p(masks), n, H, W, _p(col_cnt), _p(band_off), _p(rle_off), _s())
+    rle_cum = torch.empty(int(rle_off[n]), dtype=torch.int32, device=dev)
+    _lib.call("sam6d_mask_rle_write", _p(masks), n, H, W, _p(col_cnt), _p(band_off), _p(rle_off), _p(rle_cum), _s())
+    return rle_cum, rle_off

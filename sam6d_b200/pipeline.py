@@ -1,0 +1,283 @@
+"""SAM-6D in one process: the stages of the three template / ISM / PEM CLIs as functions on arrays and tensors, and `SAM6D`,
+which keeps the models resident, onboards an object once and runs one RGB-D frame per call.
+
+    from sam6d_b200.pipeline import SAM6D
+    sam6d = SAM6D(segmentor="sam", checkpoint_dir="checkpoints", checkpoint="checkpoints/sam-6d-pem-base.pth")
+    obj = sam6d.onboard("obj_000005.ply")                   # 42 templates rendered on the GPU, ISM + PEM template banks
+    res = sam6d(rgb_u8, depth_u16, cam_K, depth_scale, obj)  # res.ism / res.pem: the CLIs' BOP-23 records; res.R, res.t
+
+The CLIs (sam6d_b200.cli.{render_custom_templates, ism_run_inference_custom, pem_run_inference_custom}) are file I/O around
+the same stage functions, so one `SAM6D` frame computes what the chained CLIs compute from the same inputs and seeds.  Between
+the ISM and the PEM the proposal masks stay on the device: their RLE is built by a kernel (ops.mask_rle) and only the run
+ends come to the host, instead of every (H,W) float mask."""
+import time
+from dataclasses import dataclass
+from types import SimpleNamespace
+from typing import Optional
+
+import numpy as np
+import torch
+
+from . import inputs, ism, meshio, ops, render
+from .cli import ism_run_inference_custom as ism_cli
+from .cli import pem_run_inference_custom as pem_cli
+from .cli import render_custom_templates as render_cli
+
+N_ISM_CLOUD = 2048                     # points of the geometric score's template cloud (ISM/run_inference_custom.py:196)
+
+
+# ---- render + framing (Render/render_custom_templates.py) -----------------------------------------------------------------
+def render_templates(mesh: meshio.Mesh, size: int = 512, normalize: bool = True, colorize: bool = False, base_color: float = 0.05,
+                     poses_file: Optional[str] = None):
+    """the 42 level-0 views of one numpy mesh (mm) -> (render.render()'s dict for one object, poses (T,4,4) float64 in model units).
+    Framing: camera 4r away with --normalize (r = max |bbox corner|), else 2; colours: base_color with colorize, else the
+    mesh's texture / vertex colours / Blender's default grey."""
+    if normalize:
+        r = max(np.linalg.norm(mesh.vertices.max(axis=0)), np.linalg.norm(mesh.vertices.min(axis=0)))
+        distance = 4.0 * float(r)
+    else:
+        distance = 2.0
+    if colorize:
+        mesh.colors = mesh.uv = mesh.texture = None
+        grey = float(base_color)
+    else:
+        grey = render_cli.BLENDER_DEFAULT_GREY
+    poses = render_cli.view_poses(distance, poses_file)
+    out = render_cli.render_views([render.upload(mesh)], poses[None], size, [[grey] * 3])
+    return out, poses
+
+
+def template_arrays(out, o: int = 0):
+    """views of object o of render()'s output -> host arrays as the template files hold them: rgb (T,H,W,3) u8, mask (T,H,W) u8
+    (255 = object), xyz (T,H,W,3) f16 in mm"""
+    return out["rgb"][o].cpu().numpy(), out["mask"][o].cpu().numpy(), out["xyz"][o].cpu().numpy()
+
+
+# ---- ISM template references (ISM/run_inference_custom.py:129-165) ----------------------------------------------------------
+def ism_reference_features(desc, rgbs: np.ndarray, masks: np.ndarray, device):
+    """template views rgb (T,H,W,3) u8 and mask (T,H,W) u8 -> (cls (T,C), masked patch tokens (T,256,C)) of the descriptor model"""
+    boxes, templates, masks_t = [], [], []
+    for rgb, mask in zip(rgbs, masks):
+        ys, xs = np.nonzero(mask)
+        boxes.append((xs.min(), ys.min(), xs.max() + 1, ys.max() + 1))                # PIL Image.getbbox of the mask file
+        image = torch.from_numpy(rgb / 255).float()
+        m = torch.from_numpy(mask / 255).float()
+        templates.append(image * m[:, :, None])
+        masks_t.append(m.unsqueeze(-1))
+    templates = torch.stack(templates).permute(0, 3, 1, 2)
+    masks_t = torch.stack(masks_t).permute(0, 3, 1, 2)
+    boxes = torch.tensor(np.array(boxes))
+    templates = ism_cli.crop_resize_pad_images(templates, boxes).to(device)
+    masks_cropped = ism_cli.crop_resize_pad_images(masks_t, boxes).to(device)
+    return desc.compute_cls_and_patch_features(templates, masks_cropped[:, 0, :, :].contiguous())
+
+
+@dataclass
+class IsmGeometry:
+    """what the geometric score needs: template poses (T,4,4) f32 (metres), template cloud (npc,3) f32 (metres), depth (H,W) i32,
+    K (3,3) as read, depth scale -- all on the device but the scale"""
+    poses: torch.Tensor
+    cloud: torch.Tensor
+    depth: torch.Tensor
+    K: torch.Tensor
+    depth_scale: float
+
+
+def ism_geometry(poses_m, cloud_m, depth_raw, cam_K, depth_scale, device) -> IsmGeometry:
+    """the ISM CLI's conversions: poses and cloud to f32, depth to i32, K as np.array(cam_K) gives it, depth scale to a float"""
+    return IsmGeometry(poses=torch.tensor(poses_m).float().to(device), cloud=torch.from_numpy(cloud_m).float().to(device),
+                       depth=torch.from_numpy(np.asarray(depth_raw).astype(np.int32)).to(device),
+                       K=torch.tensor(np.array(cam_K).reshape(3, 3), device=device), depth_scale=float(np.array(depth_scale)))
+
+
+# ---- segment -> describe -> score (ISM/run_inference_custom.py:167-209) -------------------------------------------------------
+def ism_detect(seg, desc, ref_cls, ref_patch, rgb_u8: np.ndarray, confidence_thresh: float, geometry: Optional[IsmGeometry] = None,
+               mark=None):
+    """-> SimpleNamespace(masks (N,H,W) f32, boxes (N,4) i64 xyxy, scores (N) f32, n_proposals, reason): the proposals above the
+    semantic-score threshold with their final scores ((semantic + appearance + geometric x visible) / (2 + visible), or
+    (semantic + appearance) / 2 without geometry).  reason is None, or why there is no detection.  mark(stage) is called after
+    the segmentor, the descriptors and the scores (stage timing)."""
+    from .dinov2 import MaskedPatch_MatrixSimilarity
+    mark = mark or (lambda stage: None)
+    det = seg.generate_masks(rgb_u8)
+    det = SimpleNamespace(masks=det["masks"], boxes=det["boxes"].long(), scores=None, n_proposals=int(det["masks"].shape[0]), reason=None)
+    mark("segmentor")
+    if det.n_proposals == 0:
+        det.reason = "no mask proposal survived the filters"
+        return det
+    q_cls, q_patch = desc(rgb_u8, det)
+    mark("descriptors")
+    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_cls.unsqueeze(0), "avg_5", confidence_thresh)
+    det.masks, det.boxes, q_patch = det.masks[idx_sel], det.boxes[idx_sel], q_patch[idx_sel]
+    if idx_sel.numel() == 0:
+        det.reason = "no proposal above the semantic-score threshold"
+        mark("scores")
+        return det
+    ref_aux = ref_patch.unsqueeze(0)[pred_obj, best_t, ...]
+    appe, vis = MaskedPatch_MatrixSimilarity().scores(q_patch, ref_aux, ism_cli.VISIBLE_THRED)
+    if geometry is not None:
+        g = geometry
+        geo, _, _ = ism.compute_geometric_iou(g.poses, g.cloud, best_t, torch.zeros_like(best_t), det.masks, g.depth, g.K, g.depth_scale,
+                                              det.boxes)
+        det.scores = (sem + appe + geo * vis) / (1 + 1 + vis)
+    else:
+        det.scores = (sem + appe) / 2
+    mark("scores")
+    return det
+
+
+# ---- BOP-23 records (ISM/model/utils.py:153-216) ----------------------------------------------------------------------------
+def rle_counts(rle_cum: np.ndarray, rle_off: np.ndarray):
+    """cumulative run ends + offsets (ops.mask_rle, inputs.pack_rle) -> every mask's uncompressed COCO RLE counts as int lists,
+    exactly mask_to_rle's (a mask whose pixel (0,0) is set starts with the zero-length run: its first run end is 0)"""
+    return [np.diff(rle_cum[rle_off[i]:rle_off[i + 1]], prepend=0).tolist() for i in range(len(rle_off) - 1)]
+
+
+def ism_records(boxes_xyxy: np.ndarray, scores: np.ndarray, counts, hw, runtime: float):
+    """ISM detections -> the ISM CLI's JSON records (scene 0, image 0, category 1, bbox xywh)"""
+    b = boxes_xyxy
+    return [dict(scene_id=0, image_id=0, category_id=1, bbox=[int(b[i, 0]), int(b[i, 1]), int(b[i, 2] - b[i, 0]), int(b[i, 3] - b[i, 1])],
+                 score=float(scores[i]), time=float(runtime), segmentation={"counts": counts[i], "size": [int(hw[0]), int(hw[1])]})
+            for i in range(len(b))]
+
+
+def ism_records_from_masks(det, runtime: float):
+    """records of ism_detect's detections, RLE on the device: one host copy of the run ends, none of the masks"""
+    cum, off = ops.mask_rle(det.masks.contiguous())
+    return ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), rle_counts(cum.cpu().numpy(), off.cpu().numpy()),
+                       det.masks.shape[1:], runtime)
+
+
+# ---- PEM template bank (PEM/run_inference_custom.py:117-162) -----------------------------------------------------------------
+def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
+    """template views (uint8 rgb, uint8 mask 255 = object, float32 xyz in mm) -> (template points, template features) of the
+    PEM's ViT-B branch"""
+    cfg = pem_cli.TEST_DATASET
+    all_tem, all_tem_pts, all_tem_choose = inputs.get_templates_from_arrays(rgbs, masks, xyzs_mm, cfg["n_sample_template_point"],
+                                                                            cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device)
+    with torch.no_grad():
+        return model.feature_extraction.get_obj_feats(all_tem, all_tem_pts, all_tem_choose)
+
+
+# ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
+def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
+              generator: Optional[torch.Generator] = None, device=None, mark=None):
+    """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
+    enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
+    model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
+    else from torch's global CUDA generator (the reference's torch.rand).  mark(stage) after the inputs and after the forward."""
+    cfg = pem_cli.TEST_DATASET
+    mark = mark or (lambda stage: None)
+    input_data, img, _, model_points, kept = inputs.get_test_data(
+        [dict(d) for d in dets], rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh,
+        cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device)
+    n = input_data["pts"].size(0)
+    mark("pem_inputs")
+    out = None
+    if n:
+        with torch.no_grad():
+            input_data["dense_po"] = bank[0].repeat(n, 1, 1)
+            input_data["dense_fo"] = bank[1].repeat(n, 1, 1)
+            rand = None
+            if generator is not None:
+                rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
+            out = model(input_data, rand=rand)
+    mark("forward")
+    return SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
+
+
+def pem_records(frame):
+    """pem_frame's result -> the PEM CLI's records: the kept ISM records with the pose score, R and t (mm).  The host arrays
+    behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation."""
+    if frame.out is None:
+        return []
+    out = frame.out
+    frame.pose_scores = (out["pred_pose_score"] * out["score"]).detach().cpu().numpy()
+    frame.pred_rot = out["pred_R"].detach().cpu().numpy()
+    frame.pred_trans = out["pred_t"].detach().cpu().numpy() * 1000
+    records = frame.dets
+    for idx in range(len(records)):
+        records[idx]["score"] = float(frame.pose_scores[idx])
+        records[idx]["R"] = list(frame.pred_rot[idx].tolist())
+        records[idx]["t"] = list(frame.pred_trans[idx].tolist())
+    return records
+
+
+# ---- the whole pipeline ----------------------------------------------------------------------------------------------------
+@dataclass
+class Onboarded:
+    """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank, model points"""
+    ref_cls: torch.Tensor
+    ref_patch: torch.Tensor
+    poses_m: np.ndarray
+    cloud_m: np.ndarray
+    bank: tuple
+    model_points_m: np.ndarray
+
+
+class SAM6D:
+    """the SAM-6D models, built once (through the ISM and PEM CLIs' build_models / build_fastsam / build_model, so checkpoint
+    names, seeded weights and thresholds are theirs).  onboard() an object, then call the instance once per RGB-D frame."""
+
+    def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
+                 checkpoint_dir: Optional[str] = None, checkpoint: Optional[str] = None, random_weights: bool = False,
+                 stability_score_thresh: float = 0.97, pred_iou_thresh: float = 0.88, points_per_side: int = 32,
+                 confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
+                 device=None):
+        if segmentor not in ("sam", "fastsam"):
+            raise ValueError(f"The segmentor_model {segmentor} is not supported")
+        self.device = torch.device(device if device is not None else "cuda")
+        self.confidence_thresh = float(confidence_thresh)
+        self.det_score_thresh = float(det_score_thresh)
+        ism_args = SimpleNamespace(segmentor_model=segmentor, sam_model_type=sam_model_type, dinov2_model=dinov2_model,
+                                   checkpoint_dir=checkpoint_dir, random_weights=random_weights,
+                                   stability_score_thresh=stability_score_thresh, pred_iou_thresh=pred_iou_thresh,
+                                   points_per_side=points_per_side)
+        self.seg, self.desc = ism_cli.build_models(ism_args, self.device)
+        self.pem = pem_cli.build_model(SimpleNamespace(precision=precision, checkpoint=checkpoint, random_weights=random_weights), self.device)
+
+    def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None) -> Onboarded:
+        """render the 42 level-0 templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates'
+        framing and colours, and build everything a frame needs from them without touching a file.  Random draws, from `rng`
+        (default numpy's global RNG), in the order the chained CLIs make them: the ISM template cloud, the PEM template
+        samples, the PEM model points."""
+        mesh = meshio.load_ply_mesh(mesh_or_ply_path) if isinstance(mesh_or_ply_path, str) else mesh_or_ply_path
+        verts, faces = mesh.vertices, mesh.faces
+        out, poses = render_templates(mesh, template_size)
+        rgbs, masks, xyzs = template_arrays(out)
+        ref_cls, ref_patch = ism_reference_features(self.desc, rgbs, masks, self.device)
+        cloud = meshio.sample_surface(verts, faces, N_ISM_CLOUD, rng) / 1000.0
+        bank = pem_template_bank(self.pem, list(rgbs), list(masks), [x.astype(np.float32) for x in xyzs], rng=rng, device=self.device)
+        model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
+        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses), cloud, bank, model_points)
+
+    def __call__(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, obj: Onboarded, rng=None, mark=None):
+        """one RGB-D frame: rgb (H,W,3) u8, depth (H,W) raw u16, cam_K (9 values) and depth_scale as camera.json holds them.
+        -> SimpleNamespace(ism, pem: the CLIs' records; masks (N,H,W) f32, boxes (N,4) i64, scores (N) f32 of the ISM detections;
+        R (P,3,3), t (P,3) metres of the PEM's, on the device).  `rng` draws the observed-point samples (default numpy's global
+        RNG); the coarse stage's uniforms come from a fresh torch generator seeded with the PEM's RD_SEED, so a frame's poses
+        do not depend on earlier frames.  mark(stage), when given, is called after each stage (stage timing)."""
+        mark = mark or (lambda stage: None)
+        t0 = time.time()
+        geometry = ism_geometry(obj.poses_m, obj.cloud_m, depth_raw, cam_K, depth_scale, self.device)
+        det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark)
+        if det.reason is not None:
+            mark("rle")
+            mark("ism_records")
+            return SimpleNamespace(ism=[], pem=[], masks=det.masks, boxes=det.boxes, scores=det.scores, R=None, t=None, frame=None,
+                                   n_proposals=det.n_proposals, reason=det.reason)
+        cum, off = ops.mask_rle(det.masks.contiguous())
+        mark("rle")
+        counts = rle_counts(cum.cpu().numpy(), off.cpu().numpy())
+        records = ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), counts, det.masks.shape[1:], time.time() - t0)
+        mark("ism_records")
+        g = torch.Generator(device=self.device)
+        g.manual_seed(pem_cli.RD_SEED)
+        frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
+                          rng=rng, generator=g, device=self.device, mark=mark)
+        pem = pem_records(frame)
+        mark("pem_records")
+        R = frame.out["pred_R"] if frame.out is not None else None
+        t = frame.out["pred_t"] if frame.out is not None else None
+        return SimpleNamespace(ism=records, pem=pem, masks=det.masks, boxes=det.boxes, scores=det.scores, R=R, t=t, frame=frame,
+                               n_proposals=det.n_proposals, reason=None)
