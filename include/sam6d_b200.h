@@ -140,10 +140,10 @@ int sam6d_geo_embed_dist_tc(const float* T, long long npairs, const float* div_t
  * tabD (nd,256) bf16 at step 1/inv_hd) -> E (clouds*S*S,256) bf16 = lerp(tabD, d) + max_k lerp(tabA, a_k), written once.
  * Distances outside tabD: row 0 / column 0 of a cloud read far (clouds,2,S,256) bf16 (exact g_d of those 2 S distances, from
  * sam6d_geo_embed_dist_tc); any other pair is evaluated exactly from div_term (128 f32), WdT (256 in, 256 out) bf16 and bias.
- * precise = 1: interpolation, maximum and sum in fp32 with one rounding at the store; 0: packed bf16x2 arithmetic. */
+ * Interpolation, maximum and sum in fp32 with one rounding at the store. */
 int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const void* tabA, int na, float inv_ha, const void* tabD, int nd,
                         float inv_hd, const void* far, const float* div_term, const void* WdT_bf16, const float* bias, void* E,
-                        int precise, void* stream);
+                        void* stream);
 
 /* ---- PEM input builder (PEM/run_inference_custom.py:165-253 get_test_data; PEM/utils/data_utils.py:73-160) ----------- */
 
@@ -253,9 +253,8 @@ int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const void* x
  * the query: E (B,S,S,256) f32 or bf16, U (B*S rows of 4x256, row stride u_ld) = W_p,h^T q_h  ->  SP (B,4,S,S) */
 int sam6d_rpe_scores(const void* E, int e_is_bf16, const float* U, long long u_ld, int B, int S, float* SP, void* stream);
 /* the same term on TMA + wgmma (bf16 path, the HBM-bound stream over E): E (B,S,S,256) bf16, U (B*S, 4*256) bf16
- * contiguous, S <= 200  ->  SP (B,4,S,S) f32 */
-int sam6d_rpe_scores_tc(const void* E, const void* U, int B, int S, float* SP, void* stream);
-/* the same with padded score rows: SP (B,4,S,sp_ld), sp_ld >= S; with sp_ld a multiple of 4 sam6d_attn_tc_bias_ld streams it */
+ * contiguous, S <= 200  ->  SP (B,4,S,sp_ld) f32 with padded score rows, sp_ld >= S (columns [S, sp_ld) are not written);
+ * with sp_ld a multiple of 4 sam6d_attn_tc_bias_ld streams it */
 int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream);
 /* softmax((Q K^T + bias) * scale) V, head dim 64, Sk <= 256 (MultiHeadAttention :109-148, RPEMultiHeadAttention :369-406) */
 int sam6d_mha(const float* Q, long long q_ld, long long q_bs, const float* K, long long k_ld, long long k_bs, const float* V,

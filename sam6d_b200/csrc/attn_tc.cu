@@ -145,7 +145,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_tc_kernel(const __grid_co
   for (int hr = 0; hr < 2; ++hr) {
     const int r = wg * 64 + tc::frag_row(2 * hr, w, lane), n = n0 + r, nq = min(n, a.Sq - 1);
     const float* brow = nullptr;
-    if (BIAS_MODE == 1 || BIAS_MODE == 3) brow = a.bias + (((size_t)b * a.H + h) * a.Sq + nq) * Sk;
+    if (BIAS_MODE == 1) brow = a.bias + (((size_t)b * a.H + h) * a.Sq + nq) * Sk;
     if (BIAS_MODE == 4) brow = a.bias + (((size_t)b * a.H + h) * a.Sq + nq) * a.bias_ld;
     const float* trow = (BIAS_MODE == 2) ? scr + r * SCR_LD : nullptr;
     const int qh = (BIAS_MODE == 2) ? nq / a.Ws : 0, qw = (BIAS_MODE == 2) ? nq % a.Ws : 0;
@@ -160,7 +160,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_tc_kernel(const __grid_co
         float x = -INFINITY;
         if (c < Sk) {
           x = sacc[4 * j + 2 * hr + e];
-          if (BIAS_MODE == 1 || BIAS_MODE == 3) x += __ldg(brow + c);
+          if (BIAS_MODE == 1) x += __ldg(brow + c);
           if (BIAS_MODE == 4) x += bb[e];
           x *= a.scale;
           if (BIAS_MODE == 2) { const int kh = c / a.Ws, kw = c - kh * a.Ws; x += trow[qh - kh + a.Hs - 1] + trow[32 + qw - kw + a.Ws - 1]; }
@@ -307,12 +307,12 @@ int attn_tc_launch(const void* Q, long long q_ld, int q_col0, const void* K, lon
                    int out_is_bf16, long long out_ld, int k_brows, int k_row0, int v_col0, float* lse, void* stream,
                    long long bias_ld = 0) {
   S6_REQUIRE(Q && K && Vt && out && B >= 0 && H > 0 && Sq > 0 && Sk > 0 && Sk <= MAXK);
-  S6_REQUIRE((head_dim == 64 || head_dim == 80) && bias_mode >= 0 && bias_mode <= 4);
+  S6_REQUIRE((head_dim == 64 || head_dim == 80) && bias_mode >= 0 && bias_mode <= 4 && bias_mode != 3);
   if (bias_mode == 4)
     S6_REQUIRE(bias && head_dim == 64 && bias_ld >= Sk && (bias_ld % 4) == 0 && (reinterpret_cast<uintptr_t>(bias) & 15) == 0);
   S6_REQUIRE((q_ld % 8) == 0 && (k_ld % 8) == 0 && (vt_ld % 8) == 0 && (q_col0 % 8) == 0 && (k_col0 % 8) == 0);
   S6_REQUIRE(k_brows >= k_row0 + Sk && k_row0 >= 0 && v_col0 >= 0 && (v_col0 % 8) == 0);   // TMA boxes start on 16-byte boundaries
-  if (bias_mode == 1 || bias_mode == 3) S6_REQUIRE(bias != nullptr);
+  if (bias_mode == 1) S6_REQUIRE(bias != nullptr);
   if (bias_mode == 2) S6_REQUIRE(rel_h && Hs > 0 && Ws > 0 && Hs <= 16 && Ws <= 16 && Hs * Ws == Sk && Sq == Sk && (reinterpret_cast<uintptr_t>(rel_h) & 15) == 0);
   if (B == 0) return 0;
   S6_REQUIRE(B <= 65535 && H <= 65535);
@@ -331,13 +331,11 @@ int attn_tc_launch(const void* Q, long long q_ld, int q_col0, const void* K, lon
   if (head_dim == 64) {
     if (bias_mode == 0) return ATT_LAUNCH(64, 0);
     if (bias_mode == 1) return ATT_LAUNCH(64, 1);
-    if (bias_mode == 3) return ATT_LAUNCH(64, 3);
     if (bias_mode == 4) return ATT_LAUNCH(64, 4);
     return ATT_LAUNCH(64, 2);
   }
   if (bias_mode == 0) return ATT_LAUNCH(80, 0);
   if (bias_mode == 1) return ATT_LAUNCH(80, 1);
-  if (bias_mode == 3) return ATT_LAUNCH(80, 3);
   return ATT_LAUNCH(80, 2);
 #undef ATT_LAUNCH
 }

@@ -13,8 +13,8 @@
 //
 // Kernel: persistent, 16 warps per CTA (two pairs in flight per warp), both tables resident in shared memory.  A warp takes 32 consecutive pairs: lane l loads
 // the indices of pair l (one coalesced 512-byte read), then for each pair the four indices are broadcast by shuffles and lane l
-// interpolates channels [8l, 8l+8) as four packed bf16x2 words per table row (sub / fma / max / add on bf16x2: the same packed
-// arithmetic the tensor-core epilogue used), one 16-byte store per lane = one 512-byte row of E per warp instruction.
+// interpolates channels [8l, 8l+8) in fp32 (interpolation, maximum and sum; ONE rounding to bf16 at the store), one 16-byte store
+// per lane = one 512-byte row of E per warp instruction.
 // Bounds per 64-cloud call: E write 1.27 GB (HBM), 4 KB of table reads per pair (shared-memory bandwidth), ~70 warp
 // instructions per pair.
 //
@@ -26,33 +26,10 @@
 // hence the [0, 32) span), so the kernel is correct for any input and fast for the clouds the model produces.
 #include <cuda_bf16.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace {
 
-
-__device__ __forceinline__ uint32_t bf2_sub(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
-__device__ __forceinline__ uint32_t bf2_fma(uint32_t a, uint32_t b, uint32_t c) {
-  uint32_t d;
-  asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-  return d;
-}
-__device__ __forceinline__ uint32_t bf2_max(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("max.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
-__device__ __forceinline__ uint32_t bf2_add(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
 __device__ __forceinline__ uint32_t bf2_pack(float lo, float hi) {
   __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
@@ -67,17 +44,8 @@ __device__ __forceinline__ void lut_pos(float x, float inv_h, int nent, int& row
   t = u - (float)i;
   row = i * 32;
 }
-// linear interpolation between table rows `row` and `row + 1`: lane's 8 channels of g(x), packed bf16x2 arithmetic (t2 = (t, t))
-__device__ __forceinline__ uint4 lut_lerp(const uint4* __restrict__ tab, int row, uint32_t t2) {
-  const uint4 lo = tab[row], hi = tab[row + 32];
-  uint4 r;
-  r.x = bf2_fma(t2, bf2_sub(hi.x, lo.x), lo.x);
-  r.y = bf2_fma(t2, bf2_sub(hi.y, lo.y), lo.y);
-  r.z = bf2_fma(t2, bf2_sub(hi.z, lo.z), lo.z);
-  r.w = bf2_fma(t2, bf2_sub(hi.w, lo.w), lo.w);
-  return r;
-}
-// the same interpolation in fp32 (table entries unpacked, no intermediate rounding): 8 channels as floats
+// linear interpolation between table rows `row` and `row + 1` in fp32 (table entries unpacked, no intermediate rounding): lane's
+// 8 channels of g(x)
 __device__ __forceinline__ void lut_lerp_f32(const uint4* __restrict__ tab, int row, float t, float v[8]) {
   const uint4 lo = tab[row], hi = tab[row + 32];
   const uint32_t l[4] = {lo.x, lo.y, lo.z, lo.w}, h[4] = {hi.x, hi.y, hi.z, hi.w};
@@ -121,11 +89,10 @@ __device__ __noinline__ uint4 slow_distance(float x, const float* __restrict__ d
   return make_uint4(bf2_pack(acc[0], acc[1]), bf2_pack(acc[2], acc[3]), bf2_pack(acc[4], acc[5]), bf2_pack(acc[6], acc[7]));
 }
 
-// PRECISE: interpolation, maximum and sum in fp32, ONE rounding to bf16 at the store (rms error 1.2e-3 against 1.6e-3 for the packed
-// bf16x2 arithmetic, at about twice the instructions per pair)
-// LUT_THREADS / UNROLL: warps per CTA against pairs in flight per warp (the kernel is bound by the shared-memory pipe, warps waiting
-// on their LDS results)
-template <bool PRECISE, int LUT_THREADS, int UNROLL>
+// fp32 arithmetic was chosen over a packed bf16x2 form of the same kernel, which had rms error 1.6e-3 against 1.2e-3 (emulated in
+// torch at step 1/8) at about half the instructions per pair.  LUT_THREADS / UNROLL: warps per CTA against pairs in flight per warp (the kernel is bound by the
+// shared-memory pipe, warps waiting on their LDS results); 16 x 2 was chosen by measurement over 32 x 1 and 24 x 2.
+constexpr int LUT_THREADS = 512, UNROLL = 2;
 __global__ void __launch_bounds__(LUT_THREADS, 1) geo_embed_lut_kernel(const float4* __restrict__ T, long long npairs, int S,
                                                                       const uint4* __restrict__ tabA_g, int na, float inv_ha,
                                                                       const uint4* __restrict__ tabD_g, int nd, float inv_hd,
@@ -155,10 +122,6 @@ __global__ void __launch_bounds__(LUT_THREADS, 1) geo_embed_lut_kernel(const flo
     lut_pos(tv.z, inv_ha, na, r2, t2);
     lut_pos(tv.w, inv_hd, nd, r3, t3);
     if (!(tv.w < d_limit)) r3 = -1;
-    if constexpr (!PRECISE) {                              // the packed variant broadcasts the weight as a bf16x2 word
-      t0 = __uint_as_float(bf2_pack(t0, t0)); t1 = __uint_as_float(bf2_pack(t1, t1));
-      t2 = __uint_as_float(bf2_pack(t2, t2)); t3 = __uint_as_float(bf2_pack(t3, t3));
-    }
     const uint4* tabA_l = tabA + lane;
     const uint4* tabD_l = tabD + lane;
 #pragma unroll UNROLL
@@ -177,27 +140,15 @@ __global__ void __launch_bounds__(LUT_THREADS, 1) geo_embed_lut_kernel(const flo
         else if (m == 0) dv = far[((c * 2 + 1) * S + n) * 32 + lane];
         else dv = slow_distance(__shfl_sync(0xffffffffu, tv.w, j), div_term, WdT, bias, lane);
       }
-      uint4 o;
-      if constexpr (PRECISE) {
-        float f0[8], f1[8], f2[8], fd[8];
-        lut_lerp_f32(tabA_l, q0, w0, f0);
-        lut_lerp_f32(tabA_l, q1, w1, f1);
-        lut_lerp_f32(tabA_l, q2, w2, f2);
-        if (in_table) lut_lerp_f32(tabD_l, q3, w3, fd);
-        else unpack8(dv, fd);
+      float f0[8], f1[8], f2[8], fd[8];
+      lut_lerp_f32(tabA_l, q0, w0, f0);
+      lut_lerp_f32(tabA_l, q1, w1, f1);
+      lut_lerp_f32(tabA_l, q2, w2, f2);
+      if (in_table) lut_lerp_f32(tabD_l, q3, w3, fd);
+      else unpack8(dv, fd);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) fd[k] += fmaxf(fmaxf(f0[k], f1[k]), f2[k]);
-        o = make_uint4(bf2_pack(fd[0], fd[1]), bf2_pack(fd[2], fd[3]), bf2_pack(fd[4], fd[5]), bf2_pack(fd[6], fd[7]));
-      } else {
-        const uint4 v0 = lut_lerp(tabA_l, q0, __float_as_uint(w0));
-        const uint4 v1 = lut_lerp(tabA_l, q1, __float_as_uint(w1));
-        const uint4 v2 = lut_lerp(tabA_l, q2, __float_as_uint(w2));
-        if (in_table) dv = lut_lerp(tabD_l, q3, __float_as_uint(w3));
-        o.x = bf2_add(dv.x, bf2_max(bf2_max(v0.x, v1.x), v2.x));
-        o.y = bf2_add(dv.y, bf2_max(bf2_max(v0.y, v1.y), v2.y));
-        o.z = bf2_add(dv.z, bf2_max(bf2_max(v0.z, v1.z), v2.z));
-        o.w = bf2_add(dv.w, bf2_max(bf2_max(v0.w, v1.w), v2.w));
-      }
+      for (int k = 0; k < 8; ++k) fd[k] += fmaxf(fmaxf(f0[k], f1[k]), f2[k]);
+      const uint4 o = make_uint4(bf2_pack(fd[0], fd[1]), bf2_pack(fd[2], fd[3]), bf2_pack(fd[4], fd[5]), bf2_pack(fd[6], fd[7]));
       E[(base + j) * 32 + lane] = o;
     }
   }
@@ -207,11 +158,11 @@ __global__ void __launch_bounds__(LUT_THREADS, 1) geo_embed_lut_kernel(const flo
 
 // T (clouds*S*S, 4) f32 = (a0, a1, a2, d) indices of every pair; tabA (na, 256) bf16 = W_a emb(i / inv_ha), tabD (nd, 256) bf16 =
 // W_d emb(i / inv_hd) + bias; far (clouds, 2, S, 256) bf16 = exact g_d of row 0 ([:,0]) and column 0 ([:,1]) of every cloud;
-// div_term (128) f32, WdT (256 in, 256 out) bf16 and bias (256) f32 for the exact fallback of other out-of-table distances;
-// precise: 1 = fp32 interpolation with one final rounding, 0 = packed bf16x2 arithmetic  -> E (clouds*S*S, 256) bf16
+// div_term (128) f32, WdT (256 in, 256 out) bf16 and bias (256) f32 for the exact fallback of other out-of-table distances
+// -> E (clouds*S*S, 256) bf16
 S6_API int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const void* tabA, int na, float inv_ha, const void* tabD, int nd,
                                float inv_hd, const void* far, const float* div_term, const void* WdT_bf16, const float* bias, void* E,
-                               int precise, void* stream) {
+                               void* stream) {
   S6_REQUIRE(T && tabA && tabD && far && div_term && WdT_bf16 && bias && E && clouds >= 0 && S > 0 && na >= 2 && nd >= 2);
   S6_REQUIRE(inv_ha > 0.f && inv_hd > 0.f && (long long)(na + nd) * 512 <= 200 * 1024);
   S6_REQUIRE(((reinterpret_cast<uintptr_t>(T) | reinterpret_cast<uintptr_t>(tabA) | reinterpret_cast<uintptr_t>(tabD) | reinterpret_cast<uintptr_t>(far) |
@@ -223,31 +174,12 @@ S6_API int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const vo
   S6_CHECK(cudaGetDevice(&dev));
   S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int smem = (na + nd) * 512;
-  // launch shape (SAM6D_GEO_LUT_CFG): 1 = 16 warps x 2 pairs in flight per warp (default); 0 = 32 warps x 1 pair; 2 = 24 warps x
-  // 2 pairs
-  static const int cfg = [] { const char* e = getenv("SAM6D_GEO_LUT_CFG"); return e ? atoi(e) : 1; }();
-  const long long nblocks = (npairs + 31) / 32;
-  cudaStream_t st = s6_stream(stream);
-#define S6_LUT_LAUNCH(P, TH, UN)                                                                                                    \
-  do {                                                                                                                               \
-    auto kern = geo_embed_lut_kernel<P, TH, UN>;                                                                                     \
-    S6_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                                         \
-    const long long want = (nblocks + TH / 32 - 1) / (TH / 32);                                                                     \
-    const int grid = (int)(want < sms ? want : sms);                                                                                 \
-    kern<<<grid, TH, smem, st>>>(reinterpret_cast<const float4*>(T), npairs, S, reinterpret_cast<const uint4*>(tabA), na, inv_ha,     \
-                                 reinterpret_cast<const uint4*>(tabD), nd, inv_hd, reinterpret_cast<const uint4*>(far), div_term,  \
-                                 reinterpret_cast<const uint4*>(WdT_bf16), bias, reinterpret_cast<uint4*>(E));                       \
-  } while (0)
-  if (precise) {
-    if (cfg == 0) S6_LUT_LAUNCH(true, 1024, 1);
-    else if (cfg == 2) S6_LUT_LAUNCH(true, 768, 2);
-    else S6_LUT_LAUNCH(true, 512, 2);
-  } else {
-    if (cfg == 0) S6_LUT_LAUNCH(false, 1024, 1);
-    else if (cfg == 2) S6_LUT_LAUNCH(false, 768, 2);
-    else S6_LUT_LAUNCH(false, 512, 2);
-  }
-#undef S6_LUT_LAUNCH
+  S6_CHECK(cudaFuncSetAttribute(geo_embed_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const long long nblocks = (npairs + 31) / 32, want = (nblocks + LUT_THREADS / 32 - 1) / (LUT_THREADS / 32);
+  const int grid = (int)(want < sms ? want : sms);
+  geo_embed_lut_kernel<<<grid, LUT_THREADS, smem, s6_stream(stream)>>>(
+      reinterpret_cast<const float4*>(T), npairs, S, reinterpret_cast<const uint4*>(tabA), na, inv_ha, reinterpret_cast<const uint4*>(tabD),
+      nd, inv_hd, reinterpret_cast<const uint4*>(far), div_term, reinterpret_cast<const uint4*>(WdT_bf16), bias, reinterpret_cast<uint4*>(E));
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -11,8 +11,6 @@
 // BatchNorm is folded into the 1x1 convs on the host.  The (B,6,N,ns) grouped tensor and the (B,128,N,ns) activations of the
 // reference are never materialised; padded duplicate samples are simply recomputed (they cannot change a max).
 // Four CTAs share an SM (49 KB smem each), so one tile's serial chain hides behind the others'.
-#include <cstdlib>
-
 #include "tc.cuh"
 
 namespace {
@@ -198,8 +196,7 @@ S6_API int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, i
     S6_CHECK(cudaFuncSetAttribute(pe_tc_kernel<NSV, OT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));                     \
     /* four CTAs per SM: 4 x (49 KB + static) shared memory, 4 x 128 x 128 registers.  (The occupancy API is not used: with   */   \
     /* the default carve-out it answers fewer and the grid shrinks.)                                                             */   \
-    int per_sm = 4;                                                                                                                 \
-    if (const char* ev = getenv("SAM6D_PE_CTAS")) per_sm = atoi(ev) > 0 && atoi(ev) < per_sm ? atoi(ev) : per_sm;                   \
+    const int per_sm = 4;                                                                                                           \
     const int grid = (int)(ntiles < (long long)sms * per_sm ? ntiles : (long long)sms * per_sm);                                    \
     pe_tc_kernel<NSV, OT><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(pts, idx, N, total, W1, B1, W2, B2, W3, B3,                         \
                                                                  reinterpret_cast<OT*>(out), out_ld, out_off);                      \

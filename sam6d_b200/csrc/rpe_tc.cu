@@ -148,9 +148,10 @@ int make_map(CUtensorMap* map, const void* ptr, long long rows, int box_rows) {
 }  // namespace
 
 // E (B,S,S,256) bf16 contiguous, U (B*S, 4*256) bf16 contiguous (row = the four folded per-head queries of a token)
-// -> SP (B,4,S,S) fp32.  S <= 200.  The wgmma / TMA form of sam6d_rpe_scores (PEM/model/transformer.py:369-399).
-namespace {
-int rpe_scores_tc_launch(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream) {
+// -> SP (B,4,S,sp_ld) fp32, sp_ld >= S (columns [S, sp_ld) are left untouched).  S <= 200.  The wgmma / TMA form of
+// sam6d_rpe_scores (PEM/model/transformer.py:369-399); with sp_ld a multiple of 4 the attention kernel can stream the planes
+// with 16-byte copies (sam6d_attn_tc_bias_ld)
+S6_API int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream) {
   S6_REQUIRE(E && U && SP && B >= 0 && S > 0 && S <= SLAB_ROWS && sp_ld >= S);
   S6_REQUIRE((reinterpret_cast<uintptr_t>(E) & 15) == 0 && (reinterpret_cast<uintptr_t>(U) & 15) == 0);
   S6_REQUIRE((long long)B * S * S < 2000000000LL);
@@ -168,14 +169,4 @@ int rpe_scores_tc_launch(const void* E, const void* U, int B, int S, float* SP, 
   S6_CHECK(s6_launch_pdl(rpe_scores_tc_kernel, dim3(grid), dim3(THREADS), SMEM, s6_stream(stream), tmE, tmU, S, total, SP, sp_ld));
   S6_LAUNCH_CHECK();
   return 0;
-}
-}  // namespace
-
-S6_API int sam6d_rpe_scores_tc(const void* E, const void* U, int B, int S, float* SP, void* stream) {
-  return rpe_scores_tc_launch(E, U, B, S, SP, S, stream);
-}
-// the same with padded score rows: SP (B,4,S,sp_ld), sp_ld >= S (columns [S, sp_ld) are left untouched); with sp_ld a multiple
-// of 4 the attention kernel can stream the planes with 16-byte copies (sam6d_attn_tc_bias_ld)
-S6_API int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream) {
-  return rpe_scores_tc_launch(E, U, B, S, SP, sp_ld, stream);
 }

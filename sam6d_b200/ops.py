@@ -456,7 +456,7 @@ def geo_embed_dist_tc(T: Tensor, div_term: Tensor, Wd_bf16: Tensor, bias: Tensor
 
 
 def geo_embed_lut(T: Tensor, tabA: Tensor, inv_ha: float, tabD: Tensor, inv_hd: float, far: Tensor, div_term: Tensor, WdT_bf16: Tensor,
-                  bias: Tensor, precise: bool = True) -> Tensor:
+                  bias: Tensor) -> Tensor:
     """table-interpolation geometric embedding (csrc/geo_lut.cu): T (B,S,S,4) f32, tabA (na,256) / tabD (nd,256) bf16,
     far (B,2,S,256) bf16 -> E (B,S,S,256) bf16"""
     _check(T, torch.float32, "T", 4)
@@ -469,7 +469,7 @@ def geo_embed_lut(T: Tensor, tabA: Tensor, inv_ha: float, tabD: Tensor, inv_hd: 
         raise RuntimeError("geo_embed_lut: shape mismatch")
     E = torch.empty(b, s, s, 256, dtype=torch.bfloat16, device=T.device)
     _lib.call("sam6d_geo_embed_lut", _p(T), _ll(b), s, _p(tabA), tabA.shape[0], _f(inv_ha), _p(tabD), tabD.shape[0], _f(inv_hd), _p(far),
-              _p(div_term), _p(WdT_bf16), _p(bias), _p(E), int(bool(precise)), _s())
+              _p(div_term), _p(WdT_bf16), _p(bias), _p(E), _s())
     return E
 
 
@@ -488,31 +488,25 @@ def rpe_scores(E: Tensor, U: Tensor, u_ptr: Optional[int] = None, u_ld: int = 10
     return SP
 
 
-def rpe_scores_tc(E: Tensor, U: Tensor) -> Tensor:
-    """E (B,S,S,256) bf16, U (B*S, 1024) bf16 = the four folded per-head queries of every token -> (B,4,S,S) f32.
-    TMA + wgmma stream over E (csrc/rpe_tc.cu); S <= 200."""
+def rpe_scores_tc(E: Tensor, U: Tensor, ld: Optional[int] = None) -> Tensor:
+    """E (B,S,S,256) bf16, U (B*S, 1024) bf16 = the four folded per-head queries of every token -> (B,4,S,ld) f32 score
+    planes with row stride ld >= S (default S; columns [S, ld) are not written).  TMA + wgmma stream over E (csrc/rpe_tc.cu);
+    S <= 200."""
     _check(E, torch.bfloat16, "E", 4)
     _check(U, torch.bfloat16, "U", 2)
     B, S = E.shape[0], E.shape[1]
     if U.shape != (B * S, 1024) or E.shape[3] != 256 or E.shape[2] != S:
         raise RuntimeError("rpe_scores_tc: E (B,S,S,256), U (B*S,1024)")
-    SP = torch.empty(B, 4, S, S, dtype=torch.float32, device=E.device)
-    _lib.call("sam6d_rpe_scores_tc", _p(E), _p(U), B, S, _p(SP), _s())
+    ld = S if ld is None else ld
+    SP = torch.empty(B, 4, S, ld, dtype=torch.float32, device=E.device)
+    _lib.call("sam6d_rpe_scores_tc_ld", _p(E), _p(U), B, S, _p(SP), int(ld), _s())
     return SP
 
 
 def rpe_scores_tc_padded(E: Tensor, U: Tensor) -> Tensor:
-    """rpe_scores_tc into planes whose rows are padded to a multiple of 16 keys: returns the (B,4,S,ld) f32 buffer (columns
-    [S, ld) are not written); attn_tc_padded_bias consumes it with 16-byte copies"""
-    _check(E, torch.bfloat16, "E", 4)
-    _check(U, torch.bfloat16, "U", 2)
-    B, S = E.shape[0], E.shape[1]
-    if U.shape != (B * S, 1024) or E.shape[3] != 256 or E.shape[2] != S:
-        raise RuntimeError("rpe_scores_tc: E (B,S,S,256), U (B*S,1024)")
-    ld = (S + 15) // 16 * 16
-    SP = torch.empty(B, 4, S, ld, dtype=torch.float32, device=E.device)
-    _lib.call("sam6d_rpe_scores_tc_ld", _p(E), _p(U), B, S, _p(SP), int(ld), _s())
-    return SP
+    """rpe_scores_tc into planes whose rows are padded to a multiple of 16 keys; attn_tc_padded_bias consumes them with
+    16-byte copies"""
+    return rpe_scores_tc(E, U, ld=(E.shape[1] + 15) // 16 * 16)
 
 
 def attn_tc_padded_bias(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tensor, B: int, H: int, Sq: int, Sk: int, D: int,
@@ -574,7 +568,7 @@ def attn_global_tc(qkv: Tensor, vt: Tensor, rel_blob: Tensor, B: int, H: int, gr
 
 def attn_tc(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tensor, B: int, H: int, Sq: int, Sk: int, D: int, scale: float,
             bias: Optional[Tensor] = None, rel: Optional[tuple] = None, bv: Optional[Tensor] = None,
-            out_dtype=torch.float32, bias_variant: int = 1) -> Tensor:
+            out_dtype=torch.float32) -> Tensor:
     """tensor-core attention (<= 256 keys).  Q, K: bf16 2-D matrices (rows = batch*tokens); Vt: bf16 (B*H*D, >= ceil16(Sk));
     bias: dense fp32 (B,H,Sq,Sk); rel = (rel_h, rel_w, Hs, Ws) for the decomposed rel-pos bias.  -> (B*Sq, H*D) fp32"""
     _check(Q, torch.bfloat16, "Q", 2)
@@ -583,7 +577,7 @@ def attn_tc(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tensor, B: int, 
     mode, rh, rw, Hs, Ws = 0, None, None, 0, 0
     if bias is not None:
         _check(bias, torch.float32, "bias", 4)
-        mode = bias_variant
+        mode = 1
     elif rel is not None:
         rh, Hs, Ws = rel                     # rh: pack_rel_pos(rel_pos_h, rel_pos_w)
         mode = 2

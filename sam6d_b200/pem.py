@@ -13,7 +13,6 @@ hand-written sm_90a kernels through the C ABI (sam6d_b200/ops.py); inference onl
 losses, pose-noise augmentation -- are out of scope), and there is no CPU path.
 """
 import math
-import os
 from types import SimpleNamespace
 from typing import Dict, Optional
 
@@ -28,15 +27,10 @@ NUM_HEADS = 4  # hard-coded in the reference (coarse_point_matching.py:31, fine_
 # "bf16": wgmma tensor-core kernels -- operands rounded to bf16, fp32 accumulation in registers, geometric embedding stored
 # in bf16.  Index-valued results (FPS, ball query, labels) and the pose solvers are identical in both modes.
 PRECISIONS = ("fp32", "bf16")
-# bf16 path: linear + residual + LayerNorm + FFN + LayerNorm of every transformer layer as one kernel (csrc/tail_tc.cu);
-# False = the five-launch form (GEMM, LayerNorm, GEMM, GEMM, LayerNorm) kept as its comparator
-FUSED_TAIL = os.environ.get("SAM6D_FUSED_TAIL", "1") != "0"
-# the relative-position score stream over E on TMA + wgmma (csrc/rpe_tc.cu); False = the CUDA-core kernel (csrc/attn.cu)
-PADDED_BIAS = os.environ.get("SAM6D_PADDED_BIAS", "1") != "0"
-RPE_TC = os.environ.get("SAM6D_RPE_TC", "1") != "0"
-# bf16 path: the geometric embedding by table interpolation (csrc/geo_lut.cu); False = the wgmma projections (csrc/geo_tc.cu)
-GEO_LUT = os.environ.get("SAM6D_GEO_LUT", "1") != "0"
-GEO_LUT_PRECISE = os.environ.get("SAM6D_GEO_LUT_PRECISE", "1") != "0"   # fp32 interpolation, one rounding at the store
+# bf16 self-attention: TMA + wgmma score stream into padded planes (csrc/rpe_tc.cu); bench.py reads these to name the kernels it times
+RPE_TC = True
+PADDED_BIAS = True
+# bf16 path: the geometric embedding by table interpolation (csrc/geo_lut.cu)
 GEO_LUT_INV_H = 8.0            # table step 1/8 index unit
 GEO_LUT_D_MAX = 32.0           # distance indices below this come from the table: 6.4 object radii (the reference's input builder
                                # keeps scene points within 1.2 radii of the mask centroid: indices <= 12)
@@ -155,11 +149,18 @@ def _attn_tail(prec, x2d: torch.Tensor, hid: torch.Tensor, lw) -> torch.Tensor:
     return ops.layernorm(z, lw["g2"], lw["b2"])
 
 
-def _pack_tail(layer: _TransformerLayerParams) -> Dict[str, torch.Tensor]:
+def _pack_tail(layer: nn.Module) -> Dict[str, torch.Tensor]:
+    """the tail weights of a _TransformerLayerParams or _LinearTransformerLayerParams (same attention.linear/norm, output.*)"""
     a, o = layer.attention, layer.output
     return dict(wo=_W(a.linear.weight), bo=_f32(a.linear.bias), g1=_f32(a.norm.weight), b1=_f32(a.norm.bias),
                 we=_W(o.expand.weight), be=_f32(o.expand.bias), ws=_W(o.squeeze.weight), bs=_f32(o.squeeze.bias),
                 g2=_f32(o.norm.weight), b2=_f32(o.norm.bias))
+
+
+def _tail_bf16(x2d: torch.Tensor, hid: torch.Tensor, lw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """_attn_tail for the bf16 token stream as one kernel (csrc/tail_tc.cu): x2d, hid, out (M,256) bf16"""
+    return ops.transformer_tail_bf16(hid, x2d, lw["wo"].bf16, lw["bo"], lw["g1"], lw["b1"], lw["we"].bf16, lw["be"],
+                                     lw["ws"].bf16, lw["bs"], lw["g2"], lw["b2"], out=out)
 
 
 class GeometricTransformer(nn.Module):
@@ -198,7 +199,6 @@ class GeometricTransformer(nn.Module):
                 w_self=_W(w_self), b_self=b_self.contiguous(), tail_self=_pack_tail(self.layers[0]),
                 # tensor-core attention path: q|k|v as one bf16 GEMM, the folded rel-pos queries u as a second (fp32) one
                 w_qkv=_W(w_self[:3 * C]), b_qkv=b_self[:3 * C].contiguous(), w_u=_W(w_self[3 * C:]), b_u=b_self[3 * C:].contiguous(),
-                wq_only=_W(ca.proj_q.weight),
                 wq_c=_W(ca.proj_q.weight), bq_c=_f32(ca.proj_q.bias),
                 wkv_c=_W(torch.cat([_f32(ca.proj_k.weight), _f32(ca.proj_v.weight)], dim=0)),
                 bkv_c=torch.cat([_f32(ca.proj_k.bias), _f32(ca.proj_v.bias)], dim=0).contiguous(),
@@ -249,38 +249,23 @@ class GeometricTransformer(nn.Module):
 
     # ---- bf16 token stream (precision="bf16", both clouds in one allocation): every Linear is the persistent TMA GEMM, the
     # residual stream, LayerNorm inputs/outputs and the attention output are bf16, accumulation and statistics fp32.
-    def _tail_bf16(self, x2d, hid, lw, out=None):
-        if FUSED_TAIL:
-            return ops.transformer_tail_bf16(hid, x2d, lw["wo"].bf16, lw["bo"], lw["g1"], lw["b1"], lw["we"].bf16, lw["be"],
-                                             lw["ws"].bf16, lw["bs"], lw["g2"], lw["b2"], out=out)
-        bf = torch.bfloat16
-        y = ops.gemm_tma(hid, lw["wo"].bf16, lw["bo"], residual=x2d, out_dtype=bf)
-        y = ops.layernorm_bf16io(y, lw["g1"], lw["b1"])
-        h = ops.gemm_tma(y, lw["we"].bf16, lw["be"], act=1, out_dtype=bf)
-        z = ops.gemm_tma(h, lw["ws"].bf16, lw["bs"], residual=y, out_dtype=bf)
-        return ops.layernorm_bf16io(z, lw["g2"], lw["b2"], out=out)
-
     def _self_bf16(self, x, emb, w):
         B, S, C = x.shape
         d = C // NUM_HEADS
         x2d = x.view(B * S, C)
-        if RPE_TC and S <= 200 and emb.dtype == torch.bfloat16:
+        if S <= 200 and emb.dtype == torch.bfloat16:
             # ONE projection launch: (q | k) rows, V^T, and the folded rel-pos queries u as bf16 rows = the B operand of the TMA /
             # wgmma stream over E (csrc/rpe_tc.cu)
             qk, vt, u = ops.gemm_tma_vt2(x2d, w["w_self"].bf16, w["b_self"], 2 * C, 3 * C, S)
-            if PADDED_BIAS:
-                # score planes with 16-key padded rows: the attention kernel streams them with 16-byte cp.async copies
-                sp = ops.rpe_scores_tc_padded(emb, u)
-                hid = ops.attn_tc_padded_bias(qk, 0, qk, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), sp)
-                return self._tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
-            sp = ops.rpe_scores_tc(emb, u)
-            hid = ops.attn_tc(qk, 0, qk, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), bias=sp, out_dtype=torch.bfloat16)
-            return self._tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
+            # score planes with 16-key padded rows: the attention kernel streams them with 16-byte cp.async copies
+            sp = ops.rpe_scores_tc_padded(emb, u)
+            hid = ops.attn_tc_padded_bias(qk, 0, qk, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), sp)
+            return _tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
         qk, vt = ops.gemm_tma_vt(x2d, w["w_qkv"].bf16, w["b_qkv"], 2 * C, S)                        # (B*S, q|k) and V^T
         u = ops.gemm_tma(x2d, w["w_u"].bf16, w["b_u"])                                              # (B*S, 4*C) fp32
         sp = ops.rpe_scores(emb, None, u_ptr=u.data_ptr(), u_ld=NUM_HEADS * C)
         hid = ops.attn_tc(qk, 0, qk, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), bias=sp, out_dtype=torch.bfloat16)
-        return self._tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
+        return _tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
 
     def _forward_bf16(self, f, emb, w):
         """f (2B,S,C) bf16 = [cloud 0 ; cloud 1], emb (2B,S,S,256) -> same layout"""
@@ -295,11 +280,11 @@ class GeometricTransformer(nn.Module):
         kq, vt_all = ops.gemm_tma_vt(f.view(2 * B * S, C), w["wkqv_c"].bf16, w["bkqv_c"], 2 * C, S, slot=1)
         kq1, vt1 = kq[B * S:], vt_all[B * C:]
         hid = ops.attn_tc(kq, C, kq1, 0, vt1, B, NUM_HEADS, S, S, d, scale, out_dtype=torch.bfloat16)
-        self._tail_bf16(x0, hid, w["tail_cross"], out=out[:B].view(B * S, C))
+        _tail_bf16(x0, hid, w["tail_cross"], out=out[:B].view(B * S, C))
         # cross layer 1: cloud 1 attends to the updated cloud 0 (sequential, transformer.py:505-507)
         k0, vt0 = ops.gemm_tma_vt(out[:B].view(B * S, C), w["wkv_c"].bf16, w["bkv_c"], C, S, slot=2)
         hid = ops.attn_tc(kq1, C, k0, 0, vt0, B, NUM_HEADS, S, S, d, scale, out_dtype=torch.bfloat16)
-        self._tail_bf16(x1, hid, w["tail_cross"], out=out[B:].view(B * S, C))
+        _tail_bf16(x1, hid, w["tail_cross"], out=out[B:].view(B * S, C))
         return out
 
     @torch.no_grad()
@@ -358,7 +343,6 @@ class GeometricStructureEmbedding(nn.Module):
         if self._packed.key != key:
             self._packed.w = dict(div=_f32(self.embedding.div_term), waT=_f32(self.proj_a.weight).t().contiguous(),
                                   wdT=_f32(self.proj_d.weight).t().contiguous(),
-                                  wa_bf=_f32(self.proj_a.weight).to(torch.bfloat16).contiguous(),
                                   wd_bf=_f32(self.proj_d.weight).to(torch.bfloat16).contiguous(),
                                   bias=(_f32(self.proj_a.bias) + _f32(self.proj_d.bias)).contiguous())
             self._packed.w.update(self._tables(self._packed.w))
@@ -391,14 +375,11 @@ class GeometricStructureEmbedding(nn.Module):
     def forward(self, points):
         w = self._weights()
         T = ops.geo_indices(points.contiguous(), self.sigma_d, self.factor_a)
-        if self.precision == "bf16" and GEO_LUT:
+        if self.precision == "bf16":
             # distances of row 0 / column 0 (the background point of SAM-6D: far outside the table) go through the exact
             # tensor-core projection: 2 S values per cloud
             far = ops.geo_embed_dist_tc(torch.stack([T[:, 0, :, :], T[:, :, 0, :]], dim=1).contiguous(), w["div"], w["wd_bf"], w["bias"])
-            return ops.geo_embed_lut(T, w["tab_a"], GEO_LUT_INV_H, w["tab_d"], GEO_LUT_INV_H, far, w["div"], w["wdT_bf"], w["bias"],
-                                     precise=GEO_LUT_PRECISE)
-        if self.precision == "bf16":
-            return ops.geo_embed_tc(T, w["div"], w["wa_bf"], w["wd_bf"], w["bias"], out_dtype=torch.bfloat16)
+            return ops.geo_embed_lut(T, w["tab_a"], GEO_LUT_INV_H, w["tab_d"], GEO_LUT_INV_H, far, w["div"], w["wdT_bf"], w["bias"])
         return ops.geo_embed_f32(T, w["div"], w["waT"], w["wdT"], w["bias"])
 
 
@@ -685,16 +666,11 @@ class SparseToDenseTransformer(nn.Module):
         key = _param_key(self.dense_layer)
         if self._packed.key != key:
             la = self.dense_layer.attention.attention
-            tail = dict(wo=_W(self.dense_layer.attention.linear.weight), bo=_f32(self.dense_layer.attention.linear.bias),
-                        g1=_f32(self.dense_layer.attention.norm.weight), b1=_f32(self.dense_layer.attention.norm.bias),
-                        we=_W(self.dense_layer.output.expand.weight), be=_f32(self.dense_layer.output.expand.bias),
-                        ws=_W(self.dense_layer.output.squeeze.weight), bs=_f32(self.dense_layer.output.squeeze.bias),
-                        g2=_f32(self.dense_layer.output.norm.weight), b2=_f32(self.dense_layer.output.norm.bias))
             self._packed.w = dict(
                 wq=_W(la.proj_q.weight), bq=_f32(la.proj_q.bias),
                 wkv=_W(torch.cat([_f32(la.proj_k.weight), _f32(la.proj_v.weight)], dim=0)),
                 bkv=torch.cat([_f32(la.proj_k.bias), _f32(la.proj_v.bias)], dim=0).contiguous(),
-                sp_scale=torch.nn.functional.softplus(_f32(la.scale)).reshape(-1).contiguous(), tail=tail)
+                sp_scale=torch.nn.functional.softplus(_f32(la.scale)).reshape(-1).contiguous(), tail=_pack_tail(self.dense_layer))
             self._packed.key = key
         return self._packed.w
 
@@ -722,17 +698,8 @@ class SparseToDenseTransformer(nn.Module):
         blob, KS = ops.linattn_kv_pack_raw(kv.data_ptr(), 2 * C, J * 2 * C, kv.data_ptr() + C * 4, 2 * C, J * 2 * C, B, J, dev)
         x_att = torch.empty(B * N1, C, dtype=bf, device=dev)
         ops.linattn_tc_raw(q.data_ptr() + C * 2, C, N1 * C, blob, KS, w["sp_scale"], B, N, x_att.data_ptr() + C * 2, C, N1 * C)
-        x_att.view(B, N1, C)[:, 0, :] = 0                                   # bg rows: defined input for the GEMMs below
-        t = w["tail"]
-        if FUSED_TAIL:
-            out = ops.transformer_tail_bf16(x_att, x2d, t["wo"].bf16, t["bo"], t["g1"], t["b1"], t["we"].bf16, t["be"], t["ws"].bf16,
-                                            t["bs"], t["g2"], t["b2"]).view(B, N1, C)
-        else:
-            y = ops.gemm_tma(x_att, t["wo"].bf16, t["bo"], residual=x2d, out_dtype=bf)
-            y = ops.layernorm_bf16io(y, t["g1"], t["b1"])
-            h = ops.gemm_tma(y, t["we"].bf16, t["be"], act=1, out_dtype=bf)
-            z = ops.gemm_tma(h, t["ws"].bf16, t["bs"], residual=y, out_dtype=bf)
-            out = ops.layernorm_bf16io(z, t["g2"], t["b2"]).view(B, N1, C)
+        x_att.view(B, N1, C)[:, 0, :] = 0                                   # bg rows: defined input for the tail below
+        out = _tail_bf16(x2d, x_att, w["tail"]).view(B, N1, C)
         out[:, 0, :] = sparse[:, 0, :].to(bf)                               # replaced bg token (transformer.py:660-668)
         return out
 

@@ -589,9 +589,8 @@ def test_geo_embed_tc(ops, S, edt):
     torch.testing.assert_close(E, E32, atol=6e-2, rtol=0)
 
 
-@pytest.mark.parametrize("precise", [True, False])
 @pytest.mark.parametrize("S,far_point", [(197, False), (64, False), (197, True), (33, True)])
-def test_geo_embed_lut(ops, S, far_point, precise, monkeypatch):
+def test_geo_embed_lut(ops, S, far_point):
     """table-interpolated geometric embedding (csrc/geo_lut.cu) through the module, against the float64-index embedding: at least as
     close as the tensor-core product, incl. the background point's row / column (exact distance projection, `far`) and -- far_point
     -- an ordinary point 40 units away, whose pairs take the exact per-pair fallback"""
@@ -604,8 +603,6 @@ def test_geo_embed_lut(ops, S, far_point, precise, monkeypatch):
     geo = pem.GeometricStructureEmbedding(pem.DEFAULT_MODEL_CFG["geo_embedding"]).cuda()
     geo.load_state_dict({k[len("geo_embedding."):]: v for k, v in sd.items() if k.startswith("geo_embedding.")})
     geo.precision = "bf16"
-    monkeypatch.setattr(pem, "GEO_LUT", True)
-    monkeypatch.setattr(pem, "GEO_LUT_PRECISE", precise)     # fp32 interpolation (default) / packed bf16x2 arithmetic
     E = geo(pts.cuda())
     assert E.dtype == torch.bfloat16 and E.shape == ref.shape
     E = E.float().cpu()
@@ -615,11 +612,12 @@ def test_geo_embed_lut(ops, S, far_point, precise, monkeypatch):
     assert (err > 6e-2).float().mean().item() < 2e-3
     T = ops.geo_indices(pts.cuda(), po.SIGMA_D, 180.0 / (po.SIGMA_A * math.pi))
     w = geo._weights()
-    Etc = ops.geo_embed_tc(T, w["div"], w["wa_bf"], w["wd_bf"], w["bias"], out_dtype=torch.bfloat16).float().cpu()
+    wa_bf = geo.proj_a.weight.detach().to(torch.bfloat16).contiguous()
+    Etc = ops.geo_embed_tc(T, w["div"], wa_bf, w["wd_bf"], w["bias"], out_dtype=torch.bfloat16).float().cpu()
     # same indices: the two kernels differ only by their bf16 roundings (no knn-tie outliers)
     torch.testing.assert_close(E, Etc, atol=4e-2, rtol=0)
     rms_lut, rms_tc = (E - ref).pow(2).mean().sqrt().item(), (Etc - ref).pow(2).mean().sqrt().item()
-    print(f"geo S={S} far_point={far_point} precise={precise}: rms error vs float64-index embedding: table {rms_lut:.3e}, tensor-core {rms_tc:.3e}")
+    print(f"geo S={S} far_point={far_point}: rms error vs float64-index embedding: table {rms_lut:.3e}, tensor-core {rms_tc:.3e}")
     assert rms_lut < 1.1 * rms_tc + 1e-4
     # rows / columns whose distance index is outside the table
     far_rows = [0, 5] if far_point else [0]

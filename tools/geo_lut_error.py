@@ -46,30 +46,20 @@ def main():
         pem.GEO_LUT_INV_H = inv_h
         t = geo._tables(dict(div=geo.embedding.div_term, bias=bias.float()))
 
-        def lerp(tab, x):                                 # the kernel: packed bf16 sub / fma
-            tab = tab.double()
-            u = x.float() * inv_h
-            i = u.floor().clamp(0, tab.shape[0] - 2).long()
-            tt = bf(u - i.float())
-            lo, hi = tab[i], tab[i + 1]
-            return bf(lo + tt[..., None] * bf(hi - lo))
-
-        def lerp32(tab, x):                               # PRECISE: fp32 interpolation of the bf16 table, one rounding at the store
+        def lerp32(tab, x):                               # the kernel: fp32 interpolation of the bf16 table, one rounding at the store
             tab = tab.double()
             u = x.float() * inv_h
             i = u.floor().clamp(0, tab.shape[0] - 2).long()
             tt = (u - i.float()).double()
             return (tab[i] + tt[..., None] * (tab[i + 1] - tab[i])).float().double()
 
-        e_lut = bf(lerp(t["tab_d"], xd) + lerp(t["tab_a"], xa.reshape(-1)).reshape(n, 3, 256).max(dim=1).values)
         e_p = bf(lerp32(t["tab_d"], xd) + lerp32(t["tab_a"], xa.reshape(-1)).reshape(n, 3, 256).max(dim=1).values)
-        rows.append((inv_h, t["tab_a"].shape[0], t["tab_d"].shape[0], (e_lut - exact).pow(2).mean().sqrt().item(), (e_lut - exact).abs().max().item(),
-                     (e_p - exact).pow(2).mean().sqrt().item(), (e_p - exact).abs().max().item()))
+        rows.append((inv_h, t["tab_a"].shape[0], t["tab_d"].shape[0], (e_p - exact).pow(2).mean().sqrt().item(),
+                     (e_p - exact).abs().max().item()))
     print(f"|E| rms {exact.pow(2).mean().sqrt():.3f}; bf16 rounding of the exact E alone: rms {(bf(exact) - exact).pow(2).mean().sqrt():.2e}")
     print(f"tensor-core product (geo_tc.cu arithmetic): rms {(e_tc - exact).pow(2).mean().sqrt():.2e} max {(e_tc - exact).abs().max():.2e}")
-    for inv_h, na, nd, rms, mx, rms_p, mx_p in rows:
-        print(f"table step 1/{inv_h:g} ({na} + {nd} rows, {(na + nd) * 512 / 1024:.0f} KB): packed bf16x2 rms {rms:.2e} max {mx:.2e}; "
-              f"fp32 interpolation rms {rms_p:.2e} max {mx_p:.2e}")
+    for inv_h, na, nd, rms_p, mx_p in rows:
+        print(f"table step 1/{inv_h:g} ({na} + {nd} rows, {(na + nd) * 512 / 1024:.0f} KB): fp32 interpolation rms {rms_p:.2e} max {mx_p:.2e}")
 
 
 if __name__ == "__main__":
