@@ -216,17 +216,25 @@ int sam6d_mask_rle_write(const float* masks, int n, int H, int W, const int* col
 
 /* PositionEmbeddingRandom._pe_encoding: coords (rows,2) f32 in [0,1], G (2,128) f32 -> out (rows,256) f32 = [sin | cos] */
 int sam6d_sam_pe_encode(const float* coords, const float* G, int rows, float* out, void* stream);
-/* prompt-token self attention core (8 heads x 32): q, k, v, out (B,T,256) f32, T <= 8 */
+/* PromptEncoder.mask_downscaling (Conv2d 1->4 k2 s2, LayerNorm2d, GELU, Conv2d 4->16 k2 s2, LayerNorm2d, GELU, Conv2d 16->256 1x1;
+ * fp32, erf GELU, eps 1e-6): masks (B,256,256) f32 (16-byte aligned) -> out (B,4096,256) f32 token rows (row = y*64 + x).
+ * params (4684) f32 = conv1 w (4,1,2,2) | conv1 b (4) | ln1 w (4) | ln1 b (4) | conv2 w (16,4,2,2) | conv2 b (16) | ln2 w (16) |
+ * ln2 b (16) | conv3 w (256,16) | conv3 b (256) */
+int sam6d_sam_mask_embed(const float* masks, const float* params, int B, float* out, void* stream);
+/* prompt-token self attention core (8 heads x 32): q, k, v, out (B,T,256) f32, T <= 32 */
 int sam6d_sam_self_attn(const float* q, const float* k, const float* v, int B, int T, float* out, void* stream);
-/* tokens attend to the image (8 heads x 16): Q (B,T,128) f32; K, V bf16 (L,128) shared (kv_bs = 0) or (B,L,128) -> out (B,T,128) f32 */
+/* tokens attend to the image (8 heads x 16): Q (B,T,128) f32; K, V bf16 (L,128) shared (kv_bs = 0) or (B,L,128) -> out (B,T,128) f32;
+ * T <= 32, min(T, 8) * L * 4 <= 200 KB */
 int sam6d_sam_tok2img_attn(const float* Q, const void* K, const void* V, long long kv_bs, int B, int T, int L, float* out, void* stream);
-/* image attends to the tokens: Q bf16 (L,128) shared (q_bs = 0) or (B,L,128); Kt, Vt (B,T,128) f32 -> out (B,L,128) bf16 */
+/* image attends to the tokens: Q bf16 (L,128) shared (q_bs = 0) or (B,L,128); Kt, Vt (B,T,128) f32 -> out (B,L,128) bf16; T <= 32 */
 int sam6d_sam_img2tok_attn(const void* Q, long long q_bs, const float* Kt, const float* Vt, int B, int T, int L, void* out, void* stream);
 /* LayerNorm2d (eps 1e-6) + GELU over rows of 64 bf16 channels (output_upscaling.1, .2) */
 int sam6d_sam_ln2d_gelu(const void* x, const float* gamma, const float* beta, long long rows, void* y, void* stream);
 /* mask logits: up (B*G*G*4 rows = (b,y,x,i,j), 128 cols = (i',j',o)) bf16, hyper (B,4,32) f32 -> masks (B,3,4G,4G) f32 (mask
  * tokens 1..3), the pixel shuffles of both transposed convolutions folded into the output index */
 int sam6d_sam_mask_dot(const void* up, const float* hyper, int B, int G, float* masks, void* stream);
+/* the same product for mask tokens m0 .. m0+nm-1 (0 <= m0, m0 + nm <= 4) -> masks (B,nm,4G,4G) f32; sam6d_sam_mask_dot is (1, 3) */
+int sam6d_sam_mask_dot_range(const void* up, const float* hyper, int B, int G, int m0, int nm, float* masks, void* stream);
 /* Sam.postprocess_masks evaluated per output pixel (S -> big bilinear, crop to (in_h,in_w), -> (H,W) bilinear) + statistics:
  * low (N,S,S) f32 -> stats (N,8) i32 = [count(> thr+off), count(> thr-off), xmin, ymin, xmax, ymax of (> thr), -, -] */
 int sam6d_sam_mask_stats(const float* low, int N, int S, int big, int in_h, int in_w, int H, int W, float thr, float off, int* stats,
@@ -234,6 +242,8 @@ int sam6d_sam_mask_stats(const float* low, int N, int S, int big, int in_h, int 
 /* the selected masks at the original resolution: sel (K) i32 indices into low -> out (K,H,W) u8 = logit > thr */
 int sam6d_sam_mask_binarize(const float* low, const int* sel, int K, int S, int big, int in_h, int in_w, int H, int W, float thr,
                             unsigned char* out, void* stream);
+/* Sam.postprocess_masks: low (N,S,S) f32 -> out (N,H,W) f32 logits (the values sam6d_sam_mask_binarize thresholds) */
+int sam6d_sam_mask_upscale(const float* low, int N, int S, int big, int in_h, int in_w, int H, int W, float* out, void* stream);
 /* torchvision.ops.nms on boxes (N,4) f32 xyxy sorted by decreasing score -> keep (N) u8 */
 int sam6d_sam_nms(const float* boxes, int N, float thr, unsigned char* keep, void* stream);
 

@@ -3,14 +3,17 @@
 // The Linears of the decoder (token and image side, the two transposed convolutions written as GEMMs) run on the wgmma GEMMs
 // (sam6d_gemm_tma / sam6d_gemm_bf16); this file holds what is not a GEMM:
 //   sam_pe_encode          random-Fourier positional encoding of point prompts / of the dense 64 x 64 grid
-//   sam_self_attn          7-token self-attention of the prompt tokens (8 heads x 32)
-//   sam_tok2img_attn       prompt tokens attend to the 4096 image tokens (8 heads x 16): scores in shared memory, two passes
-//   sam_img2tok_attn       image tokens attend to the 7 prompt tokens (softmax over 7 keys per pixel and head)
+//   sam_mask_embed         PromptEncoder.mask_downscaling: (B,256,256) mask logits -> (B,4096,256) dense-embedding token rows
+//   sam_self_attn          self-attention of the T <= 32 prompt tokens (8 heads x 32)
+//   sam_tok2img_attn       prompt tokens attend to the 4096 image tokens (8 heads x 16): scores in shared memory, two passes,
+//                          at most 8 tokens per CTA
+//   sam_img2tok_attn       image tokens attend to the T <= 32 prompt tokens (softmax over T keys per pixel and head)
 //   sam_ln2d_gelu          LayerNorm2d (eps 1e-6) + GELU over 64-channel pixel rows after the first transposed convolution
-//   sam_mask_dot           GELU'd 32-channel upscaled embedding x hypernetwork vectors -> (B,3,256,256) mask logits, with the
-//                          pixel shuffle of both transposed convolutions folded into the output index
+//   sam_mask_dot(_range)   GELU'd 32-channel upscaled embedding x hypernetwork vectors -> (B,nm,256,256) mask logits of mask
+//                          tokens m0 .. m0+nm-1, with the pixel shuffle of both transposed convolutions folded into the output index
 //   sam_mask_stats         Sam.postprocess_masks (256 -> 1024 bilinear, crop, -> original size bilinear) evaluated on the fly per
 //                          output pixel + stability counts + box extremes per mask (the (64,3,1024,1024) tensor never exists)
+//   sam_mask_upscale       the same evaluation written out as logits (Sam.postprocess_masks)
 //   sam_mask_binarize      the kept masks at the original resolution
 //   sam_nms                box NMS (torchvision semantics) over score-sorted boxes
 #include "common.cuh"
@@ -19,7 +22,9 @@ namespace {
 
 constexpr int HD_X = 16;      // head dim of the cross attentions (internal dim 128 / 8 heads)
 constexpr int NH = 8;
-constexpr int MAXT = 8;       // prompt tokens per prompt (5 output tokens + point + padding point = 7)
+constexpr int TOK_SMALL = 8;  // token bound of the automatic mask generator's shapes (5 output tokens + point + padding point = 7)
+constexpr int TOK_MAX = 32;   // 5 output tokens + up to 27 prompt tokens (26 clicks + padding point, or 25 clicks + a box)
+constexpr int TOK_CHUNK = 8;  // tokens per CTA of sam_tok2img_attn (their scores over all L keys live in shared memory)
 
 __device__ __forceinline__ float bf2f(__nv_bfloat16 v) { return __bfloat162float(v); }
 
@@ -33,7 +38,88 @@ __global__ void sam_pe_encode_kernel(const float* __restrict__ coords, const flo
   out[(size_t)r * 256 + 128 + f] = cosf(v);
 }
 
+// ---- mask prompt -> dense embedding: PromptEncoder.mask_downscaling ------------------------------------------------------------------
+// Conv2d 1->4 (k2 s2) -> LayerNorm2d(4) -> GELU -> Conv2d 4->16 (k2 s2) -> LayerNorm2d(16) -> GELU -> Conv2d 16->256 (1x1), fp32.
+// Output pixel (y, x) of the 64 x 64 grid depends on input rows 4y .. 4y+3, columns 4x .. 4x+3 only, so the 4- and 16-channel
+// intermediates stay in registers / shared memory.  params (ME_NPARAM floats, see sam6d_sam_mask_embed) in the module's order.
+constexpr int ME_C1W = 0, ME_C1B = 16, ME_L1W = 20, ME_L1B = 24, ME_C2W = 28, ME_C2B = 284, ME_L2W = 300, ME_L2B = 316, ME_C3W = 332,
+              ME_C3B = 4428, ME_NPARAM = 4684;
+
+// LayerNorm2d over n channels (biased variance, eps 1e-6) + affine + erf GELU, in place
+template <int n>
+__device__ __forceinline__ void ln_gelu(float* v, const float* __restrict__ w, const float* __restrict__ b) {
+  float u = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; ++i) u += v[i];
+  u *= 1.f / n;
+  float var = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; ++i) var = fmaf(v[i] - u, v[i] - u, var);
+  const float sd = sqrtf(var * (1.f / n) + 1e-6f);
+#pragma unroll
+  for (int i = 0; i < n; ++i) v[i] = s6_act(fmaf(w[i], (v[i] - u) / sd, b[i]), 2);
+}
+
+// grid (64 rows of the embedding, B), 256 threads: threads 0..63 take one pixel of the row through the two 2x2 convolutions; then
+// thread c writes channel c of all 64 pixels (consecutive threads, consecutive channels: 1 KB per pixel row)
+__global__ void __launch_bounds__(256) sam_mask_embed_kernel(const float* __restrict__ masks, const float* __restrict__ prm,
+                                                             float* __restrict__ out) {
+  __shared__ float p[ME_C3W];
+  __shared__ float hs[64][17];
+  const int y = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  for (int i = tid; i < ME_C3W; i += 256) p[i] = prm[i];
+  __syncthreads();
+  if (tid < 64) {
+    const float* m = masks + (size_t)b * 65536 + (size_t)(4 * y) * 256 + 4 * tid;
+    float in[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const float4 v = *reinterpret_cast<const float4*>(m + r * 256);
+      in[r][0] = v.x; in[r][1] = v.y; in[r][2] = v.z; in[r][3] = v.w;
+    }
+    float a[4][4];                                   // [2x2 position (ky, kx)][channel]
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int ky = q >> 1, kx = q & 1;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        float s = p[ME_C1B + c];
+#pragma unroll
+        for (int d = 0; d < 4; ++d) s = fmaf(p[ME_C1W + c * 4 + d], in[2 * ky + (d >> 1)][2 * kx + (d & 1)], s);
+        a[q][c] = s;
+      }
+      ln_gelu<4>(a[q], p + ME_L1W, p + ME_L1B);
+    }
+    float h[16];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      float s = p[ME_C2B + c];
+#pragma unroll
+      for (int ci = 0; ci < 4; ++ci)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) s = fmaf(p[ME_C2W + (c * 4 + ci) * 4 + q], a[q][ci], s);
+      h[c] = s;
+    }
+    ln_gelu<16>(h, p + ME_L2W, p + ME_L2B);
+#pragma unroll
+    for (int c = 0; c < 16; ++c) hs[tid][c] = h[c];
+  }
+  __syncthreads();
+  float w3[16];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) w3[k] = __ldg(prm + ME_C3W + tid * 16 + k);
+  const float b3 = __ldg(prm + ME_C3B + tid);
+  float* o = out + ((size_t)b * 4096 + (size_t)y * 64) * 256 + tid;
+  for (int x = 0; x < 64; ++x) {
+    float s = b3;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s = fmaf(w3[k], hs[x][k], s);
+    o[(size_t)x * 256] = s;
+  }
+}
+
 // ---- prompt-token self-attention: q, k, v (B,T,256) f32 (already projected), 8 heads x 32; one warp per (b, h) ----------------------
+template <int MAXT>
 __global__ void __launch_bounds__(256) sam_self_attn_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                                             int B, int T, float* __restrict__ out) {
   const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -54,21 +140,26 @@ __global__ void __launch_bounds__(256) sam_self_attn_kernel(const float* __restr
 }
 
 // ---- tokens -> image: Q (B,T,128) f32; K, V (kv_bs = 0: shared (L,128), else (B,L,128)) bf16; out (B,T,128) f32 -----------------------
-// grid = B * 8 (prompt, head), 256 threads, dynamic smem T * L floats (scores) + reductions
+// grid = B * 8 * ceil(T / 8) (prompt, head, chunk of at most 8 tokens), 256 threads, dynamic smem min(T, 8) * L floats (scores) +
+// reductions; the CTAs of one (prompt, head) are adjacent, so the chunks after the first read K and V from L2.  At T <= 8 there is
+// one chunk and the CTA computes what it did before tokens were chunked.
 __global__ void __launch_bounds__(256) sam_tok2img_attn_kernel(const float* __restrict__ Q, const __nv_bfloat16* __restrict__ K,
                                                                const __nv_bfloat16* __restrict__ V, long long kv_bs, int T, int L,
                                                                float* __restrict__ out) {
-  extern __shared__ float sc[];                  // [T][L]
+  constexpr int MAXT = TOK_CHUNK;
+  extern __shared__ float sc[];                  // [Tc][L]
   __shared__ float red[MAXT][8];
   __shared__ float stat[MAXT][2];
   __shared__ float part[16][MAXT][HD_X];
   __shared__ float qs[MAXT][HD_X];
-  const int b = blockIdx.x / NH, h = blockIdx.x % NH, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nc = (T + MAXT - 1) / MAXT, c = blockIdx.x % nc, bh = blockIdx.x / nc;
+  const int b = bh / NH, h = bh % NH, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int t0 = c * MAXT, Tc = min(MAXT, T - t0);
   const __nv_bfloat16* Kb = K + (size_t)b * kv_bs + h * HD_X;
   const __nv_bfloat16* Vb = V + (size_t)b * kv_bs + h * HD_X;
   if (tid < MAXT * HD_X) {
     const int t = tid / HD_X, d = tid % HD_X;
-    qs[t][d] = t < T ? Q[((size_t)b * T + t) * 128 + h * HD_X + d] * 0.25f : 0.f;      // 1 / sqrt(16)
+    qs[t][d] = t < Tc ? Q[((size_t)b * T + t0 + t) * 128 + h * HD_X + d] * 0.25f : 0.f;      // 1 / sqrt(16)
   }
   __syncthreads();
   float mx[MAXT];
@@ -83,7 +174,7 @@ __global__ void __launch_bounds__(256) sam_tok2img_attn_kernel(const float* __re
     for (int i = 0; i < 8; ++i) { kf[2 * i] = __uint_as_float(wv[i] << 16); kf[2 * i + 1] = __uint_as_float(wv[i] & 0xffff0000u); }
 #pragma unroll
     for (int t = 0; t < MAXT; ++t) {
-      if (t < T) {
+      if (t < Tc) {
         float s = 0.f;
 #pragma unroll
         for (int d = 0; d < HD_X; ++d) s = fmaf(qs[t][d], kf[d], s);
@@ -103,7 +194,7 @@ __global__ void __launch_bounds__(256) sam_tok2img_attn_kernel(const float* __re
   for (int j = tid; j < L; j += 256) {
 #pragma unroll
     for (int t = 0; t < MAXT; ++t)
-      if (t < T) { const float p = __expf(sc[(size_t)t * L + j] - stat[t][0]); sc[(size_t)t * L + j] = p; sm[t] += p; }
+      if (t < Tc) { const float p = __expf(sc[(size_t)t * L + j] - stat[t][0]); sc[(size_t)t * L + j] = p; sm[t] += p; }
   }
 #pragma unroll
   for (int t = 0; t < MAXT; ++t) { const float v = warp_sum(sm[t]); if (lane == 0) red[t][warp] = v; }
@@ -119,21 +210,22 @@ __global__ void __launch_bounds__(256) sam_tok2img_attn_kernel(const float* __re
     const float vv = bf2f(Vb[(size_t)j * 128 + d]);
 #pragma unroll
     for (int t = 0; t < MAXT; ++t)
-      if (t < T) acc[t] = fmaf(sc[(size_t)t * L + j], vv, acc[t]);
+      if (t < Tc) acc[t] = fmaf(sc[(size_t)t * L + j], vv, acc[t]);
   }
 #pragma unroll
   for (int t = 0; t < MAXT; ++t) part[g][t][d] = acc[t];
   __syncthreads();
-  if (tid < T * HD_X) {
+  if (tid < Tc * HD_X) {
     const int t = tid / HD_X, dd = tid % HD_X;
     float v = 0.f;
     for (int gg = 0; gg < 16; ++gg) v += part[gg][t][dd];
-    out[((size_t)b * T + t) * 128 + h * HD_X + dd] = v / stat[t][1];
+    out[((size_t)b * T + t0 + t) * 128 + h * HD_X + dd] = v / stat[t][1];
   }
 }
 
 // ---- image -> tokens: Qimg (q_bs = 0: shared (L,128), else (B,L,128)) bf16; Kt, Vt (B,T,128) f32; out (B,L,128) bf16 -------------------
 // grid (L / 32, B), 256 threads: thread = (pixel of the 32, head)
+template <int MAXT>
 __global__ void __launch_bounds__(256) sam_img2tok_attn_kernel(const __nv_bfloat16* __restrict__ Q, long long q_bs, const float* __restrict__ Kt,
                                                                const float* __restrict__ Vt, int T, int L, __nv_bfloat16* __restrict__ out) {
   __shared__ float ks[MAXT][128], vs[MAXT][128];
@@ -194,10 +286,11 @@ __global__ void __launch_bounds__(256) sam_ln2d_gelu_kernel(const __nv_bfloat16*
 }
 
 // ---- mask logits: up (B*L*4 rows = (b, y, x, i, j), 128 cols = (i', j', o)) bf16 already GELU'd; hyper (B,4,32) f32 --------------------
-// masks[b, m-1, 4y + 2i + i', 4x + 2j + j'] = sum_o hyper[b, m, o] up[row, (i',j',o)]   for m = 1..3   (multimask slice)
-// thread = (row, sub-position (i',j')); grid covers B*L*4*4 threads
+// masks[b, m-m0, 4y + 2i + i', 4x + 2j + j'] = sum_o hyper[b, m, o] up[row, (i',j',o)]   for m = m0 .. m0+nm-1
+// (m0 = 1, nm = 3: the multimask slice; m0 = 0, nm = 1: the single-mask output); thread = (row, sub-position (i',j')); grid covers
+// B*L*4*4 threads
 __global__ void __launch_bounds__(256) sam_mask_dot_kernel(const __nv_bfloat16* __restrict__ up, const float* __restrict__ hyper, int B, int G,
-                                                           float* __restrict__ masks) {
+                                                           int m0, int nm, float* __restrict__ masks) {
   const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
   const long long total = (long long)B * G * G * 16;
   if (t >= total) return;
@@ -217,13 +310,12 @@ __global__ void __launch_bounds__(256) sam_mask_dot_kernel(const __nv_bfloat16* 
   }
   const int Y = 4 * y + 2 * (ij >> 1) + (sub >> 1), X = 4 * x + 2 * (ij & 1) + (sub & 1);
   const int S = 4 * G;
-#pragma unroll
-  for (int m = 1; m < 4; ++m) {
+  for (int m = m0; m < m0 + nm; ++m) {
     const float* hv = hyper + ((size_t)b * 4 + m) * 32;
     float s = 0.f;
 #pragma unroll
     for (int o = 0; o < 32; ++o) s = fmaf(__ldg(hv + o), u[o], s);
-    masks[(((size_t)b * 3 + (m - 1)) * S + Y) * S + X] = s;
+    masks[(((size_t)b * nm + (m - m0)) * S + Y) * S + X] = s;
   }
 }
 
@@ -301,6 +393,15 @@ __global__ void __launch_bounds__(256) sam_mask_binarize_kernel(const float* __r
   out[(size_t)k * H * W + i] = mask_logit(low + (size_t)sel[k] * S * S, S, big, in_h, in_w, H, W, y, x) > thr ? 1 : 0;
 }
 
+// Sam.postprocess_masks written out: low (N,S,S) -> out (N,H,W) f32; the values sam_mask_binarize thresholds
+__global__ void __launch_bounds__(256) sam_mask_upscale_kernel(const float* __restrict__ low, int S, int big, int in_h, int in_w, int H, int W,
+                                                               float* __restrict__ out) {
+  const int n = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= H * W) return;
+  const int y = i / W, x = i - y * W;
+  out[(size_t)n * H * W + i] = mask_logit(low + (size_t)n * S * S, S, big, in_h, in_w, H, W, y, x);
+}
+
 // ---- NMS over boxes sorted by decreasing score (torchvision.ops.nms): keep[i] = 1 for survivors; one CTA -----------------------------------
 __global__ void __launch_bounds__(1024) sam_nms_kernel(const float* __restrict__ boxes, int N, float thr, unsigned char* __restrict__ keep) {
   extern __shared__ unsigned char dead[];       // N
@@ -334,33 +435,51 @@ S6_API int sam6d_sam_pe_encode(const float* coords, const float* G, int rows, fl
   return 0;
 }
 
-// q, k, v, out (B,T,256) f32, T <= 8: Attention.forward core of the prompt-token self attention (8 heads x 32)
+// masks (B,256,256) f32 mask logits, params (ME_NPARAM) f32 -> out (B,4096,256) f32 dense-embedding token rows (row = y*64 + x)
+S6_API int sam6d_sam_mask_embed(const float* masks, const float* params, int B, float* out, void* stream) {
+  S6_REQUIRE(masks && params && out && B >= 0 && B <= 65535 && (reinterpret_cast<uintptr_t>(masks) & 15) == 0);
+  if (B == 0) return 0;
+  sam_mask_embed_kernel<<<dim3(64, B), 256, 0, s6_stream(stream)>>>(masks, params, out);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+// q, k, v, out (B,T,256) f32, T <= 32: Attention.forward core of the prompt-token self attention (8 heads x 32)
 S6_API int sam6d_sam_self_attn(const float* q, const float* k, const float* v, int B, int T, float* out, void* stream) {
-  S6_REQUIRE(q && k && v && out && B >= 0 && T > 0 && T <= MAXT);
+  S6_REQUIRE(q && k && v && out && B >= 0 && T > 0 && T <= TOK_MAX);
   if (B == 0) return 0;
-  sam_self_attn_kernel<<<s6_cdiv(B * NH, 8), 256, 0, s6_stream(stream)>>>(q, k, v, B, T, out);
+  if (T <= TOK_SMALL)
+    sam_self_attn_kernel<TOK_SMALL><<<s6_cdiv(B * NH, 8), 256, 0, s6_stream(stream)>>>(q, k, v, B, T, out);
+  else
+    sam_self_attn_kernel<TOK_MAX><<<s6_cdiv(B * NH, 8), 256, 0, s6_stream(stream)>>>(q, k, v, B, T, out);
   S6_LAUNCH_CHECK();
   return 0;
 }
 
-// Q (B,T,128) f32; K, V bf16 (L,128) shared by every prompt (kv_bs = 0) or (B,L,128) (kv_bs = L*128) -> out (B,T,128) f32
+// Q (B,T,128) f32; K, V bf16 (L,128) shared by every prompt (kv_bs = 0) or (B,L,128) (kv_bs = L*128) -> out (B,T,128) f32; T <= 32
 S6_API int sam6d_sam_tok2img_attn(const float* Q, const void* K, const void* V, long long kv_bs, int B, int T, int L, float* out, void* stream) {
-  S6_REQUIRE(Q && K && V && out && B >= 0 && T > 0 && T <= MAXT && L > 0 && (size_t)T * L * 4 <= 200 * 1024);
+  S6_REQUIRE(Q && K && V && out && B >= 0 && T > 0 && T <= TOK_MAX && L > 0 && (size_t)min(T, TOK_CHUNK) * L * 4 <= 200 * 1024);
   if (B == 0) return 0;
-  const size_t smem = (size_t)T * L * sizeof(float);
+  const size_t smem = (size_t)min(T, TOK_CHUNK) * L * sizeof(float);
   S6_CHECK(cudaFuncSetAttribute(sam_tok2img_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  sam_tok2img_attn_kernel<<<B * NH, 256, smem, s6_stream(stream)>>>(Q, reinterpret_cast<const __nv_bfloat16*>(K),
-                                                                   reinterpret_cast<const __nv_bfloat16*>(V), kv_bs, T, L, out);
+  const int chunks = (T + TOK_CHUNK - 1) / TOK_CHUNK;
+  sam_tok2img_attn_kernel<<<B * NH * chunks, 256, smem, s6_stream(stream)>>>(Q, reinterpret_cast<const __nv_bfloat16*>(K),
+                                                                            reinterpret_cast<const __nv_bfloat16*>(V), kv_bs, T, L, out);
   S6_LAUNCH_CHECK();
   return 0;
 }
 
-// Q bf16 (L,128) shared (q_bs = 0) or (B,L,128); Kt, Vt (B,T,128) f32 -> out (B,L,128) bf16
+// Q bf16 (L,128) shared (q_bs = 0) or (B,L,128); Kt, Vt (B,T,128) f32 -> out (B,L,128) bf16; T <= 32
 S6_API int sam6d_sam_img2tok_attn(const void* Q, long long q_bs, const float* Kt, const float* Vt, int B, int T, int L, void* out, void* stream) {
-  S6_REQUIRE(Q && Kt && Vt && out && B >= 0 && T > 0 && T <= MAXT && L > 0 && B <= 65535);
+  S6_REQUIRE(Q && Kt && Vt && out && B >= 0 && T > 0 && T <= TOK_MAX && L > 0 && B <= 65535);
   if (B == 0) return 0;
-  sam_img2tok_attn_kernel<<<dim3(s6_cdiv(L, 32), B), 256, 0, s6_stream(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(Q), q_bs, Kt, Vt, T, L,
-                                                                                  reinterpret_cast<__nv_bfloat16*>(out));
+  const dim3 grid(s6_cdiv(L, 32), B);
+  const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(Q);
+  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+  if (T <= TOK_SMALL)
+    sam_img2tok_attn_kernel<TOK_SMALL><<<grid, 256, 0, s6_stream(stream)>>>(q, q_bs, Kt, Vt, T, L, o);
+  else
+    sam_img2tok_attn_kernel<TOK_MAX><<<grid, 256, 0, s6_stream(stream)>>>(q, q_bs, Kt, Vt, T, L, o);
   S6_LAUNCH_CHECK();
   return 0;
 }
@@ -375,14 +494,19 @@ S6_API int sam6d_sam_ln2d_gelu(const void* x, const float* gamma, const float* b
   return 0;
 }
 
-// up (B*G*G*4, 128) bf16, hyper (B,4,32) f32 -> masks (B,3,4G,4G) f32
-S6_API int sam6d_sam_mask_dot(const void* up, const float* hyper, int B, int G, float* masks, void* stream) {
-  S6_REQUIRE(up && hyper && masks && B >= 0 && G > 0);
+// up (B*G*G*4, 128) bf16, hyper (B,4,32) f32 -> masks (B,nm,4G,4G) f32: the logits of mask tokens m0 .. m0+nm-1
+S6_API int sam6d_sam_mask_dot_range(const void* up, const float* hyper, int B, int G, int m0, int nm, float* masks, void* stream) {
+  S6_REQUIRE(up && hyper && masks && B >= 0 && G > 0 && m0 >= 0 && nm > 0 && m0 + nm <= 4);
   if (B == 0) return 0;
   const long long total = (long long)B * G * G * 16;
-  sam_mask_dot_kernel<<<s6_cdiv(total, 256), 256, 0, s6_stream(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(up), hyper, B, G, masks);
+  sam_mask_dot_kernel<<<s6_cdiv(total, 256), 256, 0, s6_stream(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(up), hyper, B, G, m0, nm, masks);
   S6_LAUNCH_CHECK();
   return 0;
+}
+
+// up (B*G*G*4, 128) bf16, hyper (B,4,32) f32 -> masks (B,3,4G,4G) f32 (the multimask slice)
+S6_API int sam6d_sam_mask_dot(const void* up, const float* hyper, int B, int G, float* masks, void* stream) {
+  return sam6d_sam_mask_dot_range(up, hyper, B, G, 1, 3, masks, stream);
 }
 
 // low (N,S,S) f32 low-res logits -> stats (N,8) i32 (see the kernel) at original size (H,W) through the big x big stage cropped to (in_h,in_w)
@@ -404,6 +528,15 @@ S6_API int sam6d_sam_mask_binarize(const float* low, const int* sel, int K, int 
   S6_REQUIRE(low && sel && out && K >= 0 && S > 1 && K <= 65535);
   if (K == 0) return 0;
   sam_mask_binarize_kernel<<<dim3(s6_cdiv((long long)H * W, 256), K), 256, 0, s6_stream(stream)>>>(low, sel, S, big, in_h, in_w, H, W, thr, out);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+// low (N,S,S) f32 -> out (N,H,W) f32: S -> big bilinear, crop to (in_h,in_w), -> (H,W) bilinear (Sam.postprocess_masks)
+S6_API int sam6d_sam_mask_upscale(const float* low, int N, int S, int big, int in_h, int in_w, int H, int W, float* out, void* stream) {
+  S6_REQUIRE(low && out && N >= 0 && S > 1 && big >= S && in_h > 0 && in_w > 0 && in_h <= big && in_w <= big && H > 0 && W > 0 && N <= 65535);
+  if (N == 0) return 0;
+  sam_mask_upscale_kernel<<<dim3(s6_cdiv((long long)H * W, 256), N), 256, 0, s6_stream(stream)>>>(low, S, big, in_h, in_w, H, W, out);
   S6_LAUNCH_CHECK();
   return 0;
 }
