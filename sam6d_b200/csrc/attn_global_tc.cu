@@ -14,8 +14,6 @@
 // Q, K and each rel table are DS = ceil(D/64) slabs of 64 channels (two at D = 80, the second one 16 channels deep; one at D = 64);
 // a V^T tile is two [D rows][64 keys] slabs.  Both head dims share the code; only the slab counts and the k-step counts differ.
 // The reference materialises a (16 x 4096 x 4096) fp32 score tensor per image and block; here scores never leave registers.
-#include <cuda.h>
-
 #include "epilogue.cuh"
 #include "tc.cuh"
 
@@ -224,41 +222,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_global_tc_kernel(const __
   }
 }
 
-}  // namespace
-
-namespace {
-
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeFn g_get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-int g_make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows) {
-  EncodeFn enc = g_get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
-}  // namespace
-
-namespace {
-
 template <int D, typename OT>
 int launch_global(const CUtensorMap& tqk, const CUtensorMap& tv, const GArgs& a, int B, cudaStream_t st) {
   constexpr int SMEM = Cfg<D>::SMEM_BYTES;
@@ -287,9 +250,9 @@ S6_API int sam6d_attn_global_tc_ex(const void* qkv, long long ld, const void* Vt
   S6_REQUIRE(B <= 65535 && H <= 65535);
   constexpr int L = GRID * GRID;
   CUtensorMap tqk, tv;
-  int rc = g_make_map(&tqk, qkv, (long long)B * L, ld, ld, 64, QT);
+  int rc = tc::make_map_2d(&tqk, qkv, (long long)B * L, ld, ld, 64, QT);
   if (rc) return rc;
-  rc = g_make_map(&tv, Vt, (long long)B * H * head_dim, vt_ld, vt_ld, 64, head_dim);
+  rc = tc::make_map_2d(&tv, Vt, (long long)B * H * head_dim, vt_ld, vt_ld, 64, head_dim);
   if (rc) return rc;
   GArgs a{rel_blob, out, out_ld, H, scale};
   cudaStream_t st = s6_stream(stream);

@@ -16,8 +16,6 @@
 //   epilogue : O / rowsum (+ b_v; rows of P sum to 1, so the value bias moves out of the MMA), stored from the registers
 // Rows of a tile that run past the batch (197 is not a multiple of 128) are computed on whatever the TMA box fetched (the
 // next batch's finite rows or zero fill) and never stored; keys past Sk are masked to probability 0.
-#include <cuda.h>
-
 #include "epilogue.cuh"
 #include "tc.cuh"
 
@@ -218,33 +216,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) attn_tc_kernel(const __grid_co
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-int make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows) {
-  EncodeFn enc = get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
 template <int D, int BM, typename OT>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnArgs& a, int B, cudaStream_t st) {
   constexpr int DS = (D + 63) / 64;
@@ -319,11 +290,11 @@ int attn_tc_launch(const void* Q, long long q_ld, int q_col0, const void* K, lon
   const int N1 = (Sk + 15) & ~15;
   S6_REQUIRE(vt_ld >= v_col0 + N1);
   CUtensorMap tq, tk, tv;
-  int rc = make_map(&tq, Q, (long long)B * Sq, q_ld, q_ld, 64, QT);
+  int rc = tc::make_map_2d(&tq, Q, (long long)B * Sq, q_ld, q_ld, 64, QT);
   if (rc) return rc;
-  rc = make_map(&tk, K, (long long)B * k_brows, k_ld, k_ld, 64, N1);
+  rc = tc::make_map_2d(&tk, K, (long long)B * k_brows, k_ld, k_ld, 64, N1);
   if (rc) return rc;
-  rc = make_map(&tv, Vt, (long long)B * H * head_dim, vt_ld, vt_ld, 64, head_dim);
+  rc = tc::make_map_2d(&tv, Vt, (long long)B * H * head_dim, vt_ld, vt_ld, 64, head_dim);
   if (rc) return rc;
   AttnArgs a{bias, rel_h, rel_w, Q, q_ld, q_col0, bv, out, out_ld, H, Sq, Sk, N1, Hs, Ws, k_col0, scale, k_brows, k_row0, v_col0, lse, bias_ld};   // mode 2: rel_h = packed blob
   cudaStream_t st = s6_stream(stream);

@@ -86,3 +86,15 @@ __device__ __forceinline__ float s6_act(float x, int act) {
 }
 
 static inline int s6_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// grid of a persistent kernel: min(work, per_sm x the SM count of the current device).  The device is queried on every call
+// because the caller's current device can change between calls.
+static inline cudaError_t s6_persistent_grid(long long work, int per_sm, int* grid) {
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return e;
+  const long long cap = (long long)per_sm * sms;
+  *grid = (int)(work < cap ? work : cap);
+  return cudaSuccess;
+}

@@ -15,8 +15,6 @@
 // store as bf16 or fp32 into a channel slice (row stride ldy >= Cout) through the output mapping
 //   Y[n * y_bs + ((sy * y + oy) * Wy + sx * x + ox) * ldy + c]
 // (identity for ordinary layers; sy = sx = 2 and (oy, ox) = tap for one tap of a 2x2 stride-2 transposed convolution).
-#include <cuda.h>
-
 #include "tc.cuh"
 
 namespace {
@@ -142,32 +140,6 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-
-int encode(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
-           const cuuint32_t* estr) {
-  EncodeFn enc = get_encode();
-  if (!enc) return 999;
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, strides_bytes, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
 }  // namespace
 
 // x (B, Hi, Wi, ldx) bf16 NHWC: channels [0, Cin) of each pixel row are the input (a channel slice: offset the pointer);
@@ -189,7 +161,7 @@ S6_API int sam6d_conv2d_tc(const void* x, long long ldx, int B, int Hi, int Wi, 
     cuuint64_t str[3] = {(cuuint64_t)ldx * 2, (cuuint64_t)Wi * ldx * 2, (cuuint64_t)Hi * Wi * ldx * 2};
     cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)(TX * stride), (cuuint32_t)(TY * stride), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-    int rc = encode(&tmX, x, 4, dims, str, box, estr);
+    int rc = tc::encode_map(&tmX, x, 4, dims, str, box, estr);
     if (rc) return rc;
   }
   {
@@ -197,7 +169,7 @@ S6_API int sam6d_conv2d_tc(const void* x, long long ldx, int B, int Hi, int Wi, 
     cuuint64_t str[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)k * k * Cin * 2};
     cuuint32_t box[3] = {(cuuint32_t)BK, 1, (cuuint32_t)BN};
     cuuint32_t estr[3] = {1, 1, 1};
-    int rc = encode(&tmW, w, 3, dims, str, box, estr);
+    int rc = tc::encode_map(&tmW, w, 3, dims, str, box, estr);
     if (rc) return rc;
   }
   ConvArgs g;
@@ -208,11 +180,8 @@ S6_API int sam6d_conv2d_tc(const void* x, long long ldx, int B, int Hi, int Wi, 
   S6_REQUIRE(m_tiles < (1LL << 30));
   g.m_tiles = (int)m_tiles; g.n_tiles = s6_cdiv(Cout, BN);
   g.ldr = ldr; g.r_bs = r_bs; g.ldy = ldy; g.y_bs = y_bs; g.Wy = Wy; g.sy = sy; g.sx = sx; g.oy = oy; g.ox = ox;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long ntiles = m_tiles * g.n_tiles;
-  const int grid = (int)(ntiles < sms ? ntiles : sms);
+  int grid;
+  S6_CHECK(s6_persistent_grid(m_tiles * g.n_tiles, 1, &grid));
   cudaStream_t st = s6_stream(stream);
 #define CONV_LAUNCH(OT, SL, HR)                                                                                      \
   do {                                                                                                               \

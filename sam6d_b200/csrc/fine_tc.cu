@@ -15,8 +15,6 @@
 // memory while the 256-column tiles of B stream through a 4-stage TMA ring fed by one thread of warpgroup 2.  Warpgroup g (warps 4g..4g+3) owns
 // rows [64 g, 64 g + 64) of the item: wgmma m64n256k16 into 128 registers per thread, reduced in place; a thread keeps the state
 // of its two rows across the column tiles, and the four threads of a row merge theirs with quad shuffles at the end of the item.
-#include <cuda.h>
-
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -189,33 +187,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fine_pass_kernel(const __grid_
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeFn f_get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-int f_make_map(CUtensorMap* map, const void* ptr, long long rows, int box_rows) {
-  EncodeFn enc = f_get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {256, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {512};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
 // masked template points for the ASSIGN pass: q4[b,j] = (pts2[b,j-1], 1) if column j >= 1 carries a non-background label
 __global__ void fine_masked_points_kernel(const int* __restrict__ lab2, const float* __restrict__ pts2, int S, int ld, float4* __restrict__ q4) {
   const int b = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -244,15 +215,12 @@ S6_API int sam6d_fine_pass_tc(const void* Fa, const void* Fb, int B, int S, floa
   if (mode == 2) S6_REQUIRE(q4 && wts && pred && (reinterpret_cast<uintptr_t>(q4) & 15) == 0);
   if (B == 0) return 0;
   CUtensorMap tmA, tmB;
-  int rc = f_make_map(&tmA, Fa, (long long)B * S, BM);
+  int rc = tc::make_map_2d(&tmA, Fa, (long long)B * S, 256, 256, 64, BM);
   if (rc) return rc;
-  rc = f_make_map(&tmB, Fb, (long long)B * S, BN);
+  rc = tc::make_map_2d(&tmB, Fb, (long long)B * S, 256, 256, 64, BN);
   if (rc) return rc;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int items = B * s6_cdiv(S, BM);
-  const int grid = items < sms ? items : sms;
+  int grid;
+  S6_CHECK(s6_persistent_grid(B * s6_cdiv(S, BM), 1, &grid));
   FArgs g{B, S, mode, ld_f, alpha * LOG2E, shift * LOG2E, row_f, col_f, reinterpret_cast<const float4*>(q4), out_inv, lab, wts, pred};
   cudaStream_t st = s6_stream(stream);
 #define FINE_LAUNCH(M)                                                                                              \

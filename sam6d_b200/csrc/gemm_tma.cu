@@ -8,8 +8,6 @@
 //                              into 128 fp32 registers per thread; one wgmma group stays in flight while the stage before it is
 //                              released; then alpha, bias, activation, residual -> fp32 or bf16 straight from the registers
 //                              (epilogue.cuh) while the producer already fills the ring with the next tile
-#include <cuda.h>
-
 #include "epilogue.cuh"
 #include "tc.cuh"
 
@@ -144,40 +142,6 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tma_kernel(const __grid_const
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-
-// 2-D bf16 row-major (rows, K) tensor with row stride ld (elements); box = {64, box_rows}, 128-byte swizzle
-int make_map(CUtensorMap* map, const void* ptr, long long rows, long long K, long long ld, int box_rows) {
-  EncodeFn enc = get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
-}  // namespace
-
-namespace {
-
 int launch_gemm_tma(const void* A, const void* W, const float* bias, const void* R, void* C, int c_dtype, int M, int N, int K,
                     long long lda, long long ldw, long long ldc, long long ldr, int batch, long long a_rpb, long long w_rpb,
                     long long c_bs, long long r_bs, float alpha, int act, void* stream, void* vt = nullptr, int vt_col0 = 0, int vt_S = 1,
@@ -188,15 +152,13 @@ int launch_gemm_tma(const void* A, const void* W, const float* bias, const void*
   if (M == 0 || batch == 0) return 0;
   CUtensorMap tmA, tmW;
   const long long a_rows = batch > 1 ? a_rpb * (batch - 1) + M : M, w_rows = batch > 1 ? w_rpb * (batch - 1) + N : N;
-  int rc = make_map(&tmA, A, a_rows, K, lda, BM);
+  int rc = tc::make_map_2d(&tmA, A, a_rows, K, lda, 64, BM);
   if (rc) return rc;
-  rc = make_map(&tmW, W, w_rows, K, ldw, BN);
+  rc = tc::make_map_2d(&tmW, W, w_rows, K, ldw, 64, BN);
   if (rc) return rc;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long ntiles = (long long)s6_cdiv(M, BM) * s6_cdiv(N, BN) * batch;
-  const int grid = (int)(ntiles < sms ? ntiles : sms);
+  int grid;
+  S6_CHECK(s6_persistent_grid(ntiles, 1, &grid));
   if (vt_col1 < 0) vt_col1 = N;
   Args g{bias, R, C, M, N, K, ldc, ldr, alpha, act, batch, a_rpb, w_rpb, c_bs, r_bs, vt, vt_col0, vt_S, vt_N1, vt_col1 - vt_col0,
          vt_col1, c2, ldc2};

@@ -170,13 +170,11 @@ S6_API int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const vo
   const long long npairs = clouds * S * S;
   S6_REQUIRE(npairs < (1LL << 40));
   if (npairs == 0) return 0;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const long long nblocks = (npairs + 31) / 32, want = (nblocks + LUT_THREADS / 32 - 1) / (LUT_THREADS / 32);
+  int grid;
+  S6_CHECK(s6_persistent_grid(want, 1, &grid));
   const int smem = (na + nd) * 512;
   S6_CHECK(cudaFuncSetAttribute(geo_embed_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const long long nblocks = (npairs + 31) / 32, want = (nblocks + LUT_THREADS / 32 - 1) / (LUT_THREADS / 32);
-  const int grid = (int)(want < sms ? want : sms);
   geo_embed_lut_kernel<<<grid, LUT_THREADS, smem, s6_stream(stream)>>>(
       reinterpret_cast<const float4*>(T), npairs, S, reinterpret_cast<const uint4*>(tabA), na, inv_ha, reinterpret_cast<const uint4*>(tabD),
       nd, inv_hd, reinterpret_cast<const uint4*>(far), div_term, reinterpret_cast<const uint4*>(WdT_bf16), bias, reinterpret_cast<uint4*>(E));

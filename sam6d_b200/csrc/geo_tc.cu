@@ -204,14 +204,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) geo_embed_tc_kernel(const floa
 }
 
 template <int MODE, typename ET>
-int launch_pass(const float* T, long long npairs, const float* div_term, const __nv_bfloat16* W, const float* bias, ET* E, int sms,
+int launch_pass(const float* T, long long npairs, const float* div_term, const __nv_bfloat16* W, const float* bias, ET* E,
                 cudaStream_t st) {
+  const long long per = (MODE == 0) ? 32 : 128;
+  int grid;
+  S6_CHECK(s6_persistent_grid((npairs + per - 1) / per, 1, &grid));
   auto kern = geo_embed_tc_kernel<MODE, ET>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
   if (e != cudaSuccess) return (int)e;
-  const long long per = (MODE == 0) ? 32 : 128;
-  const long long ntiles = (npairs + per - 1) / per;
-  const int grid = (int)(ntiles < sms ? ntiles : sms);
   kern<<<grid, NUM_THREADS, SMEM, st>>>(T, npairs, div_term, W, bias, E);
   return (int)cudaGetLastError();
 }
@@ -224,21 +224,18 @@ S6_API int sam6d_geo_embed_tc(const float* T, long long npairs, const float* div
                               const float* bias, void* E, int e_is_bf16, void* stream) {
   S6_REQUIRE(T && div_term && Wa_bf16 && Wd_bf16 && bias && E && npairs >= 0 && npairs < 2000000000LL);
   if (npairs == 0) return 0;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = s6_stream(stream);
   const __nv_bfloat16* Wa = reinterpret_cast<const __nv_bfloat16*>(Wa_bf16);
   const __nv_bfloat16* Wd = reinterpret_cast<const __nv_bfloat16*>(Wd_bf16);
   int rc;
   if (e_is_bf16) {
-    rc = launch_pass<1, __nv_bfloat16>(T, npairs, div_term, Wd, bias, reinterpret_cast<__nv_bfloat16*>(E), sms, st);
+    rc = launch_pass<1, __nv_bfloat16>(T, npairs, div_term, Wd, bias, reinterpret_cast<__nv_bfloat16*>(E), st);
     if (rc) return rc;
-    rc = launch_pass<0, __nv_bfloat16>(T, npairs, div_term, Wa, bias, reinterpret_cast<__nv_bfloat16*>(E), sms, st);
+    rc = launch_pass<0, __nv_bfloat16>(T, npairs, div_term, Wa, bias, reinterpret_cast<__nv_bfloat16*>(E), st);
   } else {
-    rc = launch_pass<1, float>(T, npairs, div_term, Wd, bias, reinterpret_cast<float*>(E), sms, st);
+    rc = launch_pass<1, float>(T, npairs, div_term, Wd, bias, reinterpret_cast<float*>(E), st);
     if (rc) return rc;
-    rc = launch_pass<0, float>(T, npairs, div_term, Wa, bias, reinterpret_cast<float*>(E), sms, st);
+    rc = launch_pass<0, float>(T, npairs, div_term, Wa, bias, reinterpret_cast<float*>(E), st);
   }
   return rc;
 }
@@ -249,9 +246,6 @@ S6_API int sam6d_geo_embed_dist_tc(const float* T, long long npairs, const float
                                    void* stream) {
   S6_REQUIRE(T && div_term && Wd_bf16 && bias && E && npairs >= 0 && npairs < 2000000000LL);
   if (npairs == 0) return 0;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   return launch_pass<1, __nv_bfloat16>(T, npairs, div_term, reinterpret_cast<const __nv_bfloat16*>(Wd_bf16), bias,
-                                       reinterpret_cast<__nv_bfloat16*>(E), sms, s6_stream(stream));
+                                       reinterpret_cast<__nv_bfloat16*>(E), s6_stream(stream));
 }

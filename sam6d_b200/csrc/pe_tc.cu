@@ -181,11 +181,12 @@ S6_API int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, i
   S6_REQUIRE(pts && idx && W1 && B1 && W2_bf16 && B2 && W3_bf16 && B3 && out && B >= 0 && N > 0);
   S6_REQUIRE(ns == 32 || ns == 64);
   if (B == 0) return 0;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long total = (long long)B * N;
   const long long ntiles = (total + (128 / ns) - 1) / (128 / ns);
+  // four CTAs per SM: 4 x (49 KB + static) shared memory, 4 x 128 x 128 registers.  (The occupancy API is not used: with the
+  // default carve-out it answers fewer and the grid shrinks.)
+  int grid;
+  S6_CHECK(s6_persistent_grid(ntiles, 4, &grid));
   cudaStream_t st = s6_stream(stream);
   const __nv_bfloat16* W2 = reinterpret_cast<const __nv_bfloat16*>(W2_bf16);
   const __nv_bfloat16* W3 = reinterpret_cast<const __nv_bfloat16*>(W3_bf16);
@@ -194,10 +195,6 @@ S6_API int sam6d_pe_mlp_max_tc(const float* pts, const int* idx, int B, int N, i
     S6_CHECK(cudaFuncSetAttribute(pe_tc_kernel<NSV, OT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));                 \
     /* ask for the largest shared-memory carve-out: with the default the driver sizes it for fewer resident CTAs */                   \
     S6_CHECK(cudaFuncSetAttribute(pe_tc_kernel<NSV, OT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));                     \
-    /* four CTAs per SM: 4 x (49 KB + static) shared memory, 4 x 128 x 128 registers.  (The occupancy API is not used: with   */   \
-    /* the default carve-out it answers fewer and the grid shrinks.)                                                             */   \
-    const int per_sm = 4;                                                                                                           \
-    const int grid = (int)(ntiles < (long long)sms * per_sm ? ntiles : (long long)sms * per_sm);                                    \
     pe_tc_kernel<NSV, OT><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(pts, idx, N, total, W1, B1, W2, B2, W3, B3,                         \
                                                                  reinterpret_cast<OT*>(out), out_ld, out_off);                      \
   } while (0)

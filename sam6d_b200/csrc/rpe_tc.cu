@@ -13,8 +13,6 @@
 //     threads holding a head's column write adjacent keys of s_p[b, h, n, :].
 // Persistent: one CTA per SM walks a contiguous range of the clouds*S query rows (rows are independent); warp 4 feeds a 2-stage
 // TMA ring, warps 0-3 (one warpgroup) run the MMAs and the stores.
-#include <cuda.h>
-
 #include "tc.cuh"
 
 namespace {
@@ -115,36 +113,6 @@ __global__ void __launch_bounds__(THREADS, 1) rpe_scores_tc_kernel(const __grid_
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-
-// (rows, 256) bf16 row-major, box = {64 channels, box_rows}, 128-byte swizzle
-int make_map(CUtensorMap* map, const void* ptr, long long rows, int box_rows) {
-  EncodeFn enc = get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)C * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
 }  // namespace
 
 // E (B,S,S,256) bf16 contiguous, U (B*S, 4*256) bf16 contiguous (row = the four folded per-head queries of a token)
@@ -157,14 +125,13 @@ S6_API int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, fl
   S6_REQUIRE((long long)B * S * S < 2000000000LL);
   if (B == 0) return 0;
   CUtensorMap tmE, tmU;
-  int rc = make_map(&tmE, E, (long long)B * S * S, S);
+  int rc = tc::make_map_2d(&tmE, E, (long long)B * S * S, C, C, 64, S);
   if (rc) return rc;
-  rc = make_map(&tmU, U, (long long)B * S * 4, 4);
+  rc = tc::make_map_2d(&tmU, U, (long long)B * S * 4, C, C, 64, 4);
   if (rc) return rc;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int total = B * S, grid = total < sms ? total : sms;
+  const int total = B * S;
+  int grid;
+  S6_CHECK(s6_persistent_grid(total, 1, &grid));
   S6_CHECK(cudaFuncSetAttribute(rpe_scores_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
   S6_CHECK(s6_launch_pdl(rpe_scores_tc_kernel, dim3(grid), dim3(THREADS), SMEM, s6_stream(stream), tmE, tmU, S, total, SP, sp_ld));
   S6_LAUNCH_CHECK();

@@ -18,8 +18,6 @@
 //               A row lives in the four threads of a quad: the LayerNorm statistics are two shuffles.  The warpgroups share the
 //               weight stream and nothing else.
 // Shared memory: 64 KB (hid -> y -> h half 1) + 64 KB (x -> h half 0) + 96 KB weight ring.
-#include <cuda.h>
-
 #include "tc.cuh"
 
 namespace {
@@ -212,35 +210,6 @@ __global__ void __launch_bounds__(THREADS, 1) tail_tc_kernel(const __grid_consta
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeFn>(p);
-  }
-  return fn;
-}
-
-int make_map(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_rows) {
-  EncodeFn enc = get_encode();
-  if (!enc) return 999;
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
-}
-
 }  // namespace
 
 // out = LN2(y + relu(y We^T + be) Ws^T + bs),  y = LN1(hid Wo^T + bo + x)   (PEM/model/transformer.py:176-197, 435-438)
@@ -259,15 +228,13 @@ S6_API int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const 
   if (M == 0) return 0;
   CUtensorMap tmHid, tmX, tmWo, tmWe, tmWs;
   int rc;
-  if ((rc = make_map(&tmHid, hid, M, C, ld_hid, BM))) return rc;
-  if ((rc = make_map(&tmX, x, M, C, ld_x, BM))) return rc;
-  if ((rc = make_map(&tmWo, Wo, C, C, C, 256))) return rc;
-  if ((rc = make_map(&tmWe, We, HID, C, C, 256))) return rc;
-  if ((rc = make_map(&tmWs, Ws, C, HID, HID, 256))) return rc;
-  int dev = 0, sms = 0;
-  S6_CHECK(cudaGetDevice(&dev));
-  S6_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int ntiles = s6_cdiv(M, BM), grid = ntiles < sms ? ntiles : sms;
+  if ((rc = tc::make_map_2d(&tmHid, hid, M, C, ld_hid, 64, BM))) return rc;
+  if ((rc = tc::make_map_2d(&tmX, x, M, C, ld_x, 64, BM))) return rc;
+  if ((rc = tc::make_map_2d(&tmWo, Wo, C, C, C, 64, 256))) return rc;
+  if ((rc = tc::make_map_2d(&tmWe, We, HID, C, C, 64, 256))) return rc;
+  if ((rc = tc::make_map_2d(&tmWs, Ws, C, HID, HID, 64, 256))) return rc;
+  int grid;
+  S6_CHECK(s6_persistent_grid(s6_cdiv(M, BM), 1, &grid));
   TailArgs a{bo, g1, b1, be, bs, g2, b2, M, eps};
   S6_CHECK(cudaFuncSetAttribute(tail_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
   S6_CHECK(s6_launch_pdl(tail_tc_kernel, dim3(grid), dim3(THREADS), SMEM, s6_stream(stream), tmHid, tmX, tmWo, tmWe, tmWs, a,

@@ -1,10 +1,13 @@
 // tc.cuh -- sm_90a tensor-core plumbing: mbarrier, TMA 2-D tile loads, proxy fences and warpgroup MMA (wgmma) on K-major
-// 128-byte-swizzled bf16 operands with fp32 accumulators in registers.  Inline PTX only.
+// 128-byte-swizzled bf16 operands with fp32 accumulators in registers.  Inline PTX only; the one host part is the encoding of
+// the TMA tensor maps that produce those operands.
 //
 // Accumulator fragment of one m64nN wgmma (the layout every kernel here reads its results in): thread t of the warpgroup
 // (warp w = t / 32, lane l) holds d[i], i < N/2, at row 16 w + l/4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1)
 // (frag_row / frag_col).  A row of the tile lives in the four lanes of a quad, so row reductions are two xor-shuffles.
 #pragma once
+#include <cuda.h>
+
 #include "common.cuh"
 
 namespace tc {
@@ -170,6 +173,45 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_sr
 }
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
+}
+
+// Host side: the tensor maps the loads above read.  Every map is bf16 with the 128-byte swizzle (a box of 64 channels lands as
+// the K-major slab wg_desc describes), 256-byte L2 promotion and out-of-bounds elements read as zeros.  Both encoders
+// return 0, 999 when the driver entry point is unavailable, or 1000 + the CUresult of a rejected map.
+typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+inline EncodeFn get_encode() {
+  static EncodeFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
+      return nullptr;
+    fn = reinterpret_cast<EncodeFn>(p);
+  }
+  return fn;
+}
+
+// rank-dimensional map: dims, box and element strides estr innermost first; strides_bytes of dimensions 1 .. rank-1
+inline int encode_map(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+                      const cuuint32_t* box, const cuuint32_t* estr) {
+  EncodeFn enc = get_encode();
+  if (!enc) return 999;
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, strides_bytes, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
+}
+
+// 2-D row-major (rows, cols) matrix with row stride ld (elements); box = {box_cols, box_rows}
+inline int make_map_2d(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows) {
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  return encode_map(map, ptr, 2, gdim, gstride, box, estr);
 }
 
 __device__ __forceinline__ bool elect_one() {
