@@ -151,9 +151,10 @@ int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const void* tab
  * detection concatenated, rle_off (P+1) offsets) -> mask AND depth > 0 (P,H,W) u8; stats (P,12) i32 = [0..3] raw extremes,
  * [4] pixel count, [5..8] get_bbox y1,y2,x1,x2, [9] points that survive the radius filter ||p - mean|| < thr;
  * choose2 (P,cap) i32 crop-linear pixel indices and cloud2 (P,cap,3) f32 camera-frame points of the survivors, in the
- * reference's order.  depth (H,W) f32 metres; fx, fy, cx, cy float64 intrinsics; cap >= min(H,W)^2; choose1 scratch. */
+ * reference's order.  depth (H,W) f32 metres; fx, fy, cx, cy float64 intrinsics; thr (P) f64 on the device, each detection's
+ * radius threshold float32(radius) * float32(1.2) of its object; cap >= min(H,W)^2; choose1 scratch. */
 int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
-                         double cx, double cy, double thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
+                         double cx, double cy, const double* thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
                          float* cloud2, void* stream);
 /* Stage B, the Q kept detections keep[q]: choose_idx (Q,ns) i32 sample indices (drawn by the host like the reference's
  * np.random.choice) -> pts (Q,ns,3) f32, rgb_choose (Q,ns) i64 (get_resize_rgb_choose), rgb (Q,3,S,S) f32 = crop, channel
@@ -244,8 +245,9 @@ int sam6d_sam_mask_binarize(const float* low, const int* sel, int K, int S, int 
                             unsigned char* out, void* stream);
 /* Sam.postprocess_masks: low (N,S,S) f32 -> out (N,H,W) f32 logits (the values sam6d_sam_mask_binarize thresholds) */
 int sam6d_sam_mask_upscale(const float* low, int N, int S, int big, int in_h, int in_w, int H, int W, float* out, void* stream);
-/* torchvision.ops.nms on boxes (N,4) f32 xyxy sorted by decreasing score -> keep (N) u8 */
-int sam6d_sam_nms(const float* boxes, int N, float thr, unsigned char* keep, void* stream);
+/* torchvision.ops.nms on boxes (N,4) f32 xyxy sorted by decreasing score -> keep (N) u8.  obj (N) i32 or NULL: boxes sorted by
+ * (object, decreasing score), suppression within an object only (one torchvision.ops.nms per object id) */
+int sam6d_sam_nms(const float* boxes, const int* obj, int N, float thr, unsigned char* keep, void* stream);
 
 /* ---- fused transformer-layer tail (bf16 token stream) -------------------------------------------------------------- */
 

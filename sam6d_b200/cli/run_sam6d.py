@@ -4,6 +4,10 @@ with every model built once and no file between the stages (sam6d_b200/pipeline.
     python -m sam6d_b200.cli.run_sam6d --cad_path obj.ply --rgb_path rgb.png --depth_path depth.png --cam_path camera.json \\
         --output_dir OUT [--segmentor_model sam|fastsam] [--checkpoint_dir checkpoints --checkpoint sam-6d-pem-base.pth]
 
+With several CAD models (--cad_path a.ply b.ply ... [--obj_ids 1 5 ...]) the frame runs through SAM6D.detect_objects: the ISM's
+multi-object post-processing (size filter, per-object NMS), records with category_id = the object's id (default 1, 2, ...),
+and one PEM batch across the objects; vis_pem.png draws each object's best pose with that object's points.
+
 Writes what the chained CLIs write as results: $OUT/sam6d_results/detection_ism.json, detection_pem.json and vis_pem.png,
 with the same records.  It does not write the template files ($OUT/templates/*) nor detection_ism.npz: the npz is an
 intermediate of the reference that nothing downstream reads, and writing it would copy every dense proposal mask to the
@@ -18,11 +22,19 @@ from . import ism_run_inference_custom as ism_cli
 from . import pem_run_inference_custom as pem_cli
 
 
+class _OneOrSeveral(argparse.Action):
+    """nargs="+" that stores one value as itself and several as a list"""
+
+    def __call__(self, parser, namespace, values, option_string=None):
+        setattr(namespace, self.dest, values[0] if len(values) == 1 else list(values))
+
+
 def get_parser():
     ap = argparse.ArgumentParser(description="SAM-6D: templates -> ISM -> PEM in one process")
     ap.add_argument("--segmentor_model", default="sam", choices=("sam", "fastsam"), help="The segmentor model in ISM")
     ap.add_argument("--output_dir", required=True, help="Path to root directory of the output")
-    ap.add_argument("--cad_path", required=True, help="Path to CAD(mm)")
+    ap.add_argument("--cad_path", required=True, nargs="+", action=_OneOrSeveral, help="Path to CAD(mm); several for several objects")
+    ap.add_argument("--obj_ids", type=int, nargs="+", default=None, help="category ids of the CAD models (default 1..O)")
     ap.add_argument("--rgb_path", required=True, help="Path to RGB image")
     ap.add_argument("--depth_path", required=True, help="Path to Depth image(mm)")
     ap.add_argument("--cam_path", required=True, help="Path to camera information")
@@ -51,10 +63,18 @@ def main(argv=None):
                   stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
                   points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
                   det_score_thresh=args.det_score_thresh, precision=args.precision)
-    obj = sam6d.onboard(args.cad_path, template_size=args.template_size)
+    multi = isinstance(args.cad_path, list)
+    n_cad = len(args.cad_path) if multi else 1
+    if args.obj_ids is not None and len(args.obj_ids) != n_cad:
+        raise SystemExit(f"--obj_ids: {len(args.obj_ids)} ids for {n_cad} CAD models")
+    if multi:
+        obj = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size)
+    else:
+        obj = sam6d.onboard(args.cad_path, template_size=args.template_size)
     cam = json.load(open(args.cam_path))
     rgb = pem_cli.load_im(args.rgb_path).astype("uint8")
-    res = sam6d(rgb, pem_cli.load_im(args.depth_path), cam["cam_K"], cam["depth_scale"], obj)
+    run = sam6d.detect_objects if multi else sam6d
+    res = run(rgb, pem_cli.load_im(args.depth_path), cam["cam_K"], cam["depth_scale"], obj)
     out_dir = os.path.join(args.output_dir, "sam6d_results")
     os.makedirs(out_dir, exist_ok=True)
     json.dump(res.ism, open(os.path.join(out_dir, "detection_ism.json"), "w"))
@@ -64,8 +84,26 @@ def main(argv=None):
         print(f"=> {res.reason}")
     print(f"=> {len(res.ism)} ISM detections, {len(res.pem)} poses written to {out_dir}")
     if res.pem:
-        pem_cli.write_vis(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
+        (write_vis_objects if multi else pem_cli.write_vis)(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
     return 0
+
+
+def write_vis_objects(path, frame, cam_K):
+    """vis_pem.png of a multi-object frame: the frame beside the projected box and points of each object's best-scoring poses,
+    drawn with that object's model points"""
+    print("=> visualizating ...")
+    try:
+        import cv2
+        import numpy as np
+        K = np.asarray(cam_K, dtype=np.float64).reshape(3, 3)
+        vis = frame.img
+        for o in np.unique(frame.obj):
+            rows = np.flatnonzero(frame.obj == o)
+            best = rows[frame.pose_scores[rows] == frame.pose_scores[rows].max()]
+            vis = pem_cli.draw_detections(vis, frame.pred_rot[best], frame.pred_trans[best], frame.model_points[o] * 1000, K)
+        cv2.imwrite(path, np.concatenate([frame.img, vis], axis=1)[:, :, ::-1])
+    except Exception as e:                                            # the visualisation is not part of the result
+        print(f"=> visualisation skipped: {e}", file=sys.stderr)
 
 
 if __name__ == "__main__":

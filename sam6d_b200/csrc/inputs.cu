@@ -20,7 +20,6 @@ namespace {
 struct InCfg {
   int H, W, S;               // frame size, output crop size (224)
   double fx, fy, cx, cy;
-  double thr;                // float32(radius) * float32(1.2) widened (run_inference_custom.py:209)
 };
 
 // stats row per detection (ints): 0 rmin 1 rmax 2 cmin 3 cmax (raw extremes, inclusive) 4 count | 5 y1 6 y2 7 x1 8 x2 9 n_valid
@@ -111,9 +110,11 @@ __device__ __forceinline__ int block_scan_flag(bool flag, int* warp_sums, int* t
 }
 
 // ---- 3. ordered compaction inside the bbox, centroid, radius filter (run_inference_custom.py:202-212) -----------------------
-// one CTA of 1024 threads per detection.  choose1 / choose2: (P, cap) crop-linear pixel indices, cloud2: (P, cap, 3) float32.
-__global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const unsigned char* __restrict__ mask, const float* __restrict__ depth,
-                                                           int* __restrict__ stats, int cap, int* __restrict__ choose1,
+// one CTA of 1024 threads per detection.  thr (P) float64: each detection's float32(radius) * float32(1.2) widened
+// (run_inference_custom.py:209), the radius being that of the detection's object.  choose1 / choose2: (P, cap) crop-linear pixel
+// indices, cloud2: (P, cap, 3) float32.
+__global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const double* __restrict__ thr, const unsigned char* __restrict__ mask,
+                                                           const float* __restrict__ depth, int* __restrict__ stats, int cap, int* __restrict__ choose1,
                                                            int* __restrict__ choose2, float* __restrict__ cloud2) {
   __shared__ int warp_sums[32];
   __shared__ double red[3][32];
@@ -121,6 +122,7 @@ __global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const unsign
   const int p = blockIdx.x, tid = threadIdx.x;
   int* s = stats + p * ST;
   if (s[4] <= 32) { if (tid == 0) s[9] = 0; return; }       // np.sum(mask) > 32 else continue (:199-203)
+  const double th = thr[p];
   const int y1 = s[5], y2 = s[6], x1 = s[7], x2 = s[8];
   const int ch = y2 - y1, cw = x2 - x1, area = ch * cw;
   const unsigned char* m = mask + (size_t)p * g.H * g.W;
@@ -165,7 +167,7 @@ __global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const unsign
       i = c1[k];
       cam_point(g, depth, y1 + i / cw, x1 + i % cw, px, py, pz);
       const double dx = px - center[0], dy = py - center[1], dz = pz - center[2];
-      keep = sqrt(dx * dx + dy * dy + dz * dz) < g.thr;
+      keep = sqrt(dx * dx + dy * dy + dz * dz) < th;
     }
     int tot;
     const int pos = block_scan_flag(keep, warp_sums, &tot);
@@ -264,13 +266,14 @@ __global__ void inp_init_stats_kernel(int* __restrict__ stats, int P) {
 }  // namespace
 
 // Stage A.  rle_cum: cumulative run ends of every detection's uncompressed COCO RLE (column-major), concatenated; rle_off (P+1)
-// offsets into it.  depth (H,W) f32 metres; fx, fy, cx, cy the float64 intrinsics; thr = float32(radius) * float32(1.2).
+// offsets into it.  depth (H,W) f32 metres; fx, fy, cx, cy the float64 intrinsics; thr (P) f64 on the device, per detection
+// float32(radius) * float32(1.2) of its object.
 // mask (P,H,W) u8 out.  stats (P,12) i32 out: [0..3] raw extremes, [4] pixel count, [5..8] bbox y1,y2,x1,x2, [9] points that
 // survive the radius filter.  choose1 / choose2 (P,cap) i32, cloud2 (P,cap,3) f32 scratch / out, cap >= min(H,W)^2.
 S6_API int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
-                                double cx, double cy, double thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
+                                double cx, double cy, const double* thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
                                 float* cloud2, void* stream) {
-  S6_REQUIRE(rle_cum && rle_off && depth && mask && stats && choose1 && choose2 && cloud2 && P >= 0 && H > 0 && W > 0 &&
+  S6_REQUIRE(rle_cum && rle_off && depth && thr && mask && stats && choose1 && choose2 && cloud2 && P >= 0 && H > 0 && W > 0 &&
              cap >= min(H, W) * min(H, W));
   if (P == 0) return 0;
   cudaStream_t st = s6_stream(stream);
@@ -281,8 +284,8 @@ S6_API int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, i
   S6_LAUNCH_CHECK();
   inp_bbox_kernel<<<s6_cdiv(P, 128), 128, 0, st>>>(stats, P, H, W);
   S6_LAUNCH_CHECK();
-  InCfg g{H, W, 0, fx, fy, cx, cy, thr};
-  inp_compact_kernel<<<P, 1024, 0, st>>>(g, mask, depth, stats, cap, choose1, choose2, cloud2);
+  InCfg g{H, W, 0, fx, fy, cx, cy};
+  inp_compact_kernel<<<P, 1024, 0, st>>>(g, thr, mask, depth, stats, cap, choose1, choose2, cloud2);
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -403,7 +403,10 @@ __global__ void __launch_bounds__(256) sam_mask_upscale_kernel(const float* __re
 }
 
 // ---- NMS over boxes sorted by decreasing score (torchvision.ops.nms): keep[i] = 1 for survivors; one CTA -----------------------------------
-__global__ void __launch_bounds__(1024) sam_nms_kernel(const float* __restrict__ boxes, int N, float thr, unsigned char* __restrict__ keep) {
+// With obj != null the boxes are sorted by (object, decreasing score) and a box suppresses only boxes of its own object
+// (Detections.apply_nms_per_object_id: one torchvision.ops.nms per object id, in one launch).
+__global__ void __launch_bounds__(1024) sam_nms_kernel(const float* __restrict__ boxes, const int* __restrict__ obj, int N, float thr,
+                                                       unsigned char* __restrict__ keep) {
   extern __shared__ unsigned char dead[];       // N
   for (int i = threadIdx.x; i < N; i += 1024) dead[i] = 0;
   __syncthreads();
@@ -411,8 +414,9 @@ __global__ void __launch_bounds__(1024) sam_nms_kernel(const float* __restrict__
     if (!dead[i]) {                              // uniform across the block (read after the barrier below)
       const float x1 = boxes[i * 4], y1 = boxes[i * 4 + 1], x2 = boxes[i * 4 + 2], y2 = boxes[i * 4 + 3];
       const float ai = (x2 - x1) * (y2 - y1);
+      const int oi = obj ? obj[i] : 0;
       for (int j = i + 1 + threadIdx.x; j < N; j += 1024) {
-        if (dead[j]) continue;
+        if (dead[j] || (obj && obj[j] != oi)) continue;
         const float a1 = boxes[j * 4], b1 = boxes[j * 4 + 1], a2 = boxes[j * 4 + 2], b2 = boxes[j * 4 + 3];
         const float iw = fmaxf(fminf(x2, a2) - fmaxf(x1, a1), 0.f), ih = fmaxf(fminf(y2, b2) - fmaxf(y1, b1), 0.f);
         const float inter = iw * ih, aj = (a2 - a1) * (b2 - b1);
@@ -541,12 +545,13 @@ S6_API int sam6d_sam_mask_upscale(const float* low, int N, int S, int big, int i
   return 0;
 }
 
-// boxes (N,4) f32 xyxy sorted by decreasing score -> keep (N) u8; N <= 65536
-S6_API int sam6d_sam_nms(const float* boxes, int N, float thr, unsigned char* keep, void* stream) {
+// boxes (N,4) f32 xyxy sorted by decreasing score -> keep (N) u8; N <= 65536.  obj (N) i32 or NULL: with object ids the boxes
+// are sorted by (object, decreasing score) and suppression stays within an object.
+S6_API int sam6d_sam_nms(const float* boxes, const int* obj, int N, float thr, unsigned char* keep, void* stream) {
   S6_REQUIRE(boxes && keep && N >= 0 && N <= 65536);
   if (N == 0) return 0;
   S6_CHECK(cudaFuncSetAttribute(sam_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-  sam_nms_kernel<<<1, 1024, N, s6_stream(stream)>>>(boxes, N, thr, keep);
+  sam_nms_kernel<<<1, 1024, N, s6_stream(stream)>>>(boxes, obj, N, thr, keep);
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -406,7 +406,7 @@ class FastSAM:
         keep = torch.empty(rows.shape[0], dtype=torch.uint8, device=rows.device)
         if rows.shape[0]:
             boxes = rows[:, :4].contiguous()
-            _lib.call("sam6d_sam_nms", _p(boxes), rows.shape[0], ctypes.c_float(self.iou), _p(keep), _s())
+            _lib.call("sam6d_sam_nms", _p(boxes), None, rows.shape[0], ctypes.c_float(self.iou), _p(keep), _s())
         rows = rows[keep.bool()][:self.max_det].contiguous()
         masks = torch.empty(rows.shape[0], ih, iw, dtype=torch.uint8, device=rows.device)
         if rows.shape[0]:

@@ -46,9 +46,10 @@ def pack_rle(dets: Sequence[Dict], H: int, W: int):
 
 
 class FrameInputs:
-    """device-side state of one frame between the two stages"""
+    """device-side state of one frame between the two stages.  radius: the object radius (one number for every detection) or
+    one radius per detection (several objects in a frame)"""
 
-    def __init__(self, dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, radius: float, device=None):
+    def __init__(self, dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, radius, device=None):
         self.device = torch.device(device if device is not None else "cuda")
         self.dets = list(dets)
         if image_u8.ndim == 2:                                                     # run_inference_custom.py:177-178
@@ -59,8 +60,9 @@ class FrameInputs:
         whole_depth = depth_raw.astype(np.float32) * depth_scale / 1000.0          # :179 (float32 * python floats)
         self.depth = torch.from_numpy(np.ascontiguousarray(whole_depth, dtype=np.float32)).to(self.device)
         self.image = torch.from_numpy(np.ascontiguousarray(image_u8, dtype=np.uint8)).to(self.device)
-        self.thr = float(np.float32(radius) * np.float32(1.2))                     # :209 under numpy >= 2 (weak python scalar)
         P = len(self.dets)
+        radius = np.broadcast_to(np.asarray(radius, dtype=np.float32), (P,))
+        self.thr = (radius * np.float32(1.2)).astype(np.float64)                   # :209 under numpy >= 2 (weak python scalar)
         cum, off = pack_rle(self.dets, self.H, self.W)
         self.cap = min(self.H, self.W) ** 2
         dev = self.device
@@ -72,8 +74,9 @@ class FrameInputs:
         if P:
             cum_d = torch.from_numpy(cum).to(dev) if len(cum) else torch.zeros(1, dtype=torch.int32, device=dev)
             off_d = torch.from_numpy(off).to(dev)
+            thr_d = torch.from_numpy(self.thr).to(dev)
             _lib.call("sam6d_inputs_stage_a", _p(cum_d), _p(off_d), P, self.H, self.W, _p(self.depth), float(K[0, 0]), float(K[1, 1]),
-                      float(K[0, 2]), float(K[1, 2]), self.thr, _p(self.mask), _p(self.stats), self.cap, _p(self.choose1),
+                      float(K[0, 2]), float(K[1, 2]), _p(thr_d), _p(self.mask), _p(self.stats), self.cap, _p(self.choose1),
                       _p(self.choose2), _p(self.cloud2), _stream())
         self.stats_host = self.stats.cpu().numpy() if P else np.zeros((0, ST), np.int32)
 
@@ -124,13 +127,21 @@ def draw_choose_idx(n_valid: Sequence[int], n_sample: int, rng=None) -> np.ndarr
 
 def get_test_data(dets: List[Dict], whole_image: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, model_points: np.ndarray,
                   det_score_thresh: float = 0.2, n_sample_observed_point: int = 2048, img_size: int = 224, rgb_mask_flag: bool = True,
-                  choose_idx: Optional[np.ndarray] = None, rng=None, device=None):
+                  choose_idx: Optional[np.ndarray] = None, rng=None, device=None, det_obj: Optional[Sequence[int]] = None):
     """The reference's get_test_data after its file reads (the caller loads rgb / depth / camera / detections / CAD samples).
     model_points: (n,3) float32 CAD samples in metres (the reference draws them with trimesh, :182-184).
-    -> (ret_dict, whole_image, whole_pts (H*W,3), model_points, all_dets) like the reference."""
-    dets = [d for d in dets if d["score"] > det_score_thresh]                        # :168-171
+    -> (ret_dict, whole_image, whole_pts (H*W,3), model_points, all_dets) like the reference.
+    Several objects: model_points (O,n,3) and det_obj the object index of every detection in `dets`.  Each detection then gets
+    its object's radius filter and `model` rows; ret_dict["obj"] (P) int64 holds the object index of every kept one and
+    ret_dict["choose_idx"] the sample indices drawn for it."""
+    sel = [i for i, d in enumerate(dets) if d["score"] > det_score_thresh]           # :168-171
+    dets = [dets[i] for i in sel]
     model_points = np.asarray(model_points, dtype=np.float32)
-    radius = np.max(np.linalg.norm(model_points, axis=1))                            # :184
+    if det_obj is None:
+        radius = np.max(np.linalg.norm(model_points, axis=1))                        # :184
+    else:
+        det_obj = np.asarray(det_obj, dtype=np.int64)[sel]
+        radius = np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in model_points])[det_obj]
     frame = FrameInputs(dets, whole_image, depth_raw, cam_K, depth_scale, radius, device)
     keep = frame.kept()
     if choose_idx is None:
@@ -138,10 +149,16 @@ def get_test_data(dets: List[Dict], whole_image: np.ndarray, depth_raw: np.ndarr
     pts, rgb_choose, rgb, _ = frame.sample(keep, np.asarray(choose_idx), img_size, rgb_mask_flag)
     dev = frame.device
     n = len(keep)
+    if det_obj is None:
+        model = torch.from_numpy(model_points).to(dev).unsqueeze(0).repeat(n, 1, 1)
+    else:
+        obj = torch.from_numpy(det_obj[keep]).to(dev)
+        model = torch.from_numpy(model_points).to(dev)[obj]
     ret = dict(pts=pts, rgb=rgb, rgb_choose=rgb_choose,
-               score=torch.tensor([dets[i]["score"] for i in keep], dtype=torch.float32, device=dev),
-               model=torch.from_numpy(model_points).to(dev).unsqueeze(0).repeat(n, 1, 1),
+               score=torch.tensor([dets[i]["score"] for i in keep], dtype=torch.float32, device=dev), model=model,
                K=torch.tensor(np.asarray(cam_K, dtype=np.float64).reshape(3, 3), dtype=torch.float32, device=dev).unsqueeze(0).repeat(n, 1, 1))
+    if det_obj is not None:
+        ret["obj"], ret["choose_idx"] = obj, np.asarray(choose_idx)
     return ret, whole_image, frame.whole_points(), model_points, [dets[i] for i in keep]
 
 

@@ -11,6 +11,10 @@ Geometric score (csrc/ism_geo.cu):
          Calculate_the_query_translation            ISM/model/detector.py:237-250, ISM/utils/trimesh_utils.py:77-105
          project_template_to_image                  ISM/model/detector.py:209-235
          compute_geometric_score (IoU part)         ISM/model/detector.py:311-323, ISM/utils/bbox_utils.py:197-221
+
+Multi-object post-processing of Instance_Segmentation_Model.test_step (ISM/model/detector.py:324-391):
+         Detections.remove_very_small_detections    ISM/model/utils.py:96-105
+         Detections.apply_nms_per_object_id         ISM/model/utils.py:107-119 (csrc/sam_dec.cu: sam_nms_kernel with object ids)
 """
 import ctypes
 from types import SimpleNamespace
@@ -132,3 +136,33 @@ def compute_geometric_iou(poses, pointcloud, best_pose, pred_object_idx, masks, 
     r = project_template_iou(poses, pointcloud, best_pose, pred_object_idx, tr, cam_intrinsic, (H, W), boxes)
     iou = torch.where(r["ok"].all(), r["iou"], torch.zeros_like(r["iou"]))
     return iou, r["xyxy"], tr
+
+
+# ---------------------------------------------------------------------------------------------- multi-object post-processing
+MIN_BOX_SIZE, MIN_MASK_SIZE, NMS_THRESH = 0.05, 3e-4, 0.25      # ISM/configs/model/ISM_sam.yaml post_processing_config
+
+
+@torch.no_grad()
+def remove_very_small_detections(masks, boxes, min_box_size=MIN_BOX_SIZE, min_mask_size=MIN_MASK_SIZE):
+    """Detections.remove_very_small_detections: masks (N,H,W), boxes (N,4) int64 xyxy -> keep (N,) bool on their device: box
+    and mask area relative to the image above min_box_size^2 and min_mask_size.  The areas are reduced where the masks are."""
+    img_area = masks.shape[1] * masks.shape[2]
+    box_areas = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1]) / img_area        # torchvision box_area
+    mask_areas = masks.sum(dim=(1, 2)) / img_area
+    return torch.logical_and(box_areas > min_box_size ** 2, mask_areas > min_mask_size)
+
+
+@torch.no_grad()
+def nms_per_object(boxes, scores, object_ids, nms_thresh=NMS_THRESH):
+    """Detections.apply_nms_per_object_id: one torchvision.ops.nms per object id, as one launch over the boxes sorted by
+    (object, decreasing score) -> kept indices (K,) int64 in the reference's order: object ids ascending, within an object
+    by decreasing score (ties in proposal order)"""
+    if boxes.shape[0] == 0:
+        return torch.zeros(0, dtype=torch.long, device=boxes.device)
+    order = torch.argsort(scores.float(), descending=True, stable=True)
+    order = order[torch.argsort(object_ids[order], stable=True)]
+    b = boxes[order].float().contiguous()
+    obj = object_ids[order].to(torch.int32).contiguous()
+    keep = torch.empty(b.shape[0], dtype=torch.uint8, device=b.device)
+    _lib.call("sam6d_sam_nms", _p(b), _p(obj), b.shape[0], ctypes.c_float(nms_thresh), _p(keep), _s())
+    return order[keep.bool()]

@@ -6,6 +6,11 @@ which keeps the models resident, onboards an object once and runs one RGB-D fram
     obj = sam6d.onboard("obj_000005.ply")                   # 42 templates rendered on the GPU, ISM + PEM template banks
     res = sam6d(rgb_u8, depth_u16, cam_K, depth_scale, obj)  # res.ism / res.pem: the CLIs' BOP-23 records; res.R, res.t
 
+Several known objects in a frame (Instance_Segmentation_Model.test_step for the ISM, one PEM batch across the objects):
+
+    objs = sam6d.onboard_objects(["obj_000001.ply", "obj_000005.ply"], obj_ids=[1, 5])
+    res = sam6d.detect_objects(rgb_u8, depth_u16, cam_K, depth_scale, objs)   # records carry category_id = obj_ids[object]
+
 The CLIs (sam6d_b200.cli.{render_custom_templates, ism_run_inference_custom, pem_run_inference_custom}) are file I/O around
 the same stage functions, so one `SAM6D` frame computes what the chained CLIs compute from the same inputs and seeds.  Between
 the ISM and the PEM the proposal masks stay on the device: their RLE is built by a kernel (ops.mask_rle) and only the run
@@ -75,7 +80,7 @@ def ism_reference_features(desc, rgbs: np.ndarray, masks: np.ndarray, device):
 @dataclass
 class IsmGeometry:
     """what the geometric score needs: template poses (T,4,4) f32 (metres), template cloud (npc,3) f32 (metres), depth (H,W) i32,
-    K (3,3) as read, depth scale -- all on the device but the scale"""
+    K (3,3) as read, depth scale -- all on the device but the scale.  Several objects: poses (O,T,4,4) and cloud (O,npc,3)."""
     poses: torch.Tensor
     cloud: torch.Tensor
     depth: torch.Tensor
@@ -92,33 +97,43 @@ def ism_geometry(poses_m, cloud_m, depth_raw, cam_K, depth_scale, device) -> Ism
 
 # ---- segment -> describe -> score (ISM/run_inference_custom.py:167-209) -------------------------------------------------------
 def ism_detect(seg, desc, ref_cls, ref_patch, rgb_u8: np.ndarray, confidence_thresh: float, geometry: Optional[IsmGeometry] = None,
-               mark=None):
-    """-> SimpleNamespace(masks (N,H,W) f32, boxes (N,4) i64 xyxy, scores (N) f32, n_proposals, reason): the proposals above the
-    semantic-score threshold with their final scores ((semantic + appearance + geometric x visible) / (2 + visible), or
-    (semantic + appearance) / 2 without geometry).  reason is None, or why there is no detection.  mark(stage) is called after
-    the segmentor, the descriptors and the scores (stage timing)."""
+               mark=None, remove_small: bool = False):
+    """-> SimpleNamespace(masks (N,H,W) f32, boxes (N,4) i64 xyxy, scores (N) f32, obj (N) i64, n_proposals, reason): the
+    proposals above the semantic-score threshold with their final scores ((semantic + appearance + geometric x visible) /
+    (2 + visible), or (semantic + appearance) / 2 without geometry) and the object each is assigned to.  ref_cls (T,C) and
+    ref_patch (T,256,C) of one object, or (O,T,C) and (O,T,256,C) of several (geometry then holds every object's poses and
+    cloud).  remove_small: Detections.remove_very_small_detections after the segmentor, as Instance_Segmentation_Model.test_step
+    does.  reason is None, or why there is no detection.  mark(stage) is called after the segmentor, the descriptors and the
+    scores (stage timing)."""
     from .dinov2 import MaskedPatch_MatrixSimilarity
     mark = mark or (lambda stage: None)
+    if ref_cls.dim() == 2:
+        ref_cls, ref_patch = ref_cls.unsqueeze(0), ref_patch.unsqueeze(0)
     det = seg.generate_masks(rgb_u8)
-    det = SimpleNamespace(masks=det["masks"], boxes=det["boxes"].long(), scores=None, n_proposals=int(det["masks"].shape[0]), reason=None)
+    det = SimpleNamespace(masks=det["masks"], boxes=det["boxes"].long(), scores=None, obj=None, n_proposals=int(det["masks"].shape[0]),
+                          reason=None)
+    if remove_small and det.n_proposals:
+        keep = ism.remove_very_small_detections(det.masks, det.boxes).nonzero().flatten()
+        det.masks, det.boxes = det.masks[keep], det.boxes[keep]
     mark("segmentor")
-    if det.n_proposals == 0:
+    if det.masks.shape[0] == 0:
         det.reason = "no mask proposal survived the filters"
         return det
     q_cls, q_patch = desc(rgb_u8, det)
     mark("descriptors")
-    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_cls.unsqueeze(0), "avg_5", confidence_thresh)
-    det.masks, det.boxes, q_patch = det.masks[idx_sel], det.boxes[idx_sel], q_patch[idx_sel]
+    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_cls, "avg_5", confidence_thresh)
+    det.masks, det.boxes, det.obj, q_patch = det.masks[idx_sel], det.boxes[idx_sel], pred_obj, q_patch[idx_sel]
     if idx_sel.numel() == 0:
         det.reason = "no proposal above the semantic-score threshold"
         mark("scores")
         return det
-    ref_aux = ref_patch.unsqueeze(0)[pred_obj, best_t, ...]
+    ref_aux = ref_patch[pred_obj, best_t, ...]
     appe, vis = MaskedPatch_MatrixSimilarity().scores(q_patch, ref_aux, ism_cli.VISIBLE_THRED)
     if geometry is not None:
         g = geometry
-        geo, _, _ = ism.compute_geometric_iou(g.poses, g.cloud, best_t, torch.zeros_like(best_t), det.masks, g.depth, g.K, g.depth_scale,
-                                              det.boxes)
+        # each proposal's template pose among all objects' poses (O*T,4,4): row obj*T + t
+        geo, _, _ = ism.compute_geometric_iou(g.poses.reshape(-1, 4, 4), g.cloud, pred_obj * ref_cls.shape[1] + best_t, pred_obj, det.masks,
+                                              g.depth, g.K, g.depth_scale, det.boxes)
         det.scores = (sem + appe + geo * vis) / (1 + 1 + vis)
     else:
         det.scores = (sem + appe) / 2
@@ -133,10 +148,11 @@ def rle_counts(rle_cum: np.ndarray, rle_off: np.ndarray):
     return [np.diff(rle_cum[rle_off[i]:rle_off[i + 1]], prepend=0).tolist() for i in range(len(rle_off) - 1)]
 
 
-def ism_records(boxes_xyxy: np.ndarray, scores: np.ndarray, counts, hw, runtime: float):
-    """ISM detections -> the ISM CLI's JSON records (scene 0, image 0, category 1, bbox xywh)"""
+def ism_records(boxes_xyxy: np.ndarray, scores: np.ndarray, counts, hw, runtime: float, category_ids=None):
+    """ISM detections -> the ISM CLI's JSON records (scene 0, image 0, category 1 or category_ids[i], bbox xywh)"""
     b = boxes_xyxy
-    return [dict(scene_id=0, image_id=0, category_id=1, bbox=[int(b[i, 0]), int(b[i, 1]), int(b[i, 2] - b[i, 0]), int(b[i, 3] - b[i, 1])],
+    cats = [1] * len(b) if category_ids is None else [int(c) for c in category_ids]
+    return [dict(scene_id=0, image_id=0, category_id=cats[i], bbox=[int(b[i, 0]), int(b[i, 1]), int(b[i, 2] - b[i, 0]), int(b[i, 3] - b[i, 1])],
                  score=float(scores[i]), time=float(runtime), segmentation={"counts": counts[i], "size": [int(hw[0]), int(hw[1])]})
             for i in range(len(b))]
 
@@ -161,29 +177,38 @@ def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
 
 # ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
 def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
-              generator: Optional[torch.Generator] = None, device=None, mark=None):
+              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None):
     """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
     enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
     model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
-    else from torch's global CUDA generator (the reference's torch.rand).  mark(stage) after the inputs and after the forward."""
+    else from torch's global CUDA generator (the reference's torch.rand).  mark(stage) after the inputs and after the forward.
+    Several objects: bank (O,2048,3), (O,2048,256), model_points_m (O,n,3) and det_obj the object index of every record; each
+    detection gets its object's radius filter, model points and template bank, and all run as one batch.  The frame then also
+    holds obj (P) int64, choose_idx (P,2048) and rand, the coarse stage's uniforms."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
     input_data, img, _, model_points, kept = inputs.get_test_data(
         [dict(d) for d in dets], rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh,
-        cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device)
+        cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device, det_obj=det_obj)
     n = input_data["pts"].size(0)
     mark("pem_inputs")
-    out = None
+    out = rand = None
     if n:
         with torch.no_grad():
-            input_data["dense_po"] = bank[0].repeat(n, 1, 1)
-            input_data["dense_fo"] = bank[1].repeat(n, 1, 1)
-            rand = None
+            if det_obj is None:
+                input_data["dense_po"] = bank[0].repeat(n, 1, 1)
+                input_data["dense_fo"] = bank[1].repeat(n, 1, 1)
+            else:
+                input_data["dense_po"] = bank[0][input_data["obj"]]
+                input_data["dense_fo"] = bank[1][input_data["obj"]]
             if generator is not None:
                 rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
             out = model(input_data, rand=rand)
     mark("forward")
-    return SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
+    frame = SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
+    if det_obj is not None:
+        frame.obj, frame.choose_idx, frame.rand = input_data["obj"].cpu().numpy(), input_data["choose_idx"], rand
+    return frame
 
 
 def pem_records(frame):
@@ -251,33 +276,97 @@ class SAM6D:
         model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
         return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses), cloud, bank, model_points)
 
+    def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
+        """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
+        obj_ids: the category id of every object (distinct ints), default 1..O.  The fp32 patch tokens (44 MB per object at
+        C = 1024) are copied into the stack as each object is built, so only one object's extra copy is alive at a time."""
+        meshes = list(meshes)
+        n = len(meshes)
+        obj_ids = list(range(1, n + 1)) if obj_ids is None else [int(i) for i in obj_ids]
+        if n == 0 or len(obj_ids) != n or len(set(obj_ids)) != n:
+            raise ValueError(f"onboard_objects: {n} meshes need {n} distinct obj_ids, got {obj_ids}")
+        parts, ref_patch = [], None
+        for o, mesh in enumerate(meshes):
+            ob = self.onboard(mesh, template_size, rng)
+            if ref_patch is None:
+                ref_patch = ob.ref_patch.new_empty((n,) + tuple(ob.ref_patch.shape))
+            ref_patch[o] = ob.ref_patch
+            ob.ref_patch = None
+            parts.append(ob)
+        return ObjectSet.stack(parts, ref_patch, obj_ids)
+
     def __call__(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, obj: Onboarded, rng=None, mark=None):
         """one RGB-D frame: rgb (H,W,3) u8, depth (H,W) raw u16, cam_K (9 values) and depth_scale as camera.json holds them.
         -> SimpleNamespace(ism, pem: the CLIs' records; masks (N,H,W) f32, boxes (N,4) i64, scores (N) f32 of the ISM detections;
         R (P,3,3), t (P,3) metres of the PEM's, on the device).  `rng` draws the observed-point samples (default numpy's global
         RNG); the coarse stage's uniforms come from a fresh torch generator seeded with the PEM's RD_SEED, so a frame's poses
         do not depend on earlier frames.  mark(stage), when given, is called after each stage (stage timing)."""
+        return self._frame(rgb_u8, depth_raw, cam_K, depth_scale, obj, None, rng, mark)
+
+    def detect_objects(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, objects: "ObjectSet", rng=None, mark=None):
+        """one RGB-D frame with several onboarded objects, the fields of __call__ plus obj (N) i64, the object index of every ISM
+        detection.  The ISM follows Instance_Segmentation_Model.test_step: proposals, remove_very_small_detections, descriptors,
+        semantic score over all objects, appearance score against the assigned object's best template, geometric score with
+        that object's cloud and template pose, final score, apply_nms_per_object_id (records ordered by object, then by
+        decreasing score; category_id = obj_ids[object]).  The PEM runs every kept detection in one Net.forward batch, each
+        with its object's radius filter, model points and template bank; sample indices are drawn in detection order.
+        mark(stage) as for __call__, plus "nms"."""
+        return self._frame(rgb_u8, depth_raw, cam_K, depth_scale, objects, objects.obj_ids, rng, mark)
+
+    def _frame(self, rgb_u8, depth_raw, cam_K, depth_scale, obj, obj_ids, rng, mark):
+        multi = obj_ids is not None
         mark = mark or (lambda stage: None)
         t0 = time.time()
         geometry = ism_geometry(obj.poses_m, obj.cloud_m, depth_raw, cam_K, depth_scale, self.device)
-        det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark)
+        det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark, remove_small=multi)
+        if multi and det.reason is None:
+            keep = ism.nms_per_object(det.boxes, det.scores, det.obj)
+            det.masks, det.boxes, det.scores, det.obj = det.masks[keep], det.boxes[keep], det.scores[keep], det.obj[keep]
+            mark("nms")
         if det.reason is not None:
             mark("rle")
             mark("ism_records")
             return SimpleNamespace(ism=[], pem=[], masks=det.masks, boxes=det.boxes, scores=det.scores, R=None, t=None, frame=None,
-                                   n_proposals=det.n_proposals, reason=det.reason)
+                                   n_proposals=det.n_proposals, reason=det.reason, **({"obj": det.obj} if multi else {}))
         cum, off = ops.mask_rle(det.masks.contiguous())
         mark("rle")
         counts = rle_counts(cum.cpu().numpy(), off.cpu().numpy())
-        records = ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), counts, det.masks.shape[1:], time.time() - t0)
+        det_obj = det.obj.cpu().numpy() if multi else None
+        records = ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), counts, det.masks.shape[1:], time.time() - t0,
+                              category_ids=np.asarray(obj_ids)[det_obj] if multi else None)
         mark("ism_records")
         g = torch.Generator(device=self.device)
         g.manual_seed(pem_cli.RD_SEED)
         frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
-                          rng=rng, generator=g, device=self.device, mark=mark)
+                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj)
         pem = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
         t = frame.out["pred_t"] if frame.out is not None else None
         return SimpleNamespace(ism=records, pem=pem, masks=det.masks, boxes=det.boxes, scores=det.scores, R=R, t=t, frame=frame,
-                               n_proposals=det.n_proposals, reason=None)
+                               n_proposals=det.n_proposals, reason=None, **({"obj": det.obj} if multi else {}))
+
+
+@dataclass
+class ObjectSet:
+    """several objects after SAM6D.onboard_objects, stacked along a leading object axis O: ISM references ref_cls (O,T,C) and
+    ref_patch (O,T,256,C), template poses poses_m (O,T,4,4) (the framing distance depends on the mesh), geometric-score clouds
+    cloud_m (O,2048,3), PEM template banks (O,2048,3) and (O,2048,256), model points model_points_m (O,Nm,3), each object's
+    radius (O,) (the PEM's max |model point|) and category ids obj_ids"""
+    ref_cls: torch.Tensor
+    ref_patch: torch.Tensor
+    poses_m: np.ndarray
+    cloud_m: np.ndarray
+    bank: tuple
+    model_points_m: np.ndarray
+    radii: np.ndarray
+    obj_ids: list
+
+    @staticmethod
+    def stack(parts, ref_patch, obj_ids) -> "ObjectSet":
+        """Onboarded objects (their ref_patch already stacked into `ref_patch`) -> ObjectSet"""
+        mp = np.stack([np.asarray(p.model_points_m, dtype=np.float32) for p in parts])
+        return ObjectSet(ref_cls=torch.stack([p.ref_cls for p in parts]), ref_patch=ref_patch,
+                         poses_m=np.stack([p.poses_m for p in parts]), cloud_m=np.stack([p.cloud_m for p in parts]),
+                         bank=tuple(torch.stack([p.bank[i].reshape(p.bank[i].shape[-2:]) for p in parts]) for i in range(2)),
+                         model_points_m=mp, radii=np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp]), obj_ids=list(obj_ids))

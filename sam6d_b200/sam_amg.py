@@ -729,7 +729,7 @@ class CustomSamAutomaticMaskGenerator:
         order = torch.argsort(scores, descending=True, stable=True)
         b = boxes[order].float().contiguous()
         keep = torch.empty(b.shape[0], dtype=torch.uint8, device=b.device)
-        _lib.call("sam6d_sam_nms", _p(b), b.shape[0], ctypes.c_float(thr), _p(keep), _s())
+        _lib.call("sam6d_sam_nms", _p(b), None, b.shape[0], ctypes.c_float(thr), _p(keep), _s())
         return order[keep.bool()]
 
     @torch.no_grad()

@@ -14,7 +14,12 @@ descriptor model runs on all of them in any case), and det_score_thresh is set b
 score so that --pem_dets detections reach the PEM.  The count after each filter is reported beside the times.
 The card's name, power limit and SM clocks are read with nvidia-smi in the same run.  Without a CUDA device it fails.
 
-    python tools/sam6d_frame_bench.py [--frames 10] [--warmup 2] [--pem_dets 8] [--configs sam_vit_h,sam_vit_b,fastsam] --out FILE"""
+With --objects 1,8,21 the first configuration instead times SAM6D.detect_objects on O onboarded objects for each O (the
+example CAD at O distinct scales, ids 1..O): the stages above plus the per-object NMS ("nms"), onboard_objects' cost, and the
+counts after each filter.
+
+    python tools/sam6d_frame_bench.py [--frames 10] [--warmup 2] [--pem_dets 8] [--configs sam_vit_h,sam_vit_b,fastsam]
+                                      [--objects 1,8,21] --out FILE"""
 import argparse
 import json
 import os
@@ -35,6 +40,7 @@ CONFIGS = {
     "fastsam": dict(segmentor="fastsam"),
 }
 STAGES = ("segmentor", "descriptors", "scores", "rle", "ism_records", "pem_inputs", "forward", "pem_records")
+MULTI_STAGES = ("segmentor", "descriptors", "scores", "nms", "rle", "ism_records", "pem_inputs", "forward", "pem_records")
 
 
 def _card():
@@ -68,8 +74,8 @@ def _example(tmp):
 class StageClock:
     """mark(stage): synchronise the device, add the host time since the previous mark to that stage"""
 
-    def __init__(self):
-        self.acc = {s: 0.0 for s in STAGES}
+    def __init__(self, stages=STAGES):
+        self.acc = {s: 0.0 for s in stages}
         self.t = None
 
     def start(self):
@@ -145,12 +151,55 @@ def bench(name, cad, frame, args):
     return out
 
 
+def bench_objects(name, cad, frame, n_objects, args):
+    """one detect_objects frame on n_objects objects: the example CAD scaled by 0.6 .. 1.4, ids 1..O"""
+    from sam6d_b200 import meshio
+    from sam6d_b200.pipeline import SAM6D
+    model = SAM6D(**CONFIGS[name], dinov2_model="dinov2_vitl14", precision="bf16", random_weights=True, confidence_thresh=-1,
+                  det_score_thresh=-1)
+    base = meshio.load_ply_mesh(cad)
+    scales = np.linspace(0.6, 1.4, n_objects) if n_objects > 1 else [1.0]
+    meshes = [meshio.Mesh(vertices=(base.vertices * s).astype(np.float32), faces=base.faces, colors=base.colors) for s in scales]
+    model.onboard_objects(meshes[:1], template_size=512, rng=np.random.RandomState(0))      # warm-up
+    torch.cuda.synchronize()
+    t = time.perf_counter()
+    objs = model.onboard_objects(meshes, template_size=512, rng=np.random.RandomState(0))
+    torch.cuda.synchronize()
+    onboard_ms = (time.perf_counter() - t) * 1e3
+    res = model.detect_objects(*frame, objs, rng=np.random.RandomState(5))
+    s = sorted((r["score"] for r in res.ism), reverse=True)
+    if len(s) > args.pem_dets:
+        model.det_score_thresh = 0.5 * (s[args.pem_dets - 1] + s[args.pem_dets])
+    for _ in range(args.warmup):
+        res = model.detect_objects(*frame, objs, rng=np.random.RandomState(5))
+    clock = StageClock(MULTI_STAGES)
+    for _ in range(args.frames):
+        clock.start()
+        res = model.detect_objects(*frame, objs, rng=np.random.RandomState(5), mark=clock)
+    stages_ms = {k: round(v * 1e3 / args.frames, 2) for k, v in clock.acc.items()}
+    torch.cuda.synchronize()
+    t = time.perf_counter()
+    for _ in range(args.frames):
+        model.detect_objects(*frame, objs, rng=np.random.RandomState(5))
+    torch.cuda.synchronize()
+    frame_ms = (time.perf_counter() - t) * 1e3 / args.frames
+    counts = dict(proposals=res.n_proposals, ism_after_nms=len(res.ism), objects_detected=len({r["category_id"] for r in res.ism}),
+                  above_det_score_thresh=sum(r["score"] > model.det_score_thresh for r in res.ism), pem_kept=len(res.pem))
+    out = dict(objects=n_objects, stages_ms=stages_ms, stage_sum_ms=round(sum(stages_ms.values()), 2), frame_ms=round(frame_ms, 2),
+               frames_per_s=round(1e3 / frame_ms, 2), onboard_objects_ms=round(onboard_ms, 1), counts=counts,
+               det_score_thresh=model.det_score_thresh, ref_patch_bytes=int(objs.ref_patch.numel() * objs.ref_patch.element_size()))
+    del model, objs, res
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--pem_dets", type=int, default=8, help="detections that reach the PEM (sets det_score_thresh)")
     ap.add_argument("--configs", default=",".join(CONFIGS))
+    ap.add_argument("--objects", default=None, help="comma-separated object counts: time detect_objects instead (first config)")
     ap.add_argument("--out", required=True, help="JSON file to write")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -158,9 +207,15 @@ def main():
     res = dict(card_before=_card(), frames=args.frames, warmup=args.warmup, pem_dets=args.pem_dets)
     with tempfile.TemporaryDirectory() as tmp:
         cad, frame = _example(tmp)
-        for name in args.configs.split(","):
-            res[name] = bench(name, cad, frame, args)
-            print(name, json.dumps(res[name]), flush=True)
+        if args.objects:
+            name = args.configs.split(",")[0]
+            for n in (int(x) for x in args.objects.split(",")):
+                res[f"{name}_objects_{n}"] = bench_objects(name, cad, frame, n, args)
+                print(name, json.dumps(res[f"{name}_objects_{n}"]), flush=True)
+        else:
+            for name in args.configs.split(","):
+                res[name] = bench(name, cad, frame, args)
+                print(name, json.dumps(res[name]), flush=True)
     res["card_after"] = _card()
     with open(args.out, "w") as fh:
         json.dump(res, fh, indent=1)
