@@ -373,6 +373,14 @@ int sam6d_attn_global_tc_ex(const void* qkv, long long ld, const void* Vt, long 
                             int head_dim, float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
 
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
+/* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):
+ * 0 mean, 1 median (torch.median's lower median), 2 max, 3 avg_5.  sim_out (P,O,T) optional; obj_score (P,O) f32 and obj_tmpl
+ * (P,O) i32 caller-owned: per (proposal, object) score and first-max template.  best_obj / best_score / best_tmpl (P): the
+ * first-max object, its score and its best template.  -22 when O > 65535 or the per-CTA shared memory (8 x (C + T) floats,
+ * T rounded up to a power of two for the median) exceeds the device's opt-in limit. */
+int sam6d_template_score_agg(const float* Qn, const float* Rn, int P, int O, int T, int C, int aggregation, float* sim_out,
+                             float* obj_score, int* obj_tmpl, int* best_obj, float* best_score, int* best_tmpl, void* stream);
+/* avg_5; obj_score optional (scratch is then allocated on the stream). */
 int sam6d_template_score(const float* Qn, const float* Rn, int P, int O, int T, int C, float* sim_out, float* obj_score,
                          int* best_obj, float* best_score, int* best_tmpl, void* stream);
 

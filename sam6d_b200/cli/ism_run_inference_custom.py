@@ -23,7 +23,12 @@ only the DINOv2 checkpoint besides.  The rest of the pipeline and the output fil
 
 `--dinov2_model {dinov2_vits14,dinov2_vitb14,dinov2_vitl14,dinov2_vitg14}` picks the descriptor backbone (the reference's hydra
 `model.descriptor_model.model_name`, default dinov2_vitl14) and its checkpoint `{checkpoint_dir}/dinov2/<name>_pretrain.pth`.
-dinov2_vitg14 is built with the SwiGLU FFN its published checkpoint holds (sam6d_b200/dinov2.py: FFN_OF_MODEL)."""
+dinov2_vitg14 is built with the SwiGLU FFN its published checkpoint holds (sam6d_b200/dinov2.py: FFN_OF_MODEL).
+
+`--aggregation_function {mean,median,max,avg_5}` (the reference's matching_config, default avg_5) reduces each object's template
+similarities to its semantic score.  `--level_templates {0,1,2}` and `--pose_distribution {all,upper}` (onboarding_config) pick
+the ISM's views among templates rendered by render_custom_templates with the same two flags (render.template_view_set's
+layout: the 42 level-0 views first); the defaults use every view in the directory, as before."""
 import argparse
 import glob
 import json
@@ -61,6 +66,12 @@ def get_parser():
     ap.add_argument("--points_per_side", default=32, type=int)
     ap.add_argument("--pred_iou_thresh", default=0.88, type=float)
     ap.add_argument("--confidence_thresh", default=CONFIDENCE_THRESH, type=float, help="semantic-score threshold (ISM_sam.yaml: 0.2)")
+    ap.add_argument("--aggregation_function", default="avg_5", choices=("mean", "median", "max", "avg_5"),
+                    help="matching_config.aggregation_function: how an object's template similarities become its semantic score")
+    ap.add_argument("--level_templates", default=0, type=int, choices=(0, 1, 2),
+                    help="onboarding_config.level_templates: the ISM's views, 0 / 1 / 2 = 42 / 162 / 642")
+    ap.add_argument("--pose_distribution", default="all", choices=("all", "upper"),
+                    help="onboarding_config.pose_distribution: all, or upper (cameras with z >= 0)")
     return ap
 
 
@@ -163,6 +174,20 @@ def build_models(args, device):
     return seg, desc
 
 
+def ism_views(n_files: int, level_templates: int = 0, pose_distribution: str = "all") -> np.ndarray:
+    """indices of the ISM's template files among the n_files views of a template directory: all of them for the default
+    view set, else render.template_view_set(level_templates, pose_distribution)'s ISM views, whose layout the directory
+    must have"""
+    from .. import render
+    if (level_templates, pose_distribution) == (0, "all"):
+        return np.arange(n_files)
+    union, index = render.template_view_set(level_templates, pose_distribution)
+    if n_files != len(union):
+        raise ValueError(f"--level_templates {level_templates} --pose_distribution {pose_distribution} needs the {len(union)} views "
+                         f"render_custom_templates writes with the same flags; the template directory holds {n_files}")
+    return index
+
+
 def main(argv=None):
     args = get_parser().parse_args(argv)
     if args.segmentor_model not in ("sam", "fastsam"):
@@ -176,21 +201,23 @@ def main(argv=None):
     # ---- templates (run_inference_custom.py:129-165) ---------------------------------------------------------------------
     tdir = os.path.join(args.output_dir, "templates")
     n_t = len(glob.glob(f"{tdir}/*.npy")) - int(os.path.exists(os.path.join(tdir, "template_poses.npy")))
-    rgbs = np.stack([np.array(Image.open(os.path.join(tdir, f"rgb_{i}.png")).convert("RGB")) for i in range(n_t)])
-    masks = np.stack([np.array(Image.open(os.path.join(tdir, f"mask_{i}.png")).convert("L")) for i in range(n_t)])
+    views = ism_views(n_t, args.level_templates, args.pose_distribution)
+    rgbs = np.stack([np.array(Image.open(os.path.join(tdir, f"rgb_{i}.png")).convert("RGB")) for i in views])
+    masks = np.stack([np.array(Image.open(os.path.join(tdir, f"mask_{i}.png")).convert("L")) for i in views])
     ref_cls, ref_patch = pipeline.ism_reference_features(desc, rgbs, masks, device)
     pose_path = args.template_poses or os.path.join(tdir, "template_poses.npy")
     geometry = None
     if os.path.exists(pose_path):
         cam = json.load(open(args.cam_path))
         verts, faces, _ = meshio.load_ply(args.cad_path)
-        geometry = pipeline.ism_geometry(np.load(pose_path), meshio.sample_surface(verts, faces, pipeline.N_ISM_CLOUD) / 1000.0,
+        geometry = pipeline.ism_geometry(np.load(pose_path)[views], meshio.sample_surface(verts, faces, pipeline.N_ISM_CLOUD) / 1000.0,
                                          np.array(Image.open(args.depth_path)), cam["cam_K"], cam["depth_scale"], device)
     else:
         print("=> no template poses: final score = (semantic + appearance) / 2", file=sys.stderr)
     # ---- proposals + descriptors + scores (:167-209) ----------------------------------------------------------------------------
     rgb = np.array(Image.open(args.rgb_path).convert("RGB"))
-    det = pipeline.ism_detect(seg, desc, ref_cls, ref_patch, rgb, args.confidence_thresh, geometry)
+    det = pipeline.ism_detect(seg, desc, ref_cls, ref_patch, rgb, args.confidence_thresh, geometry,
+                              aggregation_function=args.aggregation_function)
     out_json = f"{args.output_dir}/sam6d_results/detection_ism.json"
     if det.reason is not None:
         json.dump([], open(out_json, "w"))

@@ -11,7 +11,12 @@ Framing as in the reference: with --normalize the model is scaled by 1/(2r), r =
 it d = 2.  The views are sam6d_b200.render.level0_template_poses() (elevation, then azimuth ascending); --poses takes the
 reference's obj_poses_level0.npy (or any (T,4,4) file whose translation is in mm for a camera 1000 mm away) to render in its
 order.  Colours: --colorize paints the model in --base_color; otherwise the texture, else the vertex colours, else Blender's
-default grey 0.8.  Shading is ambient + Lambert from a point light at 2.5x the camera position, not Cycles."""
+default grey 0.8.  Shading is ambient + Lambert from a point light at 2.5x the camera position, not Cycles.
+
+Denser view sets for the ISM (the reference's onboarding_config): --level_templates {0,1,2} (42 / 162 / 642 views) and
+--pose_distribution {all,upper} (upper: cameras with z >= 0).  The directory then holds render.template_view_set()'s layout:
+the 42 level-0 views first as rgb_0..41 (what the PEM reads, the same files as the defaults write), then the chosen set's other
+views; template_poses.npy follows the same order.  The ISM CLI given the same two flags finds its views among them."""
 import argparse
 import os
 
@@ -37,13 +42,32 @@ def get_parser():
     return ap
 
 
+def view_set_parser():
+    """the view-set flags, not in the reference's argument list (get_parser): parsed from what get_parser leaves"""
+    ap = argparse.ArgumentParser(add_help=False)
+    ap.add_argument("--level_templates", type=int, default=0, choices=sorted(render.VIEW_COUNTS),
+                    help="onboarding_config.level_templates: 0 / 1 / 2 = 42 / 162 / 642 views")
+    ap.add_argument("--pose_distribution", default="all", choices=render.POSE_DISTRIBUTIONS,
+                    help="onboarding_config.pose_distribution: all, or upper (cameras with z >= 0)")
+    return ap
+
+
 def view_poses(distance, poses_file=None):
     """(T,4,4) float64 object -> camera poses with the camera `distance` model units from the origin"""
+    return view_set(distance, poses_file)[0]
+
+
+def view_set(distance, poses_file=None, level_templates=0, pose_distribution="all"):
+    """-> (poses (N,4,4) float64 with the camera `distance` model units from the origin, ism_index (T,) int64):
+    render.template_view_set's layout, or poses_file's views (then all of them are the ISM's, and the view set must be the
+    default one)"""
     if poses_file is None:
-        return render.level0_template_poses(distance)
+        return render.template_view_set(level_templates, pose_distribution, distance)
+    if (level_templates, pose_distribution) != (0, "all"):
+        raise ValueError("--poses renders the file's views: it takes no --level_templates / --pose_distribution")
     P = np.asarray(np.load(poses_file), dtype=np.float64).reshape(-1, 4, 4).copy()
     P[:, :3, 3] *= distance / 1000.0
-    return P
+    return P, np.arange(len(P), dtype=np.int64)
 
 
 def render_views(meshes_dev, poses, size, base_colors):
@@ -71,10 +95,18 @@ def to_metres(poses_mm):
     return P
 
 
+def parse_args(argv=None):
+    """get_parser()'s arguments plus view_set_parser()'s, in one namespace"""
+    args, rest = get_parser().parse_known_args(argv)
+    view_set_parser().parse_args(rest, namespace=args)
+    return args
+
+
 def main(argv=None):
-    args = get_parser().parse_args(argv)
+    args = parse_args(argv)
     from ..pipeline import render_templates
-    out, poses = render_templates(meshio.load_ply_mesh(args.cad_path), args.size, args.normalize, args.colorize, args.base_color, args.poses)
+    out, poses = render_templates(meshio.load_ply_mesh(args.cad_path), args.size, args.normalize, args.colorize, args.base_color, args.poses,
+                                  args.level_templates, args.pose_distribution)
     dropped = int(out["dropped"][0])
     if dropped:
         print(f"=> WARNING: {dropped} triangle views dropped (vertex behind the camera or outside the guard band)")

@@ -47,6 +47,12 @@ def get_parser():
     ap.add_argument("--points_per_side", default=32, type=int)
     ap.add_argument("--pred_iou_thresh", default=0.88, type=float)
     ap.add_argument("--confidence_thresh", default=ism_cli.CONFIDENCE_THRESH, type=float, help="semantic-score threshold")
+    ap.add_argument("--aggregation_function", default="avg_5", choices=("mean", "median", "max", "avg_5"),
+                    help="matching_config.aggregation_function of the semantic score")
+    ap.add_argument("--level_templates", default=0, type=int, choices=(0, 1, 2),
+                    help="the ISM's views (onboarding_config): 0 / 1 / 2 = 42 / 162 / 642; the PEM keeps the 42 level-0 views")
+    ap.add_argument("--pose_distribution", default="all", choices=("all", "upper"),
+                    help="onboarding_config.pose_distribution: all, or upper (cameras with z >= 0)")
     # the PEM CLI's options
     ap.add_argument("--det_score_thresh", default=0.2, type=float, help="The score threshold of detection")
     ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth (default: the PEM CLI's)")
@@ -62,7 +68,8 @@ def main(argv=None):
                   checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
                   stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
                   points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
-                  det_score_thresh=args.det_score_thresh, precision=args.precision)
+                  det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
+                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function)
     multi = isinstance(args.cad_path, list)
     n_cad = len(args.cad_path) if multi else 1
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:

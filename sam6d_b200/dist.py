@@ -3,6 +3,7 @@ data-path collective; the only exchange is one all-gather of the final poses (16
 over NCCL / NVLink.  ISM template scoring shards the O x T reference descriptors by object instead (every rank scores all
 proposals against its objects; one all-gather of 12 bytes per proposal and rank picks the winner).  One process per GPU,
 torch.distributed for the rendezvous."""
+import functools
 from typing import Dict, Tuple
 
 import torch
@@ -50,23 +51,24 @@ def all_gather_poses(local: torch.Tensor, counts=None) -> torch.Tensor:
     return torch.cat([out[r * mx: r * mx + counts[r]] for r in range(world)], dim=0)
 
 
-def _local_best(proposal_descriptors: torch.Tensor, ref_descriptors: torch.Tensor):
-    """fused kernel on this rank's object shard: per proposal (best local object, its avg-5 score, its best template)"""
-    from . import ops
-    qn = ops.l2norm_rows(proposal_descriptors.float().contiguous())
+def _local_best(proposal_descriptors: torch.Tensor, ref_descriptors: torch.Tensor, aggregation_function: str = "avg_5"):
+    """fused kernel on this rank's object shard: per proposal (best local object, its aggregated score, its best template)"""
+    from . import ism, ops
+    qn = ism._normalized(proposal_descriptors)
     rn = ops.l2norm_rows(ref_descriptors.float().contiguous())
-    _, _, best_obj, best_score, best_tmpl = ops.template_score(qn, rn, want_sim=False)
+    _, _, best_obj, best_score, best_tmpl = ops.template_score(qn, rn, want_sim=False, aggregation=aggregation_function)
     return best_obj.long(), best_score, best_tmpl.long()
 
 
 def sharded_semantic_score(proposal_descriptors: torch.Tensor, local_ref_descriptors: torch.Tensor, obj_lo: int,
-                           confidence_thresh: float = 0.2, local_best=None):
+                           confidence_thresh: float = 0.2, local_best=None, aggregation_function: str = "avg_5"):
     """compute_semantic_score (ISM/model/detector.py:260-296) with the reference descriptors sharded by object:
     this rank holds objects [obj_lo, obj_lo + O_local) (shard_range over the O objects, ascending with the rank).
     Every rank returns the same (idx_selected_proposals, pred_idx_objects, semantic_score, best_template) the unsharded call
     gives: per-object scores do not depend on the sharding, and ties go to the lowest object index (first maximum) because
-    lower ranks own lower indices.  `local_best(desc, refs)` defaults to the CUDA kernel; tests inject the CPU oracle."""
-    fn = local_best or _local_best
+    lower ranks own lower indices.  aggregation_function: as ism.compute_semantic_score.  `local_best(desc, refs)` defaults
+    to the CUDA kernel with that aggregation; tests inject the CPU oracle (which then applies its own aggregation)."""
+    fn = local_best or functools.partial(_local_best, aggregation_function=aggregation_function)
     P = proposal_descriptors.shape[0]
     if local_ref_descriptors.shape[0] == 0:                       # a rank may own no object (O < world)
         score = torch.full((P,), -1.0, dtype=torch.float32, device=proposal_descriptors.device)

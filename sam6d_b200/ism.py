@@ -4,8 +4,8 @@ Mirrors  PairwiseSimilarity                         ISM/model/loss.py:21-44
          Instance_Segmentation_Model.compute_semantic_score / best_template_pose
                                                     ISM/model/detector.py:198-207, 260-296
 with the same call signatures and return values.  One fused sm_90a kernel (csrc/ism.cu) computes the clamped cosine
-matrix, the avg-5 aggregation, the object argmax and the best-template argmax; the reference's P-fold replication of the
-reference descriptors is never formed.
+matrix, the template aggregation (mean, median, max or avg-5) and the best-template argmax, and a second one the object
+argmax; the reference's P-fold replication of the reference descriptors is never formed.
 
 Geometric score (csrc/ism_geo.cu):
          Calculate_the_query_translation            ISM/model/detector.py:237-250, ISM/utils/trimesh_utils.py:77-105
@@ -42,14 +42,20 @@ class PairwiseSimilarity(nn.Module):
         return sim
 
 
+def _normalized(x):
+    x = x.float().contiguous()
+    return ops.l2norm_rows(x) if x.numel() else x
+
+
 def compute_semantic_score(proposal_descriptors, ref_descriptors, aggregation_function="avg_5", confidence_thresh=0.2):
     """detector.py:260-296 -> (idx_selected_proposals, pred_idx_objects, semantic_score, best_template), all int64/f32
-    like the reference.  Only 'avg_5' (ISM/configs/model/ISM_sam.yaml) runs fused."""
-    if aggregation_function != "avg_5":
-        raise NotImplementedError("SAM-6D's ISM configuration uses aggregation_function='avg_5'")
-    qn = ops.l2norm_rows(proposal_descriptors.float().contiguous())
+    like the reference.  aggregation_function (matching_config): 'mean', 'median' (the lower median, as torch.median),
+    'max' or 'avg_5' (ISM/configs/model/ISM_sam.yaml), all in the one fused kernel."""
+    if aggregation_function not in ops.TEMPLATE_AGGREGATIONS:
+        raise NotImplementedError(f"aggregation_function {aggregation_function!r}: one of {sorted(ops.TEMPLATE_AGGREGATIONS)}")
+    qn = _normalized(proposal_descriptors)
     rn = ops.l2norm_rows(ref_descriptors.float().contiguous())
-    _, _, best_obj, best_score, best_tmpl = ops.template_score(qn, rn, want_sim=False)
+    _, _, best_obj, best_score, best_tmpl = ops.template_score(qn, rn, want_sim=False, aggregation=aggregation_function)
     keep = best_score > confidence_thresh
     idx_selected = torch.arange(best_score.shape[0], device=best_score.device)[keep]
     return idx_selected, best_obj[keep].long(), best_score[keep], best_tmpl[keep].long()

@@ -846,19 +846,27 @@ def bilinear_gather(up: Tensor, choose: Tensor, G: int, sub: int, C: int, H: int
     return out
 
 
-def template_score(Qn: Tensor, Rn: Tensor, want_sim: bool = True):
-    """Qn (P,C), Rn (O,T,C): F.normalize'd descriptors -> sim (P,O,T), obj_score (P,O), best_obj, best_score, best_tmpl."""
+TEMPLATE_AGGREGATIONS = {"mean": 0, "median": 1, "max": 2, "avg_5": 3}     # csrc/ism.cu, matching_config.aggregation_function
+
+
+def template_score(Qn: Tensor, Rn: Tensor, want_sim: bool = True, aggregation: str = "avg_5"):
+    """Qn (P,C), Rn (O,T,C): F.normalize'd descriptors -> sim (P,O,T), obj_score (P,O), best_obj, best_score, best_tmpl.
+    aggregation: how obj_score reduces the T similarities, one of TEMPLATE_AGGREGATIONS."""
     _check(Qn, torch.float32, "query", 2)
     _check(Rn, torch.float32, "reference", 3)
+    if aggregation not in TEMPLATE_AGGREGATIONS:
+        raise NotImplementedError(f"template aggregation {aggregation!r}: one of {sorted(TEMPLATE_AGGREGATIONS)}")
     P, C = Qn.shape
     O, T, _ = Rn.shape
     dev = Qn.device
     sim = torch.empty(P, O, T, dtype=torch.float32, device=dev) if want_sim else None
     obj = torch.empty(P, O, dtype=torch.float32, device=dev)
+    obj_t = torch.empty(P, O, dtype=torch.int32, device=dev)
     bo = torch.zeros(P, dtype=torch.int32, device=dev)
     bs = torch.zeros(P, dtype=torch.float32, device=dev)
     bt = torch.zeros(P, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_template_score", _p(Qn), _p(Rn), P, O, T, C, _p(sim), _p(obj), _p(bo), _p(bs), _p(bt), _s())
+    _lib.call("sam6d_template_score_agg", _p(Qn), _p(Rn), P, O, T, C, TEMPLATE_AGGREGATIONS[aggregation], _p(sim), _p(obj), _p(obj_t),
+              _p(bo), _p(bs), _p(bt), _s())
     return sim, obj, bo, bs, bt
 
 

@@ -4,6 +4,7 @@ which keeps the models resident, onboards an object once and runs one RGB-D fram
     from sam6d_b200.pipeline import SAM6D
     sam6d = SAM6D(segmentor="sam", checkpoint_dir="checkpoints", checkpoint="checkpoints/sam-6d-pem-base.pth")
     obj = sam6d.onboard("obj_000005.ply")                   # 42 templates rendered on the GPU, ISM + PEM template banks
+    # denser ISM view sets and other aggregations: SAM6D(..., level_templates=2, pose_distribution="upper", aggregation_function="median")
     res = sam6d(rgb_u8, depth_u16, cam_K, depth_scale, obj)  # res.ism / res.pem: the CLIs' BOP-23 records; res.R, res.t
 
 Several known objects in a frame (Instance_Segmentation_Model.test_step for the ISM, one PEM batch across the objects):
@@ -33,10 +34,11 @@ N_ISM_CLOUD = 2048                     # points of the geometric score's templat
 
 # ---- render + framing (Render/render_custom_templates.py) -----------------------------------------------------------------
 def render_templates(mesh: meshio.Mesh, size: int = 512, normalize: bool = True, colorize: bool = False, base_color: float = 0.05,
-                     poses_file: Optional[str] = None):
-    """the 42 level-0 views of one numpy mesh (mm) -> (render.render()'s dict for one object, poses (T,4,4) float64 in model units).
-    Framing: camera 4r away with --normalize (r = max |bbox corner|), else 2; colours: base_color with colorize, else the
-    mesh's texture / vertex colours / Blender's default grey."""
+                     poses_file: Optional[str] = None, level_templates: int = 0, pose_distribution: str = "all"):
+    """the template views of one numpy mesh (mm) -> (render.render()'s dict for one object, poses (T,4,4) float64 in model units):
+    the views of render.template_view_set(level_templates, pose_distribution), the 42 level-0 views first (the defaults: those
+    42 only), or poses_file's.  Framing: camera 4r away with --normalize (r = max |bbox corner|), else 2; colours: base_color
+    with colorize, else the mesh's texture / vertex colours / Blender's default grey."""
     if normalize:
         r = max(np.linalg.norm(mesh.vertices.max(axis=0)), np.linalg.norm(mesh.vertices.min(axis=0)))
         distance = 4.0 * float(r)
@@ -47,7 +49,7 @@ def render_templates(mesh: meshio.Mesh, size: int = 512, normalize: bool = True,
         grey = float(base_color)
     else:
         grey = render_cli.BLENDER_DEFAULT_GREY
-    poses = render_cli.view_poses(distance, poses_file)
+    poses, _ = render_cli.view_set(distance, poses_file, level_templates, pose_distribution)
     out = render_cli.render_views([render.upload(mesh)], poses[None], size, [[grey] * 3])
     return out, poses
 
@@ -97,13 +99,14 @@ def ism_geometry(poses_m, cloud_m, depth_raw, cam_K, depth_scale, device) -> Ism
 
 # ---- segment -> describe -> score (ISM/run_inference_custom.py:167-209) -------------------------------------------------------
 def ism_detect(seg, desc, ref_cls, ref_patch, rgb_u8: np.ndarray, confidence_thresh: float, geometry: Optional[IsmGeometry] = None,
-               mark=None, remove_small: bool = False):
+               mark=None, remove_small: bool = False, aggregation_function: str = "avg_5"):
     """-> SimpleNamespace(masks (N,H,W) f32, boxes (N,4) i64 xyxy, scores (N) f32, obj (N) i64, n_proposals, reason): the
     proposals above the semantic-score threshold with their final scores ((semantic + appearance + geometric x visible) /
     (2 + visible), or (semantic + appearance) / 2 without geometry) and the object each is assigned to.  ref_cls (T,C) and
     ref_patch (T,256,C) of one object, or (O,T,C) and (O,T,256,C) of several (geometry then holds every object's poses and
     cloud).  remove_small: Detections.remove_very_small_detections after the segmentor, as Instance_Segmentation_Model.test_step
-    does.  reason is None, or why there is no detection.  mark(stage) is called after the segmentor, the descriptors and the
+    does.  aggregation_function: how the semantic score reduces each object's template similarities (ism.compute_semantic_score).
+    reason is None, or why there is no detection.  mark(stage) is called after the segmentor, the descriptors and the
     scores (stage timing)."""
     from .dinov2 import MaskedPatch_MatrixSimilarity
     mark = mark or (lambda stage: None)
@@ -121,7 +124,7 @@ def ism_detect(seg, desc, ref_cls, ref_patch, rgb_u8: np.ndarray, confidence_thr
         return det
     q_cls, q_patch = desc(rgb_u8, det)
     mark("descriptors")
-    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_cls, "avg_5", confidence_thresh)
+    idx_sel, pred_obj, sem, best_t = ism.compute_semantic_score(q_cls, ref_cls, aggregation_function, confidence_thresh)
     det.masks, det.boxes, det.obj, q_patch = det.masks[idx_sel], det.boxes[idx_sel], pred_obj, q_patch[idx_sel]
     if idx_sel.numel() == 0:
         det.reason = "no proposal above the semantic-score threshold"
@@ -242,15 +245,25 @@ class Onboarded:
 
 class SAM6D:
     """the SAM-6D models, built once (through the ISM and PEM CLIs' build_models / build_fastsam / build_model, so checkpoint
-    names, seeded weights and thresholds are theirs).  onboard() an object, then call the instance once per RGB-D frame."""
+    names, seeded weights and thresholds are theirs).  onboard() an object, then call the instance once per RGB-D frame.
+
+    The ISM settings of the reference's configuration: level_templates (0 / 1 / 2 = 42 / 162 / 642 views) and pose_distribution
+    ("all", or "upper": cameras with z >= 0) choose the views the ISM matches against (onboarding_config); aggregation_function
+    ("mean", "median", "max", "avg_5") how each object's template similarities become its semantic score (matching_config).
+    The PEM always uses the 42 level-0 views."""
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
                  checkpoint_dir: Optional[str] = None, checkpoint: Optional[str] = None, random_weights: bool = False,
                  stability_score_thresh: float = 0.97, pred_iou_thresh: float = 0.88, points_per_side: int = 32,
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
-                 device=None):
+                 device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5"):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
+        render.template_view_set(level_templates, pose_distribution)          # ValueError on an unknown view set
+        if aggregation_function not in ops.TEMPLATE_AGGREGATIONS:
+            raise ValueError(f"aggregation_function must be one of {sorted(ops.TEMPLATE_AGGREGATIONS)}, got {aggregation_function!r}")
+        self.level_templates, self.pose_distribution = int(level_templates), pose_distribution
+        self.aggregation_function = aggregation_function
         self.device = torch.device(device if device is not None else "cuda")
         self.confidence_thresh = float(confidence_thresh)
         self.det_score_thresh = float(det_score_thresh)
@@ -262,19 +275,25 @@ class SAM6D:
         self.pem = pem_cli.build_model(SimpleNamespace(precision=precision, checkpoint=checkpoint, random_weights=random_weights), self.device)
 
     def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None) -> Onboarded:
-        """render the 42 level-0 templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates'
-        framing and colours, and build everything a frame needs from them without touching a file.  Random draws, from `rng`
-        (default numpy's global RNG), in the order the chained CLIs make them: the ISM template cloud, the PEM template
+        """render the templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates' framing
+        and colours, and build everything a frame needs from them without touching a file: every view of
+        render.template_view_set(level_templates, pose_distribution) is rendered once; the ISM references and the
+        geometric-score poses come from the ISM's views, the PEM template bank from the 42 level-0 views.  Random draws, from
+        `rng` (default numpy's global RNG), in the order the chained CLIs make them: the ISM template cloud, the PEM template
         samples, the PEM model points."""
         mesh = meshio.load_ply_mesh(mesh_or_ply_path) if isinstance(mesh_or_ply_path, str) else mesh_or_ply_path
         verts, faces = mesh.vertices, mesh.faces
-        out, poses = render_templates(mesh, template_size)
+        out, poses = render_templates(mesh, template_size, level_templates=self.level_templates, pose_distribution=self.pose_distribution)
+        ism_index = render.template_view_set(self.level_templates, self.pose_distribution)[1]
         rgbs, masks, xyzs = template_arrays(out)
-        ref_cls, ref_patch = ism_reference_features(self.desc, rgbs, masks, self.device)
+        del out
+        ref_cls, ref_patch = ism_reference_features(self.desc, rgbs[ism_index], masks[ism_index], self.device)
         cloud = meshio.sample_surface(verts, faces, N_ISM_CLOUD, rng) / 1000.0
-        bank = pem_template_bank(self.pem, list(rgbs), list(masks), [x.astype(np.float32) for x in xyzs], rng=rng, device=self.device)
+        n0 = pem_cli.TEST_DATASET["n_template_view"]
+        bank = pem_template_bank(self.pem, list(rgbs[:n0]), list(masks[:n0]), [x.astype(np.float32) for x in xyzs[:n0]], rng=rng,
+                                 device=self.device)
         model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
-        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses), cloud, bank, model_points)
+        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points)
 
     def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
         """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
@@ -318,7 +337,8 @@ class SAM6D:
         mark = mark or (lambda stage: None)
         t0 = time.time()
         geometry = ism_geometry(obj.poses_m, obj.cloud_m, depth_raw, cam_K, depth_scale, self.device)
-        det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark, remove_small=multi)
+        det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark, remove_small=multi,
+                         aggregation_function=self.aggregation_function)
         if multi and det.reason is None:
             keep = ism.nms_per_object(det.boxes, det.scores, det.obj)
             det.masks, det.boxes, det.scores, det.obj = det.masks[keep], det.boxes[keep], det.scores[keep], det.obj[keep]

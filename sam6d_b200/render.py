@@ -83,6 +83,109 @@ def level0_template_poses(distance: float = 1.0) -> np.ndarray:
     return poses
 
 
+VIEW_COUNTS = {0: 42, 1: 162, 2: 642}          # onboarding_config.level_templates -> views of the CNOS view set
+POSE_DISTRIBUTIONS = ("all", "upper")
+
+
+def _icosphere_points(level: int) -> np.ndarray:
+    """camera directions of the level-`level` view set: the level-0 vertices (_icosphere_level0) refined `level` times by 1-to-4
+    midpoint subdivision with re-normalisation, as Blender's icosphere of subdivision level + 2 -> (VIEW_COUNTS[level], 3)"""
+    pts = _icosphere_level0()
+    d = np.linalg.norm(pts[:12, None] - pts[None, :12], axis=2)
+    edge = d[d > 1e-9].min()
+    adj = d < edge * 1.001
+    # the icosahedron's 20 faces, each cut into 4 with its three edge midpoints (rows 12.. of _icosphere_level0, in its order)
+    mid = {}
+    k = 12
+    for i in range(12):
+        for j in range(i + 1, 12):
+            if adj[i, j]:
+                mid[(i, j)] = mid[(j, i)] = k
+                k += 1
+    faces = []
+    for a in range(12):
+        for b in range(a + 1, 12):
+            for c in range(b + 1, 12):
+                if adj[a, b] and adj[b, c] and adj[a, c]:
+                    ab, bc, ca = mid[(a, b)], mid[(b, c)], mid[(c, a)]
+                    faces += [(a, ab, ca), (ab, b, bc), (ca, bc, c), (ab, bc, ca)]
+    for _ in range(level):
+        pts, faces = _subdivide(pts, faces)
+    assert pts.shape == (VIEW_COUNTS[level], 3)
+    return pts
+
+
+def _subdivide(pts, faces):
+    """one 1-to-4 split of every triangle; each edge's midpoint is added once, normalised onto the unit sphere"""
+    pts = list(pts)
+    mid = {}
+
+    def m(i, j):
+        key = (min(i, j), max(i, j))
+        if key not in mid:
+            v = pts[i] + pts[j]
+            pts.append(v / np.linalg.norm(v))
+            mid[key] = len(pts) - 1
+        return mid[key]
+    out = []
+    for a, b, c in faces:
+        ab, bc, ca = m(a, b), m(b, c), m(c, a)
+        out += [(a, ab, ca), (ab, b, bc), (ca, bc, c), (ab, bc, ca)]
+    return np.asarray(pts), out
+
+
+def _poses_at(pos: np.ndarray, distance: float) -> np.ndarray:
+    """unit camera positions -> (n,4,4) object -> camera poses, ordered by elevation ascending, then azimuth ascending"""
+    el = np.arctan2(pos[:, 2], np.hypot(pos[:, 0], pos[:, 1]))
+    az = np.arctan2(pos[:, 0], pos[:, 1])
+    order = np.lexsort((np.round(az, 9), np.round(el, 9)))
+    poses = np.zeros((len(pos), 4, 4))
+    for i, k in enumerate(order):
+        R = _look_at(pos[k]).T                                       # world -> camera
+        poses[i, :3, :3] = R
+        poses[i, :3, 3] = -R @ (pos[k] * distance)
+        poses[i, 3, 3] = 1.0
+    return poses
+
+
+def camera_centres(poses: np.ndarray) -> np.ndarray:
+    """(n,4,4) object -> camera poses -> (n,3) camera centres in the object frame, -R^T t"""
+    return -np.einsum("tji,tj->ti", poses[:, :3, :3], poses[:, :3, 3])
+
+
+def template_poses(level: int = 0, pose_distribution: str = "all", distance: float = 1.0) -> np.ndarray:
+    """-> (T,4,4) float64 object -> camera poses of the CNOS view set onboarding_config.level_templates = level (0 / 1 / 2 =
+    42 / 162 / 642 views, ISM/utils/poses/pose_utils.py:70-100) with the camera `distance` from the origin, ordered by
+    elevation, then azimuth, ascending.  pose_distribution "upper" keeps the cameras with z >= 0, the equator included
+    (26 / 91 / 341 views): an object resting on a table is never seen from below.  Level 0 "all" is level0_template_poses()."""
+    if level not in VIEW_COUNTS:
+        raise ValueError(f"level_templates must be one of {sorted(VIEW_COUNTS)}, got {level!r}")
+    if pose_distribution not in POSE_DISTRIBUTIONS:
+        raise ValueError(f"pose_distribution must be one of {POSE_DISTRIBUTIONS}, got {pose_distribution!r}")
+    poses = level0_template_poses(distance) if level == 0 else _poses_at(_icosphere_points(level), distance)
+    if pose_distribution == "upper":
+        # equator cameras are sums of mirror-image pairs, so their z is 0 exactly; the margin only absorbs -R^T t's rounding
+        poses = poses[camera_centres(poses)[:, 2] >= -1e-9 * max(distance, 1.0)]
+    return poses
+
+
+def template_view_set(level: int = 0, pose_distribution: str = "all", distance: float = 1.0):
+    """the template directory's view layout -> (poses (N,4,4) float64, ism_index (T,) int64).  The 42 level-0 views come first,
+    in level0_template_poses()'s order (so rgb_0..41, which the PEM reads, are always those views), then the views of
+    template_poses(level, pose_distribution) that are not level-0 views, in that set's order.  ism_index lists, in the set's
+    own order, where each of its T views sits among the N: the ISM scores against poses[ism_index]."""
+    base = level0_template_poses(distance)
+    chosen = template_poses(level, pose_distribution, distance)
+    cb, cc = camera_centres(base), camera_centres(chosen)
+    d = np.linalg.norm(cc[:, None] - cb[None], axis=2)
+    tol = 1e-6 * max(distance, 1.0)
+    in_base = d.min(axis=1) < tol
+    extra = chosen[~in_base]
+    index = np.where(in_base, d.argmin(axis=1), 0)
+    index[~in_base] = len(base) + np.arange(len(extra))
+    return np.concatenate([base, extra]), index.astype(np.int64)
+
+
 def template_K(size: int = 512) -> np.ndarray:
     """the template camera: f = 560 px, principal point at the centre of a 512 x 512 image, scaled to size x size"""
     s = size / 512.0
