@@ -414,6 +414,8 @@ int sam6d_conv2d_tc(const void* x, long long ldx, int B, int Hi, int Wi, int Cin
 /* stem: img (B,H,W,3) u8 letterboxed, channel-flipped and /255 on the fly; w (80,3,3,3) f32 (out,ky,kx,in), bias (80) f32 ->
  * out (B,ceil(H/2),ceil(W/2),80) bf16 = SiLU(3x3 stride-2 conv) */
 int sam6d_yolo_stem(const unsigned char* img, int B, int H, int W, const float* w, const float* bias, void* out, void* stream);
+/* the stem at C output channels (C % 16 == 0, C <= 80; 32 for FastSAM-s): w (C,3,3,3), bias (C) -> out (B,ceil(H/2),ceil(W/2),C) */
+int sam6d_yolo_stem_c(const unsigned char* img, int B, int H, int W, int C, const float* w, const float* bias, void* out, void* stream);
 /* SPPF pools: buf (B,H,W,ld) bf16, channels [0,C) -> [C,2C), [2C,3C), [3C,4C) = 5x5, 9x9, 13x13 max (-inf padding) */
 int sam6d_yolo_sppf(void* buf, long long ld, int B, int H, int W, int C, void* stream);
 /* nearest x2: x (B,H,W,ldx) channels [0,C) -> y (B,2H,2W,ldy) channels [0,C); C, ldx, ldy % 8 == 0 */

@@ -17,9 +17,11 @@ reference's predefined level-0 poses with --template_poses); without it the fina
 default vit_h) and its checkpoint `{checkpoint_dir}/segment-anything/sam_vit_{h_4b8939,l_0b3195,b_01ec64}.pth` through
 sam_amg.load_sam.
 
-`--segmentor_model fastsam` (ISM_fastsam.yaml) replaces SAM by FastSAM (sam6d_b200/fast_sam.py: YOLOv8x-seg, conf 0.25, iou 0.9,
-max_det 200) built from `{checkpoint_dir}/FastSAM/FastSAM-x.pt` or the reference's `./checkpoints/FastSAM/FastSAM-x.pt`; it needs
-only the DINOv2 checkpoint besides.  The rest of the pipeline and the output files are the same.
+`--segmentor_model fastsam` (ISM_fastsam.yaml) replaces SAM by FastSAM (sam6d_b200/fast_sam.py: YOLOv8x-seg or YOLOv8s-seg, conf
+0.25, iou 0.9, max_det 200) built from `{checkpoint_dir}/FastSAM/<--fastsam_model>.pt` or the reference's
+`./checkpoints/FastSAM/<--fastsam_model>.pt` (`--fastsam_model {FastSAM-x,FastSAM-s}`, default FastSAM-x; the reference's hydra
+`model.segmentor_model.checkpoint_path`); it needs only the DINOv2 checkpoint besides.  The rest of the pipeline and the output
+files are the same.
 
 `--dinov2_model {dinov2_vits14,dinov2_vitb14,dinov2_vitl14,dinov2_vitg14}` picks the descriptor backbone (the reference's hydra
 `model.descriptor_model.model_name`, default dinov2_vitl14) and its checkpoint `{checkpoint_dir}/dinov2/<name>_pretrain.pth`.
@@ -42,6 +44,7 @@ import torch.nn.functional as F
 
 VISIBLE_THRED = 0.5            # ISM/configs/model/ISM_sam.yaml
 CONFIDENCE_THRESH = 0.2
+FASTSAM_MODELS = {"FastSAM-x": "x", "FastSAM-s": "s"}          # checkpoint name -> YOLOv8-seg scale
 
 
 def get_parser():
@@ -55,10 +58,12 @@ def get_parser():
     ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
     # not in the reference: where weights / template poses come from
     ap.add_argument("--checkpoint_dir", default=None,
-                    help="directory with segment-anything/sam_vit_h_4b8939.pth (or the --sam_model_type's file, or FastSAM/FastSAM-x.pt) "
+                    help="directory with segment-anything/sam_vit_h_4b8939.pth (or the --sam_model_type's file, or FastSAM/<--fastsam_model>.pt) "
                          "and dinov2/<--dinov2_model>_pretrain.pth")
     ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"),
                     help="not in the reference: the hydra `model.segmentor_model.sam.model_type` (SAM backbone)")
+    ap.add_argument("--fastsam_model", default="FastSAM-x", choices=FASTSAM_MODELS,
+                    help="not in the reference: the FastSAM checkpoint of --segmentor_model fastsam (FastSAM-x: YOLOv8x-seg, FastSAM-s: YOLOv8s-seg)")
     ap.add_argument("--dinov2_model", default="dinov2_vitl14", choices=("dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"),
                     help="not in the reference: the hydra `model.descriptor_model.model_name` (DINOv2 descriptor backbone)")
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
@@ -122,18 +127,22 @@ def build_fastsam(args, device):
     from ..fast_sam import FastSAM
     desc = _new_desc(args, device)
     ck = args.checkpoint_dir
-    cands = ([os.path.join(ck, "FastSAM", "FastSAM-x.pt")] if ck else []) + [os.path.join(".", "checkpoints", "FastSAM", "FastSAM-x.pt")]
+    name = getattr(args, "fastsam_model", "FastSAM-x")
+    if name not in FASTSAM_MODELS:
+        raise ValueError(f"fastsam_model must be one of {sorted(FASTSAM_MODELS)}, got {name!r}")
+    scale = FASTSAM_MODELS[name]
+    cands = ([os.path.join(ck, "FastSAM", name + ".pt")] if ck else []) + [os.path.join(".", "checkpoints", "FastSAM", name + ".pt")]
     fs_ck = next((c for c in cands if os.path.exists(c)), None)
     dino_ck = _dino_checkpoint(args)
     cfg = dict(iou_threshold=0.9, conf_threshold=0.05, max_det=200)
     if fs_ck and dino_ck and os.path.exists(dino_ck):
-        seg = FastSAM(fs_ck, cfg, segmentor_width_size=640, device=device)
+        seg = FastSAM(fs_ck, cfg, segmentor_width_size=640, device=device, scale=scale)
         desc.model.load_state_dict(torch.load(dino_ck, map_location="cpu"), strict=True)
     elif args.random_weights:
         from .. import synth
         print("=> WARNING: no checkpoints, seeded random weights (detections are meaningless; plumbing run)", file=sys.stderr)
-        seg = FastSAM(None, cfg, segmentor_width_size=640, device=device)
-        seg.model.load_state_dict(synth.make_fastsam_state_dict(seed=1), strict=True)
+        seg = FastSAM(None, cfg, segmentor_width_size=640, device=device, scale=scale)
+        seg.model.load_state_dict(synth.make_fastsam_state_dict(seed=1, scale=scale), strict=True)
         desc.model.load_state_dict(_seeded_dino_state_dict(desc.model), strict=True)
     else:
         raise FileNotFoundError("FastSAM / DINOv2 checkpoints not found (pass --checkpoint_dir, or --random_weights for a plumbing run)")

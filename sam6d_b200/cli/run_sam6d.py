@@ -2,7 +2,7 @@
 with every model built once and no file between the stages (sam6d_b200/pipeline.py: SAM6D).
 
     python -m sam6d_b200.cli.run_sam6d --cad_path obj.ply --rgb_path rgb.png --depth_path depth.png --cam_path camera.json \\
-        --output_dir OUT [--segmentor_model sam|fastsam] [--checkpoint_dir checkpoints --checkpoint sam-6d-pem-base.pth]
+        --output_dir OUT [--segmentor_model sam|fastsam [--fastsam_model FastSAM-x|FastSAM-s]] [--checkpoint_dir checkpoints --checkpoint sam-6d-pem-base.pth]
 
 With several CAD models (--cad_path a.ply b.ply ... [--obj_ids 1 5 ...]) the frame runs through SAM6D.detect_objects: the ISM's
 multi-object post-processing (size filter, per-object NMS), records with category_id = the object's id (default 1, 2, ...),
@@ -43,6 +43,7 @@ def get_parser():
     ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
     ap.add_argument("--checkpoint_dir", default=None, help="the ISM CLI's --checkpoint_dir (SAM / FastSAM and DINOv2 weights)")
     ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"))
+    ap.add_argument("--fastsam_model", default="FastSAM-x", choices=tuple(ism_cli.FASTSAM_MODELS))
     ap.add_argument("--dinov2_model", default="dinov2_vitl14", choices=("dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"))
     ap.add_argument("--points_per_side", default=32, type=int)
     ap.add_argument("--pred_iou_thresh", default=0.88, type=float)
@@ -64,7 +65,8 @@ def get_parser():
 def main(argv=None):
     args = get_parser().parse_args(argv)
     from ..pipeline import SAM6D
-    sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, dinov2_model=args.dinov2_model,
+    sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
+                  dinov2_model=args.dinov2_model,
                   checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
                   stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
                   points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,

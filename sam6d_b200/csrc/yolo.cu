@@ -1,5 +1,6 @@
 // yolo.cu -- the parts of YOLOv8-seg (FastSAM-x) that are not convolutions on wgmma (those are csrc/conv_tc.cu):
-//   stem      letterboxed u8 frame -> channel flip, /255 -> 3x3 stride-2 conv (3 -> 80, BatchNorm folded) + SiLU -> NHWC bf16
+//   stem      letterboxed u8 frame -> channel flip, /255 -> 3x3 stride-2 conv (3 -> C, BatchNorm folded) + SiLU -> NHWC bf16
+//             (C = 80 for FastSAM-x, 32 for FastSAM-s)
 //   sppf      the three cascaded 5x5 max-pools of SPPF written into their concat slices
 //   upsample  nearest x2 into a concat slice
 //   decode    Detect / Segment head decode (DFL, dist2bbox, sigmoid) + confidence filter with an ordered compaction
@@ -8,12 +9,13 @@
 
 namespace {
 
-constexpr int STEM_C = 80, HEAD_W = 64 + 1 + 32, ROW_W = 6 + 32, NM = 32;
+constexpr int HEAD_W = 64 + 1 + 32, ROW_W = 6 + 32, NM = 32;
 
 __device__ __forceinline__ float silu(float x) { return x / (1.f + expf(-x)); }
 __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
-// thread = one output pixel x 16 output channels (blockIdx.y picks the group of 16)
+// thread = one output pixel x 16 output channels (blockIdx.y picks the group of 16); C output channels per pixel
+template <int C>
 __global__ void __launch_bounds__(128) yolo_stem_kernel(const uint8_t* __restrict__ img, int B, int H, int W, int Ho, int Wo,
                                                         const float* __restrict__ w, const float* __restrict__ bias,
                                                         __nv_bfloat16* __restrict__ out) {
@@ -44,7 +46,7 @@ __global__ void __launch_bounds__(128) yolo_stem_kernel(const uint8_t* __restric
     __nv_bfloat162 h = __floats2bfloat162_rn(silu(a0), silu(a1));
     packed[o / 2] = *reinterpret_cast<uint32_t*>(&h);
   }
-  uint4* dst = reinterpret_cast<uint4*>(out + p * STEM_C + o0);
+  uint4* dst = reinterpret_cast<uint4*>(out + p * C + o0);
   dst[0] = make_uint4(packed[0], packed[1], packed[2], packed[3]);
   dst[1] = make_uint4(packed[4], packed[5], packed[6], packed[7]);
 }
@@ -197,17 +199,31 @@ __global__ void yolo_mask_up_kernel(const float* __restrict__ low, int N, int mh
 
 }  // namespace
 
-// img (B,H,W,3) u8 letterboxed frames (channel order as given: the network sees channel 2 - c as its channel c); w (80,3,3,3)
-// f32 folded weights in (out, ky, kx, in) order, bias (80) f32 -> out (B, ceil(H/2), ceil(W/2), 80) bf16
-S6_API int sam6d_yolo_stem(const unsigned char* img, int B, int H, int W, const float* w, const float* bias, void* out, void* stream) {
+// img (B,H,W,3) u8 letterboxed frames (channel order as given: the network sees channel 2 - c as its channel c); w (C,3,3,3)
+// f32 folded weights in (out, ky, kx, in) order, bias (C) f32 -> out (B, ceil(H/2), ceil(W/2), C) bf16; C in {16, 32, 48, 64, 80}
+S6_API int sam6d_yolo_stem_c(const unsigned char* img, int B, int H, int W, int C, const float* w, const float* bias, void* out, void* stream) {
   S6_REQUIRE(img && w && bias && out && B >= 0 && H > 0 && W > 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0);
+  S6_REQUIRE(C > 0 && C <= 80 && (C % 16) == 0);
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   const long long P = (long long)B * Ho * Wo;
   if (P == 0) return 0;
-  yolo_stem_kernel<<<dim3(s6_cdiv(P, 128), STEM_C / 16), 128, 0, s6_stream(stream)>>>(img, B, H, W, Ho, Wo, w, bias,
-                                                                                      reinterpret_cast<__nv_bfloat16*>(out));
+  const dim3 grid(s6_cdiv(P, 128), C / 16);
+  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+  cudaStream_t st = s6_stream(stream);
+  switch (C) {
+    case 16: yolo_stem_kernel<16><<<grid, 128, 0, st>>>(img, B, H, W, Ho, Wo, w, bias, o); break;
+    case 32: yolo_stem_kernel<32><<<grid, 128, 0, st>>>(img, B, H, W, Ho, Wo, w, bias, o); break;
+    case 48: yolo_stem_kernel<48><<<grid, 128, 0, st>>>(img, B, H, W, Ho, Wo, w, bias, o); break;
+    case 64: yolo_stem_kernel<64><<<grid, 128, 0, st>>>(img, B, H, W, Ho, Wo, w, bias, o); break;
+    default: yolo_stem_kernel<80><<<grid, 128, 0, st>>>(img, B, H, W, Ho, Wo, w, bias, o); break;
+  }
   S6_LAUNCH_CHECK();
   return 0;
+}
+
+// sam6d_yolo_stem_c at C = 80 (FastSAM-x)
+S6_API int sam6d_yolo_stem(const unsigned char* img, int B, int H, int W, const float* w, const float* bias, void* out, void* stream) {
+  return sam6d_yolo_stem_c(img, B, H, W, 80, w, bias, out, stream);
 }
 
 // buf (B,H,W,ld) bf16: channels [0, C) in, [C, 4C) out (MaxPool2d(5, 1, 2) applied once, twice, three times == 5x5, 9x9, 13x13)

@@ -1,16 +1,18 @@
-"""FastSAM segmentor of the ISM (ISM/model/fast_sam.py): YOLOv8x-seg -- the ultralytics 8.0.135 `SegmentationModel` of
-`yolov8x-seg.yaml` at nc = 1, what `FastSAM-x.pt` holds -- on sm_90a kernels, with the reference's `FastSAM` wrapper contract.
+"""FastSAM segmentor of the ISM (ISM/model/fast_sam.py): YOLOv8x-seg or YOLOv8s-seg -- the ultralytics 8.0.135
+`SegmentationModel` of `yolov8-seg.yaml` at scale x or s and nc = 1, what `FastSAM-x.pt` and `FastSAM-s.pt` hold -- on sm_90a
+kernels, with the reference's `FastSAM` wrapper contract.
 
 Network.  `YOLOv8Seg` has ultralytics' module tree and state_dict keys (`model.0.conv.weight`, `model.22.proto.upsample.bias`, ...),
 so a real checkpoint loads with strict=True through `load_fastsam_checkpoint` (no ultralytics needed).  BatchNorm is folded into
 each convolution in fp32 as ultralytics' fuse_conv_and_bn does (AutoBackend(fuse=True)), then rounded to bf16 once per parameter
 version.  Activations are NHWC bf16 with fp32 accumulation:
   * every 1x1 / 3x3 convolution is one `sam6d_conv2d_tc` launch (implicit GEMM on wgmma, csrc/conv_tc.cu); the first layer
-    (Cin = 3) is `sam6d_yolo_stem`, which also does the channel flip and /255 of the letterboxed u8 frame;
+    (Cin = 3) is `sam6d_yolo_stem_c`, which also does the channel flip and /255 of the letterboxed u8 frame;
   * concatenation is free: C2f's chunk / cat, SPPF's four-way cat and the head's Concat layers are channel slices of one
     preallocated NHWC buffer that the producing layers write into;
   * the first 3x3 convolutions of the box, class and mask-coefficient branches of a level share their input and run as one
-    launch (Cout 80 + 320 + 80); their last 1x1 convolutions run as one block-diagonal 480 -> 97 launch that writes the level's
+    launch (Cout 80 + 320 + 80 at x, 64 + 128 + 32 at s); their last 1x1 convolutions run as one block-diagonal launch
+    (480 -> 97 at x, 224 -> 97 at s) that writes the level's
     rows of the fp32 head matrix (B, anchors, 64 DFL logits | class logit | 32 coefficients);
   * Proto's 2x2 stride-2 transposed convolution is four 1x1 launches, one per tap, written interleaved.
 
@@ -19,9 +21,10 @@ order) -> stable sort by descending confidence (ties go to the lower anchor inde
 order of exact ties is unspecified) -> `sam6d_sam_nms` (torchvision.ops.nms restated; class-aware NMS is plain NMS at nc = 1) ->
 the first max_det -> `sam6d_yolo_masks` (process_mask with upsample=True) -> scale_boxes / clip_boxes -> postprocess_resize."""
 import ctypes
+import math
 import pickle
 from types import SimpleNamespace
-from typing import Any, Dict
+from typing import Any, Dict, Optional
 
 import numpy as np
 import torch
@@ -35,6 +38,22 @@ bf = torch.bfloat16
 REG_MAX, NM, NC = 16, 32, 1
 HEAD_W = 4 * REG_MAX + NC + NM          # 97 columns per anchor
 STRIDES = (8, 16, 32)
+
+# yolov8-seg.yaml's scales that FastSAM publishes: (depth multiple, width multiple, max channels)
+SCALES = {"x": (1.00, 1.25, 512), "s": (0.33, 0.50, 1024)}
+
+
+def scale_layout(scale: str) -> SimpleNamespace:
+    """the layer widths and C2f depths of a scale, by ultralytics' parse_model rules: width make_divisible(min(c, max_channels)
+    * width, 8) of the yaml's 64 / 128 / 256 / 512 / 1024, depth max(round(n * depth), 1) of its 3 / 6 repeats.
+    -> c (c0..c4), n3, n6 (the backbone's C2f depths; the head's are n3), npr (Proto width)"""
+    if scale not in SCALES:
+        raise ValueError(f"FastSAM scale must be one of {sorted(SCALES)}, got {scale!r}")
+    depth, width, max_c = SCALES[scale]
+    ch = lambda c: int(math.ceil(min(c, max_c) * width / 8) * 8)        # noqa: E731
+    n = lambda k: max(round(k * depth), 1)                              # noqa: E731
+    c = tuple(ch(v) for v in (64, 128, 256, 512, 1024))
+    return SimpleNamespace(scale=scale, c=c, n3=n(3), n6=n(6), npr=c[2])
 
 
 def _p(t):
@@ -139,17 +158,22 @@ def _cw(m: Conv) -> _CW:
 
 # =====================================================================================================================
 class YOLOv8Seg(nn.Module):
-    """ultralytics SegmentationModel('yolov8x-seg.yaml', nc=1): width 1.25, depth 1.0, max channels 640.
+    """ultralytics SegmentationModel('yolov8{scale}-seg.yaml', nc=1), scale "x" (FastSAM-x: widths 80 / 160 / 320 / 640 / 640,
+    C2f depths 3 / 6 / 6 / 3) or "s" (FastSAM-s: widths 32 / 64 / 128 / 256 / 512, depths 1 / 2 / 2 / 1).
     forward(frames (B,H,W,3) u8 letterboxed, H and W multiples of 32) -> head (B,A,97) f32, proto (B,H/4,W/4,32) f32."""
 
-    def __init__(self):
+    def __init__(self, scale: str = "x"):
         super().__init__()
-        L = [Conv(3, 80, 3, 2), Conv(80, 160, 3, 2), C2f(160, 160, 3, True), Conv(160, 320, 3, 2), C2f(320, 320, 6, True),
-             Conv(320, 640, 3, 2), C2f(640, 640, 6, True), Conv(640, 640, 3, 2), C2f(640, 640, 3, True), SPPF(640, 640),
-             _Layer(), _Layer(), C2f(1280, 640, 3, False), _Layer(), _Layer(), C2f(960, 320, 3, False),
-             Conv(320, 320, 3, 2), _Layer(), C2f(960, 640, 3, False), Conv(640, 640, 3, 2), _Layer(), C2f(1280, 640, 3, False),
-             Segment()]
+        lay = scale_layout(scale)
+        c0, c1, c2, c3, c4 = lay.c
+        n3, n6 = lay.n3, lay.n6
+        L = [Conv(3, c0, 3, 2), Conv(c0, c1, 3, 2), C2f(c1, c1, n3, True), Conv(c1, c2, 3, 2), C2f(c2, c2, n6, True),
+             Conv(c2, c3, 3, 2), C2f(c3, c3, n6, True), Conv(c3, c4, 3, 2), C2f(c4, c4, n3, True), SPPF(c4, c4),
+             _Layer(), _Layer(), C2f(c4 + c3, c3, n3, False), _Layer(), _Layer(), C2f(c3 + c2, c2, n3, False),
+             Conv(c2, c2, 3, 2), _Layer(), C2f(c2 + c3, c3, n3, False), Conv(c3, c3, 3, 2), _Layer(), C2f(c3 + c4, c4, n3, False),
+             Segment(npr=lay.npr, ch=(c2, c3, c4))]
         self.model = nn.ModuleList(L)
+        self.scale = scale
         self._packed = _Packed()
 
     # ---- packing ------------------------------------------------------------------------------------------------------
@@ -234,34 +258,37 @@ class YOLOv8Seg(nn.Module):
         w = self._weights()
         frames = frames.contiguous()
         dev = frames.device
+        lay = scale_layout(self.scale)
+        c0, c1, c2, c3, c4 = lay.c
+        npr, conv = lay.npr, self._conv
         e = lambda h, ww, c, dt=bf: torch.empty(B, h, ww, c, dtype=dt, device=dev)   # noqa: E731
         s2, s4, s8, s16, s32 = (H // 2, W // 2), (H // 4, W // 4), (H // 8, W // 8), (H // 16, W // 16), (H // 32, W // 32)
-        x0 = e(*s2, 80)
-        _lib.call("sam6d_yolo_stem", _p(frames), B, H, W, _p(w["stem"][0]), _p(w["stem"][1]), _p(x0), _s())
-        x1 = self._conv(x0, w[1], e(*s4, 160), stride=2)
-        x2 = self._c2f(x1, w[2], e(*s4, 160))
-        x3 = self._conv(x2, w[3], e(*s8, 320), stride=2)
-        cat14 = e(*s8, 960)                                             # [up(12) | 4]
-        self._c2f(x3, w[4], cat14[..., 640:])
-        x5 = self._conv(cat14[..., 640:], w[5], e(*s16, 640), stride=2)
-        cat11 = e(*s16, 1280)                                           # [up(9) | 6]
-        self._c2f(x5, w[6], cat11[..., 640:])
-        x7 = self._conv(cat11[..., 640:], w[7], e(*s32, 640), stride=2)
-        x8 = self._c2f(x7, w[8], e(*s32, 640))
-        sppf = e(*s32, 1280)
-        self._conv(x8, w[9].cv1, sppf[..., :320])
-        _lib.call("sam6d_yolo_sppf", _p(sppf), ctypes.c_longlong(1280), B, s32[0], s32[1], 320, _s())
-        cat20 = e(*s32, 1280)                                           # [19 | 9]
-        self._conv(sppf, w[9].cv2, cat20[..., 640:])
-        self._up(cat20[..., 640:], cat11[..., :640])
-        cat17 = e(*s16, 960)                                            # [16 | 12]
-        self._c2f(cat11, w[12], cat17[..., 320:])
-        self._up(cat17[..., 320:], cat14[..., :640])
-        p3 = self._c2f(cat14, w[15], e(*s8, 320))
-        self._conv(p3, w[16], cat17[..., :320], stride=2)
-        p4 = self._c2f(cat17, w[18], e(*s16, 640))
-        self._conv(p4, w[19], cat20[..., :640], stride=2)
-        p5 = self._c2f(cat20, w[21], e(*s32, 640))
+        x0 = e(*s2, c0)
+        _lib.call("sam6d_yolo_stem_c", _p(frames), B, H, W, c0, _p(w["stem"][0]), _p(w["stem"][1]), _p(x0), _s())
+        x1 = conv(x0, w[1], e(*s4, c1), stride=2)
+        x2 = self._c2f(x1, w[2], e(*s4, c1))
+        x3 = conv(x2, w[3], e(*s8, c2), stride=2)
+        cat14 = e(*s8, c3 + c2)                                         # [up(12) | 4]
+        self._c2f(x3, w[4], cat14[..., c3:])
+        x5 = conv(cat14[..., c3:], w[5], e(*s16, c3), stride=2)
+        cat11 = e(*s16, c4 + c3)                                        # [up(9) | 6]
+        self._c2f(x5, w[6], cat11[..., c4:])
+        x7 = conv(cat11[..., c4:], w[7], e(*s32, c4), stride=2)
+        x8 = self._c2f(x7, w[8], e(*s32, c4))
+        sppf = e(*s32, 2 * c4)                                          # [cv1 | 5x5 | 9x9 | 13x13], c4 / 2 each
+        conv(x8, w[9].cv1, sppf[..., :c4 // 2])
+        _lib.call("sam6d_yolo_sppf", _p(sppf), ctypes.c_longlong(2 * c4), B, s32[0], s32[1], c4 // 2, _s())
+        cat20 = e(*s32, c3 + c4)                                        # [19 | 9]
+        conv(sppf, w[9].cv2, cat20[..., c3:])
+        self._up(cat20[..., c3:], cat11[..., :c4])
+        cat17 = e(*s16, c2 + c3)                                        # [16 | 12]
+        self._c2f(cat11, w[12], cat17[..., c2:])
+        self._up(cat17[..., c2:], cat14[..., :c3])
+        p3 = self._c2f(cat14, w[15], e(*s8, c2))
+        conv(p3, w[16], cat17[..., :c2], stride=2)
+        p4 = self._c2f(cat17, w[18], e(*s16, c3))
+        conv(p4, w[19], cat20[..., :c3], stride=2)
+        p5 = self._c2f(cat20, w[21], e(*s32, c4))
         # ---- Segment head: rows of all anchors, level after level
         sizes = (s8, s16, s32)
         A = sum(h * ww for h, ww in sizes)
@@ -269,20 +296,20 @@ class YOLOv8Seg(nn.Module):
         off = 0
         for hw, x, hc in zip(sizes, (p3, p4, p5), w["head"]):
             t1, t2 = e(*hw, sum(hc.widths)), e(*hw, sum(hc.widths))
-            self._conv(x, hc.first, t1)
+            conv(x, hc.first, t1)
             c = 0
             for cw, wd in zip(hc.second, hc.widths):
-                self._conv(t1[..., c:c + wd], cw, t2[..., c:c + wd])
+                conv(t1[..., c:c + wd], cw, t2[..., c:c + wd])
                 c += wd
-            self._conv(t2, hc.last, head[:, off:off + hw[0] * hw[1]].unflatten(1, hw), silu=False)
+            conv(t2, hc.last, head[:, off:off + hw[0] * hw[1]].unflatten(1, hw), silu=False)
             off += hw[0] * hw[1]
-        pr1 = self._conv(p3, w["p1"], e(*s8, 320))
-        up = e(*s4, 320)
+        pr1 = conv(p3, w["p1"], e(*s8, npr))
+        up = e(*s4, npr)
         for i in range(2):
             for j in range(2):
-                self._conv(pr1, w["up"][i][j], up, silu=False, tap=(i, j))
-        pr2 = self._conv(up, w["p2"], e(*s4, 320))
-        proto = self._conv(pr2, w["p3"], e(*s4, NM, torch.float32))
+                conv(pr1, w["up"][i][j], up, silu=False, tap=(i, j))
+        pr2 = conv(up, w["p2"], e(*s4, npr))
+        proto = conv(pr2, w["p3"], e(*s4, NM, torch.float32))
         return head, proto
 
 
@@ -315,20 +342,98 @@ _pickle_module = SimpleNamespace(Unpickler=_FastSAMUnpickler, load=lambda f, **k
                                  __name__="sam6d_b200.fast_sam._pickle")
 
 
+def checkpoint_scale(sd: Dict[str, torch.Tensor]) -> Optional[str]:
+    """the scale whose layout a state_dict's shapes announce -- model.0's output channels, the bottleneck counts of model.2 and
+    model.4, model.9.cv2's output channels -- or None"""
+    try:
+        found = (sd["model.0.conv.weight"].shape[0], _bottlenecks(sd, "model.2"), _bottlenecks(sd, "model.4"), sd["model.9.cv2.conv.weight"].shape[0])
+    except KeyError:
+        return None
+    for name in SCALES:
+        lay = scale_layout(name)
+        if found == (lay.c[0], lay.n3, lay.n6, lay.c[4]):
+            return name
+    return None
+
+
+def _bottlenecks(sd, prefix):
+    return len({k.split(".")[3] for k in sd if k.startswith(prefix + ".m.")})
+
+
+def _found(sd):
+    """what a state_dict holds, in the words of the rejection message"""
+    def out_ch(k):
+        return sd[k].shape[0] if k in sd and sd[k].dim() else "none"
+    return (f"stem width {out_ch('model.0.conv.weight')}, SPPF width {out_ch('model.9.cv2.conv.weight')}, "
+            f"C2f depths {_bottlenecks(sd, 'model.2')} / {_bottlenecks(sd, 'model.4')} in model.2 / model.4")
+
+
 def load_fastsam_checkpoint(path) -> Dict[str, torch.Tensor]:
-    """the ultralytics checkpoint `path` (FastSAM-x.pt) -> fp32 state_dict with YOLOv8Seg's keys (checked)"""
+    """the ultralytics checkpoint `path` (FastSAM-x.pt or FastSAM-s.pt) -> fp32 state_dict with YOLOv8Seg's keys, checked
+    against the layout of the scale its shapes announce (checkpoint_scale)"""
     ckpt = torch.load(path, map_location="cpu", weights_only=False, pickle_module=_pickle_module)
     model = (ckpt.get("ema") or ckpt["model"]) if isinstance(ckpt, dict) else None
     if not isinstance(model, nn.Module):
         raise ValueError(f"{path}: no 'ema' / 'model' module in the checkpoint")
     sd = {k: v.float() if v.is_floating_point() else v for k, v in model.float().state_dict().items()}
-    ref = YOLOv8Seg().state_dict()
+    scale = checkpoint_scale(sd)
+    ref = YOLOv8Seg(scale or "x").state_dict()
     missing = sorted(set(ref) - set(sd))
     unexpected = sorted(set(sd) - set(ref))
     shapes = sorted(f"{k}: {tuple(sd[k].shape)} vs {tuple(ref[k].shape)}" for k in set(sd) & set(ref) if sd[k].shape != ref[k].shape)
+    if scale is None:
+        known = "; ".join(f"{n}: stem width {scale_layout(n).c[0]}, SPPF width {scale_layout(n).c[4]}, C2f depths "
+                          f"{scale_layout(n).n3} / {scale_layout(n).n6}" for n in SCALES)
+        raise ValueError(f"{path} is not a YOLOv8x-seg or YOLOv8s-seg (nc=1) checkpoint: found {_found(sd)} (known scales {known}); "
+                         f"against YOLOv8x-seg: missing {missing}, unexpected {unexpected}, mis-shaped {shapes}")
     if missing or unexpected or shapes:
-        raise ValueError(f"{path} is not a YOLOv8x-seg (nc=1) checkpoint: missing {missing}, unexpected {unexpected}, mis-shaped {shapes}")
+        raise ValueError(f"{path} is not a YOLOv8{scale}-seg (nc=1) checkpoint: found {_found(sd)}; missing {missing}, "
+                         f"unexpected {unexpected}, mis-shaped {shapes}")
     return sd
+
+
+def conv_shapes(scale: str, H: int, W: int):
+    """every convolution of the network at an H x W frame, in forward order: dicts (name, Cin, Cout, k, s, H, W, Ho, Wo); the
+    Proto upsample is listed once as its four 1 x 1 taps' combined Cout"""
+    lay = scale_layout(scale)
+    c0, c1, c2, c3, c4 = lay.c
+    n3, n6, npr = lay.n3, lay.n6, lay.npr
+    out = []
+
+    def add(name, cin, cout, k, s, h, w):
+        ho, wo = (h + 2 * (k // 2) - k) // s + 1, (w + 2 * (k // 2) - k) // s + 1
+        out.append(dict(name=name, Cin=cin, Cout=cout, k=k, s=s, H=h, W=w, Ho=ho, Wo=wo))
+        return ho, wo
+
+    def c2f(name, ci, co, n, h, w):
+        c = co // 2
+        add(name + ".cv1", ci, 2 * c, 1, 1, h, w)
+        for i in range(n):
+            add(f"{name}.m.{i}.cv1", c, c, 3, 1, h, w)
+            add(f"{name}.m.{i}.cv2", c, c, 3, 1, h, w)
+        add(name + ".cv2", (2 + n) * c, co, 1, 1, h, w)
+
+    h2 = add("model.0", 3, c0, 3, 2, H, W)
+    h4 = add("model.1", c0, c1, 3, 2, *h2); c2f("model.2", c1, c1, n3, *h4)
+    h8 = add("model.3", c1, c2, 3, 2, *h4); c2f("model.4", c2, c2, n6, *h8)
+    h16 = add("model.5", c2, c3, 3, 2, *h8); c2f("model.6", c3, c3, n6, *h16)
+    h32 = add("model.7", c3, c4, 3, 2, *h16); c2f("model.8", c4, c4, n3, *h32)
+    add("model.9.cv1", c4, c4 // 2, 1, 1, *h32); add("model.9.cv2", 2 * c4, c4, 1, 1, *h32)
+    c2f("model.12", c4 + c3, c3, n3, *h16); c2f("model.15", c3 + c2, c2, n3, *h8)
+    add("model.16", c2, c2, 3, 2, *h8); c2f("model.18", c2 + c3, c3, n3, *h16)
+    add("model.19", c3, c3, 3, 2, *h16); c2f("model.21", c3 + c4, c4, n3, *h32)
+    seg = Segment(npr=npr, ch=(c2, c3, c4))
+    widths = [seg.cv2[0][0].conv.out_channels, seg.cv3[0][0].conv.out_channels, seg.cv4[0][0].conv.out_channels]
+    for i, (ch, hw) in enumerate(((c2, h8), (c3, h16), (c4, h32))):
+        add(f"model.22.head.{i}.first", ch, sum(widths), 3, 1, *hw)
+        for name, wd in zip(("cv2", "cv3", "cv4"), widths):
+            add(f"model.22.{name}.{i}.1", wd, wd, 3, 1, *hw)
+        add(f"model.22.head.{i}.last", sum(widths), HEAD_W, 1, 1, *hw)
+    add("model.22.proto.cv1", c2, npr, 3, 1, *h8)
+    add("model.22.proto.upsample", npr, 4 * npr, 1, 1, *h8)
+    add("model.22.proto.cv2", npr, npr, 3, 1, h8[0] * 2, h8[1] * 2)
+    add("model.22.proto.cv3", npr, NM, 1, 1, h8[0] * 2, h8[1] * 2)
+    return out
 
 
 # =====================================================================================================================
@@ -377,16 +482,24 @@ class FastSAM:
         original size (float masks); boxes are scale_boxes + clip_boxes in original pixels.
     Where the reference fails (no detection: `masks.data` of None), empty tensors are returned."""
 
-    def __init__(self, checkpoint_path=None, config=None, segmentor_width_size=640, device=None):
+    def __init__(self, checkpoint_path=None, config=None, segmentor_width_size=640, device=None, scale: Optional[str] = None):
+        """scale: "x" or "s".  With a checkpoint the network is the scale the checkpoint holds (a different `scale` raises);
+        without one it is `scale`, default "x"."""
         cfg = config if config is not None else SimpleNamespace(iou_threshold=0.9, conf_threshold=0.05, max_det=200)
         get = (lambda k: cfg[k]) if isinstance(cfg, dict) else (lambda k: getattr(cfg, k))
         self.iou, self.max_det = float(get("iou_threshold")), int(get("max_det"))
         self.conf = 0.25                                 # fast_sam.py:39 overrides the config's conf_threshold
         self.segmentor_width_size = segmentor_width_size
         self.current_device = torch.device(device) if device is not None else torch.device("cuda")
-        self.model = YOLOv8Seg().to(self.current_device).eval()
-        if checkpoint_path is not None:
-            self.model.load_state_dict(load_fastsam_checkpoint(checkpoint_path), strict=True)
+        sd = load_fastsam_checkpoint(checkpoint_path) if checkpoint_path is not None else None
+        if sd is not None:
+            held = checkpoint_scale(sd)
+            if scale is not None and scale != held:
+                raise ValueError(f"scale={scale!r} but {checkpoint_path} holds YOLOv8{held}-seg")
+            scale = held
+        self.model = YOLOv8Seg(scale or "x").to(self.current_device).eval()
+        if sd is not None:
+            self.model.load_state_dict(sd, strict=True)
 
     @torch.no_grad()
     def postprocess(self, head: torch.Tensor, proto: torch.Tensor, shape) -> Dict[str, torch.Tensor]:

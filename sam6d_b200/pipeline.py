@@ -250,15 +250,19 @@ class SAM6D:
     The ISM settings of the reference's configuration: level_templates (0 / 1 / 2 = 42 / 162 / 642 views) and pose_distribution
     ("all", or "upper": cameras with z >= 0) choose the views the ISM matches against (onboarding_config); aggregation_function
     ("mean", "median", "max", "avg_5") how each object's template similarities become its semantic score (matching_config).
-    The PEM always uses the 42 level-0 views."""
+    The PEM always uses the 42 level-0 views.  fastsam_model ("FastSAM-x" or "FastSAM-s") picks the FastSAM checkpoint and
+    network when segmentor is "fastsam"."""
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
                  checkpoint_dir: Optional[str] = None, checkpoint: Optional[str] = None, random_weights: bool = False,
                  stability_score_thresh: float = 0.97, pred_iou_thresh: float = 0.88, points_per_side: int = 32,
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
-                 device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5"):
+                 device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5",
+                 fastsam_model: str = "FastSAM-x"):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
+        if fastsam_model not in ism_cli.FASTSAM_MODELS:
+            raise ValueError(f"fastsam_model must be one of {sorted(ism_cli.FASTSAM_MODELS)}, got {fastsam_model!r}")
         render.template_view_set(level_templates, pose_distribution)          # ValueError on an unknown view set
         if aggregation_function not in ops.TEMPLATE_AGGREGATIONS:
             raise ValueError(f"aggregation_function must be one of {sorted(ops.TEMPLATE_AGGREGATIONS)}, got {aggregation_function!r}")
@@ -267,7 +271,7 @@ class SAM6D:
         self.device = torch.device(device if device is not None else "cuda")
         self.confidence_thresh = float(confidence_thresh)
         self.det_score_thresh = float(det_score_thresh)
-        ism_args = SimpleNamespace(segmentor_model=segmentor, sam_model_type=sam_model_type, dinov2_model=dinov2_model,
+        ism_args = SimpleNamespace(segmentor_model=segmentor, sam_model_type=sam_model_type, fastsam_model=fastsam_model, dinov2_model=dinov2_model,
                                    checkpoint_dir=checkpoint_dir, random_weights=random_weights,
                                    stability_score_thresh=stability_score_thresh, pred_iou_thresh=pred_iou_thresh,
                                    points_per_side=points_per_side)

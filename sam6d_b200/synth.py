@@ -381,8 +381,15 @@ def make_image_embedding(seed=1, size=64) -> torch.Tensor:
     return emb.unsqueeze(0)
 
 
-def make_fastsam_state_dict(seed: int = 1) -> SD:
-    """Seeded YOLOv8x-seg (nc=1) weights under ultralytics' keys (the layout of FastSAM-x.pt).  Convolutions are drawn at
+# the heads' last layers in make_fastsam_state_dict: scales of the DFL (cv2), class (cv3) and coefficient (cv4) weights, the
+# coefficient bias, and the class bias of each level.  At s the class features of a level vary little around a level-dependent
+# mean, so the class weights are scaled up and each level's bias centres its logits near -2.5.
+_FASTSAM_HEAD_SCALES = {"x": (20.0, 35.0, 300.0, 0.065, (0.0, 0.0, 0.0)), "s": (20.0, 140.0, 200.0, 20.0, (-19.8, 13.0, 13.6))}
+
+
+def make_fastsam_state_dict(seed: int = 1, scale: str = "x") -> SD:
+    """Seeded YOLOv8{scale}-seg (nc=1) weights under ultralytics' keys (the layout of FastSAM-x.pt / FastSAM-s.pt; the x draw
+    is the one this function made before it took a scale).  Convolutions are drawn at
     1/sqrt(fan_in) and BatchNorm statistics are randomised, so activations stay O(1) through the 23 layers and folding is
     exercised.  The heads' last layers are scaled so decoded boxes vary, masks are crisp (few pixels near the 0.5 threshold) and,
     on the test frames, several hundred anchors pass conf 0.25 and more than max_det = 200 survive NMS, so the max_det cut is
@@ -390,7 +397,7 @@ def make_fastsam_state_dict(seed: int = 1) -> SD:
     from .fast_sam import YOLOv8Seg
     g = torch.Generator().manual_seed(seed)
     sd: SD = {}
-    for k, v in YOLOv8Seg().state_dict().items():
+    for k, v in YOLOv8Seg(scale).state_dict().items():
         if k.endswith("num_batches_tracked"):
             sd[k] = torch.zeros((), dtype=torch.long)
         elif k.endswith("dfl.conv.weight"):
@@ -409,12 +416,13 @@ def make_fastsam_state_dict(seed: int = 1) -> SD:
     # the heads' last 1x1 convolutions: zero-sum rows (the SiLU features have a positive mean, which would otherwise give every
     # anchor the same offset), scaled so DFL logits have std ~2.4 and class logits ~N(-2.5, 1.5) (~18 % of anchors pass 0.25);
     # the mask coefficients are scaled and biased so that coeffs . proto is ~0 on average over anchors with std ~1.6 within a mask
+    s_box, s_cls, s_mc, b_mc, b_cls = _FASTSAM_HEAD_SCALES[scale]
     for i in range(3):
-        for name, scale in (("cv2", 20.0), ("cv3", 35.0), ("cv4", 300.0)):
+        for name, f in (("cv2", s_box), ("cv3", s_cls), ("cv4", s_mc)):
             w = sd[f"model.22.{name}.{i}.2.weight"]
-            sd[f"model.22.{name}.{i}.2.weight"] = (w - w.mean(dim=1, keepdim=True)) * scale
-        sd[f"model.22.cv3.{i}.2.bias"].zero_()
-        sd[f"model.22.cv4.{i}.2.bias"].fill_(0.065)
+            sd[f"model.22.{name}.{i}.2.weight"] = (w - w.mean(dim=1, keepdim=True)) * f
+        sd[f"model.22.cv3.{i}.2.bias"].fill_(b_cls[i])
+        sd[f"model.22.cv4.{i}.2.bias"].fill_(b_mc)
     return sd
 
 

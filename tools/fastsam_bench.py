@@ -1,11 +1,11 @@
-"""Times the FastSAM segmentor on one GPU and prints one JSON line: the YOLOv8x-seg forward on a 480 x 640 frame at B = 1 and
-B = 8 (CUDA events, algorithmic GFLOP from the layer shapes over time), FastSAM.generate_masks end to end per frame, the five
-largest convolution layers alone with achieved TFLOP/s, and two yardsticks measured in the same run: torch / cuDNN bf16
-channels_last convolutions of the same network (the oracle's fused layers), and the SAM path's
+"""Times the FastSAM segmentor on one GPU and prints one JSON line: the YOLOv8x-seg or YOLOv8s-seg (--scale x / s) forward on
+a 480 x 640 frame at B = 1 and B = 8 (CUDA events, GFLOP of the executed convolutions over time); FastSAM.generate_masks end
+to end per frame; every distinct convolution shape alone at B = 1 and B = 8 with achieved TFLOP/s; and two yardsticks measured in the same run: torch /
+cuDNN bf16 channels_last convolutions of the same network (the oracle's fused layers), and the SAM path's
 CustomSamAutomaticMaskGenerator.generate_masks on the same frame.  Seeded weights (speed does not depend on their values).
 The card's name, power limit and maximum SM clock are read with nvidia-smi in the same run.
 
-    python tools/fastsam_bench.py [--iters 20]"""
+    python tools/fastsam_bench.py [--scale x] [--iters 20]"""
 import argparse
 import json
 import os
@@ -35,21 +35,23 @@ def _time(fn, iters, warmup=3):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--scale", default="x", choices=("x", "s"))
     ap.add_argument("--iters", type=int, default=20)
     args = ap.parse_args()
     from oracle import fastsam_oracle as fo
     from sam6d_b200 import synth
-    from sam6d_b200.fast_sam import FastSAM, YOLOv8Seg, _CW
+    from sam6d_b200.fast_sam import FastSAM, YOLOv8Seg, _CW, conv_shapes
 
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
                           text=True).stdout.strip().splitlines()[0]
     dev = torch.device("cuda")
-    sd = synth.make_fastsam_state_dict(1)
+    sd = synth.make_fastsam_state_dict(1, args.scale)
     frame = synth.make_fastsam_frame(480, 640, 0)
-    gflop = fo.flops((480, 640))
-    res = dict(card=card, frame="480x640", gflop_per_frame=round(gflop, 2))
+    shapes = conv_shapes(args.scale, 480, 640)
+    gflop = sum(2.0 * l["Cout"] * l["Cin"] * l["k"] ** 2 * l["Ho"] * l["Wo"] for l in shapes) / 1e9
+    res = dict(card=card, scale=args.scale, frame="480x640", gflop_per_frame=round(gflop, 2))
 
-    net = YOLOv8Seg().to(dev).eval()
+    net = YOLOv8Seg(args.scale).to(dev).eval()
     net.load_state_dict(sd, strict=True)
     for B in (1, 8):
         x = torch.from_numpy(np.stack([frame] * B)).to(dev)
@@ -57,24 +59,30 @@ def main():
         res[f"forward_b{B}_ms"] = round(ms, 3)
         res[f"forward_b{B}_tflops"] = round(gflop * B / ms, 1)
 
-    seg = FastSAM(None, dict(iou_threshold=0.9, conf_threshold=0.05, max_det=200), device=dev)
+    seg = FastSAM(None, dict(iou_threshold=0.9, conf_threshold=0.05, max_det=200), device=dev, scale=args.scale)
     seg.model.load_state_dict(sd, strict=True)
     res["generate_masks_ms"] = round(_time(lambda: seg.generate_masks(frame), args.iters), 3)
     res["generate_masks_detections"] = int(seg.generate_masks(frame)["masks"].shape[0])
 
-    # five largest convolutions alone (B = 1)
-    layers = sorted(fo.conv_shapes(480, 640), key=lambda l: -l["Cout"] * l["Cin"] * l["k"] ** 2 * l["Ho"] * l["Wo"])
-    big = []
+    # every distinct convolution shape alone (the Cin = 3 stem is its own kernel; the Proto upsample runs as 1 x 1 taps)
+    seen, layers = set(), []
     g = torch.Generator(device=dev).manual_seed(0)
-    for l in [l for l in layers if l["Cin"] != 3 and "upsample" not in l["name"]][:5]:
-        x = torch.randn(1, l["H"], l["W"], l["Cin"], device=dev, generator=g).to(torch.bfloat16)
+    for l in shapes:
+        key = (l["H"], l["W"], l["Cin"], l["Cout"], l["k"], l["s"])
+        if l["Cin"] == 3 or "upsample" in l["name"] or key in seen:
+            continue
+        seen.add(key)
         cw = _CW(torch.randn(l["Cout"], l["Cin"], l["k"], l["k"], device=dev, generator=g) * 0.05, torch.zeros(l["Cout"], device=dev))
-        y = torch.empty(1, l["Ho"], l["Wo"], l["Cout"], device=dev, dtype=torch.bfloat16)
-        ms = _time(lambda: YOLOv8Seg._conv(x, cw, y, stride=l["s"]), 4 * args.iters)
-        fl = 2.0 * l["Cout"] * l["Cin"] * l["k"] ** 2 * l["Ho"] * l["Wo"]
-        big.append(dict(layer=l["name"], shape=f"{l['Cin']}->{l['Cout']} k{l['k']} s{l['s']} {l['H']}x{l['W']}", us=round(ms * 1e3, 1),
-                        tflops=round(fl / ms / 1e9, 1)))
-    res["largest_convs"] = big
+        row = dict(layer=l["name"], shape=f"{l['Cin']}->{l['Cout']} k{l['k']} s{l['s']} {l['H']}x{l['W']}")
+        for B in (1, 8):
+            x = torch.randn(B, l["H"], l["W"], l["Cin"], device=dev, generator=g).to(torch.bfloat16)
+            y = torch.empty(B, l["Ho"], l["Wo"], l["Cout"], device=dev, dtype=torch.bfloat16)
+            fl = 2.0 * B * l["Cout"] * l["Cin"] * l["k"] ** 2 * l["Ho"] * l["Wo"]
+            ms = _time(lambda: YOLOv8Seg._conv(x, cw, y, stride=l["s"]), 4 * args.iters)
+            row[f"b{B}_us"] = round(ms * 1e3, 1)
+            row[f"b{B}_tflops"] = round(fl / ms / 1e9, 1)
+        layers.append(row)
+    res["layers"] = layers
 
     # yardstick 1: the oracle's network (fused as ultralytics fuses it) in torch / cuDNN, bf16 channels_last
     class _Cudnn(fo.Net):

@@ -1,6 +1,6 @@
 """Times one whole SAM-6D frame (480 x 640, templates -> ISM -> PEM) through a resident sam6d_b200.pipeline.SAM6D and writes
 one JSON file:
-  * configurations: SAM ViT-H, SAM ViT-B and FastSAM as the segmentor, DINOv2 ViT-L descriptors, PEM in bf16; seeded weights
+  * configurations: SAM ViT-H, SAM ViT-B, FastSAM-x and FastSAM-s as the segmentor, DINOv2 ViT-L descriptors, PEM in bf16; seeded weights
     (speed does not depend on their values);
   * frame: the repository's example frame (tests/golden/pem_input.pt) and the convex hull of its object's samples as the CAD;
   * per stage (segmentor, descriptors, scores, RLE, ISM records, PEM inputs, Net.forward, PEM records): host clock between
@@ -18,7 +18,7 @@ With --objects 1,8,21 the first configuration instead times SAM6D.detect_objects
 example CAD at O distinct scales, ids 1..O): the stages above plus the per-object NMS ("nms"), onboard_objects' cost, and the
 counts after each filter.
 
-    python tools/sam6d_frame_bench.py [--frames 10] [--warmup 2] [--pem_dets 8] [--configs sam_vit_h,sam_vit_b,fastsam]
+    python tools/sam6d_frame_bench.py [--frames 10] [--warmup 2] [--pem_dets 8] [--configs sam_vit_h,sam_vit_b,fastsam,fastsam_s]
                                       [--objects 1,8,21] --out FILE"""
 import argparse
 import json
@@ -38,6 +38,7 @@ CONFIGS = {
     "sam_vit_h": dict(segmentor="sam", sam_model_type="vit_h", stability_score_thresh=0.0, pred_iou_thresh=-10, points_per_side=32),
     "sam_vit_b": dict(segmentor="sam", sam_model_type="vit_b", stability_score_thresh=0.0, pred_iou_thresh=-10, points_per_side=32),
     "fastsam": dict(segmentor="fastsam"),
+    "fastsam_s": dict(segmentor="fastsam", fastsam_model="FastSAM-s"),
 }
 STAGES = ("segmentor", "descriptors", "scores", "rle", "ism_records", "pem_inputs", "forward", "pem_records")
 MULTI_STAGES = ("segmentor", "descriptors", "scores", "nms", "rle", "ism_records", "pem_inputs", "forward", "pem_records")
