@@ -177,6 +177,12 @@ int sam6d_crop_resize_normalize(const unsigned char* images, const unsigned char
  * pmask (P,T,T) f32 (same geometry); either output may be NULL */
 int sam6d_crop_resize_pad(const unsigned char* image, const float* masks, const int* boxes, int P, int H, int W, int T, float* rgb,
                           float* pmask, void* stream);
+/* BOPTemplatePBR.__getitem__ (ISM/provider/bop_pbr.py) for R references cut from a stack of F decoded frames (F,H,W,3) u8 RGB:
+ * frame_idx (R) i32 the frame of each reference, masks (R,H,W) u8 its visible mask (any value 0..255) -> boxes (R,4) i32 the mask's
+ * Image.getbbox (nonzero pixels, exclusive max; (0,0,0,0) when empty), rgb (R,3,T,T) f32 Normalize(CropResizePad(composite(frame,
+ * black, mask) / 255)), pmask (R,T,T) f32 CropResizePad(mask / 255); crop geometry as sam6d_crop_resize_pad; R <= 65535 */
+int sam6d_pbr_reference_crops(const unsigned char* frames, int F, int H, int W, const int* frame_idx, const unsigned char* masks, int R,
+                              int T, int* boxes, float* rgb, float* pmask, void* stream);
 /* compute_cls_and_patch_features tail: patch token (p,t) = tokens + p*tok_bs + t*tok_ld (C f32); kept when the mean of its
  * patch x patch block of pmask (P, G*patch, G*patch) exceeds thresh, then L2-normalised, else zero -> out_f32 / out_bf16
  * (P, G*G, C) (either NULL), valid (P, G*G) u8 or NULL */

@@ -8,6 +8,10 @@ With several CAD models (--cad_path a.ply b.ply ... [--obj_ids 1 5 ...]) the fra
 multi-object post-processing (size filter, per-object NMS), records with category_id = the object's id (default 1, 2, ...),
 and one PEM batch across the objects; vis_pem.png draws each object's best pose with that object's points.
 
+--rendering_type pbr --pbr_root DATASET [--pbr_split train_pbr] takes the ISM references from the BOP PBR split DATASET/train_pbr
+instead of GPU renders (the reference's default onboarding_config.rendering_type; sam6d_b200/pbr.py).  It needs --obj_ids, the
+BOP ids of the CAD models, and --pose_distribution all.
+
 Writes what the chained CLIs write as results: $OUT/sam6d_results/detection_ism.json, detection_pem.json and vis_pem.png,
 with the same records.  It does not write the template files ($OUT/templates/*) nor detection_ism.npz: the npz is an
 intermediate of the reference that nothing downstream reads, and writing it would copy every dense proposal mask to the
@@ -54,6 +58,10 @@ def get_parser():
                     help="the ISM's views (onboarding_config): 0 / 1 / 2 = 42 / 162 / 642; the PEM keeps the 42 level-0 views")
     ap.add_argument("--pose_distribution", default="all", choices=("all", "upper"),
                     help="onboarding_config.pose_distribution: all, or upper (cameras with z >= 0)")
+    ap.add_argument("--rendering_type", default="pyrender", choices=("pyrender", "pbr"),
+                    help="onboarding_config.rendering_type: ISM references rendered from the CAD model, or frames of a BOP PBR split")
+    ap.add_argument("--pbr_root", default=None, help="with --rendering_type pbr: the BOP dataset directory (holding --pbr_split)")
+    ap.add_argument("--pbr_split", default="train_pbr", help="with --rendering_type pbr: the split whose frames become the references")
     # the PEM CLI's options
     ap.add_argument("--det_score_thresh", default=0.2, type=float, help="The score threshold of detection")
     ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth (default: the PEM CLI's)")
@@ -63,7 +71,10 @@ def get_parser():
 
 
 def main(argv=None):
-    args = get_parser().parse_args(argv)
+    ap = get_parser()
+    args = ap.parse_args(argv)
+    if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
+        ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
     from ..pipeline import SAM6D
     sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
                   dinov2_model=args.dinov2_model,
@@ -71,7 +82,8 @@ def main(argv=None):
                   stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
                   points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
                   det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
-                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function)
+                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
+                  rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split)
     multi = isinstance(args.cad_path, list)
     n_cad = len(args.cad_path) if multi else 1
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:
@@ -79,7 +91,8 @@ def main(argv=None):
     if multi:
         obj = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size)
     else:
-        obj = sam6d.onboard(args.cad_path, template_size=args.template_size)
+        obj = sam6d.onboard(args.cad_path, template_size=args.template_size,
+                            obj_id=args.obj_ids[0] if args.rendering_type == "pbr" else None)
     cam = json.load(open(args.cam_path))
     rgb = pem_cli.load_im(args.rgb_path).astype("uint8")
     run = sam6d.detect_objects if multi else sam6d

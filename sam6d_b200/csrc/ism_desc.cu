@@ -8,11 +8,9 @@
 //   * appearance_reduce : MaskedPatch_MatrixSimilarity.compute_straight / compute_visible_ratio (ISM/model/loss.py:52-77) on the
 //                       (P, 256, 256) patch-similarity matrices the batched tensor-core GEMM produced
 #include "common.cuh"
+#include "crop_geom.cuh"
 
 namespace {
-
-// F.interpolate(mode='nearest', scale_factor=s): out = floor(in * s) (double), src = min(floor(dst * (1/s) as float), in - 1)
-__device__ __forceinline__ int nearest_src(int dst, float inv_scale, int in_size) { return min((int)floorf((float)dst * inv_scale), in_size - 1); }
 
 // grid (T, P), block T threads: output (P, C, T, T) f32.  RGB: C = 3, value = ((img/255 - mean)/std) * mask[p]; MASK: C = 1, value = mask.
 template <bool RGB>
@@ -20,27 +18,8 @@ __global__ void crop_resize_pad_kernel(const unsigned char* __restrict__ image, 
                                        int H, int W, int T, float* __restrict__ out) {
   const int p = blockIdx.y, oy = blockIdx.x, ox = threadIdx.x;
   if (ox >= T) return;
-  const int x1 = boxes[p * 4], y1 = boxes[p * 4 + 1], x2 = boxes[p * 4 + 2], y2 = boxes[p * 4 + 3];
-  const int bw = x2 - x1, bh = y2 - y1;
-  // scale_factor = target_max / max(box size) as a float32 tensor element, .item() -> double (bbox_utils.py:99-105)
-  // `target_max / tensor` is torch.Tensor.__rtruediv__ = tensor.reciprocal() * target_max: two float32 roundings
-  const float scale_f = __fmul_rn(__frcp_rn((float)max(bw, bh)), (float)T);
-  const double scale = (double)scale_f;
-  const int rh = (int)floor((double)bh * scale), rw = (int)floor((double)bw * scale);
-  const float inv = (float)(1.0 / scale);                 // ATen: scale = 1 / scale_factor, computed in double, used as float
-  // padding (bbox_utils.py:111-118); a square resized crop (target ratio == original ratio) is not padded
-  int pt = 0, pl = 0, side = rh;                          // side of the (square) image after the optional padding
-  if ((double)rw / (double)rh != 1.0) { pt = max((T - rh) / 2, 0); pl = max((T - rw) / 2, 0); side = T; }
-  // final F.interpolate(scale_factor = T / side) (:122-124): the identity unless an unpadded square crop came out one pixel short
-  int py = oy, px = ox;
-  if (side != T) {
-    const float inv2 = (float)(1.0 / ((double)T / (double)side));
-    py = nearest_src(oy, inv2, side); px = nearest_src(ox, inv2, side);
-  }
-  const int yy = py - pt, xx = px - pl;
-  const bool inside = yy >= 0 && yy < rh && xx >= 0 && xx < rw;
-  int sy = 0, sx = 0;
-  if (inside) { sy = y1 + nearest_src(yy, inv, bh); sx = x1 + nearest_src(xx, inv, bw); }
+  int sy, sx;
+  const bool inside = crop_resize_pad_src(boxes[p * 4], boxes[p * 4 + 1], boxes[p * 4 + 2], boxes[p * 4 + 3], T, oy, ox, sy, sx);
   const float m = inside ? masks[((size_t)p * H + sy) * W + sx] : 0.f;
   if (RGB) {
     const float mean[3] = {0.485f, 0.456f, 0.406f}, sd[3] = {0.229f, 0.224f, 0.225f};

@@ -5,6 +5,8 @@ which keeps the models resident, onboards an object once and runs one RGB-D fram
     sam6d = SAM6D(segmentor="sam", checkpoint_dir="checkpoints", checkpoint="checkpoints/sam-6d-pem-base.pth")
     obj = sam6d.onboard("obj_000005.ply")                   # 42 templates rendered on the GPU, ISM + PEM template banks
     # denser ISM view sets and other aggregations: SAM6D(..., level_templates=2, pose_distribution="upper", aggregation_function="median")
+    # ISM references from a BOP PBR split (rendering_type: pbr): SAM6D(..., rendering_type="pbr", pbr_root="datasets/ycbv")
+    #   obj = sam6d.onboard("obj_000005.ply", obj_id=5)
     res = sam6d(rgb_u8, depth_u16, cam_K, depth_scale, obj)  # res.ism / res.pem: the CLIs' BOP-23 records; res.R, res.t
 
 Several known objects in a frame (Instance_Segmentation_Model.test_step for the ISM, one PEM batch across the objects):
@@ -24,26 +26,31 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import inputs, ism, meshio, ops, render
+from . import inputs, ism, meshio, ops, pbr, render
 from .cli import ism_run_inference_custom as ism_cli
 from .cli import pem_run_inference_custom as pem_cli
 from .cli import render_custom_templates as render_cli
 
 N_ISM_CLOUD = 2048                     # points of the geometric score's template cloud (ISM/run_inference_custom.py:196)
+RENDERING_TYPES = ("pyrender", "pbr")  # onboarding_config.rendering_type: the ISM references are renders, or BOP PBR frames
 
 
 # ---- render + framing (Render/render_custom_templates.py) -----------------------------------------------------------------
+def template_distance(mesh: meshio.Mesh, normalize: bool = True) -> float:
+    """the template camera's distance from the origin: 4r with --normalize (r = max |bbox corner|), else 2"""
+    if normalize:
+        r = max(np.linalg.norm(mesh.vertices.max(axis=0)), np.linalg.norm(mesh.vertices.min(axis=0)))
+        return 4.0 * float(r)
+    return 2.0
+
+
 def render_templates(mesh: meshio.Mesh, size: int = 512, normalize: bool = True, colorize: bool = False, base_color: float = 0.05,
                      poses_file: Optional[str] = None, level_templates: int = 0, pose_distribution: str = "all"):
     """the template views of one numpy mesh (mm) -> (render.render()'s dict for one object, poses (T,4,4) float64 in model units):
     the views of render.template_view_set(level_templates, pose_distribution), the 42 level-0 views first (the defaults: those
     42 only), or poses_file's.  Framing: camera 4r away with --normalize (r = max |bbox corner|), else 2; colours: base_color
     with colorize, else the mesh's texture / vertex colours / Blender's default grey."""
-    if normalize:
-        r = max(np.linalg.norm(mesh.vertices.max(axis=0)), np.linalg.norm(mesh.vertices.min(axis=0)))
-        distance = 4.0 * float(r)
-    else:
-        distance = 2.0
+    distance = template_distance(mesh, normalize)
     if colorize:
         mesh.colors = mesh.uv = mesh.texture = None
         grey = float(base_color)
@@ -251,14 +258,22 @@ class SAM6D:
     ("all", or "upper": cameras with z >= 0) choose the views the ISM matches against (onboarding_config); aggregation_function
     ("mean", "median", "max", "avg_5") how each object's template similarities become its semantic score (matching_config).
     The PEM always uses the 42 level-0 views.  fastsam_model ("FastSAM-x" or "FastSAM-s") picks the FastSAM checkpoint and
-    network when segmentor is "fastsam"."""
+    network when segmentor is "fastsam".
+
+    rendering_type (onboarding_config): "pyrender", the ISM references are GPU renders of the CAD model; "pbr", they are
+    frames of the BOP split pbr_root/pbr_split (sam6d_b200/pbr.py: for each view the frame whose object pose is nearest it,
+    cut out with its visible mask), which needs each object's BOP id and pose_distribution "all".  The split is scanned once,
+    at the first onboarding.  The geometric-score poses, the template cloud, the PEM bank and the model points come from the
+    mesh either way."""
+    rendering_type = "pyrender"
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
                  checkpoint_dir: Optional[str] = None, checkpoint: Optional[str] = None, random_weights: bool = False,
                  stability_score_thresh: float = 0.97, pred_iou_thresh: float = 0.88, points_per_side: int = 32,
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
                  device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5",
-                 fastsam_model: str = "FastSAM-x"):
+                 fastsam_model: str = "FastSAM-x", rendering_type: str = "pyrender", pbr_root: Optional[str] = None,
+                 pbr_split: str = "train_pbr"):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
         if fastsam_model not in ism_cli.FASTSAM_MODELS:
@@ -266,6 +281,15 @@ class SAM6D:
         render.template_view_set(level_templates, pose_distribution)          # ValueError on an unknown view set
         if aggregation_function not in ops.TEMPLATE_AGGREGATIONS:
             raise ValueError(f"aggregation_function must be one of {sorted(ops.TEMPLATE_AGGREGATIONS)}, got {aggregation_function!r}")
+        if rendering_type not in RENDERING_TYPES:
+            raise ValueError(f"rendering_type must be one of {RENDERING_TYPES}, got {rendering_type!r}")
+        if rendering_type == "pbr":
+            if pbr_root is None:
+                raise ValueError('rendering_type "pbr" needs pbr_root, the BOP dataset directory that holds the pbr_split')
+            if pose_distribution != "all":
+                raise NotImplementedError(f'rendering_type "pbr" selects references for pose_distribution "all" only, got {pose_distribution!r}')
+            pbr.list_scenes(pbr_root, pbr_split)                              # FileNotFoundError without the split
+        self.rendering_type, self.pbr_root, self.pbr_split, self._pbr_rows = rendering_type, pbr_root, pbr_split, None
         self.level_templates, self.pose_distribution = int(level_templates), pose_distribution
         self.aggregation_function = aggregation_function
         self.device = torch.device(device if device is not None else "cuda")
@@ -278,20 +302,47 @@ class SAM6D:
         self.seg, self.desc = ism_cli.build_models(ism_args, self.device)
         self.pem = pem_cli.build_model(SimpleNamespace(precision=precision, checkpoint=checkpoint, random_weights=random_weights), self.device)
 
-    def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None) -> Onboarded:
+    def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None, obj_id: Optional[int] = None) -> Onboarded:
         """render the templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates' framing
         and colours, and build everything a frame needs from them without touching a file: every view of
         render.template_view_set(level_templates, pose_distribution) is rendered once; the ISM references and the
         geometric-score poses come from the ISM's views, the PEM template bank from the 42 level-0 views.  Random draws, from
         `rng` (default numpy's global RNG), in the order the chained CLIs make them: the ISM template cloud, the PEM template
-        samples, the PEM model points."""
+        samples, the PEM model points.
+
+        rendering_type "pbr": obj_id, the object's BOP id, is required; the ISM references are the split's frames chosen by
+        pbr.select_references, whose draws come first from `rng`, then the draws above; only the 42 level-0 views are rendered."""
+        if self.rendering_type == "pbr":
+            if obj_id is None:
+                raise ValueError('rendering_type "pbr" needs the BOP object id: onboard(..., obj_id=)')
+            ref_cls, ref_patch = self._pbr_references([obj_id], rng)
+            return self._onboard_mesh(mesh_or_ply_path, template_size, rng, (ref_cls[0], ref_patch[0]))
+        return self._onboard_mesh(mesh_or_ply_path, template_size, rng)
+
+    def _pbr_references(self, obj_ids, rng):
+        """the PBR references of every object of obj_ids -> (ref_cls (O,T,C), ref_patch (O,T,256,C)) for the ISM's views"""
+        if self._pbr_rows is None:
+            self._pbr_rows = pbr.scan_split(self.pbr_root, self.pbr_split)
+        union, index = render.template_view_set(self.level_templates, "all")
+        sel = pbr.select_references(self._pbr_rows, obj_ids, union[index], rng)
+        return pbr.reference_features(self.desc, self._pbr_rows, sel, self.device)
+
+    def _onboard_mesh(self, mesh_or_ply_path, template_size, rng, refs=None) -> Onboarded:
+        """onboard() from the mesh, with the ISM references `refs` (ref_cls, ref_patch) when they are given"""
         mesh = meshio.load_ply_mesh(mesh_or_ply_path) if isinstance(mesh_or_ply_path, str) else mesh_or_ply_path
         verts, faces = mesh.vertices, mesh.faces
-        out, poses = render_templates(mesh, template_size, level_templates=self.level_templates, pose_distribution=self.pose_distribution)
-        ism_index = render.template_view_set(self.level_templates, self.pose_distribution)[1]
-        rgbs, masks, xyzs = template_arrays(out)
-        del out
-        ref_cls, ref_patch = ism_reference_features(self.desc, rgbs[ism_index], masks[ism_index], self.device)
+        if refs is None:
+            out, poses = render_templates(mesh, template_size, level_templates=self.level_templates, pose_distribution=self.pose_distribution)
+            ism_index = render.template_view_set(self.level_templates, self.pose_distribution)[1]
+            rgbs, masks, xyzs = template_arrays(out)
+            del out
+            ref_cls, ref_patch = ism_reference_features(self.desc, rgbs[ism_index], masks[ism_index], self.device)
+        else:
+            out, _ = render_templates(mesh, template_size)                    # the PEM's 42 level-0 views
+            rgbs, masks, xyzs = template_arrays(out)
+            del out
+            ref_cls, ref_patch = refs
+            poses, ism_index = render_cli.view_set(template_distance(mesh), None, self.level_templates, "all")
         cloud = meshio.sample_surface(verts, faces, N_ISM_CLOUD, rng) / 1000.0
         n0 = pem_cli.TEST_DATASET["n_template_view"]
         bank = pem_template_bank(self.pem, list(rgbs[:n0]), list(masks[:n0]), [x.astype(np.float32) for x in xyzs[:n0]], rng=rng,
@@ -302,12 +353,22 @@ class SAM6D:
     def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
         """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
         obj_ids: the category id of every object (distinct ints), default 1..O.  The fp32 patch tokens (44 MB per object at
-        C = 1024) are copied into the stack as each object is built, so only one object's extra copy is alive at a time."""
+        C = 1024) are copied into the stack as each object is built, so only one object's extra copy is alive at a time.
+
+        rendering_type "pbr": obj_ids are required and are the objects' BOP ids.  The references of all objects are selected
+        first (pbr.select_references' draws, object after object, as the reference's load_processed_metaData makes them), then
+        built in one pass over the split's frames straight into the stacks; then each mesh is onboarded with its draws."""
         meshes = list(meshes)
         n = len(meshes)
+        if self.rendering_type == "pbr" and obj_ids is None:
+            raise ValueError('rendering_type "pbr" needs the BOP id of every object: onboard_objects(meshes, obj_ids)')
         obj_ids = list(range(1, n + 1)) if obj_ids is None else [int(i) for i in obj_ids]
         if n == 0 or len(obj_ids) != n or len(set(obj_ids)) != n:
             raise ValueError(f"onboard_objects: {n} meshes need {n} distinct obj_ids, got {obj_ids}")
+        if self.rendering_type == "pbr":
+            ref_cls, ref_patch = self._pbr_references(obj_ids, rng)
+            parts = [self._onboard_mesh(mesh, template_size, rng, (ref_cls[o], None)) for o, mesh in enumerate(meshes)]
+            return ObjectSet.stack(parts, ref_patch, obj_ids)
         parts, ref_patch = [], None
         for o, mesh in enumerate(meshes):
             ob = self.onboard(mesh, template_size, rng)
