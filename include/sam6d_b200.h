@@ -156,6 +156,12 @@ int sam6d_geo_embed_lut(const float* T, long long clouds, int S, const void* tab
 int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
                          double cx, double cy, const double* thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
                          float* cloud2, void* stream);
+/* Stage A with the pixel-count cut min_count (sam6d_inputs_stage_a is this with 32): a detection with min_count or fewer pixels of
+ * mask AND depth > 0 gets stats[9] = 0; thr (P) f64 any radius threshold per detection (BOPTestset.get_instance: 8 and
+ * diameter * 0.6) */
+int sam6d_inputs_stage_a_min(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
+                             double cx, double cy, const double* thr, int min_count, unsigned char* mask, int* stats, int cap,
+                             int* choose1, int* choose2, float* cloud2, void* stream);
 /* Stage B, the Q kept detections keep[q]: choose_idx (Q,ns) i32 sample indices (drawn by the host like the reference's
  * np.random.choice) -> pts (Q,ns,3) f32, rgb_choose (Q,ns) i64 (get_resize_rgb_choose), rgb (Q,3,S,S) f32 = crop, channel
  * flip, mask, cv2.INTER_LINEAR resize (uint8 fixed point, bit exact), ToTensor + Normalize; rgb_u8 (Q,S,S,3) or NULL. */

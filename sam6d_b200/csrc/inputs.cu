@@ -112,8 +112,8 @@ __device__ __forceinline__ int block_scan_flag(bool flag, int* warp_sums, int* t
 // ---- 3. ordered compaction inside the bbox, centroid, radius filter (run_inference_custom.py:202-212) -----------------------
 // one CTA of 1024 threads per detection.  thr (P) float64: each detection's float32(radius) * float32(1.2) widened
 // (run_inference_custom.py:209), the radius being that of the detection's object.  choose1 / choose2: (P, cap) crop-linear pixel
-// indices, cloud2: (P, cap, 3) float32.
-__global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const double* __restrict__ thr, const unsigned char* __restrict__ mask,
+// indices, cloud2: (P, cap, 3) float32.  A detection of min_count pixels or fewer is skipped (n_valid 0).
+__global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, int min_count, const double* __restrict__ thr, const unsigned char* __restrict__ mask,
                                                            const float* __restrict__ depth, int* __restrict__ stats, int cap, int* __restrict__ choose1,
                                                            int* __restrict__ choose2, float* __restrict__ cloud2) {
   __shared__ int warp_sums[32];
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(1024) inp_compact_kernel(InCfg g, const double
   __shared__ double center[3];
   const int p = blockIdx.x, tid = threadIdx.x;
   int* s = stats + p * ST;
-  if (s[4] <= 32) { if (tid == 0) s[9] = 0; return; }       // np.sum(mask) > 32 else continue (:199-203)
+  if (s[4] <= min_count) { if (tid == 0) s[9] = 0; return; }  // np.sum(mask) > 32 else continue (:199-203)
   const double th = thr[p];
   const int y1 = s[5], y2 = s[6], x1 = s[7], x2 = s[8];
   const int ch = y2 - y1, cw = x2 - x1, area = ch * cw;
@@ -265,6 +265,10 @@ __global__ void inp_init_stats_kernel(int* __restrict__ stats, int P) {
 
 }  // namespace
 
+S6_API int sam6d_inputs_stage_a_min(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
+                                    double cx, double cy, const double* thr, int min_count, unsigned char* mask, int* stats, int cap,
+                                    int* choose1, int* choose2, float* cloud2, void* stream);
+
 // Stage A.  rle_cum: cumulative run ends of every detection's uncompressed COCO RLE (column-major), concatenated; rle_off (P+1)
 // offsets into it.  depth (H,W) f32 metres; fx, fy, cx, cy the float64 intrinsics; thr (P) f64 on the device, per detection
 // float32(radius) * float32(1.2) of its object.
@@ -273,8 +277,18 @@ __global__ void inp_init_stats_kernel(int* __restrict__ stats, int P) {
 S6_API int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
                                 double cx, double cy, const double* thr, unsigned char* mask, int* stats, int cap, int* choose1, int* choose2,
                                 float* cloud2, void* stream) {
+  return sam6d_inputs_stage_a_min(rle_cum, rle_off, P, H, W, depth, fx, fy, cx, cy, thr, 32, mask, stats, cap, choose1, choose2, cloud2,
+                                  stream);
+}
+
+// Stage A with the pixel-count cut as a parameter: a detection whose mask AND depth > 0 has min_count pixels or fewer gets no
+// radius filter (stats[9] = 0).  32 is run_inference_custom.py:199-203, 8 is BOPTestset.get_instance's minimum_n_point; thr is any
+// float64 threshold per detection (BOP: diameter * 0.6).
+S6_API int sam6d_inputs_stage_a_min(const int* rle_cum, const int* rle_off, int P, int H, int W, const float* depth, double fx, double fy,
+                                    double cx, double cy, const double* thr, int min_count, unsigned char* mask, int* stats, int cap,
+                                    int* choose1, int* choose2, float* cloud2, void* stream) {
   S6_REQUIRE(rle_cum && rle_off && depth && thr && mask && stats && choose1 && choose2 && cloud2 && P >= 0 && H > 0 && W > 0 &&
-             cap >= min(H, W) * min(H, W));
+             cap >= min(H, W) * min(H, W) && min_count >= 0);
   if (P == 0) return 0;
   cudaStream_t st = s6_stream(stream);
   inp_init_stats_kernel<<<s6_cdiv(P * ST, 256), 256, 0, st>>>(stats, P);
@@ -285,7 +299,7 @@ S6_API int sam6d_inputs_stage_a(const int* rle_cum, const int* rle_off, int P, i
   inp_bbox_kernel<<<s6_cdiv(P, 128), 128, 0, st>>>(stats, P, H, W);
   S6_LAUNCH_CHECK();
   InCfg g{H, W, 0, fx, fy, cx, cy};
-  inp_compact_kernel<<<P, 1024, 0, st>>>(g, thr, mask, depth, stats, cap, choose1, choose2, cloud2);
+  inp_compact_kernel<<<P, 1024, 0, st>>>(g, min_count, thr, mask, depth, stats, cap, choose1, choose2, cloud2);
   S6_LAUNCH_CHECK();
   return 0;
 }

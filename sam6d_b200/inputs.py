@@ -47,9 +47,14 @@ def pack_rle(dets: Sequence[Dict], H: int, W: int):
 
 class FrameInputs:
     """device-side state of one frame between the two stages.  radius: the object radius (one number for every detection) or
-    one radius per detection (several objects in a frame)"""
+    one radius per detection (several objects in a frame).
 
-    def __init__(self, dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, radius, device=None):
+    BOPTestset.get_instance (sam6d_b200/bop.py) uses the same stages with its own rules: depth_m, the (H,W) float32 depth map in
+    metres that replaces the custom path's (depth_raw then only gives the frame size), thr, the float64 radius threshold of every
+    detection that replaces radius * 1.2, and min_count, the pixel count a mask must exceed (kept() takes the rest of the rule)."""
+
+    def __init__(self, dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, radius, device=None,
+                 depth_m: Optional[np.ndarray] = None, thr: Optional[np.ndarray] = None, min_count: int = 32):
         self.device = torch.device(device if device is not None else "cuda")
         self.dets = list(dets)
         if image_u8.ndim == 2:                                                     # run_inference_custom.py:177-178
@@ -57,12 +62,18 @@ class FrameInputs:
         self.H, self.W = depth_raw.shape
         K = np.asarray(cam_K, dtype=np.float64).reshape(3, 3)
         self.K = K
-        whole_depth = depth_raw.astype(np.float32) * depth_scale / 1000.0          # :179 (float32 * python floats)
+        if depth_m is None:
+            whole_depth = depth_raw.astype(np.float32) * depth_scale / 1000.0      # :179 (float32 * python floats)
+        else:
+            whole_depth = depth_m
         self.depth = torch.from_numpy(np.ascontiguousarray(whole_depth, dtype=np.float32)).to(self.device)
         self.image = torch.from_numpy(np.ascontiguousarray(image_u8, dtype=np.uint8)).to(self.device)
         P = len(self.dets)
-        radius = np.broadcast_to(np.asarray(radius, dtype=np.float32), (P,))
-        self.thr = (radius * np.float32(1.2)).astype(np.float64)                   # :209 under numpy >= 2 (weak python scalar)
+        if thr is None:
+            radius = np.broadcast_to(np.asarray(radius, dtype=np.float32), (P,))
+            self.thr = (radius * np.float32(1.2)).astype(np.float64)               # :209 under numpy >= 2 (weak python scalar)
+        else:
+            self.thr = np.array(np.broadcast_to(np.asarray(thr, dtype=np.float64), (P,)))
         cum, off = pack_rle(self.dets, self.H, self.W)
         self.cap = min(self.H, self.W) ** 2
         dev = self.device
@@ -75,15 +86,16 @@ class FrameInputs:
             cum_d = torch.from_numpy(cum).to(dev) if len(cum) else torch.zeros(1, dtype=torch.int32, device=dev)
             off_d = torch.from_numpy(off).to(dev)
             thr_d = torch.from_numpy(self.thr).to(dev)
-            _lib.call("sam6d_inputs_stage_a", _p(cum_d), _p(off_d), P, self.H, self.W, _p(self.depth), float(K[0, 0]), float(K[1, 1]),
-                      float(K[0, 2]), float(K[1, 2]), _p(thr_d), _p(self.mask), _p(self.stats), self.cap, _p(self.choose1),
-                      _p(self.choose2), _p(self.cloud2), _stream())
+            _lib.call("sam6d_inputs_stage_a_min", _p(cum_d), _p(off_d), P, self.H, self.W, _p(self.depth), float(K[0, 0]),
+                      float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), _p(thr_d), int(min_count), _p(self.mask), _p(self.stats), self.cap,
+                      _p(self.choose1), _p(self.choose2), _p(self.cloud2), _stream())
         self.stats_host = self.stats.cpu().numpy() if P else np.zeros((0, ST), np.int32)
 
-    # what the reference's loop decides per detection (run_inference_custom.py:199-212)
-    def kept(self) -> np.ndarray:
+    # what the reference's loop decides per detection (run_inference_custom.py:199-212: more than 32 pixels, at least 4 points
+    # after the radius filter; BOPTestset.get_instance: 8 and 8)
+    def kept(self, min_count: int = 32, min_valid: int = 4) -> np.ndarray:
         s = self.stats_host
-        return np.flatnonzero((s[:, 4] > 32) & (s[:, 9] >= 4)) if len(s) else np.zeros(0, np.int64)
+        return np.flatnonzero((s[:, 4] > min_count) & (s[:, 9] >= min_valid)) if len(s) else np.zeros(0, np.int64)
 
     def n_valid(self) -> np.ndarray:
         return self.stats_host[:, 9]

@@ -18,6 +18,7 @@ The CLIs (sam6d_b200.cli.{render_custom_templates, ism_run_inference_custom, pem
 the same stage functions, so one `SAM6D` frame computes what the chained CLIs compute from the same inputs and seeds.  Between
 the ISM and the PEM the proposal masks stay on the device: their RLE is built by a kernel (ops.mask_rle) and only the run
 ends come to the host, instead of every (H,W) float mask."""
+import json
 import time
 from dataclasses import dataclass
 from types import SimpleNamespace
@@ -26,7 +27,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import inputs, ism, meshio, ops, pbr, render
+from . import bop, inputs, ism, meshio, ops, pbr, render
 from .cli import ism_run_inference_custom as ism_cli
 from .cli import pem_run_inference_custom as pem_cli
 from .cli import render_custom_templates as render_cli
@@ -387,32 +388,120 @@ class SAM6D:
         do not depend on earlier frames.  mark(stage), when given, is called after each stage (stage timing)."""
         return self._frame(rgb_u8, depth_raw, cam_K, depth_scale, obj, None, rng, mark)
 
-    def detect_objects(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, objects: "ObjectSet", rng=None, mark=None):
+    def detect_objects(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, objects: "ObjectSet", rng=None, mark=None,
+                       pem: bool = True):
         """one RGB-D frame with several onboarded objects, the fields of __call__ plus obj (N) i64, the object index of every ISM
         detection.  The ISM follows Instance_Segmentation_Model.test_step: proposals, remove_very_small_detections, descriptors,
         semantic score over all objects, appearance score against the assigned object's best template, geometric score with
         that object's cloud and template pose, final score, apply_nms_per_object_id (records ordered by object, then by
         decreasing score; category_id = obj_ids[object]).  The PEM runs every kept detection in one Net.forward batch, each
         with its object's radius filter, model points and template bank; sample indices are drawn in detection order.
-        mark(stage) as for __call__, plus "nms"."""
-        return self._frame(rgb_u8, depth_raw, cam_K, depth_scale, objects, objects.obj_ids, rng, mark)
+        mark(stage) as for __call__, plus "nms".  pem=False stops after the ISM records (pem [], R and t None).  The result's
+        ism_time is the host seconds from the segmentor to the end of the NMS, test_step's proposal + matching time."""
+        return self._frame(rgb_u8, depth_raw, cam_K, depth_scale, objects, objects.obj_ids, rng, mark, pem)
 
-    def _frame(self, rgb_u8, depth_raw, cam_K, depth_scale, obj, obj_ids, rng, mark):
+    # ---- a BOP test split (ISM/run_inference.py, PEM/test_bop.py; sam6d_b200/bop.py) ------------------------------------------
+    def onboard_bop(self, bop_root: str, dataset_name: str, template_size: int = 512, rng=None) -> "ObjectSet":
+        """onboard_objects() of every object of the dataset (bop.load_objects: sorted model ids, the ids passed as obj_ids)"""
+        objs = bop.load_objects(bop_root, dataset_name)
+        return self.onboard_objects(objs.ply_paths, obj_ids=objs.ids, template_size=template_size, rng=rng)
+
+    def run_bop_ism(self, bop_root: str, dataset_name: str, objects: "ObjectSet", out_path: Optional[str] = None,
+                    max_frames: Optional[int] = None, mark=None):
+        """Instance_Segmentation_Model.test_step over every frame of bop.scan_test_split (the first max_frames), then
+        test_epoch_end's result file: detect_objects (ISM only) on the image test_step segments (bop.round_trip of the decoded
+        frame), records with scene_id, image_id = frame id, category_id = bop.category_ids of the object index (the objects in
+        onboarding order, which is load_objects' order for onboard_bop) and time = proposal + matching seconds.  Frames in scan
+        order.  Writes the list to out_path with a plain json.dump (save_json_bop23) and returns it.  mark(stage) is called
+        after "decode" and after each stage of detect_objects."""
+        mark = mark or (lambda stage: None)
+        cats = bop.category_ids(dataset_name, len(objects.obj_ids))
+        records = []
+        for f in bop.scan_test_split(bop_root, dataset_name)[:max_frames]:
+            rgb = bop.round_trip(bop.decode_rgb(f.rgb_path))
+            depth = bop.decode_depth(f.depth_path)
+            mark("decode")
+            res = self.detect_objects(rgb, depth, f.cam_K, f.depth_scale, objects, mark=mark, pem=False)
+            for r, o in zip(res.ism, res.obj.tolist() if res.ism else []):
+                r.update(scene_id=f.scene_id, image_id=f.frame_id, category_id=cats[o], time=float(res.ism_time))
+            records += res.ism
+        if out_path is not None:
+            with open(out_path, "w") as fh:
+                json.dump(records, fh)
+        return records
+
+    def run_bop_pem(self, detections_path: str, bop_root: str, dataset_name: str, template_dir: str, out_path: Optional[str] = None,
+                    rng=None, max_frames: Optional[int] = None, mark=None):
+        """test_bop.py over a detection file (ours or the reference ISM's; uncompressed RLE): per image of the file (bop.
+        group_detections, the first max_frames), bop.pem_instances, then Net.forward on all of the image's instances with the
+        coarse-stage uniforms of test_bop.py (bop.pem_rand: one CUDA generator seeded RD_SEED for the run, one torch.rand per
+        chunk of 16).  Random draws from `rng` (default numpy's global RNG): the model points of every object, each object's
+        42 template samples, then the observed points in detection order.  An image none of whose detections survives is
+        skipped (the reference fails there).  Writes the CSV lines to out_path and returns them.  mark(stage) after
+        "onboard", and per image after "decode", "pem_inputs" and "forward"."""
+        mark = mark or (lambda stage: None)
+        rng = rng if rng is not None else np.random
+        cfg = pem_cli.TEST_DATASET
+        objs = bop.load_objects(bop_root, dataset_name)
+        meshes = [meshio.load_ply_mesh(p) for p in objs.ply_paths]
+        model_points = np.stack([meshio.sample_surface(m.vertices, m.faces, bop.N_SAMPLE_MODEL_POINT, rng) / 1000.0 for m in meshes])
+        model_points = model_points.astype(np.float32)
+        banks = [pem_template_bank(self.pem, *bop.load_templates(template_dir, dataset_name, i, cfg["n_template_view"]), rng=rng,
+                                   device=self.device) for i in objs.ids]
+        bank = tuple(torch.stack([b[k].reshape(b[k].shape[-2:]) for b in banks]) for k in range(2))
+        del banks
+        mark("onboard")
+        with open(detections_path) as fh:
+            groups = bop.group_detections(json.load(fh))
+        g = torch.Generator(device=self.device)
+        g.manual_seed(pem_cli.RD_SEED)
+        n_rand = self.pem.coarse_point_matching.cfg.nproposal1 * 3
+        lines = []
+        for (scene_id, image_id), dets in groups[:max_frames]:
+            rgb_path, depth_path, cam_K, depth_scale = bop.frame_paths(bop_root, dataset_name, scene_id, image_id)
+            image, raw = bop.decode_pem_image(rgb_path), bop.decode_depth(depth_path)
+            mark("decode")
+            torch.cuda.synchronize(self.device)
+            t0 = time.time()
+            data, kept, _ = bop.pem_instances(dets, image, raw, cam_K, depth_scale, objs, model_points, rng=rng,
+                                              n_sample=cfg["n_sample_observed_point"], img_size=cfg["img_size"], device=self.device)
+            mark("pem_inputs")
+            n = len(kept)
+            if n == 0:
+                continue
+            data["dense_po"], data["dense_fo"] = bank[0][data["obj"]], bank[1][data["obj"]]
+            rand = bop.pem_rand(g, n, n_rand, self.device)
+            with torch.no_grad():
+                out = self.pem(data, rand=rand)
+            scores = (out["pred_pose_score"] * data["score"]).cpu().numpy()
+            R = out["pred_R"].reshape(-1, 9).cpu().numpy()
+            t = out["pred_t"].cpu().numpy() * 1000
+            image_time = time.time() - t0 + float(np.float32(dets[0]["time"]))
+            mark("forward")
+            lines += bop.csv_rows(scene_id, image_id, [d["category_id"] for d in kept], scores, R, t, image_time)
+        if out_path is not None:
+            with open(out_path, "w+") as fh:
+                fh.writelines(lines)
+        return lines
+
+    def _frame(self, rgb_u8, depth_raw, cam_K, depth_scale, obj, obj_ids, rng, mark, pem=True):
         multi = obj_ids is not None
         mark = mark or (lambda stage: None)
         t0 = time.time()
         geometry = ism_geometry(obj.poses_m, obj.cloud_m, depth_raw, cam_K, depth_scale, self.device)
+        t_ism = time.time()
         det = ism_detect(self.seg, self.desc, obj.ref_cls, obj.ref_patch, rgb_u8, self.confidence_thresh, geometry, mark, remove_small=multi,
                          aggregation_function=self.aggregation_function)
         if multi and det.reason is None:
             keep = ism.nms_per_object(det.boxes, det.scores, det.obj)
             det.masks, det.boxes, det.scores, det.obj = det.masks[keep], det.boxes[keep], det.scores[keep], det.obj[keep]
             mark("nms")
+        ism_time = time.time() - t_ism
         if det.reason is not None:
             mark("rle")
             mark("ism_records")
             return SimpleNamespace(ism=[], pem=[], masks=det.masks, boxes=det.boxes, scores=det.scores, R=None, t=None, frame=None,
-                                   n_proposals=det.n_proposals, reason=det.reason, **({"obj": det.obj} if multi else {}))
+                                   n_proposals=det.n_proposals, reason=det.reason, ism_time=ism_time, **({"obj": det.obj} if multi else {}))
         cum, off = ops.mask_rle(det.masks.contiguous())
         mark("rle")
         counts = rle_counts(cum.cpu().numpy(), off.cpu().numpy())
@@ -420,16 +509,19 @@ class SAM6D:
         records = ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), counts, det.masks.shape[1:], time.time() - t0,
                               category_ids=np.asarray(obj_ids)[det_obj] if multi else None)
         mark("ism_records")
+        if not pem:
+            return SimpleNamespace(ism=records, pem=[], masks=det.masks, boxes=det.boxes, scores=det.scores, R=None, t=None, frame=None,
+                                   n_proposals=det.n_proposals, reason=None, ism_time=ism_time, **({"obj": det.obj} if multi else {}))
         g = torch.Generator(device=self.device)
         g.manual_seed(pem_cli.RD_SEED)
         frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
                           rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj)
-        pem = pem_records(frame)
+        pem_recs = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
         t = frame.out["pred_t"] if frame.out is not None else None
-        return SimpleNamespace(ism=records, pem=pem, masks=det.masks, boxes=det.boxes, scores=det.scores, R=R, t=t, frame=frame,
-                               n_proposals=det.n_proposals, reason=None, **({"obj": det.obj} if multi else {}))
+        return SimpleNamespace(ism=records, pem=pem_recs, masks=det.masks, boxes=det.boxes, scores=det.scores, R=R, t=t, frame=frame,
+                               n_proposals=det.n_proposals, reason=None, ism_time=ism_time, **({"obj": det.obj} if multi else {}))
 
 
 @dataclass
