@@ -413,6 +413,22 @@ int sam6d_render_meshes(const float* verts, const int* faces, const int* mesh_in
                         float znear, float ambient, int* vrec, unsigned long long* vis, int* big, int big_cap, int* counters,
                         unsigned char* rgb, unsigned char* mask, void* xyz, int* tri, float* depth, void* stream);
 
+/* ---- BOP19 pose errors (sam6d_b200/bop_eval.py; csrc/bop_eval.cu) --------------------------------------------------- */
+
+/* MSSD and MSPD of P (estimate, GT) pairs.  est, gt (P,12) f32: R row-major (9) then t (3), mm; pair_obj (P) i32 object index
+ * in [0, O); K (P,4) f32 = fx, fy, cx, cy of each pair's image.  verts (n,3) f32 of all objects packed in order, vert_off (O+1) i32;
+ * syms (m,12) f32 symmetry transforms (R row-major, t) packed the same way, sym_off (O+1) i32, every object with at least one
+ * and max_sym >= the largest count.  out (P,2) f32 = min over symmetries of the max over vertices of the 3D distance (mm) and
+ * of the projected distance (px). */
+int sam6d_bop_mssd_mspd(const float* est, const float* gt, const int* pair_obj, const float* K, int P, const float* verts,
+                        const int* vert_off, const float* syms, const int* sym_off, int O, int max_sym, float* out, void* stream);
+/* VSD pixel counts of P pairs of one image size H x W and one K: depth_est, depth_gt (P,H,W) f32 rendered camera z (0 = empty),
+ * depth_test (n_img,H,W) f32 test depth in mm, pair_img (P) i32 its image; delta and diameter in mm, taus (10) f32 fractions of
+ * the diameter.  out (P,12) i32 = |U|, |I|, then per tau #{p in I : |dist_g - dist_e| / diameter >= tau}.  P <= 65535. */
+int sam6d_bop_vsd_counts(const float* depth_est, const float* depth_gt, const float* depth_test, const int* pair_img, int P,
+                         int H, int W, float fx, float fy, float cx, float cy, float delta, float diameter, const float* taus,
+                         int* out, void* stream);
+
 /* ---- FastSAM segmentor: YOLOv8x-seg (ultralytics SegmentationModel behind ISM/model/fast_sam.py; csrc/conv_tc.cu, csrc/yolo.cu) */
 
 /* Implicit-GEMM convolution on wgmma, NHWC bf16: x (B,Hi,Wi,ldx) channels [0,Cin) (a channel slice: offset the pointer),
