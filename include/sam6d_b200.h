@@ -429,6 +429,23 @@ int sam6d_bop_vsd_counts(const float* depth_est, const float* depth_gt, const fl
                          int H, int W, float fx, float fy, float cx, float cy, float delta, float diameter, const float* taus,
                          int* out, void* stream);
 
+/* ---- BOP detection / segmentation: COCO mask IoU (sam6d_b200/bop_eval_coco.py; csrc/bop_eval.cu) ----------------------- */
+/* Packed masks: mask i holds the 32-bit words bits[word_off[i] .. word_off[i] + ceil(H_i W_i / 32)), bit k (LSB first) of the
+ * mask = pixel x = k / H_i, y = k % H_i (COCO's column-major RLE order); bits past H_i W_i are 0. */
+
+/* n uncompressed COCO RLEs -> packed masks.  rle_cum / rle_off (n+1): the cumulative run ends of each mask concatenated
+ * (inputs.pack_rle's layout; runs alternate background / foreground, starting with background; the last end is H_i W_i),
+ * hw (n,2) i32 = H_i, W_i, word_off (n) i32.  Writes every word of every mask. */
+int sam6d_bop_pack_rle(const int* rle_cum, const int* rle_off, const int* hw, const int* word_off, int n, unsigned* bits, void* stream);
+/* n decoded masks (n,H,W) u8 row-major (set where > 0) -> packed masks at word_off (n) (bits may be NULL: nothing packed), area
+ * (n) i32 pixel count and box (n,4) i32 = x_min, y_min, x_max, y_max of the set pixels (all -1 when the mask is empty). */
+int sam6d_bop_pack_u8(const unsigned char* masks, int n, int H, int W, const int* word_off, unsigned* bits, int* area, int* box,
+                      void* stream);
+/* out (P) i32 = |A & B| of P pairs (pair_a, pair_b index masks of word_off (n+1)) of one size each.  bits is 16-byte aligned and
+ * every word_off is a multiple of 4; the words between masks are 0. */
+int sam6d_bop_mask_pair_counts(const unsigned* bits, const int* word_off, const int* pair_a, const int* pair_b, int P, int* out,
+                               void* stream);
+
 /* ---- FastSAM segmentor: YOLOv8x-seg (ultralytics SegmentationModel behind ISM/model/fast_sam.py; csrc/conv_tc.cu, csrc/yolo.cu) */
 
 /* Implicit-GEMM convolution on wgmma, NHWC bf16: x (B,Hi,Wi,ldx) channels [0,Cin) (a channel slice: offset the pointer),

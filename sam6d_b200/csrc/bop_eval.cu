@@ -9,6 +9,10 @@
 // VSD (same paper; Hodan et al., ECCV 2016 workshop): per pair, integer counts over the pixels of |U|, |I| and, per tau,
 // #{p in I : |dist_g - dist_e| / diameter >= tau}, from the rendered depths of the estimate and the GT and the test depth;
 // the host forms e(tau) = (cost + |U| - |I|) / |U|.  No distance or visibility image is written.
+//
+// COCO mask IoU of the BOP detection / segmentation task (sam6d_b200/bop_eval_coco.py, oracle/bop_coco_oracle.py): masks are
+// bit-packed in COCO's RLE order (column-major, bit k = x H + y, LSB first in 32-bit words), from run ends or from decoded PNG
+// masks, and |A & B| of a pair is the popcount of the AND of their words.  Every result is an exact integer.
 #include "common.cuh"
 
 namespace {
@@ -159,6 +163,126 @@ __global__ void __launch_bounds__(BE_THREADS) bop_vsd_kernel(const float* __rest
   if (threadIdx.x < 2 + BE_NTAU && cnt[threadIdx.x]) atomicAdd(out + p * (2 + BE_NTAU) + threadIdx.x, cnt[threadIdx.x]);
 }
 
+// ---- COCO masks ----------------------------------------------------------------------------------------------------------------
+constexpr int BM_THREADS = 256;
+constexpr int BM_WARPS = BM_THREADS / 32;
+
+// grid (n masks).  Each thread builds whole words: the run holding the word's first pixel by a binary search over the mask's run
+// ends (the first end > that pixel), then the runs up to the word's last pixel; odd runs are foreground.  Zero-length runs are
+// skipped by the search and add no bits.  Every word of the mask is written, so no clearing pass is needed.
+__global__ void __launch_bounds__(BM_THREADS) bop_pack_rle_kernel(const int* __restrict__ rle_cum, const int* __restrict__ rle_off,
+                                                                  const int* __restrict__ hw, const int* __restrict__ word_off,
+                                                                  unsigned* __restrict__ bits) {
+  const int i = blockIdx.x;
+  const int* cum = rle_cum + rle_off[i];
+  const int nr = rle_off[i + 1] - rle_off[i];
+  const long long npix = (long long)hw[2 * i] * hw[2 * i + 1];
+  const int nw = (int)((npix + 31) >> 5);
+  unsigned* out = bits + word_off[i];
+  for (int w = threadIdx.x; w < nw; w += BM_THREADS) {
+    const long long p0 = (long long)w << 5, p1 = p0 + 32;
+    int lo = 0, hi = nr;
+    while (lo < hi) {                                // first k with cum[k] > p0
+      const int mid = (lo + hi) >> 1;
+      if (cum[mid] > p0) hi = mid; else lo = mid + 1;
+    }
+    unsigned word = 0u;
+    for (int k = lo; k < nr; ++k) {
+      const long long a = k ? cum[k - 1] : 0, b = cum[k];
+      if (a >= p1) break;
+      if ((k & 1) && b > a) {
+        const int s = (int)max(a - p0, 0LL), e = (int)min(b - p0, 32LL);      // bits [s, e) of this word
+        word |= (e - s == 32) ? 0xffffffffu : (((1u << (e - s)) - 1u) << s);
+      }
+    }
+    out[w] = word;
+  }
+}
+
+__device__ __forceinline__ int bm_block_reduce(int v, bool is_max, int* sh) {
+  // warp then block min / max; sh holds BM_WARPS ints; every thread gets the result
+  for (int o = 16; o > 0; o >>= 1) {
+    const int u = __shfl_xor_sync(0xffffffffu, v, o);
+    v = is_max ? max(v, u) : min(v, u);
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = sh[0];
+#pragma unroll
+  for (int w = 1; w < BM_WARPS; ++w) v = is_max ? max(v, sh[w]) : min(v, sh[w]);
+  return v;
+}
+
+// grid (n masks).  Warp-per-word: lane j tests pixel 32 w + j (x = p / H, y = p % H, read from the row-major mask) and a ballot
+// forms the word.  The 32 rows a warp reads share their cache sectors with the next 31 columns' reads, which follow within the
+// same CTA.  Area by popcount of the words, the tight box by block min / max; bits may be NULL (area and box only).
+__global__ void __launch_bounds__(BM_THREADS) bop_pack_u8_kernel(const unsigned char* __restrict__ masks, int H, int W,
+                                                                 const int* __restrict__ word_off, unsigned* __restrict__ bits,
+                                                                 int* __restrict__ area, int* __restrict__ box) {
+  __shared__ int sh[BM_WARPS];
+  __shared__ int sh_area[BM_WARPS];
+  const int i = blockIdx.x;
+  const long long npix = (long long)H * W;
+  const unsigned char* m = masks + (long long)i * npix;
+  const int nw = (int)((npix + 31) >> 5);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int cnt = 0, x0 = INT_MAX, y0 = INT_MAX, x1 = -1, y1 = -1;
+  for (int w = warp; w < nw; w += BM_WARPS) {
+    const long long p = ((long long)w << 5) + lane;
+    bool on = false;
+    int x = 0, y = 0;
+    if (p < npix) {
+      x = (int)(p / H);
+      y = (int)(p - (long long)x * H);
+      on = m[(long long)y * W + x] != 0;
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) {
+      if (bits) bits[word_off[i] + w] = word;
+      cnt += __popc(word);
+    }
+    if (on) { x0 = min(x0, x); x1 = max(x1, x); y0 = min(y0, y); y1 = max(y1, y); }
+  }
+  if (lane == 0) sh_area[warp] = cnt;
+  x0 = bm_block_reduce(x0, false, sh);
+  y0 = bm_block_reduce(y0, false, sh);
+  x1 = bm_block_reduce(x1, true, sh);
+  y1 = bm_block_reduce(y1, true, sh);
+  if (threadIdx.x == 0) {
+    int a = 0;
+#pragma unroll
+    for (int w = 0; w < BM_WARPS; ++w) a += sh_area[w];
+    area[i] = a;
+    const bool empty = a == 0;
+    box[4 * i] = empty ? -1 : x0;
+    box[4 * i + 1] = empty ? -1 : y0;
+    box[4 * i + 2] = empty ? -1 : x1;
+    box[4 * i + 3] = empty ? -1 : y1;
+  }
+}
+
+// grid (ceil(P / BM_WARPS)), one warp per pair: 16-byte loads of both masks' words (offsets and lengths are multiples of 4
+// words), popcount of the AND, a warp sum.  Order-free integer sums, so deterministic.
+__global__ void __launch_bounds__(BM_THREADS) bop_pair_counts_kernel(const unsigned* __restrict__ bits, const int* __restrict__ word_off,
+                                                                     const int* __restrict__ pair_a, const int* __restrict__ pair_b, int P,
+                                                                     int* __restrict__ out) {
+  const int p = blockIdx.x * BM_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (p >= P) return;
+  const int a = pair_a[p], b = pair_b[p];
+  const int nq = min(word_off[a + 1] - word_off[a], word_off[b + 1] - word_off[b]) >> 2;
+  const uint4* A = reinterpret_cast<const uint4*>(bits + word_off[a]);
+  const uint4* B = reinterpret_cast<const uint4*>(bits + word_off[b]);
+  int c = 0;
+#pragma unroll 4
+  for (int j = lane; j < nq; j += 32) {
+    const uint4 u = __ldg(A + j), v = __ldg(B + j);
+    c += __popc(u.x & v.x) + __popc(u.y & v.y) + __popc(u.z & v.z) + __popc(u.w & v.w);
+  }
+  c = __reduce_add_sync(0xffffffffu, c);
+  if (lane == 0) out[p] = c;
+}
+
 }  // namespace
 
 S6_API int sam6d_bop_mssd_mspd(const float* est, const float* gt, const int* pair_obj, const float* K, int P, const float* verts,
@@ -187,6 +311,39 @@ S6_API int sam6d_bop_vsd_counts(const float* depth_est, const float* depth_gt, c
   S6_CHECK(cudaMemsetAsync(out, 0, (size_t)P * (2 + BE_NTAU) * sizeof(int), st));
   dim3 grid(s6_cdiv((long long)H * W, BE_VSD_PIX), P);
   bop_vsd_kernel<<<grid, BE_THREADS, 0, st>>>(depth_est, depth_gt, depth_test, pair_img, H, W, fx, fy, cx, cy, delta, diameter, taus, out);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+S6_API int sam6d_bop_pack_rle(const int* rle_cum, const int* rle_off, const int* hw, const int* word_off, int n, unsigned* bits,
+                              void* stream) {
+  S6_REQUIRE(rle_off && hw && word_off && bits && n >= 0);
+  cudaStream_t st = s6_stream(stream);
+  if (n == 0) return 0;
+  S6_REQUIRE(rle_cum);
+  bop_pack_rle_kernel<<<n, BM_THREADS, 0, st>>>(rle_cum, rle_off, hw, word_off, bits);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+S6_API int sam6d_bop_pack_u8(const unsigned char* masks, int n, int H, int W, const int* word_off, unsigned* bits, int* area, int* box,
+                             void* stream) {
+  S6_REQUIRE(masks && area && box && n >= 0 && H > 0 && W > 0 && (long long)H * W < (1LL << 31));
+  S6_REQUIRE(!bits || word_off);
+  cudaStream_t st = s6_stream(stream);
+  if (n == 0) return 0;
+  bop_pack_u8_kernel<<<n, BM_THREADS, 0, st>>>(masks, H, W, word_off, bits, area, box);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+S6_API int sam6d_bop_mask_pair_counts(const unsigned* bits, const int* word_off, const int* pair_a, const int* pair_b, int P, int* out,
+                                      void* stream) {
+  S6_REQUIRE(bits && word_off && pair_a && pair_b && out && P >= 0);
+  S6_REQUIRE((reinterpret_cast<uintptr_t>(bits) & 15) == 0);
+  cudaStream_t st = s6_stream(stream);
+  if (P == 0) return 0;
+  bop_pair_counts_kernel<<<s6_cdiv(P, BM_WARPS), BM_THREADS, 0, st>>>(bits, word_off, pair_a, pair_b, P, out);
   S6_LAUNCH_CHECK();
   return 0;
 }
