@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(1024) topk_smallest_kernel(const float* __rest
     if (i < n) {
       float f = v[(size_t)b * n + i];
       unsigned u = __float_as_uint(f);
-      u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // order-preserving map; NaN sorts last-ish
+      u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // order-preserving map of the bit pattern (see sam6d_topk_smallest)
       key = ((unsigned long long)u << 32) | (unsigned)i;
     }
     keys[i] = key;
@@ -361,7 +361,9 @@ S6_API int sam6d_coarse_hypotheses(const int* idx, const float* pts1, const floa
   return 0;
 }
 
-// v (B,n) -> out (B,k): indices of the k smallest values, ascending by (value, index)   (model_utils.py:235)
+// v (B,n) -> out (B,k): indices of the k smallest values, ascending by (value, index)   (model_utils.py:235).
+// The order is that of the fp32 bit patterns: -0.0 sorts before +0.0 whatever their indices, a NaN with the sign bit set
+// before every value and any other NaN after +inf.  The residuals this ranks are norms, never -0 or NaN from finite points.
 S6_API int sam6d_topk_smallest(const float* v, int B, int n, int k, int* out, void* stream) {
   S6_REQUIRE(v && out && B >= 0 && n > 0 && k > 0 && k <= n);
   if (B == 0) return 0;
