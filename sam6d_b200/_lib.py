@@ -4,6 +4,10 @@ import ctypes
 import os
 import re
 
+import torch
+
+_Tensor = torch.Tensor
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "sam6d_b200.h")
 LIB_PATH = os.path.join(_HERE, "libsam6d_b200.so")
@@ -42,6 +46,7 @@ class Sam6dError(RuntimeError):
 
 _lib = None
 _protos = None
+_fns = {}        # name -> (ctypes function, number of parameters before a trailing stream, or -1 if there is none)
 
 
 def lib():
@@ -57,6 +62,7 @@ def lib():
             fn = getattr(_lib, name)
             fn.restype = ret
             fn.argtypes = [t for t, _ in args]
+            _fns[name] = (fn, len(args) - 1 if args and args[-1][1] == "stream" else -1)
     return _lib
 
 
@@ -92,11 +98,18 @@ def timed_events(name: str):
 
 
 def call(name: str, *args):
+    """calls C-ABI function `name`.  The trailing stream may be left out, and is then the current CUDA stream.  A tensor
+    argument is passed as its device address; it must be a CUDA tensor, since every pointer the header declares is a
+    device pointer.  Everything else goes to ctypes as it is: ints, floats, bools and None for NULL."""
     global _launches
-    fn = getattr(lib(), name)
+    if _lib is None:
+        lib()
+    fn, n_before_stream = _fns[name]
+    args = [(a.data_ptr() if a.is_cuda else _not_device(name, a)) if isinstance(a, _Tensor) else a for a in args]
+    if len(args) == n_before_stream:
+        args.append(torch.cuda.current_stream().cuda_stream)
     rec = _timed.get(name)
     if rec is not None:
-        import torch
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         rc = fn(*args)
@@ -110,6 +123,10 @@ def call(name: str, *args):
             raise Sam6dError(f"{name}: invalid argument (see include/sam6d_b200.h)")
         raise Sam6dError(f"{name}: CUDA error {rc}")
     return rc
+
+
+def _not_device(name: str, t: torch.Tensor):
+    raise Sam6dError(f"{name}: a {t.device} tensor where the C ABI takes a device pointer")
 
 
 def version() -> str:

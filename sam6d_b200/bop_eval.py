@@ -38,7 +38,6 @@ import numpy as np
 import torch
 
 from . import _lib, bop, meshio, pbr, render
-from .render import _p, _stream
 
 ERROR_TYPES = ("vsd", "mssd", "mspd")
 VSD_TAUS = np.arange(0.05, 0.51, 0.05)           # misfit tolerance, fraction of the diameter
@@ -172,8 +171,7 @@ def mssd_mspd(est, gt, pair_obj, K, verts, syms, device="cuda") -> torch.Tensor:
     voff = _dev(np.concatenate([[0], np.cumsum(nv)]), torch.int32, device)
     soff = _dev(np.concatenate([[0], np.cumsum(ns)]), torch.int32, device)
     out = torch.empty(P, 2, dtype=torch.float32, device=device)
-    _lib.call("sam6d_bop_mssd_mspd", _p(est), _p(gt), _p(pair_obj), _p(K), P, _p(V), _p(voff), _p(S), _p(soff), O, max(ns), _p(out),
-              _stream())
+    _lib.call("sam6d_bop_mssd_mspd", est, gt, pair_obj, K, P, V, voff, S, soff, O, max(ns), out)
     return out
 
 
@@ -199,8 +197,8 @@ def vsd_counts(depth_est, depth_gt, depth_test, pair_img, K, delta: float, diame
     K = np.asarray(K.cpu() if isinstance(K, torch.Tensor) else K, np.float64).reshape(3, 3)
     de, dg, dt = depth_est.contiguous(), depth_gt.contiguous(), depth_test.contiguous()
     out = torch.empty(P, 12, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_bop_vsd_counts", _p(de), _p(dg), _p(dt), _p(pair_img), P, H, W, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]),
-              float(K[1, 2]), float(delta), float(diameter), _p(taus), _p(out), _stream())
+    _lib.call("sam6d_bop_vsd_counts", de, dg, dt, pair_img, P, H, W, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]),
+              float(delta), float(diameter), taus, out)
     return out
 
 

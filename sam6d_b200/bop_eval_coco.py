@@ -57,7 +57,6 @@ import torch
 from . import _lib, bop, pbr
 from .bop_eval import _image_size, load_targets
 from .pbr import _tick
-from .render import _p, _stream
 
 IOU_TYPES = ("segm", "bbox")
 BBOX_TYPES = ("amodal", "modal")
@@ -157,7 +156,7 @@ def pack_u8(masks: torch.Tensor, word_off=None, bits: torch.Tensor = None):
             raise ValueError("pack_u8: one word offset per mask")
         _check_bits(bits, woff_h, mask_words(H, W))
         woff = torch.as_tensor(woff_h.astype(np.int32), device=dev)
-    _lib.call("sam6d_bop_pack_u8", _p(masks), n, H, W, _p(woff), _p(bits), _p(area), _p(box), _stream())
+    _lib.call("sam6d_bop_pack_u8", masks, n, H, W, woff, bits, area, box)
     return area, box
 
 
@@ -178,7 +177,7 @@ def pack_rle(rle_cum, rle_off, hw, word_off, bits: torch.Tensor):
     off_d = torch.as_tensor(rle_off, device=dev)
     hw_d = torch.as_tensor(hw.astype(np.int32), device=dev)
     woff = torch.as_tensor(np.asarray(word_off, np.int32), device=dev)
-    _lib.call("sam6d_bop_pack_rle", _p(cum), _p(off_d), _p(hw_d), _p(woff), n, _p(bits), _stream())
+    _lib.call("sam6d_bop_pack_rle", cum, off_d, hw_d, woff, n, bits)
 
 
 def mask_pair_counts(bits: torch.Tensor, word_off, pair_a, pair_b) -> torch.Tensor:
@@ -199,7 +198,7 @@ def mask_pair_counts(bits: torch.Tensor, word_off, pair_a, pair_b) -> torch.Tens
     out = torch.empty(P, dtype=torch.int32, device=dev)
     woff_d = torch.as_tensor(woff.astype(np.int32), device=dev)
     a_d, b_d = torch.as_tensor(a.astype(np.int32), device=dev), torch.as_tensor(b.astype(np.int32), device=dev)
-    _lib.call("sam6d_bop_mask_pair_counts", _p(bits), _p(woff_d), _p(a_d), _p(b_d), P, _p(out), _stream())
+    _lib.call("sam6d_bop_mask_pair_counts", bits, woff_d, a_d, b_d, P, out)
     return out
 
 

@@ -18,7 +18,6 @@ The trunk is a pre-norm ViT with LayerScale: parameter names are the reference's
     masked, normalised patch tokens                        -> sam6d_masked_patch_normalize
     appearance score + visible ratio                       -> sam6d_gemm_tma_batched (256 x 256 x C per proposal) + sam6d_appearance_reduce
 There is no CPU path.  The positional-embedding interpolation (bicubic, once per input size) is weight preprocessing in torch."""
-import ctypes
 import math
 from typing import Optional
 
@@ -30,14 +29,6 @@ from . import _lib, ops
 from .pem import _W, _f32, _Packed, _param_key
 
 _ACT_GELU = 2
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 class _PatchEmbed(nn.Module):
@@ -192,8 +183,7 @@ class DinoVisionTransformer(nn.Module):
         patches[:, :K] = x.float().reshape(B, Cin, Gh, P, Gw, P).permute(0, 2, 4, 1, 3, 5).reshape(B * L, K)
         tok = torch.empty(B, S, C, dtype=torch.float32, device=x.device)
         tok[:, 0, :] = cls
-        ops.gemm_tc_raw(patches.data_ptr(), 0, w["pe_w"].bf16.data_ptr(), 1, w["pe_b"], pos.data_ptr(), tok.data_ptr() + C * 4, 0,
-                        L, C, Kp, Kp, Kp, C, C, batch=B, sA=L * Kp, sW=0, sC=S * C, sR=0)
+        ops.gemm_tc(patches.view(B, L, Kp), w["pe_w"].bf16, w["pe_b"], residual=pos.expand(B, L, C), out=tok[:, 1:, :])
         tok = tok.view(B * S, C)
         act = ops.ACT_SWIGLU if self.ffn_layer == "swiglufused" else _ACT_GELU
         for bw in w["blocks"]:
@@ -268,7 +258,7 @@ def crop_resize_pad(image_u8: Optional[torch.Tensor], masks: torch.Tensor, boxes
     rgb = torch.empty(P, 3, target, target, dtype=torch.float32, device=dev) if want_rgb else None
     pm = torch.empty(P, target, target, dtype=torch.float32, device=dev) if want_mask else None
     img = image_u8.contiguous() if want_rgb else None
-    _lib.call("sam6d_crop_resize_pad", _p(img), _p(m), _p(b), P, H, W, target, _p(rgb), _p(pm), _s())
+    _lib.call("sam6d_crop_resize_pad", img, m, b, P, H, W, target, rgb, pm)
     return rgb, pm
 
 
@@ -315,9 +305,8 @@ class CustomDINOv2(nn.Module):
             cls[i:i + n] = f["x_norm_clstoken"]
             pt = f["x_norm_patchtokens"]                                     # view of (n, S, C): row stride C, batch stride S*C
             mk = masks[i:i + n].contiguous()                                 # named: must outlive the launch
-            _lib.call("sam6d_masked_patch_normalize", _p(pt), ctypes.c_longlong(pt.stride(1)), ctypes.c_longlong(pt.stride(0)),
-                      _p(mk), n, G, self.patch_size, C, ctypes.c_float(self.validpatch_thresh), _p(pf[i:i + n]),
-                      _p(pb[i:i + n]) if want_bf16 else None, _p(valid[i:i + n]), _s())
+            _lib.call("sam6d_masked_patch_normalize", pt, pt.stride(1), pt.stride(0), mk, n, G, self.patch_size, C, self.validpatch_thresh,
+                      pf[i:i + n], pb[i:i + n] if want_bf16 else None, valid[i:i + n])
         self.last_patch_bf16, self.last_valid = pb, valid
         return cls, pf
 
@@ -351,12 +340,11 @@ class MaskedPatch_MatrixSimilarity(nn.Module):
         r = reference.to(torch.bfloat16).contiguous()
         ld = (N + 3) // 4 * 4
         sim = torch.empty(P, N, ld, dtype=torch.float32, device=query.device)
-        ops.gemm_tma_batched(q, r, sim, N, N, ld, N * ld)
+        ops.gemm_tma_batched(q, r, sim[:, :, :N])
         qvalid = (query.abs().amax(dim=-1) > 0).to(torch.uint8).contiguous()
         appe = torch.empty(P, dtype=torch.float32, device=query.device)
         vis = torch.empty(P, dtype=torch.float32, device=query.device)
-        _lib.call("sam6d_appearance_reduce", _p(sim), ctypes.c_longlong(ld), ctypes.c_longlong(N * ld), P, N, _p(qvalid), ctypes.c_float(thred),
-                  _p(appe), _p(vis), _s())
+        _lib.call("sam6d_appearance_reduce", sim, ld, N * ld, P, N, qvalid, thred, appe, vis)
         return appe, vis
 
     def compute_straight(self, query, reference):

@@ -20,7 +20,6 @@ Post-processing (SegmentationPredictor.postprocess): `sam6d_yolo_decode` (DFL, d
 order) -> stable sort by descending confidence (ties go to the lower anchor index; ultralytics' argsort is not stable, so its
 order of exact ties is unspecified) -> `sam6d_sam_nms` (torchvision.ops.nms restated; class-aware NMS is plain NMS at nc = 1) ->
 the first max_det -> `sam6d_yolo_masks` (process_mask with upsample=True) -> scale_boxes / clip_boxes -> postprocess_resize."""
-import ctypes
 import math
 import pickle
 from types import SimpleNamespace
@@ -54,14 +53,6 @@ def scale_layout(scale: str) -> SimpleNamespace:
     n = lambda k: max(round(k * depth), 1)                              # noqa: E731
     c = tuple(ch(v) for v in (64, 128, 256, 512, 1024))
     return SimpleNamespace(scale=scale, c=c, n3=n(3), n6=n(6), npr=c[2])
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # =====================================================================================================================
@@ -225,10 +216,9 @@ class YOLOv8Seg(nn.Module):
         if Cin != cw.cin or x.stride(3) != 1 or out.stride(3) != 1:
             raise ValueError("conv operand layout")
         sy, sx, oy, ox = (2, 2, tap[0], tap[1]) if tap is not None else (1, 1, 0, 0)
-        _lib.call("sam6d_conv2d_tc", _p(x), ctypes.c_longlong(x.stride(2)), B, Hi, Wi, Cin, _p(cw.w), cw.k, stride, cw.cout, _p(cw.b),
-                  int(silu), _p(res), ctypes.c_longlong(res.stride(2) if res is not None else 0),
-                  ctypes.c_longlong(res.stride(0) if res is not None else 0), _p(out), int(out.dtype == torch.float32),
-                  ctypes.c_longlong(out.stride(2)), ctypes.c_longlong(out.stride(0)), out.shape[2], sy, sx, oy, ox, _s())
+        _lib.call("sam6d_conv2d_tc", x, x.stride(2), B, Hi, Wi, Cin, cw.w, cw.k, stride, cw.cout, cw.b, int(silu), res,
+                  res.stride(2) if res is not None else 0, res.stride(0) if res is not None else 0, out, int(out.dtype == torch.float32),
+                  out.stride(2), out.stride(0), out.shape[2], sy, sx, oy, ox)
         return out
 
     def _c2f(self, x, cw, out):
@@ -246,7 +236,7 @@ class YOLOv8Seg(nn.Module):
     @staticmethod
     def _up(x, out):
         B, H, W, C = x.shape
-        _lib.call("sam6d_yolo_upsample2x", _p(x), ctypes.c_longlong(x.stride(2)), B, H, W, C, _p(out), ctypes.c_longlong(out.stride(2)), _s())
+        _lib.call("sam6d_yolo_upsample2x", x, x.stride(2), B, H, W, C, out, out.stride(2))
 
     @torch.no_grad()
     def forward(self, frames: torch.Tensor):
@@ -264,7 +254,7 @@ class YOLOv8Seg(nn.Module):
         e = lambda h, ww, c, dt=bf: torch.empty(B, h, ww, c, dtype=dt, device=dev)   # noqa: E731
         s2, s4, s8, s16, s32 = (H // 2, W // 2), (H // 4, W // 4), (H // 8, W // 8), (H // 16, W // 16), (H // 32, W // 32)
         x0 = e(*s2, c0)
-        _lib.call("sam6d_yolo_stem_c", _p(frames), B, H, W, c0, _p(w["stem"][0]), _p(w["stem"][1]), _p(x0), _s())
+        _lib.call("sam6d_yolo_stem_c", frames, B, H, W, c0, w["stem"][0], w["stem"][1], x0)
         x1 = conv(x0, w[1], e(*s4, c1), stride=2)
         x2 = self._c2f(x1, w[2], e(*s4, c1))
         x3 = conv(x2, w[3], e(*s8, c2), stride=2)
@@ -277,7 +267,7 @@ class YOLOv8Seg(nn.Module):
         x8 = self._c2f(x7, w[8], e(*s32, c4))
         sppf = e(*s32, 2 * c4)                                          # [cv1 | 5x5 | 9x9 | 13x13], c4 / 2 each
         conv(x8, w[9].cv1, sppf[..., :c4 // 2])
-        _lib.call("sam6d_yolo_sppf", _p(sppf), ctypes.c_longlong(2 * c4), B, s32[0], s32[1], c4 // 2, _s())
+        _lib.call("sam6d_yolo_sppf", sppf, 2 * c4, B, s32[0], s32[1], c4 // 2)
         cat20 = e(*s32, c3 + c4)                                        # [19 | 9]
         conv(sppf, w[9].cv2, cat20[..., c3:])
         self._up(cat20[..., c3:], cat11[..., :c4])
@@ -511,21 +501,21 @@ class FastSAM:
         A = head.shape[0]
         cand = torch.empty(A, 6 + NM, dtype=torch.float32, device=head.device)
         count = torch.empty(1, dtype=torch.int32, device=head.device)
-        _lib.call("sam6d_yolo_decode", _p(head), ctypes.c_longlong(head.stride(0)), ctypes.c_longlong(A * head.stride(0)), 1,
-                  *[v for hw in sizes for v in hw], ctypes.c_float(self.conf), _p(cand), _p(count), _s())
+        _lib.call("sam6d_yolo_decode", head, head.stride(0), A * head.stride(0), 1, *[v for hw in sizes for v in hw], self.conf, cand,
+                  count)
         rows = cand[:int(count.item())]
         order = torch.argsort(rows[:, 4], descending=True, stable=True)
         rows = rows[order]
         keep = torch.empty(rows.shape[0], dtype=torch.uint8, device=rows.device)
         if rows.shape[0]:
             boxes = rows[:, :4].contiguous()
-            _lib.call("sam6d_sam_nms", _p(boxes), None, rows.shape[0], ctypes.c_float(self.iou), _p(keep), _s())
+            _lib.call("sam6d_sam_nms", boxes, None, rows.shape[0], self.iou, keep)
         rows = rows[keep.bool()][:self.max_det].contiguous()
         masks = torch.empty(rows.shape[0], ih, iw, dtype=torch.uint8, device=rows.device)
         if rows.shape[0]:
             low = torch.empty(rows.shape[0], mh, mw, dtype=torch.float32, device=rows.device)
-            _lib.call("sam6d_yolo_masks", _p(proto.contiguous()), mh, mw, _p(rows), ctypes.c_longlong(rows.stride(0)), rows.shape[0], ih, iw,
-                      ctypes.c_float(mw / iw), ctypes.c_float(mh / ih), _p(low), _p(masks), _s())
+            _lib.call("sam6d_yolo_masks", proto.contiguous(), mh, mw, rows, rows.stride(0), rows.shape[0], ih, iw, mw / iw, mh / ih, low,
+                      masks)
         return {"rows": rows, "masks": masks}
 
     def postprocess_resize(self, detections, orig_size):

@@ -6,7 +6,6 @@ come back in between so that the host can draw the sample indices with numpy's R
     ret_dict, whole_image, whole_pts, model_points, all_dets = get_test_data(dets, image, depth, cam_K, depth_scale, model_points, ...)
 
 ret_dict carries the reference's keys: pts (P,2048,3), rgb (P,3,224,224), rgb_choose (P,2048) int64, score (P), model, K."""
-import ctypes
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -15,14 +14,6 @@ import torch
 from . import _lib
 
 ST = 12   # ints per detection in the stats array (csrc/inputs.cu)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def pack_rle(dets: Sequence[Dict], H: int, W: int):
@@ -86,9 +77,9 @@ class FrameInputs:
             cum_d = torch.from_numpy(cum).to(dev) if len(cum) else torch.zeros(1, dtype=torch.int32, device=dev)
             off_d = torch.from_numpy(off).to(dev)
             thr_d = torch.from_numpy(self.thr).to(dev)
-            _lib.call("sam6d_inputs_stage_a_min", _p(cum_d), _p(off_d), P, self.H, self.W, _p(self.depth), float(K[0, 0]),
-                      float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), _p(thr_d), int(min_count), _p(self.mask), _p(self.stats), self.cap,
-                      _p(self.choose1), _p(self.choose2), _p(self.cloud2), _stream())
+            _lib.call("sam6d_inputs_stage_a_min", cum_d, off_d, P, self.H, self.W, self.depth, float(K[0, 0]), float(K[1, 1]),
+                      float(K[0, 2]), float(K[1, 2]), thr_d, int(min_count), self.mask, self.stats, self.cap, self.choose1, self.choose2,
+                      self.cloud2)
         self.stats_host = self.stats.cpu().numpy() if P else np.zeros((0, ST), np.int32)
 
     # what the reference's loop decides per detection (run_inference_custom.py:199-212: more than 32 pixels, at least 4 points
@@ -114,9 +105,8 @@ class FrameInputs:
         if Q:
             keep_d = torch.from_numpy(np.ascontiguousarray(keep, dtype=np.int32)).to(dev)
             ci = torch.from_numpy(np.ascontiguousarray(choose_idx, dtype=np.int32)).to(dev)
-            _lib.call("sam6d_inputs_stage_b", _p(self.stats), _p(keep_d), Q, self.H, self.W, self.cap, _p(self.choose2), _p(self.cloud2),
-                      _p(ci), ns, img_size, _p(self.image), _p(self.mask), int(rgb_mask_flag), _p(pts), _p(rgb_choose), _p(rgb), _p(u8),
-                      _stream())
+            _lib.call("sam6d_inputs_stage_b", self.stats, keep_d, Q, self.H, self.W, self.cap, self.choose2, self.cloud2, ci, ns, img_size,
+                      self.image, self.mask, int(rgb_mask_flag), pts, rgb_choose, rgb, u8)
         return pts, rgb_choose, rgb, u8
 
     def whole_points(self) -> torch.Tensor:
@@ -208,7 +198,7 @@ def get_templates_from_arrays(rgbs: Sequence[np.ndarray], masks: Sequence[np.nda
     mask_d = torch.from_numpy(m.astype(np.uint8)).to(dev)
     bbox_d = torch.from_numpy(bbox).to(dev)
     rgb = torch.empty(T, 3, img_size, img_size, dtype=torch.float32, device=dev)
-    _lib.call("sam6d_crop_resize_normalize", _p(img_d), _p(mask_d), _p(bbox_d), T, H, W, img_size, int(rgb_mask_flag), _p(rgb), None, _stream())
+    _lib.call("sam6d_crop_resize_normalize", img_d, mask_d, bbox_d, T, H, W, img_size, int(rgb_mask_flag), rgb, None)
     rng = rng if rng is not None else np.random
     all_tem, all_pts, all_choose = [], [], []
     for t in range(T):

@@ -16,14 +16,12 @@ Multi-object post-processing of Instance_Segmentation_Model.test_step (ISM/model
          Detections.remove_very_small_detections    ISM/model/utils.py:96-105
          Detections.apply_nms_per_object_id         ISM/model/utils.py:107-119 (csrc/sam_dec.cu: sam_nms_kernel with object ids)
 """
-import ctypes
 from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .ops import _p, _s
 
 
 class PairwiseSimilarity(nn.Module):
@@ -95,7 +93,7 @@ def calculate_the_query_translation(proposal, depth, cam_intrinsic, depth_scale)
     d = depth.reshape(H, W).to(device=m.device, dtype=torch.int32).contiguous()
     K = _k64(cam_intrinsic, m.device)
     out = torch.empty(N, 3, dtype=torch.float32, device=m.device)
-    _lib.call("sam6d_query_translation", _p(m), _p(d), N, H, W, _p(K), ctypes.c_double(float(depth_scale)), _p(out), _s())
+    _lib.call("sam6d_query_translation", m, d, N, H, W, K, float(depth_scale), out)
     return out
 
 
@@ -124,8 +122,7 @@ def project_template_iou(poses, pointcloud, best_pose, pred_object_idx, translat
     iou = torch.empty(N, dtype=torch.float32, device=dev)
     ok = torch.empty(N, dtype=torch.uint8, device=dev)
     tr = translate.to(torch.float32).contiguous()      # a named tensor: a temporary inside the argument list would be freed before the launch
-    _lib.call("sam6d_project_template_iou", _p(poses), poses.shape[0], _p(pc), pc.shape[0], npc, _p(bp), _p(po),
-              _p(tr), _p(K), N, H, W, _p(bx), _p(vu), _p(xyxy), _p(iou), _p(ok), _s())
+    _lib.call("sam6d_project_template_iou", poses, poses.shape[0], pc, pc.shape[0], npc, bp, po, tr, K, N, H, W, bx, vu, xyxy, iou, ok)
     out = dict(xyxy=xyxy, iou=iou, ok=ok.bool())
     if want_image_vu:
         out["image_vu"] = vu
@@ -170,5 +167,5 @@ def nms_per_object(boxes, scores, object_ids, nms_thresh=NMS_THRESH):
     b = boxes[order].float().contiguous()
     obj = object_ids[order].to(torch.int32).contiguous()
     keep = torch.empty(b.shape[0], dtype=torch.uint8, device=b.device)
-    _lib.call("sam6d_sam_nms", _p(b), _p(obj), b.shape[0], ctypes.c_float(nms_thresh), _p(keep), _s())
+    _lib.call("sam6d_sam_nms", b, obj, b.shape[0], nms_thresh, keep)
     return order[keep.bool()]

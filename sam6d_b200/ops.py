@@ -2,9 +2,12 @@
 
 PyTorch is used here only as the owner of device memory and of the current CUDA stream; every function validates its
 arguments the way the reference's native layer does (CUDA, contiguous, dtype -- PEM/model/pointnet2/_ext_src/include/utils.h:10-30
-raise through TORCH_CHECK -> RuntimeError) and then hands raw pointers to libsam6d_b200.so.
+raise through TORCH_CHECK -> RuntimeError) and then hands the tensors to libsam6d_b200.so through _lib.call.
+
+A "row view" is a 2-D (rows, C) or 3-D (batch, rows, C) tensor whose last stride is 1, such as a column slice of a fused
+projection or the rows behind a sequence's first token; its row and batch strides are read from .stride(), and a batch
+stride of 0 (expand) shares one matrix across the batch.
 """
-import ctypes
 from typing import Optional, Tuple
 
 import torch
@@ -27,20 +30,14 @@ def _check(t: Tensor, dtype, name: str, ndim: Optional[int] = None):
         raise RuntimeError(f"{name} must have {ndim} dims, got {t.dim()}")
 
 
-def _p(t: Optional[Tensor]):
-    return ctypes.c_void_p(0 if t is None else t.data_ptr())
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ll(v):
-    return ctypes.c_longlong(int(v))
-
-
-def _f(v):
-    return ctypes.c_float(float(v))
+def _rows(t: Tensor) -> Tuple[int, int, int]:
+    """row view -> the (rows per batch, batch stride, row stride) triple of the header's row-op convention"""
+    if t.dim() not in (2, 3) or t.stride(-1) != 1:
+        raise RuntimeError(f"a row view is a 2-D or 3-D tensor with unit last stride, got shape {tuple(t.shape)} "
+                           f"strides {t.stride()}")
+    if t.dim() == 2:
+        return t.shape[0], 0, t.stride(0)
+    return t.shape[1], t.stride(0), t.stride(1)
 
 
 # ---------------------------------------------------------------------------------------------- point-cloud ops
@@ -52,7 +49,7 @@ def furthest_point_sampling(xyz: Tensor, m: int) -> Tensor:
         raise RuntimeError("points must be (B,N,3)")
     idx = torch.zeros(b, m, dtype=torch.int32, device=xyz.device)
     temp = torch.empty(b, n, dtype=torch.float32, device=xyz.device) if n > 4096 else None
-    _lib.call("sam6d_fps", _p(xyz), b, n, int(m), _p(temp), _p(idx), _s())
+    _lib.call("sam6d_fps", xyz, b, n, int(m), temp, idx)
     return idx
 
 
@@ -62,7 +59,7 @@ def furthest_point_sampling_single_cta(xyz: Tensor, m: int) -> Tensor:
     b, n, _ = xyz.shape
     idx = torch.zeros(b, m, dtype=torch.int32, device=xyz.device)
     temp = torch.empty(b, n, dtype=torch.float32, device=xyz.device)
-    _lib.call("sam6d_fps_single_cta", _p(xyz), b, n, int(m), _p(temp), _p(idx), _s())
+    _lib.call("sam6d_fps_single_cta", xyz, b, n, int(m), temp, idx)
     return idx
 
 
@@ -73,7 +70,7 @@ def gather_points(points: Tensor, idx: Tensor) -> Tensor:
     b, c, n = points.shape
     m = idx.shape[1]
     out = torch.zeros(b, c, m, dtype=torch.float32, device=points.device)
-    _lib.call("sam6d_gather_points", _p(points), _p(idx), b, c, n, m, _p(out), _s())
+    _lib.call("sam6d_gather_points", points, idx, b, c, n, m, out)
     return out
 
 
@@ -84,7 +81,7 @@ def gather_rows(src: Tensor, idx: Tensor, n_rows: Optional[int] = None) -> Tenso
     b, n, c = src.shape
     m = idx.shape[1]
     out = torch.empty(b, m, c, dtype=torch.float32, device=src.device)
-    _lib.call("sam6d_gather_rows", _p(src), _p(idx), b, n, m, c, _ll(n * c), _p(out), _s())
+    _lib.call("sam6d_gather_rows", src, idx, b, n, m, c, n * c, out)
     return out
 
 
@@ -96,7 +93,7 @@ def ball_query(new_xyz: Tensor, xyz: Tensor, radius: float, nsample: int, return
     n = xyz.shape[1]
     idx = torch.zeros(b, m, nsample, dtype=torch.int32, device=xyz.device)
     cnt = torch.zeros(b, m, dtype=torch.int32, device=xyz.device) if return_count else None
-    _lib.call("sam6d_ball_query", _p(new_xyz), _p(xyz), b, n, m, _f(radius), int(nsample), _p(idx), _p(cnt), _s())
+    _lib.call("sam6d_ball_query", new_xyz, xyz, b, n, m, radius, int(nsample), idx, cnt)
     return (idx, cnt) if return_count else idx
 
 
@@ -111,8 +108,7 @@ def ball_query_pair(new_xyz: Tensor, xyz: Tensor, ra: float, nsa: int, rb: float
     ib = torch.empty(b, m, nsb, dtype=torch.int32, device=dev)
     ca = torch.empty(b, m, dtype=torch.int32, device=dev)
     cb = torch.empty(b, m, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_ball_query_pair", _p(new_xyz), _p(xyz), b, n, m, _f(ra), int(nsa), _f(rb), int(nsb), _p(ia), _p(ib), _p(ca),
-              _p(cb), _s())
+    _lib.call("sam6d_ball_query_pair", new_xyz, xyz, b, n, m, ra, int(nsa), rb, int(nsb), ia, ib, ca, cb)
     return ia, ca, ib, cb
 
 
@@ -123,62 +119,48 @@ def group_points(points: Tensor, idx: Tensor) -> Tensor:
     b, c, n = points.shape
     _, npnt, ns = idx.shape
     out = torch.zeros(b, c, npnt, ns, dtype=torch.float32, device=points.device)
-    _lib.call("sam6d_group_points", _p(points), _p(idx), b, c, n, npnt, ns, _p(out), _s())
+    _lib.call("sam6d_group_points", points, idx, b, c, n, npnt, ns, out)
     return out
 
 
 # ---------------------------------------------------------------------------------------------- dense algebra
+def _gemm_dims(A: Tensor, W: Tensor, residual: Optional[Tensor], out: Tensor):
+    """(M, N, K, lda, ldw, ldc, ldr, batch, sA, sW, sC, sR) of the strided / batched GEMM contract: A, residual, out row views,
+    W (N,K) shared by every problem or (batch, N, K)"""
+    M, sA, lda = _rows(A)
+    K, N = A.shape[-1], W.shape[-2]
+    if W.shape[-1] != K or W.stride(-1) != 1 or W.dim() not in (2, 3):
+        raise RuntimeError("gemm: W must be (N,K) or (batch,N,K) with A's inner dimension and unit last stride")
+    _, sC, ldc = _rows(out)
+    _, sR, ldr = (0, 0, 0) if residual is None else _rows(residual)
+    return (M, N, K, lda, W.stride(-2), ldc, ldr, A.shape[0] if A.dim() == 3 else 1, sA, W.stride(0) if W.dim() == 3 else 0,
+            sC, sR)
+
+
 def gemm(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optional[Tensor] = None,
          out: Optional[Tensor] = None, relu=False, alpha: float = 1.0) -> Tensor:
-    """out = alpha * A @ W^T (+bias) (act) (+residual); A (M,K), W (N,K) contiguous f32.  relu: False/True or the activation
-    code (0 none, 1 ReLU, 2 GELU)."""
-    _check(A, torch.float32, "A", 2)
-    _check(W, torch.float32, "W", 2)
-    M, K = A.shape
-    N = W.shape[0]
-    if W.shape[1] != K:
-        raise RuntimeError("gemm: inner dimensions differ")
+    """out = alpha * A @ W^T (+bias) (act) (+residual), f32: A, residual, out row views (M,K), (M,N) or batched (batch,M,K),
+    (batch,M,N); W (N,K) shared or (batch,N,K).  relu: False/True or the activation code (0 none, 1 ReLU, 2 GELU)."""
+    if A.dtype != torch.float32 or W.dtype != torch.float32:
+        raise RuntimeError("gemm: A and W must be float32")
     if out is None:
-        out = torch.empty(M, N, dtype=torch.float32, device=A.device)
-    _lib.call("sam6d_gemm_f32", _p(A), _p(W), _p(bias), _p(residual), _p(out), M, N, K, _ll(K), _ll(K), _ll(N), _ll(N),
-              1, _ll(0), _ll(0), _ll(0), _ll(0), _f(alpha), int(relu), _s())
+        out = torch.empty(*A.shape[:-1], W.shape[-2], dtype=torch.float32, device=A.device)
+    _lib.call("sam6d_gemm_f32", A, W, bias, residual, out, *_gemm_dims(A, W, residual, out), alpha, relu)
     return out
-
-
-def gemm_raw(A_ptr, W_ptr, bias, R_ptr, C_ptr, M, N, K, lda, ldw, ldc, ldr, batch=1, sA=0, sW=0, sC=0, sR=0,
-             alpha=1.0, relu=False):
-    """strided / batched form over raw device addresses (ints)."""
-    _lib.call("sam6d_gemm_f32", ctypes.c_void_p(A_ptr), ctypes.c_void_p(W_ptr), _p(bias), ctypes.c_void_p(R_ptr or 0),
-              ctypes.c_void_p(C_ptr), int(M), int(N), int(K), _ll(lda), _ll(ldw), _ll(ldc), _ll(ldr), int(batch), _ll(sA),
-              _ll(sW), _ll(sC), _ll(sR), _f(alpha), int(relu), _s())
 
 
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 
 
-def gemm_tc_raw(A_ptr, a_dt, W_ptr, w_dt, bias, R_ptr, C_ptr, c_dt, M, N, K, lda, ldw, ldc, ldr, batch=1, sA=0, sW=0, sC=0, sR=0,
-                alpha=1.0, relu=False):
-    """wgmma bf16 GEMM over raw device addresses; *_dt: 0 = fp32, 1 = bf16"""
-    _lib.call("sam6d_gemm_bf16", ctypes.c_void_p(A_ptr), int(a_dt), ctypes.c_void_p(W_ptr), int(w_dt), _p(bias),
-              ctypes.c_void_p(R_ptr or 0), ctypes.c_void_p(C_ptr), int(c_dt), int(M), int(N), int(K), _ll(lda), _ll(ldw), _ll(ldc),
-              _ll(ldr), int(batch), _ll(sA), _ll(sW), _ll(sC), _ll(sR), _f(alpha), int(relu), _s())
-
-
 def gemm_tc(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Optional[Tensor] = None, out: Optional[Tensor] = None,
             relu: bool = False, alpha: float = 1.0, out_dtype=torch.float32) -> Tensor:
-    """tensor-core form of gemm(): A (M,K) fp32|bf16, W (N,K) fp32|bf16 -> (M,N) fp32|bf16, fp32 accumulate"""
-    for t, n in ((A, "A"), (W, "W")):
-        if t.dtype not in _DT:
-            raise RuntimeError(f"{n} must be float32 or bfloat16")
-        _check(t, t.dtype, n, 2)
-    M, K = A.shape
-    N = W.shape[0]
-    if W.shape[1] != K:
-        raise RuntimeError("gemm: inner dimensions differ")
+    """tensor-core form of gemm(): A, W fp32|bf16 -> out fp32|bf16, fp32 accumulate"""
+    if A.dtype not in _DT or W.dtype not in _DT:
+        raise RuntimeError("gemm_tc: A and W must be float32 or bfloat16")
     if out is None:
-        out = torch.empty(M, N, dtype=out_dtype, device=A.device)
-    gemm_tc_raw(A.data_ptr(), _DT[A.dtype], W.data_ptr(), _DT[W.dtype], bias, residual.data_ptr() if residual is not None else 0,
-                out.data_ptr(), _DT[out.dtype], M, N, K, K, K, N, N, alpha=alpha, relu=relu)
+        out = torch.empty(*A.shape[:-1], W.shape[-2], dtype=out_dtype, device=A.device)
+    _lib.call("sam6d_gemm_bf16", A, _DT[A.dtype], W, _DT[W.dtype], bias, residual, out, _DT[out.dtype], *_gemm_dims(A, W, residual, out),
+              alpha, relu)
     return out
 
 
@@ -197,8 +179,7 @@ def gemm_tma(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Opti
         out = torch.empty(M, Nout, dtype=torch.bfloat16 if act == ACT_SWIGLU else out_dtype, device=A.device)
     if residual is not None:
         _check(residual, out.dtype, "residual", 2)          # the residual stream has the element type of the output
-    _lib.call("sam6d_gemm_tma", _p(A), _p(W), _p(bias), _p(residual), _p(out), _DT[out.dtype], M, N, K, _ll(K), _ll(K), _ll(Nout), _ll(N),
-              _f(alpha), int(act), _s())
+    _lib.call("sam6d_gemm_tma", A, W, bias, residual, out, _DT[out.dtype], M, N, K, K, K, Nout, N, alpha, int(act))
     return out
 
 
@@ -244,8 +225,7 @@ def gemm_tma_vt(A: Tensor, W: Tensor, bias: Tensor, vt_col0: int, S: int, slot: 
     n1 = (S + 15) // 16 * 16
     out = torch.empty(M, vt_col0, dtype=torch.bfloat16, device=A.device)
     vt = _vt_buffer((M // S) * (N - vt_col0), n1, A.device, slot)
-    _lib.call("sam6d_gemm_tma_vt", _p(A), _p(W), _p(bias), _p(out), M, N, K, _ll(K), _ll(K), _ll(vt_col0), _p(vt), int(vt_col0), int(S),
-              int(n1), _s())
+    _lib.call("sam6d_gemm_tma_vt", A, W, bias, out, M, N, K, K, K, vt_col0, vt, int(vt_col0), int(S), int(n1))
     return out, vt
 
 
@@ -261,24 +241,21 @@ def gemm_tma_vt2(A: Tensor, W: Tensor, bias: Tensor, vt_col0: int, vt_col1: int,
     out = torch.empty(M, vt_col0, dtype=torch.bfloat16, device=A.device)
     out2 = torch.empty(M, N - vt_col1, dtype=torch.bfloat16, device=A.device)
     vt = _vt_buffer((M // S) * (vt_col1 - vt_col0), n1, A.device, slot)
-    _lib.call("sam6d_gemm_tma_vt2", _p(A), _p(W), _p(bias), _p(out), M, N, K, _ll(K), _ll(K), _ll(vt_col0), _p(vt), int(vt_col0),
-              int(vt_col1), int(S), int(n1), _p(out2), _ll(N - vt_col1), _s())
+    _lib.call("sam6d_gemm_tma_vt2", A, W, bias, out, M, N, K, K, K, vt_col0, vt, int(vt_col0), int(vt_col1), int(S), int(n1), out2,
+              N - vt_col1)
     return out, vt, out2
 
 
-def layernorm_raw(x_ptr, x_view, y_ptr, y_view, gamma: Tensor, beta: Tensor, rows: int, C: int, eps: float = 1e-5):
-    _lib.call("sam6d_layernorm", ctypes.c_void_p(x_ptr), _ll(x_view[0]), _ll(x_view[1]), _ll(x_view[2]),
-              ctypes.c_void_p(y_ptr), _ll(y_view[0]), _ll(y_view[1]), _ll(y_view[2]), _p(gamma), _p(beta), _ll(rows), int(C),
-              _f(eps), _s())
-
-
 def layernorm(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5, out: Optional[Tensor] = None) -> Tensor:
-    _check(x, torch.float32, "x")
+    """LayerNorm over the last dim of f32 rows: x and out contiguous (any rank) or row views"""
+    if x.dtype != torch.float32:
+        raise RuntimeError(f"x must be torch.float32, got {x.dtype}")
     C = x.shape[-1]
-    rows = x.numel() // C
     if out is None:
         out = torch.empty_like(x)
-    layernorm_raw(x.data_ptr(), (rows, 0, C), out.data_ptr(), (rows, 0, C), gamma, beta, rows, C, eps)
+    xv = x.view(-1, C) if x.is_contiguous() else x
+    yv = out.view(-1, C) if out.is_contiguous() else out
+    _lib.call("sam6d_layernorm", xv, *_rows(xv), yv, *_rows(yv), gamma, beta, x.numel() // C, C, eps)
     return out
 
 
@@ -288,8 +265,7 @@ def layernorm_bf16(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5) ->
     C = x.shape[-1]
     rows = x.numel() // C
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    _lib.call("sam6d_layernorm_bf16", _p(x), _ll(rows), _ll(0), _ll(C), _p(out), _ll(rows), _ll(0), _ll(C), _p(gamma), _p(beta),
-              _ll(rows), int(C), _f(eps), _s())
+    _lib.call("sam6d_layernorm_bf16", x, rows, 0, C, out, rows, 0, C, gamma, beta, rows, int(C), eps)
     return out
 
 
@@ -300,8 +276,7 @@ def layernorm_bf16io(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5, 
     rows = x.numel() // C
     if out is None:
         out = torch.empty_like(x)
-    _lib.call("sam6d_layernorm_bf16io", _p(x), _ll(max(rows, 1)), _ll(0), _ll(C), _p(out), _ll(max(rows, 1)), _ll(0), _ll(C),
-              _p(gamma), _p(beta), _ll(rows), int(C), _f(eps), _s())
+    _lib.call("sam6d_layernorm_bf16io", x, max(rows, 1), 0, C, out, max(rows, 1), 0, C, gamma, beta, rows, int(C), eps)
     return out
 
 
@@ -319,8 +294,7 @@ def transformer_tail_bf16(hid: Tensor, x: Tensor, wo: Tensor, bo: Tensor, g1: Te
     if out is None:
         out = torch.empty_like(hid)
     _check(out, torch.bfloat16, "out", 2)
-    _lib.call("sam6d_transformer_tail_bf16", _p(hid), _ll(256), _p(x), _ll(256), _p(wo), _p(bo), _p(g1), _p(b1), _p(we), _p(be), _p(ws),
-              _p(bs), _p(g2), _p(b2), _p(out), _ll(256), int(M), _f(eps), _s())
+    _lib.call("sam6d_transformer_tail_bf16", hid, 256, x, 256, wo, bo, g1, b1, we, be, ws, bs, g2, b2, out, 256, int(M), eps)
     return out
 
 
@@ -331,7 +305,7 @@ def gather_rows_bf16_f32(src: Tensor, idx: Tensor) -> Tensor:
     b, n, c = src.shape
     m = idx.shape[1]
     out = torch.empty(b, m, c, dtype=torch.float32, device=src.device)
-    _lib.call("sam6d_gather_rows_bf16_f32", _p(src), _p(idx), b, n, m, c, _ll(n * c), _p(out), _s())
+    _lib.call("sam6d_gather_rows_bf16_f32", src, idx, b, n, m, c, n * c, out)
     return out
 
 
@@ -342,7 +316,7 @@ def gather_rows_bf16(src: Tensor, idx: Tensor) -> Tensor:
     b, n, c = src.shape
     m = idx.shape[1]
     out = torch.empty(b, m, c, dtype=torch.bfloat16, device=src.device)
-    _lib.call("sam6d_gather_rows", _p(src), _p(idx), b, n, m, c // 2, _ll(n * c // 2), _p(out), _s())
+    _lib.call("sam6d_gather_rows", src, idx, b, n, m, c // 2, n * c // 2, out)
     return out
 
 
@@ -351,7 +325,7 @@ def l2norm_rows(x: Tensor) -> Tensor:
     C = x.shape[-1]
     rows = x.numel() // C
     out = torch.empty_like(x)
-    _lib.call("sam6d_l2norm_rows", _p(x), _ll(rows), _ll(0), _ll(C), _p(out), _ll(rows), _ll(0), _ll(C), _ll(rows), C, _s())
+    _lib.call("sam6d_l2norm_rows", x, rows, 0, C, out, rows, 0, C, rows, C)
     return out
 
 
@@ -361,33 +335,38 @@ def l2norm_rows_bf16(x: Tensor) -> Tensor:
     C = x.shape[-1]
     rows = x.numel() // C
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    _lib.call("sam6d_l2norm_rows_bf16", _p(x), _ll(max(rows, 1)), _ll(0), _ll(C), _p(out), _ll(max(rows, 1)), _ll(0), _ll(C), _ll(rows), C,
-              _s())
+    _lib.call("sam6d_l2norm_rows_bf16", x, max(rows, 1), 0, C, out, max(rows, 1), 0, C, rows, C)
     return out
 
 
-def gemm_tma_batched(A: Tensor, W: Tensor, out: Tensor, M: int, N: int, ldc: int, c_bs: int, alpha: float = 1.0,
-                     bias: Optional[Tensor] = None, residual: Optional[Tensor] = None, ldr: int = 0, r_bs: int = 0) -> Tensor:
-    """A (batch, a_rows, K) bf16; W (batch, w_rows, K) bf16 or one shared (N, K) matrix ->
-    out[z, :M, :N] = alpha * A[z,:M] @ W[z,:N]^T (+ bias) (+ residual[z]) for every z, written with row stride ldc and problem
-    stride c_bs (elements) into `out` (fp32 or bf16; the residual has out's element type, row stride ldr, problem stride r_bs)"""
+def gemm_tma_batched(A: Tensor, W: Tensor, out: Tensor, alpha: float = 1.0, bias: Optional[Tensor] = None,
+                     residual: Optional[Tensor] = None) -> Tensor:
+    """A (batch, a_rows, K) bf16; W (batch, w_rows, K) bf16 or one shared (N, K) matrix; out a (batch, M, N) row view (fp32 or
+    bf16, M <= a_rows, N <= w_rows) -> out[z] = alpha * A[z,:M] @ W[z,:N]^T (+ bias) (+ residual[z]) for every z; the residual
+    is a row view with out's shape and element type (batch stride 0 shares one matrix)"""
     _check(A, torch.bfloat16, "A", 3)
     _check(W, torch.bfloat16, "W")
     batch, a_rows, K = A.shape
+    M, c_bs, ldc = _rows(out)
+    N = out.shape[-1]
     shared = W.dim() == 2
-    if W.shape[-1] != K or a_rows < M or (not shared and (W.shape[0] != batch or W.shape[1] < N)) or (shared and W.shape[0] != N):
+    if (W.shape[-1] != K or a_rows < M or out.dim() != 3 or out.shape[0] != batch
+            or (not shared and (W.shape[0] != batch or W.shape[1] < N)) or (shared and W.shape[0] != N)):
         raise RuntimeError("gemm_tma_batched: shape mismatch")
     if residual is not None and residual.dtype != out.dtype:
         raise RuntimeError("gemm_tma_batched: the residual must have the output's element type")
-    _lib.call("sam6d_gemm_tma_batched", _p(A), _p(W), _p(bias), _p(residual), _p(out), _DT[out.dtype], int(M), int(N), int(K), _ll(K),
-              _ll(K), _ll(ldc), _ll(ldr), int(batch), _ll(a_rows), _ll(0 if shared else W.shape[1]), _ll(c_bs), _ll(r_bs), _f(alpha), 0,
-              _s())
+    _, r_bs, ldr = (0, 0, 0) if residual is None else _rows(residual)
+    _lib.call("sam6d_gemm_tma_batched", A, W, bias, residual, out, _DT[out.dtype], M, N, K, K, K, ldc, ldr, batch, a_rows,
+              0 if shared else W.shape[1], c_bs, r_bs, alpha, 0)
     return out
 
 
-def focus_rows_raw(x_ptr, x_view, y_ptr, y_view, sp_scale: Tensor, rows: int, C: int):
-    _lib.call("sam6d_focus_rows", ctypes.c_void_p(x_ptr), _ll(x_view[0]), _ll(x_view[1]), _ll(x_view[2]),
-              ctypes.c_void_p(y_ptr), _ll(y_view[0]), _ll(y_view[1]), _ll(y_view[2]), _p(sp_scale), _ll(rows), int(C), _s())
+def focus_rows(x: Tensor, sp_scale: Tensor, out: Optional[Tensor] = None) -> Tensor:
+    """focused-linear-attention feature map of f32 row views; out may be x itself"""
+    if out is None:
+        out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    _lib.call("sam6d_focus_rows", x, *_rows(x), out, *_rows(out), sp_scale, x.numel() // x.shape[-1], x.shape[-1])
+    return out
 
 
 def rigid_warp(p: Tensor, R: Tensor, t: Tensor) -> Tensor:
@@ -395,14 +374,14 @@ def rigid_warp(p: Tensor, R: Tensor, t: Tensor) -> Tensor:
     _check(R, torch.float32, "R", 3)
     _check(t, torch.float32, "t", 2)
     out = torch.empty_like(p)
-    _lib.call("sam6d_rigid_warp", _p(p), _p(R), _p(t), p.shape[0], p.shape[1], _p(out), _s())
+    _lib.call("sam6d_rigid_warp", p, R, t, p.shape[0], p.shape[1], out)
     return out
 
 
 def cloud_radius(po: Tensor) -> Tensor:
     _check(po, torch.float32, "dense_po", 3)
     r = torch.empty(po.shape[0], dtype=torch.float32, device=po.device)
-    _lib.call("sam6d_cloud_radius", _p(po), po.shape[0], po.shape[1], _p(r), _s())
+    _lib.call("sam6d_cloud_radius", po, po.shape[0], po.shape[1], r)
     return r
 
 
@@ -411,7 +390,7 @@ def scale_by_radius(x: Tensor, radius: Tensor) -> Tensor:
     _check(radius, torch.float32, "radius", 1)
     out = torch.empty_like(x)
     b = x.shape[0]
-    _lib.call("sam6d_scale_by_radius", _p(x), _p(radius), b, _ll(x.numel() // max(b, 1)), _p(out), _s())
+    _lib.call("sam6d_scale_by_radius", x, radius, b, x.numel() // max(b, 1), out)
     return out
 
 
@@ -420,7 +399,7 @@ def geo_indices(pts: Tensor, sigma_d: float, factor_a: float) -> Tensor:
     _check(pts, torch.float32, "points", 3)
     b, s, _ = pts.shape
     T = torch.empty(b, s, s, 4, dtype=torch.float32, device=pts.device)
-    _lib.call("sam6d_geo_indices", _p(pts), b, s, _f(sigma_d), _f(factor_a), _p(T), _s())
+    _lib.call("sam6d_geo_indices", pts, b, s, sigma_d, factor_a, T)
     return T
 
 
@@ -428,7 +407,7 @@ def geo_embed_f32(T: Tensor, div_term: Tensor, WaT: Tensor, WdT: Tensor, bias: T
     _check(T, torch.float32, "T", 4)
     b, s, _, _ = T.shape
     E = torch.empty(b, s, s, 256, dtype=torch.float32, device=T.device)
-    _lib.call("sam6d_geo_embed_f32", _p(T), _ll(b * s * s), _p(div_term), _p(WaT), _p(WdT), _p(bias), _p(E), _s())
+    _lib.call("sam6d_geo_embed_f32", T, b * s * s, div_term, WaT, WdT, bias, E)
     return E
 
 
@@ -439,8 +418,7 @@ def geo_embed_tc(T: Tensor, div_term: Tensor, Wa_bf16: Tensor, Wd_bf16: Tensor, 
     _check(Wd_bf16, torch.bfloat16, "Wd", 2)
     b, s, _, _ = T.shape
     E = torch.empty(b, s, s, 256, dtype=out_dtype, device=T.device)
-    _lib.call("sam6d_geo_embed_tc", _p(T), _ll(b * s * s), _p(div_term), _p(Wa_bf16), _p(Wd_bf16), _p(bias), _p(E),
-              int(out_dtype == torch.bfloat16), _s())
+    _lib.call("sam6d_geo_embed_tc", T, b * s * s, div_term, Wa_bf16, Wd_bf16, bias, E, int(out_dtype == torch.bfloat16))
     return E
 
 
@@ -451,7 +429,7 @@ def geo_embed_dist_tc(T: Tensor, div_term: Tensor, Wd_bf16: Tensor, bias: Tensor
     _check(Wd_bf16, torch.bfloat16, "Wd", 2)
     n = T.numel() // 4
     E = torch.empty(*T.shape[:-1], 256, dtype=torch.bfloat16, device=T.device)
-    _lib.call("sam6d_geo_embed_dist_tc", _p(T), _ll(n), _p(div_term), _p(Wd_bf16), _p(bias), _p(E), _s())
+    _lib.call("sam6d_geo_embed_dist_tc", T, n, div_term, Wd_bf16, bias, E)
     return E
 
 
@@ -468,23 +446,24 @@ def geo_embed_lut(T: Tensor, tabA: Tensor, inv_ha: float, tabD: Tensor, inv_hd: 
     if far.shape != (b, 2, s, 256) or tabA.shape[1] != 256 or tabD.shape[1] != 256 or T.shape[3] != 4:
         raise RuntimeError("geo_embed_lut: shape mismatch")
     E = torch.empty(b, s, s, 256, dtype=torch.bfloat16, device=T.device)
-    _lib.call("sam6d_geo_embed_lut", _p(T), _ll(b), s, _p(tabA), tabA.shape[0], _f(inv_ha), _p(tabD), tabD.shape[0], _f(inv_hd), _p(far),
-              _p(div_term), _p(WdT_bf16), _p(bias), _p(E), _s())
+    _lib.call("sam6d_geo_embed_lut", T, b, s, tabA, tabA.shape[0], inv_ha, tabD, tabD.shape[0], inv_hd, far, div_term, WdT_bf16, bias, E)
     return E
 
 
 # ---------------------------------------------------------------------------------------------- attention
-def rpe_scores(E: Tensor, U: Tensor, u_ptr: Optional[int] = None, u_ld: int = 1024) -> Tensor:
-    """E (B,S,S,256) f32|bf16, U (B,S,4,256) f32 (or a raw address + row stride) -> (B,4,S,S) f32."""
+def rpe_scores(E: Tensor, U: Tensor) -> Tensor:
+    """E (B,S,S,256) f32|bf16, U (B,S,4,256) f32 contiguous or a (B*S, 4*256) f32 row view (e.g. the u columns of a fused
+    projection) -> (B,4,S,S) f32."""
     if E.dtype not in (torch.float32, torch.bfloat16):
         raise RuntimeError("E must be float32 or bfloat16")
     _check(E, E.dtype, "E", 4)
-    if u_ptr is None:
-        _check(U, torch.float32, "U", 4)
-        u_ptr = U.data_ptr()
     B, S = E.shape[0], E.shape[1]
+    if U.dim() == 4:
+        U = U.view(B * S, -1)
+    if U.dtype != torch.float32 or U.dim() != 2 or U.shape != (B * S, 1024) or U.stride(1) != 1:
+        raise RuntimeError("rpe_scores: U must be a (B*S, 1024) float32 row view")
     SP = torch.empty(B, 4, S, S, dtype=torch.float32, device=E.device)
-    _lib.call("sam6d_rpe_scores", _p(E), int(E.dtype == torch.bfloat16), ctypes.c_void_p(u_ptr), _ll(u_ld), B, S, _p(SP), _s())
+    _lib.call("sam6d_rpe_scores", E, int(E.dtype == torch.bfloat16), U, U.stride(0), B, S, SP)
     return SP
 
 
@@ -499,7 +478,7 @@ def rpe_scores_tc(E: Tensor, U: Tensor, ld: Optional[int] = None) -> Tensor:
         raise RuntimeError("rpe_scores_tc: E (B,S,S,256), U (B*S,1024)")
     ld = S if ld is None else ld
     SP = torch.empty(B, 4, S, ld, dtype=torch.float32, device=E.device)
-    _lib.call("sam6d_rpe_scores_tc_ld", _p(E), _p(U), B, S, _p(SP), int(ld), _s())
+    _lib.call("sam6d_rpe_scores_tc_ld", E, U, B, S, SP, int(ld))
     return SP
 
 
@@ -519,17 +498,21 @@ def attn_tc_padded_bias(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tens
     if bias.shape[:3] != (B, H, Sq) or bias.shape[3] < Sk or bias.shape[3] % 4:
         raise RuntimeError("attn_tc_padded_bias: bias (B,H,Sq,ld), ld >= Sk, ld % 4 == 0")
     out = torch.empty(B * Sq, H * D, dtype=out_dtype, device=Q.device)
-    _lib.call("sam6d_attn_tc_bias_ld", _p(Q), _ll(Q.shape[1]), int(q_col0), _p(K), _ll(K.shape[1]), int(k_col0), _p(Vt), _ll(Vt.shape[1]),
-              int(B), int(H), int(Sq), int(Sk), int(D), _p(bias), _ll(bias.shape[3]), _f(scale), _p(out),
-              int(out_dtype == torch.bfloat16), _ll(H * D), _s())
+    _lib.call("sam6d_attn_tc_bias_ld", Q, Q.shape[1], int(q_col0), K, K.shape[1], int(k_col0), Vt, Vt.shape[1], int(B), int(H), int(Sq),
+              int(Sk), int(D), bias, bias.shape[3], scale, out, int(out_dtype == torch.bfloat16), H * D)
     return out
 
 
-def mha_raw(q_ptr, q_ld, q_bs, k_ptr, k_ld, k_bs, v_ptr, v_ld, v_bs, bias: Optional[Tensor], B, H, Sq, Sk, scale,
-            o_ptr, o_ld, o_bs):
-    _lib.call("sam6d_mha", ctypes.c_void_p(q_ptr), _ll(q_ld), _ll(q_bs), ctypes.c_void_p(k_ptr), _ll(k_ld), _ll(k_bs),
-              ctypes.c_void_p(v_ptr), _ll(v_ld), _ll(v_bs), _p(bias), int(B), int(H), int(Sq), int(Sk), _f(scale),
-              ctypes.c_void_p(o_ptr), _ll(o_ld), _ll(o_bs), _s())
+def mha(q: Tensor, k: Tensor, v: Tensor, bias: Optional[Tensor], scale: float, out: Tensor) -> Tensor:
+    """softmax((q k^T + bias) * scale) v per head of 64 channels: q, out (B,Sq,H*64), k, v (B,Sk,H*64) f32 row views (e.g.
+    column slices of a fused qkv projection); bias (B,H,Sq,Sk) f32 or None"""
+    B, Sq, HD = q.shape
+    _, q_bs, q_ld = _rows(q)
+    _, k_bs, k_ld = _rows(k)
+    _, v_bs, v_ld = _rows(v)
+    _, o_bs, o_ld = _rows(out)
+    _lib.call("sam6d_mha", q, q_ld, q_bs, k, k_ld, k_bs, v, v_ld, v_bs, bias, B, HD // 64, Sq, k.shape[1], scale, out, o_ld, o_bs)
+    return out
 
 
 def pack_rel_pos(rel_h: Tensor, rel_w: Tensor, slab_rows: int = 32) -> Tensor:
@@ -561,8 +544,8 @@ def attn_global_tc(qkv: Tensor, vt: Tensor, rel_blob: Tensor, B: int, H: int, gr
     _check(rel_blob, torch.bfloat16, "rel_blob", 1)
     L = grid * grid
     out = torch.empty(B * L, H * D, dtype=out_dtype, device=qkv.device)
-    _lib.call("sam6d_attn_global_tc_ex", _p(qkv), _ll(qkv.shape[1]), _p(vt), _ll(vt.shape[1]), _p(rel_blob), int(B), int(H), int(grid),
-              int(D), _f(scale), _p(out), int(out_dtype == torch.bfloat16), _ll(H * D), _s())
+    _lib.call("sam6d_attn_global_tc_ex", qkv, qkv.shape[1], vt, vt.shape[1], rel_blob, int(B), int(H), int(grid), int(D), scale, out,
+              int(out_dtype == torch.bfloat16), H * D)
     return out
 
 
@@ -582,9 +565,8 @@ def attn_tc(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tensor, B: int, 
         rh, Hs, Ws = rel                     # rh: pack_rel_pos(rel_pos_h, rel_pos_w)
         mode = 2
     out = torch.empty(B * Sq, H * D, dtype=out_dtype, device=Q.device)
-    _lib.call("sam6d_attn_tc", _p(Q), _ll(Q.shape[1]), int(q_col0), _p(K), _ll(K.shape[1]), int(k_col0), _p(Vt), _ll(Vt.shape[1]),
-              int(B), int(H), int(Sq), int(Sk), int(D), mode, _p(bias), _p(rh), _p(rw), int(Hs), int(Ws), _p(bv), _f(scale), _p(out),
-              int(out_dtype == torch.bfloat16), _ll(H * D), _s())
+    _lib.call("sam6d_attn_tc", Q, Q.shape[1], int(q_col0), K, K.shape[1], int(k_col0), Vt, Vt.shape[1], int(B), int(H), int(Sq), int(Sk),
+              int(D), mode, bias, rh, rw, int(Hs), int(Ws), bv, scale, out, int(out_dtype == torch.bfloat16), H * D)
     return out
 
 
@@ -597,9 +579,8 @@ def attn_tc_ex(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tensor, B: in
     _check(Vt, torch.bfloat16, "Vt", 2)
     out = torch.empty(B * Sq, H * D, dtype=out_dtype, device=Q.device)
     lse = torch.empty(B, H, Sq, dtype=torch.float32, device=Q.device) if want_lse else None
-    _lib.call("sam6d_attn_tc_ex", _p(Q), _ll(Q.shape[1]), int(q_col0), _p(K), _ll(K.shape[1]), int(k_col0), _p(Vt), _ll(Vt.shape[1]),
-              int(B), int(H), int(Sq), int(Sk), int(D), _f(scale), int(k_brows), int(k_row0), int(v_col0), _p(lse), _p(out),
-              int(out_dtype == torch.bfloat16), _ll(H * D), _s())
+    _lib.call("sam6d_attn_tc_ex", Q, Q.shape[1], int(q_col0), K, K.shape[1], int(k_col0), Vt, Vt.shape[1], int(B), int(H), int(Sq), int(Sk),
+              int(D), scale, int(k_brows), int(k_row0), int(v_col0), lse, out, int(out_dtype == torch.bfloat16), H * D)
     return out, lse
 
 
@@ -609,8 +590,8 @@ def attn_merge_key(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, k_brows: int,
     attn_tc_ex (head dim 64), in place"""
     _check(out, torch.bfloat16, "out", 2)
     _check(lse, torch.float32, "lse", 3)
-    _lib.call("sam6d_attn_merge_key", _p(Q), _ll(Q.shape[1]), int(q_col0), _p(K), _ll(K.shape[1]), int(k_col0), int(k_brows), int(key_row),
-              _p(Vt), _ll(Vt.shape[1]), int(key_col), _p(lse), int(B), int(H), int(Sq), _f(scale), _p(out), _ll(out.shape[1]), _s())
+    _lib.call("sam6d_attn_merge_key", Q, Q.shape[1], int(q_col0), K, K.shape[1], int(k_col0), int(k_brows), int(key_row), Vt, Vt.shape[1],
+              int(key_col), lse, int(B), int(H), int(Sq), scale, out, out.shape[1])
     return out
 
 
@@ -619,43 +600,51 @@ def transpose_tokens(src: Tensor, col0: int, C: int, nB: int, L: int) -> Tensor:
     _check(src, torch.bfloat16, "src", 2)
     N1 = (L + 15) // 16 * 16
     out = torch.empty(nB * C, N1, dtype=torch.bfloat16, device=src.device)
-    _lib.call("sam6d_transpose_tokens_bf16", _p(src), _ll(src.shape[1]), int(col0), int(C), int(nB), int(L), int(N1), _p(out), _s())
+    _lib.call("sam6d_transpose_tokens_bf16", src, src.shape[1], int(col0), int(C), int(nB), int(L), int(N1), out)
     return out
 
 
-def linattn_kv_raw(k_ptr, k_ld, k_bs, v_ptr, v_ld, v_bs, B, H, J, KV: Tensor, KS: Tensor):
-    _lib.call("sam6d_linattn_kv", ctypes.c_void_p(k_ptr), _ll(k_ld), _ll(k_bs), ctypes.c_void_p(v_ptr), _ll(v_ld), _ll(v_bs),
-              int(B), int(H), int(J), _p(KV), _p(KS), _s())
+def linattn_kv(k: Tensor, v: Tensor, KV: Tensor, KS: Tensor):
+    """kv-first branch of LinearAttention: focused keys k and values v ((B,J,H*64) f32 row views) -> KV (B,H,64,64), KS (B,H,64)"""
+    B, J, _ = k.shape
+    _, k_bs, k_ld = _rows(k)
+    _, v_bs, v_ld = _rows(v)
+    _lib.call("sam6d_linattn_kv", k, k_ld, k_bs, v, v_ld, v_bs, B, KV.shape[1], J, KV, KS)
 
 
-def linattn_apply_raw(q_ptr, q_rpb, q_bs, q_ld, KV: Tensor, KS: Tensor, B, H, x_ptr, x_bs, x_ld):
-    _lib.call("sam6d_linattn_apply", ctypes.c_void_p(q_ptr), _ll(q_rpb), _ll(q_bs), _ll(q_ld), _p(KV), _p(KS), int(B), int(H),
-              ctypes.c_void_p(x_ptr), _ll(x_bs), _ll(x_ld), _s())
+def linattn_apply(q: Tensor, KV: Tensor, KS: Tensor, out: Tensor):
+    """out[b,i,h] = (q'_h KV_h) / (q'_h . KS_h + 1e-6) for focused queries q and out (B,N,H*64) f32 row views"""
+    _, x_bs, x_ld = _rows(out)
+    _lib.call("sam6d_linattn_apply", q, *_rows(q), KV, KS, q.shape[0], KV.shape[1], out, x_bs, x_ld)
 
 
-# ---------------------------------------------------------------------------------------------- coarse pose
-def linattn_kv_pack_raw(k_ptr, k_ld, k_bs, v_ptr, v_ld, v_bs, B, J, device):
-    """focused keys / values ((B,J,256) fp32 views) -> (blob: B x 32 KB bf16 wgmma image of KV_h^T, KS (B,4,64) fp32)"""
-    blob = torch.empty(B, 4 * 64 * 64, dtype=torch.bfloat16, device=device)
-    KS = torch.empty(B, 4, 64, dtype=torch.float32, device=device)
-    _lib.call("sam6d_linattn_kv_pack", ctypes.c_void_p(k_ptr), _ll(k_ld), _ll(k_bs), ctypes.c_void_p(v_ptr), _ll(v_ld), _ll(v_bs),
-              int(B), int(J), _p(blob), _p(KS), _s())
+def linattn_kv_pack(k: Tensor, v: Tensor) -> Tuple[Tensor, Tensor]:
+    """focused keys / values ((B,J,256) fp32 row views) -> (blob: B x 32 KB bf16 wgmma image of KV_h^T, KS (B,4,64) fp32)"""
+    B, J, _ = k.shape
+    _, k_bs, k_ld = _rows(k)
+    _, v_bs, v_ld = _rows(v)
+    blob = torch.empty(B, 4 * 64 * 64, dtype=torch.bfloat16, device=k.device)
+    KS = torch.empty(B, 4, 64, dtype=torch.float32, device=k.device)
+    _lib.call("sam6d_linattn_kv_pack", k, k_ld, k_bs, v, v_ld, v_bs, B, J, blob, KS)
     return blob, KS
 
 
-def linattn_tc_raw(q_ptr, q_ld, q_bs, blob: Tensor, KS: Tensor, sp_scale: Tensor, B, rpb, x_ptr, x_ld, x_bs):
-    """dense tokens (bf16): focusing feature map + per-head (q' KV) / (q' . ksum) on wgmma"""
-    _lib.call("sam6d_linattn_tc", ctypes.c_void_p(q_ptr), _ll(q_ld), _ll(q_bs), _p(blob), _p(KS), _p(sp_scale), int(B), int(rpb),
-              ctypes.c_void_p(x_ptr), _ll(x_ld), _ll(x_bs), _s())
+def linattn_tc(q: Tensor, blob: Tensor, KS: Tensor, sp_scale: Tensor, out: Tensor):
+    """dense tokens (bf16 row views q, out (B,rows,256)): focusing feature map + per-head (q' KV) / (q' . ksum) on wgmma"""
+    B, rpb, _ = q.shape
+    _, q_bs, q_ld = _rows(q)
+    _, x_bs, x_ld = _rows(out)
+    _lib.call("sam6d_linattn_tc", q, q_ld, q_bs, blob, KS, sp_scale, B, rpb, out, x_ld, x_bs)
 
 
+# ---------------------------------------------------------------------------------------------- coarse pose
 def coarse_assign(A: Tensor) -> Tuple[Tensor, Tensor]:
     _check(A, torch.float32, "atten", 3)
     B, S, _ = A.shape
     n = S - 1
     W = torch.empty(B, n * n, dtype=torch.float32, device=A.device)
     w1 = torch.empty(B, n, dtype=torch.float32, device=A.device)
-    _lib.call("sam6d_coarse_assign", _p(A), B, S, _p(W), _p(w1), _s())
+    _lib.call("sam6d_coarse_assign", A, B, S, W, w1)
     return W, w1
 
 
@@ -665,7 +654,7 @@ def coarse_sample(W: Tensor, rand: Tensor) -> Tensor:
     B, L = W.shape
     nr = rand.shape[1]
     idx = torch.empty(B, nr, dtype=torch.int32, device=W.device)
-    _lib.call("sam6d_coarse_sample", _p(W), B, L, _p(rand), nr, _p(idx), _s())
+    _lib.call("sam6d_coarse_sample", W, B, L, rand, nr, idx)
     return idx
 
 
@@ -677,7 +666,7 @@ def coarse_hypotheses(idx: Tensor, pts1: Tensor, pts2: Tensor) -> Tuple[Tensor, 
     n1 = idx.shape[1] // 3
     Rt = torch.empty(B, n1, 12, dtype=torch.float32, device=idx.device)
     resid = torch.empty(B, n1, dtype=torch.float32, device=idx.device)
-    _lib.call("sam6d_coarse_hypotheses", _p(idx), _p(pts1), _p(pts2), B, n, n1, _p(Rt), _p(resid), _s())
+    _lib.call("sam6d_coarse_hypotheses", idx, pts1, pts2, B, n, n1, Rt, resid)
     return Rt, resid
 
 
@@ -685,7 +674,7 @@ def topk_smallest(v: Tensor, k: int) -> Tensor:
     _check(v, torch.float32, "v", 2)
     B, n = v.shape
     out = torch.empty(B, k, dtype=torch.int32, device=v.device)
-    _lib.call("sam6d_topk_smallest", _p(v), B, n, int(k), _p(out), _s())
+    _lib.call("sam6d_topk_smallest", v, B, n, int(k), out)
     return out
 
 
@@ -699,8 +688,7 @@ def coarse_select(Rt: Tensor, top: Tensor, pts1: Tensor, w1: Tensor, model: Tens
     scores = torch.empty(B, n2, dtype=torch.float32, device=Rt.device)
     R = torch.empty(B, 3, 3, dtype=torch.float32, device=Rt.device)
     t = torch.empty(B, 3, dtype=torch.float32, device=Rt.device)
-    _lib.call("sam6d_coarse_select", _p(Rt), _p(top), B, n1, n2, _p(pts1), _p(w1), n, _p(model), model.shape[1], _p(scores),
-              _p(R), _p(t), _s())
+    _lib.call("sam6d_coarse_select", Rt, top, B, n1, n2, pts1, w1, n, model, model.shape[1], scores, R, t)
     return R, t, scores
 
 
@@ -712,8 +700,7 @@ def pe_mlp_max(pts: Tensor, idx: Tensor, cnt: Tensor, weights, out: Tensor, out_
     B, N, _ = pts.shape
     ns = idx.shape[2]
     W1, B1, W2, B2, W3, B3 = weights
-    _lib.call("sam6d_pe_mlp_max", _p(pts), _p(idx), _p(cnt), B, N, ns, _p(W1), _p(B1), _p(W2), _p(B2), _p(W3), _p(B3),
-              _p(out), out.shape[-1], int(out_off), _s())
+    _lib.call("sam6d_pe_mlp_max", pts, idx, cnt, B, N, ns, W1, B1, W2, B2, W3, B3, out, out.shape[-1], int(out_off))
 
 
 def pe_mlp_max_tc(pts: Tensor, idx: Tensor, weights, out: Tensor, out_off: int):
@@ -727,8 +714,8 @@ def pe_mlp_max_tc(pts: Tensor, idx: Tensor, weights, out: Tensor, out_off: int):
     _check(W3, torch.bfloat16, "W3", 2)
     if out.dtype not in (torch.float32, torch.bfloat16):
         raise RuntimeError("pe_mlp_max_tc: out must be float32 or bfloat16")
-    _lib.call("sam6d_pe_mlp_max_tc", _p(pts), _p(idx), B, N, ns, _p(W1), _p(B1), _p(W2), _p(B2), _p(W3), _p(B3), _p(out),
-              int(out.dtype == torch.bfloat16), out.shape[-1], int(out_off), _s())
+    _lib.call("sam6d_pe_mlp_max_tc", pts, idx, B, N, ns, W1, B1, W2, B2, W3, B3, out, int(out.dtype == torch.bfloat16), out.shape[-1],
+              int(out_off))
 
 
 def fine_assign(A: Tensor, pts2: Tensor, shift: float):
@@ -756,8 +743,7 @@ def fine_assign(A: Tensor, pts2: Tensor, shift: float):
     lab2 = torch.zeros(B, S, dtype=torch.int32, device=dev)
     wts = torch.empty(B, S - 1, dtype=torch.float32, device=dev)
     pred = torch.empty(B, S - 1, 3, dtype=torch.float32, device=dev)
-    _lib.call("sam6d_fine_assign", _p(A), B, S, int(ld), _f(shift), _p(pts2), _p(rsum), _p(csum), _p(cpart), _p(cpi), _p(lab1),
-              _p(lab2), _p(wts), _p(pred), _s())
+    _lib.call("sam6d_fine_assign", A, B, S, int(ld), shift, pts2, rsum, csum, cpart, cpi, lab1, lab2, wts, pred)
     return lab1, lab2, wts, pred
 
 
@@ -780,13 +766,11 @@ def fine_assign_tc(f1n: Tensor, f2n: Tensor, pts2: Tensor, alpha: float):
     lab2 = torch.zeros(B, S, dtype=torch.int32, device=dev)
     wts = torch.empty(B, S - 1, dtype=torch.float32, device=dev)
     pred = torch.empty(B, S - 1, 3, dtype=torch.float32, device=dev)
-    a, sh = _f(alpha), _f(alpha)
-    _lib.call("sam6d_fine_pass_tc", _p(f1n), _p(f2n), B, S, a, sh, 0, None, None, ld, None, _p(rinv), None, None, None, _s())
-    _lib.call("sam6d_fine_pass_tc", _p(f2n), _p(f1n), B, S, a, sh, 0, None, None, ld, None, _p(cinv), None, None, None, _s())
-    _lib.call("sam6d_fine_pass_tc", _p(f2n), _p(f1n), B, S, a, sh, 1, _p(cinv), _p(rinv), ld, None, None, _p(lab2), None, None, _s())
-    _lib.call("sam6d_fine_masked_points", _p(lab2), _p(pts2), B, S, ld, _p(q4), _s())
-    _lib.call("sam6d_fine_pass_tc", _p(f1n), _p(f2n), B, S, a, sh, 2, _p(rinv), _p(cinv), ld, _p(q4), None, _p(lab1), _p(wts), _p(pred),
-              _s())
+    _lib.call("sam6d_fine_pass_tc", f1n, f2n, B, S, alpha, alpha, 0, None, None, ld, None, rinv, None, None, None)
+    _lib.call("sam6d_fine_pass_tc", f2n, f1n, B, S, alpha, alpha, 0, None, None, ld, None, cinv, None, None, None)
+    _lib.call("sam6d_fine_pass_tc", f2n, f1n, B, S, alpha, alpha, 1, cinv, rinv, ld, None, None, lab2, None, None)
+    _lib.call("sam6d_fine_masked_points", lab2, pts2, B, S, ld, q4)
+    _lib.call("sam6d_fine_pass_tc", f1n, f2n, B, S, alpha, alpha, 2, rinv, cinv, ld, q4, None, lab1, wts, pred)
     return lab1, lab2, wts, pred
 
 
@@ -797,7 +781,7 @@ def weighted_procrustes(src: Tensor, ref: Tensor, wts: Tensor, weight_thresh: fl
     B, N, _ = src.shape
     R = torch.empty(B, 3, 3, dtype=torch.float32, device=src.device)
     t = torch.empty(B, 3, dtype=torch.float32, device=src.device)
-    _lib.call("sam6d_weighted_procrustes", _p(src), _p(ref), _p(wts), B, N, _f(weight_thresh), _f(eps), _p(R), _p(t), _s())
+    _lib.call("sam6d_weighted_procrustes", src, ref, wts, B, N, weight_thresh, eps, R, t)
     return R, t
 
 
@@ -807,8 +791,7 @@ def pose_score(pts1: Tensor, lab1: Tensor, R: Tensor, t: Tensor, model: Tensor, 
     B, N, _ = pts1.shape
     score = torch.empty(B, dtype=torch.float32, device=pts1.device)
     ts = torch.empty(B, 3, dtype=torch.float32, device=pts1.device)
-    _lib.call("sam6d_pose_score", _p(pts1), _p(lab1), B, N, _p(R), _p(t), _p(model), model.shape[1], _f(dis_thres),
-              _p(radius), _p(score), _p(ts), _s())
+    _lib.call("sam6d_pose_score", pts1, lab1, B, N, R, t, model, model.shape[1], dis_thres, radius, score, ts)
     return score, ts
 
 
@@ -824,8 +807,8 @@ def attn_relpos(qkv: Tensor, nW: int, Hs: int, Ws: int, nH: int, rel_h: Tensor, 
     if T != nW * Hs * Ws or rel_h.shape[0] != 2 * Hs - 1 or rel_w.shape[0] != 2 * Ws - 1:
         raise RuntimeError("attn_relpos: shape mismatch")
     out = torch.empty(T, C, dtype=out_dtype, device=qkv.device)
-    _lib.call("sam6d_attn_relpos", _p(qkv), _ll(C3), int(nW), int(Hs), int(Ws), int(nH), C // nH, _p(rel_h), _p(rel_w), _f(scale),
-              _p(out), int(out_dtype == torch.bfloat16), _ll(C), _s())
+    _lib.call("sam6d_attn_relpos", qkv, C3, int(nW), int(Hs), int(Ws), int(nH), C // nH, rel_h, rel_w, scale, out,
+              int(out_dtype == torch.bfloat16), C)
     return out
 
 
@@ -841,8 +824,8 @@ def bilinear_gather(up: Tensor, choose: Tensor, G: int, sub: int, C: int, H: int
     if up.shape != (B, G * G, sub * sub * C):
         raise RuntimeError("bilinear_gather: shape mismatch")
     out = torch.empty(B, K, C, dtype=torch.float32, device=up.device)
-    _lib.call("sam6d_bilinear_gather", _p(up), int(up.dtype == torch.bfloat16), _p(choose), int(B), int(K), int(G), int(sub), int(C),
-              int(H), int(W), _p(out), _s())
+    _lib.call("sam6d_bilinear_gather", up, int(up.dtype == torch.bfloat16), choose, int(B), int(K), int(G), int(sub), int(C), int(H),
+              int(W), out)
     return out
 
 
@@ -865,8 +848,7 @@ def template_score(Qn: Tensor, Rn: Tensor, want_sim: bool = True, aggregation: s
     bo = torch.zeros(P, dtype=torch.int32, device=dev)
     bs = torch.zeros(P, dtype=torch.float32, device=dev)
     bt = torch.zeros(P, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_template_score_agg", _p(Qn), _p(Rn), P, O, T, C, TEMPLATE_AGGREGATIONS[aggregation], _p(sim), _p(obj), _p(obj_t),
-              _p(bo), _p(bs), _p(bt), _s())
+    _lib.call("sam6d_template_score_agg", Qn, Rn, P, O, T, C, TEMPLATE_AGGREGATIONS[aggregation], sim, obj, obj_t, bo, bs, bt)
     return sim, obj, bo, bs, bt
 
 
@@ -881,7 +863,7 @@ def mask_rle(masks: Tensor) -> Tuple[Tensor, Tensor]:
     col_cnt = torch.empty(n, W, dtype=torch.int32, device=dev)
     band_off = torch.empty(n, (W + 31) // 32, dtype=torch.int32, device=dev)
     rle_off = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_mask_rle_count", _p(masks), n, H, W, _p(col_cnt), _p(band_off), _p(rle_off), _s())
+    _lib.call("sam6d_mask_rle_count", masks, n, H, W, col_cnt, band_off, rle_off)
     rle_cum = torch.empty(int(rle_off[n]), dtype=torch.int32, device=dev)
-    _lib.call("sam6d_mask_rle_write", _p(masks), n, H, W, _p(col_cnt), _p(band_off), _p(rle_off), _p(rle_cum), _s())
+    _lib.call("sam6d_mask_rle_write", masks, n, H, W, col_cnt, band_off, rle_off, rle_cum)
     return rle_cum, rle_off

@@ -24,7 +24,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .render import _p, _stream
 
 MAX_NUM_SCENES = 10
 MAX_NUM_FRAMES = 1000
@@ -179,8 +178,7 @@ def crop_frames(frames: torch.Tensor, frame_idx: torch.Tensor, masks: torch.Tens
     rgb = torch.empty(R, 3, target, target, dtype=torch.float32, device=dev)
     pmask = torch.empty(R, target, target, dtype=torch.float32, device=dev)
     frames, frame_idx, masks = frames.contiguous(), frame_idx.contiguous(), masks.contiguous()
-    _lib.call("sam6d_pbr_reference_crops", _p(frames), F, H, W, _p(frame_idx), _p(masks), R, target, _p(boxes), _p(rgb), _p(pmask),
-              _stream())
+    _lib.call("sam6d_pbr_reference_crops", frames, F, H, W, frame_idx, masks, R, target, boxes, rgb, pmask)
     return boxes, rgb, pmask
 
 

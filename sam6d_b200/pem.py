@@ -45,21 +45,14 @@ class _W:
         self.bf16 = self.f32.to(torch.bfloat16).contiguous()
 
 
-def _gemm(prec, A, W: "_W", bias=None, residual=None, relu=False):
+def _gemm(prec, A, W: "_W", bias=None, residual=None, relu=False, out=None):
+    """A, residual and out are row views (ops.gemm)"""
     if prec == "bf16":
-        if A.dtype == torch.bfloat16 and residual is None and A.is_contiguous() and A.shape[1] % 64 == 0:
+        if A.dtype == torch.bfloat16 and residual is None and out is None and A.is_contiguous() and A.shape[1] % 64 == 0:
             # bf16 token matrix: the persistent TMA kernel (fp32 output); the register-staged kernel below is for fp32 operands
             return ops.gemm_tma(A, W.bf16, bias, act=1 if relu else 0)
-        return ops.gemm_tc(A, W.bf16, bias, residual=residual, relu=relu)
-    return ops.gemm(A, W.f32, bias, residual=residual, relu=relu)
-
-
-def _gemm_raw(prec, A_ptr, W: "_W", bias, R_ptr, C_ptr, M, N, K, lda, ldc, ldr=0, batch=1, sA=0, sC=0, sR=0):
-    if prec == "bf16":
-        ops.gemm_tc_raw(A_ptr, 0, W.bf16.data_ptr(), 1, bias, R_ptr, C_ptr, 0, M, N, K, lda, K, ldc, ldr, batch=batch, sA=sA, sW=0,
-                        sC=sC, sR=sR)
-    else:
-        ops.gemm_raw(A_ptr, W.f32.data_ptr(), bias, R_ptr, C_ptr, M, N, K, lda, K, ldc, ldr, batch=batch, sA=sA, sW=0, sC=sC, sR=sR)
+        return ops.gemm_tc(A, W.bf16, bias, residual=residual, out=out, relu=relu)
+    return ops.gemm(A, W.f32, bias, residual=residual, out=out, relu=relu)
 
 
 def _cfg(cfg, **defaults):
@@ -216,17 +209,15 @@ class GeometricTransformer(nn.Module):
             d = C // NUM_HEADS
             qkv = ops.gemm_tc(x2d, w["w_qkv"].bf16, w["b_qkv"], out_dtype=torch.bfloat16)          # (B*S, q|k|v) bf16
             u = ops.gemm_tc(x2d, w["w_u"].bf16, w["b_u"])                                            # (B*S, 4*C) fp32
-            sp = ops.rpe_scores(emb, None, u_ptr=u.data_ptr(), u_ld=NUM_HEADS * C)
+            sp = ops.rpe_scores(emb, u)
             vt = ops.transpose_tokens(qkv, 2 * C, C, B, S)
             hid = ops.attn_tc(qkv, 0, qkv, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), bias=sp)
             return _attn_tail(self.precision, x2d, hid, w["tail_self"]).view(B, S, C)
-        ld = 3 * C + NUM_HEADS * C
         qkvu = _gemm(self.precision, x2d, w["w_self"], w["b_self"])              # (B*S, q|k|v|u0..u3)
-        base, f = qkvu.data_ptr(), 4
-        sp = ops.rpe_scores(emb, None, u_ptr=base + 3 * C * f, u_ld=ld)          # (B,H,S,S)
+        sp = ops.rpe_scores(emb, qkvu[:, 3 * C:])                                  # (B,H,S,S)
         hid = torch.empty(B * S, C, dtype=torch.float32, device=x.device)
-        ops.mha_raw(base, ld, S * ld, base + C * f, ld, S * ld, base + 2 * C * f, ld, S * ld, sp, B, NUM_HEADS, S, S,
-                    1.0 / math.sqrt(C // NUM_HEADS), hid.data_ptr(), C, S * C)
+        qkv = qkvu.view(B, S, -1)
+        ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:3 * C], sp, 1.0 / math.sqrt(C // NUM_HEADS), hid.view(B, S, C))
         return _attn_tail(self.precision, x2d, hid, w["tail_self"]).view(B, S, C)
 
     def _cross_layer(self, x: torch.Tensor, mem: torch.Tensor, w) -> torch.Tensor:
@@ -241,10 +232,9 @@ class GeometricTransformer(nn.Module):
             hid = ops.attn_tc(q, 0, kv, 0, vt, B, NUM_HEADS, S, Sm, d, 1.0 / math.sqrt(d))
             return _attn_tail(self.precision, x2d, hid, w["tail_cross"]).view(B, S, C)
         q = _gemm(self.precision, x2d, w["wq_c"], w["bq_c"])
-        kv = _gemm(self.precision, mem.reshape(B * Sm, C), w["wkv_c"], w["bkv_c"])
+        kv = _gemm(self.precision, mem.reshape(B * Sm, C), w["wkv_c"], w["bkv_c"]).view(B, Sm, 2 * C)
         hid = torch.empty(B * S, C, dtype=torch.float32, device=x.device)
-        ops.mha_raw(q.data_ptr(), C, S * C, kv.data_ptr(), 2 * C, Sm * 2 * C, kv.data_ptr() + C * 4, 2 * C, Sm * 2 * C, None,
-                    B, NUM_HEADS, S, Sm, 1.0 / math.sqrt(C // NUM_HEADS), hid.data_ptr(), C, S * C)
+        ops.mha(q.view(B, S, C), kv[..., :C], kv[..., C:], None, 1.0 / math.sqrt(C // NUM_HEADS), hid.view(B, S, C))
         return _attn_tail(self.precision, x2d, hid, w["tail_cross"]).view(B, S, C)
 
     # ---- bf16 token stream (precision="bf16", both clouds in one allocation): every Linear is the persistent TMA GEMM, the
@@ -263,7 +253,7 @@ class GeometricTransformer(nn.Module):
             return _tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
         qk, vt = ops.gemm_tma_vt(x2d, w["w_qkv"].bf16, w["b_qkv"], 2 * C, S)                        # (B*S, q|k) and V^T
         u = ops.gemm_tma(x2d, w["w_u"].bf16, w["b_u"])                                              # (B*S, 4*C) fp32
-        sp = ops.rpe_scores(emb, None, u_ptr=u.data_ptr(), u_ld=NUM_HEADS * C)
+        sp = ops.rpe_scores(emb, u)
         hid = ops.attn_tc(qk, 0, qk, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), bias=sp, out_dtype=torch.bfloat16)
         return _tail_bf16(x2d, hid, w["tail_self"]).view(B, S, C)
 
@@ -407,12 +397,11 @@ def compute_feature_similarity(feat1, feat2, type='cosine', temp=1.0, normalize_
         # normalised bf16 tokens -> persistent TMA GEMM over all proposals (tiles that run past a proposal's rows are masked)
         f1 = ops.l2norm_rows_bf16(feat1.contiguous()) if normalize_feat else feat1.contiguous().to(torch.bfloat16)
         f2 = ops.l2norm_rows_bf16(feat2.contiguous()) if normalize_feat else feat2.contiguous().to(torch.bfloat16)
-        ops.gemm_tma_batched(f1, f2, store, N, M, ld, N * ld, alpha=1.0 / temp)
+        ops.gemm_tma_batched(f1, f2, store[:, :, :M], alpha=1.0 / temp)
     else:
         f1 = ops.l2norm_rows(feat1.contiguous()) if normalize_feat else feat1.contiguous()
         f2 = ops.l2norm_rows(feat2.contiguous()) if normalize_feat else feat2.contiguous()
-        ops.gemm_raw(f1.data_ptr(), f2.data_ptr(), None, 0, store.data_ptr(), N, M, C, C, C, ld, 0, batch=B, sA=N * C, sW=M * C,
-                     sC=N * ld, alpha=1.0 / temp)
+        ops.gemm(f1, f2, out=store[:, :, :M], alpha=1.0 / temp)
     return store[:, :, :M]                     # (B,N,M) like the reference; dense rows, row stride ld
 
 
@@ -488,13 +477,11 @@ class CoarsePointMatching(nn.Module):
         if self.precision == "bf16":                          # the sparse token stream is bf16 in this mode
             out = torch.empty(B, n + 1, H, dtype=torch.bfloat16, device=f.device)
             out[:, 0, :] = self.bg_token.detach().reshape(1, -1).to(torch.bfloat16)
-            ops.gemm_tc_raw(f.data_ptr(), 0, w["w_in"].bf16.data_ptr(), 1, w["b_in"], 0, out.data_ptr() + H * 2, 1, n, H, C, C, C, H, 0,
-                            batch=B, sA=n * C, sW=0, sC=(n + 1) * H)
+            ops.gemm_tc(f, w["w_in"].bf16, w["b_in"], out=out[:, 1:, :])
             return out
         out = torch.empty(B, n + 1, H, dtype=torch.float32, device=f.device)
         out[:, 0, :] = self.bg_token.detach().reshape(1, -1)
-        _gemm_raw(self.precision, f.data_ptr(), w["w_in"], w["b_in"], 0, out.data_ptr() + H * 4, n, H, C, C, H, 0, batch=B,
-                  sA=n * C, sC=(n + 1) * H)
+        _gemm(self.precision, f, w["w_in"], w["b_in"], out=out[:, 1:, :])
         return out
 
     @torch.no_grad()
@@ -691,13 +678,12 @@ class SparseToDenseTransformer(nn.Module):
         x2d = dense.view(B * N1, C)
         q = ops.gemm_tma(x2d, w["wq"].bf16, w["bq"], out_dtype=bf)
         kv = torch.empty(B * J, 2 * C, dtype=torch.float32, device=dev)
-        s_bf = sparse.dtype == torch.bfloat16
-        ops.gemm_tc_raw(sparse.data_ptr() + C * (2 if s_bf else 4), int(s_bf), w["wkv"].bf16.data_ptr(), 1, w["bkv"], 0, kv.data_ptr(), 0,
-                        J, 2 * C, C, C, C, 2 * C, 0, batch=B, sA=(J + 1) * C, sW=0, sC=J * 2 * C)
-        ops.focus_rows_raw(kv.data_ptr(), (B * J, 0, 2 * C), kv.data_ptr(), (B * J, 0, 2 * C), w["sp_scale"], B * J, C)
-        blob, KS = ops.linattn_kv_pack_raw(kv.data_ptr(), 2 * C, J * 2 * C, kv.data_ptr() + C * 4, 2 * C, J * 2 * C, B, J, dev)
+        ops.gemm_tc(sparse[:, 1:, :], w["wkv"].bf16, w["bkv"], out=kv.view(B, J, 2 * C))
+        ops.focus_rows(kv[:, :C], w["sp_scale"], out=kv[:, :C])
+        kv3 = kv.view(B, J, 2 * C)
+        blob, KS = ops.linattn_kv_pack(kv3[..., :C], kv3[..., C:])
         x_att = torch.empty(B * N1, C, dtype=bf, device=dev)
-        ops.linattn_tc_raw(q.data_ptr() + C * 2, C, N1 * C, blob, KS, w["sp_scale"], B, N, x_att.data_ptr() + C * 2, C, N1 * C)
+        ops.linattn_tc(q.view(B, N1, C)[:, 1:, :], blob, KS, w["sp_scale"], x_att.view(B, N1, C)[:, 1:, :])
         x_att.view(B, N1, C)[:, 0, :] = 0                                   # bg rows: defined input for the tail below
         out = _tail_bf16(x2d, x_att, w["tail"]).view(B, N1, C)
         out[:, 0, :] = sparse[:, 0, :].to(bf)                               # replaced bg token (transformer.py:660-668)
@@ -707,31 +693,29 @@ class SparseToDenseTransformer(nn.Module):
         """LinearTransformerLayer on dense[:,1:,:] with memory sparse[:,1:,:]; returns the new (B,N+1,C) sequence."""
         B, N1, C = dense.shape
         N, J = N1 - 1, sparse.shape[1] - 1
-        f = 4
         dev = dense.device
-        x_ptr, x_view = dense.data_ptr() + C * f, (N, N1 * C, C)          # rows 1..N of every proposal
+        x = dense[:, 1:, :]                                                 # rows 1..N of every proposal
         q = torch.empty(B * N, C, dtype=torch.float32, device=dev)
         prec = self.precision
-        _gemm_raw(prec, x_ptr, w["wq"], w["bq"], 0, q.data_ptr(), N, C, C, C, C, 0, batch=B, sA=N1 * C, sC=N * C)
+        _gemm(prec, x, w["wq"], w["bq"], out=q.view(B, N, C))
         kv = torch.empty(B * J, 2 * C, dtype=torch.float32, device=dev)
-        _gemm_raw(prec, sparse.data_ptr() + C * f, w["wkv"], w["bkv"], 0, kv.data_ptr(), J, 2 * C, C, C, 2 * C, 0, batch=B,
-                  sA=(J + 1) * C, sC=J * 2 * C)
-        ops.focus_rows_raw(q.data_ptr(), (B * N, 0, C), q.data_ptr(), (B * N, 0, C), w["sp_scale"], B * N, C)
-        ops.focus_rows_raw(kv.data_ptr(), (B * J, 0, 2 * C), kv.data_ptr(), (B * J, 0, 2 * C), w["sp_scale"], B * J, C)
+        _gemm(prec, sparse[:, 1:, :], w["wkv"], w["bkv"], out=kv.view(B, J, 2 * C))
+        ops.focus_rows(q, w["sp_scale"], out=q)
+        ops.focus_rows(kv[:, :C], w["sp_scale"], out=kv[:, :C])
         KV = torch.empty(B, NUM_HEADS, 64, 64, dtype=torch.float32, device=dev)
         KS = torch.empty(B, NUM_HEADS, 64, dtype=torch.float32, device=dev)
-        ops.linattn_kv_raw(kv.data_ptr(), 2 * C, J * 2 * C, kv.data_ptr() + C * f, 2 * C, J * 2 * C, B, NUM_HEADS, J, KV, KS)
+        kv3 = kv.view(B, J, 2 * C)
+        ops.linattn_kv(kv3[..., :C], kv3[..., C:], KV, KS)
         x_att = torch.empty(B * N, C, dtype=torch.float32, device=dev)
-        ops.linattn_apply_raw(q.data_ptr(), N, N * C, C, KV, KS, B, NUM_HEADS, x_att.data_ptr(), N * C, C)
+        ops.linattn_apply(q.view(B, N, C), KV, KS, x_att.view(B, N, C))
         t = w["tail"]
         y = torch.empty(B * N, C, dtype=torch.float32, device=dev)
-        _gemm_raw(prec, x_att.data_ptr(), t["wo"], t["bo"], x_ptr, y.data_ptr(), N, C, C, C, C, C, batch=B, sA=N * C, sC=N * C,
-                  sR=N1 * C)
+        _gemm(prec, x_att.view(B, N, C), t["wo"], t["bo"], residual=x, out=y.view(B, N, C))
         y = ops.layernorm(y, t["g1"], t["b1"])
         h = _gemm(prec, y, t["we"], t["be"], relu=True)
         z = _gemm(prec, h, t["ws"], t["bs"], residual=y)
         out = torch.empty(B, N1, C, dtype=torch.float32, device=dev)
-        ops.layernorm_raw(z.data_ptr(), (B * N, 0, C), out.data_ptr() + C * f, (N, N1 * C, C), t["g2"], t["b2"], B * N, C)
+        ops.layernorm(z, t["g2"], t["b2"], out=out[:, 1:, :])
         out[:, 0, :] = sparse[:, 0, :]                                      # replaced bg token (transformer.py:660-668)
         return out
 
@@ -801,14 +785,12 @@ class FinePointMatching(nn.Module):
                 tmp = ops.gemm_tc(f2d, w["w_in"].bf16, w["b_in"], out_dtype=torch.bfloat16)
             out = torch.empty(B, N + 1, H, dtype=torch.bfloat16, device=f.device)
             out[:, 0, :] = self.bg_token.detach().reshape(1, -1).to(torch.bfloat16)
-            ops.gemm_tma_batched(local, pw["w3"].bf16, out[:, 1:, :], N, H, H, (N + 1) * H, bias=pw["b3"],
-                                 residual=tmp.view(B, N, H), ldr=H, r_bs=N * H)
+            ops.gemm_tma_batched(local, pw["w3"].bf16, out[:, 1:, :], bias=pw["b3"], residual=tmp.view(B, N, H))
             return out
         tmp = _gemm(self.precision, f.reshape(B * N, C), w["w_in"], w["b_in"])
         out = torch.empty(B, N + 1, H, dtype=torch.float32, device=f.device)
         out[:, 0, :] = self.bg_token.detach().reshape(1, -1)
-        _gemm_raw(self.precision, local.data_ptr(), pw["w3"], pw["b3"], tmp.data_ptr(), out.data_ptr() + H * 4, N, H, 256, 256, H, H,
-                  batch=B, sA=N * 256, sC=(N + 1) * H, sR=N * H)
+        _gemm(self.precision, local, pw["w3"], pw["b3"], residual=tmp.view(B, N, H), out=out[:, 1:, :])
         return out
 
     @torch.no_grad()

@@ -8,7 +8,6 @@ The rasteriser's visibility is exact (fixed-point edge functions, top-left rule,
 face id), so oracle/render_oracle.py reproduces it bit for bit.  Shading is a documented stand-in for Cycles: albedo (vertex
 colour, bilinear texture or base colour) x (ambient + (1 - ambient) max(0, n.l)) with a point light at 2.5x the camera
 position (render_custom_templates.py:68-72), no shadows, no BSDF."""
-import ctypes
 import math
 from typing import Sequence
 
@@ -21,14 +20,6 @@ from .meshio import Mesh
 # the (O*T*H*W) u64 visibility buffer of one rasteriser call stays within this many bytes; more objects are rendered in chunks
 VIS_BUDGET_BYTES = 1 << 30
 BIG_LIST_CAP = 1 << 20
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _icosphere_level0():
@@ -304,8 +295,7 @@ def _render_chunk(meshes, poses, K, H, W, ambient, base, znear, out):
     big_cap = min(T * f0, BIG_LIST_CAP)
     big = torch.empty(max(big_cap, 1), 2, dtype=torch.int32, device=dev)
     counters = torch.empty(O + 1, dtype=torch.int32, device=dev)
-    _lib.call("sam6d_render_meshes", _p(verts), _p(faces), _p(info_d), O, v0, f0, _p(cols), _p(uvs), _p(texs), _p(tex_off_d), _p(base_d),
-              _p(poses), T, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), H, W, float(znear), float(ambient),
-              _p(vrec), _p(vis), _p(big), big_cap, _p(counters), _p(out["rgb"]), _p(out["mask"]), _p(out["xyz"]), _p(out["tri"]),
-              _p(out["depth"]), _stream())
+    _lib.call("sam6d_render_meshes", verts, faces, info_d, O, v0, f0, cols, uvs, texs, tex_off_d, base_d, poses, T, float(K[0, 0]),
+              float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), H, W, float(znear), float(ambient), vrec, vis, big, big_cap, counters,
+              out["rgb"], out["mask"], out["xyz"], out["tri"], out["depth"])
     out["dropped"].copy_(counters[1:])

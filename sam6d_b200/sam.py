@@ -187,12 +187,8 @@ class ImageEncoderViT(nn.Module):
         tok = torch.empty(B * L, C, dtype=torch.float32, device=x.device)
         if w["pos"] is not None:
             Wm = w["pe_w"]
-            if prec == "bf16":
-                ops.gemm_tc_raw(patches.data_ptr(), 0, Wm.bf16.data_ptr(), 1, w["pe_b"], w["pos"].data_ptr(), tok.data_ptr(), 0, L, C,
-                                Cin * P * P, Cin * P * P, Cin * P * P, C, C, batch=B, sA=L * Cin * P * P, sW=0, sC=L * C, sR=0)
-            else:
-                ops.gemm_raw(patches.data_ptr(), Wm.f32.data_ptr(), w["pe_b"], w["pos"].data_ptr(), tok.data_ptr(), L, C, Cin * P * P,
-                             Cin * P * P, Cin * P * P, C, C, batch=B, sA=L * Cin * P * P, sW=0, sC=L * C, sR=0)
+            gemm, pe_w = (ops.gemm_tc, Wm.bf16) if prec == "bf16" else (ops.gemm, Wm.f32)
+            gemm(patches.view(B, L, -1), pe_w, w["pe_b"], residual=w["pos"].expand(B, L, C), out=tok.view(B, L, C))
         else:
             tok = _gemm(prec, patches, w["pe_w"], w["pe_b"])
         ws = max((b.window_size for b in self.blocks), default=0) or 14

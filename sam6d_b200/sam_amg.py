@@ -20,7 +20,6 @@ post-processing.  Three algebraic savings over the reference's formulation, all 
   * `Sam.postprocess_masks` (256 -> 1024 bilinear, crop, -> frame size bilinear) is evaluated per output pixel inside the statistics
     kernel: the (64, 3, 1024, 1024) and (64, 3, H, W) logit tensors never exist; only kept masks are materialised (binary).
 The reference's RLE encode / decode round trip inside `_generate_masks` is the identity and is skipped."""
-import ctypes
 import math
 import os
 from typing import Any, Dict, Optional, Tuple
@@ -33,14 +32,6 @@ from . import _lib, ops
 from .pem import _W, _f32, _Packed, _param_key
 
 bf = torch.bfloat16
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 class LayerNorm2d(nn.Module):
@@ -60,7 +51,7 @@ def _pe_encode(coords01: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
     c = coords01.float().contiguous()
     g = G.float().contiguous()                           # named: must outlive the launch
     out = torch.empty(c.shape[0], 256, dtype=torch.float32, device=c.device)
-    _lib.call("sam6d_sam_pe_encode", _p(c), _p(g), c.shape[0], _p(out), _s())
+    _lib.call("sam6d_sam_pe_encode", c, g, c.shape[0], out)
     return out
 
 
@@ -125,7 +116,7 @@ class PromptEncoder(nn.Module):
         m = masks.to(device=self.no_mask_embed.weight.device, dtype=torch.float32).contiguous()
         prm = self._mask_params()
         rows = torch.empty(B, h * w, self.embed_dim, dtype=torch.float32, device=m.device)
-        _lib.call("sam6d_sam_mask_embed", _p(m), _p(prm), B, _p(rows), _s())
+        _lib.call("sam6d_sam_mask_embed", m, prm, B, rows)
         return rows.view(B, h, w, self.embed_dim).permute(0, 3, 1, 2)
 
     @torch.no_grad()
@@ -300,7 +291,7 @@ class MaskDecoder(nn.Module):
         src_bf = src.to(bf).view(B * L, 256)
         srcpe_bf = (src + pe_rows).to(bf).view(B * L, 256)
         del src
-        f = dict(L=L, src0_bf=src_bf, src_bs=L * 256, kv_bs=L * 128)
+        f = dict(L=L, src0_bf=src_bf, kv_bs=L * 128)
         a = w["t2i0"]
         f["K0"] = ops.gemm_tma(srcpe_bf, a["k"].bf16, a["kb"], out_dtype=bf)
         f["V0"] = ops.gemm_tma(src_bf, a["v"].bf16, a["vb"], out_dtype=bf)
@@ -311,7 +302,7 @@ class MaskDecoder(nn.Module):
     def _img_proj(self, keys_bf, W, b, pe_term, B, L):
         """proj(keys + pe) = keys W^T + b + (pe W^T): (B,L,256) bf16 -> (B,L,128) bf16, the pe term as a residual shared by all prompts"""
         out = torch.empty(B, L, 128, dtype=bf, device=keys_bf.device)
-        return ops.gemm_tma_batched(keys_bf, W, out, L, 128, 128, L * 128, bias=b, residual=pe_term, ldr=128, r_bs=0)
+        return ops.gemm_tma_batched(keys_bf, W, out, bias=b, residual=pe_term.expand(B, L, 128))
 
     @staticmethod
     def _shared_dense(dense) -> bool:
@@ -333,10 +324,10 @@ class MaskDecoder(nn.Module):
         pe_rows = image_pe[0].reshape(256, -1).t().contiguous() if image_pe.dim() == 4 else image_pe
         if self._shared_dense(dense_prompt_embeddings):
             f = self._frame_terms(image_embeddings, pe_rows, dense_prompt_embeddings[0, :, 0, 0])
-            kv_bs0, src_bs0 = 0, 0
+            kv_bs0 = 0
         else:
             f = self._prompt_terms(image_embeddings, pe_rows, dense_prompt_embeddings)
-            kv_bs0, src_bs0 = f["kv_bs"], f["src_bs"]
+            kv_bs0 = f["kv_bs"]
         L = f["L"]
         out_tokens = torch.cat([self.iou_token.weight, self.mask_tokens.weight], dim=0)
         tokens = torch.cat((out_tokens.unsqueeze(0).expand(B, -1, -1), sparse_prompt_embeddings), dim=1).float().contiguous()   # (B,T,256)
@@ -345,19 +336,19 @@ class MaskDecoder(nn.Module):
         def self_attn(a, q_in, k_in, v_in):
             q, k, v = _lin(q_in, a.q_proj), _lin(k_in, a.k_proj), _lin(v_in, a.v_proj)
             o = torch.empty_like(q)
-            _lib.call("sam6d_sam_self_attn", _p(q), _p(k), _p(v), B, T, _p(o), _s())
+            _lib.call("sam6d_sam_self_attn", q, k, v, B, T, o)
             return o
 
         def tok2img(a, aw, q_in, K, V, kv_bs):
             q = _lin(q_in, a.q_proj)                                             # (B*T,128)
             o = torch.empty_like(q)
-            _lib.call("sam6d_sam_tok2img_attn", _p(q), _p(K), _p(V), ctypes.c_longlong(kv_bs), B, T, L, _p(o), _s())
+            _lib.call("sam6d_sam_tok2img_attn", q, K, V, kv_bs, B, T, L, o)
             return o
 
         def img2tok(a, Qimg, q_bs, k_in, v_in):
             kt, vt = _lin(k_in, a.k_proj), _lin(v_in, a.v_proj)                 # (B*T,128)
             o = torch.empty(B, L, 128, dtype=bf, device=dev)
-            _lib.call("sam6d_sam_img2tok_attn", _p(Qimg), ctypes.c_longlong(q_bs), _p(kt), _p(vt), B, T, L, _p(o), _s())
+            _lib.call("sam6d_sam_img2tok_attn", Qimg, q_bs, kt, vt, B, T, L, o)
             return o
 
         # ---- block 0 (skip_first_layer_pe) ----------------------------------------------------------------------------------
@@ -368,7 +359,7 @@ class MaskDecoder(nn.Module):
         q = _ln(_lin(_lin(q, l0.mlp.lin1, relu=True), l0.mlp.lin2, residual=q), l0.norm3)
         a = img2tok(l0.cross_attn_image_to_token, f["Q0"], kv_bs0, q + tok2, q)
         keys = torch.empty(B, L, 256, dtype=bf, device=dev)
-        ops.gemm_tma_batched(a, w["i2t0"]["o"].bf16, keys, L, 256, 256, L * 256, bias=w["i2t0"]["ob"], residual=f["src0_bf"], ldr=256, r_bs=src_bs0)
+        ops.gemm_tma_batched(a, w["i2t0"]["o"].bf16, keys, bias=w["i2t0"]["ob"], residual=f["src0_bf"].view(-1, L, 256).expand(B, L, 256))
         keys = ops.layernorm_bf16io(keys.view(B * L, 256), _f32(l0.norm4.weight), _f32(l0.norm4.bias), eps=l0.norm4.eps).view(B, L, 256)
         # ---- block 1 -----------------------------------------------------------------------------------------------------------
         qp = q + tok2
@@ -392,12 +383,12 @@ class MaskDecoder(nn.Module):
         G = int(math.isqrt(L))
         u1 = ops.gemm_tma(keys.view(B * L, 256), w["ct1"].bf16, w["ct1b"], out_dtype=bf)                   # (B*L, 4*64): cols (i,j,o)
         u1n = torch.empty_like(u1)
-        _lib.call("sam6d_sam_ln2d_gelu", _p(u1), _p(w["ln2w"]), _p(w["ln2b"]), ctypes.c_longlong(B * L * 4), _p(u1n), _s())
+        _lib.call("sam6d_sam_ln2d_gelu", u1, w["ln2w"], w["ln2b"], B * L * 4, u1n)
         u2 = ops.gemm_tma(u1n.view(B * L * 4, 64), w["ct2"].bf16, w["ct2b"], act=2, out_dtype=bf)          # (B*L*4, 4*32), GELU'd
         hyper = torch.stack([self._mlp(self.output_hypernetworks_mlps[i], hs[:, 1 + i, :]) for i in range(self.num_mask_tokens)], dim=1).contiguous()
         m0, nm = (1, 3) if multimask_output else (0, 1)                                    # MaskDecoder.forward's mask_slice
         masks = torch.empty(B, nm, 4 * G, 4 * G, dtype=torch.float32, device=dev)
-        _lib.call("sam6d_sam_mask_dot_range", _p(u2), _p(hyper), B, G, m0, nm, _p(masks), _s())
+        _lib.call("sam6d_sam_mask_dot_range", u2, hyper, B, G, m0, nm, masks)
         iou = self._mlp(self.iou_prediction_head, hs[:, 0, :])
         return masks, iou[:, m0:m0 + nm].contiguous()
 
@@ -443,8 +434,7 @@ class Sam(nn.Module):
         H, W = int(original_size[0]), int(original_size[1])
         low = masks.float().contiguous()
         out = torch.empty(B, C, H, W, dtype=torch.float32, device=low.device)
-        _lib.call("sam6d_sam_mask_upscale", _p(low), B * C, S, self.image_encoder.img_size, int(input_size[0]), int(input_size[1]), H, W,
-                  _p(out), _s())
+        _lib.call("sam6d_sam_mask_upscale", low, B * C, S, self.image_encoder.img_size, int(input_size[0]), int(input_size[1]), H, W, out)
         return out
 
     def binarize_masks(self, masks: torch.Tensor, input_size: Tuple[int, ...], original_size: Tuple[int, ...]) -> torch.Tensor:
@@ -454,8 +444,8 @@ class Sam(nn.Module):
         low = masks.float().contiguous()
         sel = torch.arange(B * C, dtype=torch.int32, device=low.device)
         out = torch.empty(B, C, H, W, dtype=torch.uint8, device=low.device)
-        _lib.call("sam6d_sam_mask_binarize", _p(low), _p(sel), B * C, S, self.image_encoder.img_size, int(input_size[0]), int(input_size[1]),
-                  H, W, ctypes.c_float(self.mask_threshold), _p(out), _s())
+        _lib.call("sam6d_sam_mask_binarize", low, sel, B * C, S, self.image_encoder.img_size, int(input_size[0]), int(input_size[1]), H, W,
+                  self.mask_threshold, out)
         return out.view(torch.bool)
 
 
@@ -703,8 +693,8 @@ class CustomSamAutomaticMaskGenerator:
         n = low.shape[0] * 3
         low = low.view(n, low.shape[-2], low.shape[-1])
         stats = torch.empty(n, 8, dtype=torch.int32, device=dev)
-        _lib.call("sam6d_sam_mask_stats", _p(low), n, low.shape[-1], self.sam.image_encoder.img_size, nh, nw, H, W,
-                  ctypes.c_float(self.sam.mask_threshold), ctypes.c_float(self.stability_score_offset), _p(stats), _s())
+        _lib.call("sam6d_sam_mask_stats", low, n, low.shape[-1], self.sam.image_encoder.img_size, nh, nw, H, W, self.sam.mask_threshold,
+                  self.stability_score_offset, stats)
         iou_f = iou.reshape(-1)
         st = stats.cpu()
         iou_h = iou_f.cpu()
@@ -717,8 +707,8 @@ class CustomSamAutomaticMaskGenerator:
         masks = torch.empty(len(sel), H, W, dtype=torch.uint8, device=dev)
         if len(sel):
             sel_d = sel.to(device=dev, dtype=torch.int32)
-            _lib.call("sam6d_sam_mask_binarize", _p(low), _p(sel_d), len(sel), low.shape[-1], self.sam.image_encoder.img_size, nh, nw, H, W,
-                      ctypes.c_float(self.sam.mask_threshold), _p(masks), _s())
+            _lib.call("sam6d_sam_mask_binarize", low, sel_d, len(sel), low.shape[-1], self.sam.image_encoder.img_size, nh, nw, H, W,
+                      self.sam.mask_threshold, masks)
         return masks, boxes.to(dev), iou_f[sel.to(dev)], low, iou_f, stats
 
     @staticmethod
@@ -729,7 +719,7 @@ class CustomSamAutomaticMaskGenerator:
         order = torch.argsort(scores, descending=True, stable=True)
         b = boxes[order].float().contiguous()
         keep = torch.empty(b.shape[0], dtype=torch.uint8, device=b.device)
-        _lib.call("sam6d_sam_nms", _p(b), None, b.shape[0], ctypes.c_float(thr), _p(keep), _s())
+        _lib.call("sam6d_sam_nms", b, None, b.shape[0], thr, keep)
         return order[keep.bool()]
 
     @torch.no_grad()

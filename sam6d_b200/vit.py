@@ -111,9 +111,8 @@ class ViT(nn.Module):
         xn = ops.layernorm(tok, bw["n1w"], bw["n1b"], eps=bw["eps1"])
         qkv = ops.gemm(xn, bw["qkv"].f32, bw["qkv_b"])
         att = torch.empty(B * S, C, dtype=torch.float32, device=tok.device)
-        base, ld, f = qkv.data_ptr(), 3 * C, 4
-        ops.mha_raw(base, ld, S * ld, base + C * f, ld, S * ld, base + 2 * C * f, ld, S * ld, None, B, H, S, S, d ** -0.5,
-                    att.data_ptr(), C, S * C)
+        qkv = qkv.view(B, S, 3 * C)
+        ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], None, d ** -0.5, att.view(B, S, C))
         tok = ops.gemm(att, bw["proj"].f32, bw["proj_b"], residual=tok)
         xn = ops.layernorm(tok, bw["n2w"], bw["n2b"], eps=bw["eps2"])
         h = ops.gemm(xn, bw["f1"].f32, bw["f1b"], relu=_ACT_GELU)
@@ -136,12 +135,8 @@ class ViT(nn.Module):
         tok[:, 0, :] = w["cls"]                                      # cls_token + pos_embed[0]
         K = Cin * P * P
         # patch tokens = patches W^T + b + pos_embed[1:], written behind the cls row of every image
-        if self.precision == "bf16":
-            ops.gemm_tc_raw(patches.data_ptr(), 0, w["pe_w"].bf16.data_ptr(), 1, w["pe_b"], w["pos"].data_ptr(), tok.data_ptr() + C * 4, 0,
-                            L, C, K, K, K, C, C, batch=B, sA=L * K, sW=0, sC=S * C, sR=0)
-        else:
-            ops.gemm_raw(patches.data_ptr(), w["pe_w"].f32.data_ptr(), w["pe_b"], w["pos"].data_ptr(), tok.data_ptr() + C * 4, L, C, K,
-                         K, K, C, C, batch=B, sA=L * K, sW=0, sC=S * C, sR=0)
+        gemm, pe_w = (ops.gemm_tc, w["pe_w"].bf16) if self.precision == "bf16" else (ops.gemm, w["pe_w"].f32)
+        gemm(patches.view(B, L, K), pe_w, w["pe_b"], residual=w["pos"].expand(B, L, C), out=tok[:, 1:, :])
         tok = tok.view(B * S, C)
         d = self.depth
         n = d // 4

@@ -47,6 +47,14 @@ def test_ops_reject_cpu_tensors():
         ops.gemm(torch.zeros(2, 2), torch.zeros(2, 2))
 
 
+def test_call_rejects_cpu_tensor_arguments(libpath):
+    """every pointer of the C ABI is a device pointer: a host tensor is refused before the stream is read or anything launches"""
+    before = _lib.launch_count()
+    with pytest.raises(_lib.Sam6dError, match="device pointer"):
+        _lib.call("sam6d_cloud_radius", torch.zeros(1, 8, 3), 1, 8, None)
+    assert _lib.launch_count() == before
+
+
 def test_net_state_dict_layout_matches_reference_names():
     from oracle import pem_oracle as po
     from sam6d_b200.pem import Net

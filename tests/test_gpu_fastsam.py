@@ -115,14 +115,12 @@ def test_conv_edge_cases(case):
     _run_conv(**case)
 
 
-def test_sppf_kernel_matches_cascaded_pools():
+def test_sppf_kernel_matches_cascaded_pools_tensor_args():
     from sam6d_b200 import _lib
-    from sam6d_b200.fast_sam import _p, _s
-    import ctypes
     g = torch.Generator(device="cuda").manual_seed(3)
     buf = torch.zeros(2, 15, 20, 1280, device="cuda", dtype=torch.bfloat16)
     buf[..., :320] = torch.randn(2, 15, 20, 320, device="cuda", generator=g).to(torch.bfloat16)
-    _lib.call("sam6d_yolo_sppf", _p(buf), ctypes.c_longlong(1280), 2, 15, 20, 320, _s())
+    _lib.call("sam6d_yolo_sppf", buf, 1280, 2, 15, 20, 320)
     x = buf[..., :320].float().permute(0, 3, 1, 2)
     y1 = F.max_pool2d(x, 5, 1, 2); y2 = F.max_pool2d(y1, 5, 1, 2); y3 = F.max_pool2d(y2, 5, 1, 2)
     ref = torch.cat((y1, y2, y3), 1).permute(0, 2, 3, 1)
@@ -131,19 +129,16 @@ def test_sppf_kernel_matches_cascaded_pools():
 
 def _decode_all(head, sizes):
     """GPU decode of every anchor (threshold below any sigmoid) -> (A, 38) rows in anchor order"""
-    import ctypes
     from sam6d_b200 import _lib
-    from sam6d_b200.fast_sam import _p, _s
     B, A, _ = head.shape
     cand = torch.empty(B, A, 38, device="cuda")
     count = torch.empty(B, dtype=torch.int32, device="cuda")
-    _lib.call("sam6d_yolo_decode", _p(head), ctypes.c_longlong(head.stride(1)), ctypes.c_longlong(head.stride(0)), B,
-              *[v for hw in sizes for v in hw], ctypes.c_float(-1.0), _p(cand), _p(count), _s())
+    _lib.call("sam6d_yolo_decode", head, head.stride(1), head.stride(0), B, *[v for hw in sizes for v in hw], -1.0, cand, count)
     assert (count.cpu() == A).all()
     return cand
 
 
-def test_network_matches_oracle(sd, frames, oracle_out):
+def test_network_matches_oracle_tensor_args(sd, frames, oracle_out):
     """whole network, two frames in one batch, bf16 activations vs the fp32 oracle.  Error model: every layer rounds its output
     to bf16 once (relative u_bf16 = 2^-8 at most, ~2^-10 rms); about 60 such roundings lie on the longest path and the seeded
     layers neither amplify nor damp much (activations stay O(1)), so the errors add up like a random walk to ~sqrt(60) x 2^-10

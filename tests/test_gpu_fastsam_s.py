@@ -1,7 +1,6 @@
 """GPU: FastSAM-s (YOLOv8s-seg) on sm_90a.  The s network, post-processing and CLIs against the fp32 CPU restatement
 oracle/fastsam_oracle.py on seeded weights (synth.make_fastsam_state_dict(scale="s")); every convolution shape of s and the
 narrow-channel edge cases of its layers (Cout <= 64 in one 128-wide N tile) against fp64; the stem at 32 channels."""
-import ctypes
 import json
 import os
 
@@ -134,9 +133,8 @@ def test_conv_fp32_output_32_channels():
     assert ((y.double() - ref).abs() <= bound).all()
 
 
-def test_stem_32_channels_matches_fp64():
+def test_stem_32_channels_matches_fp64_tensor_args():
     from sam6d_b200 import _lib
-    from sam6d_b200.fast_sam import _p, _s
     g = torch.Generator().manual_seed(2)
     img = np.random.RandomState(3).randint(0, 256, (2, 33, 47, 3)).astype(np.uint8)    # odd sizes: the ceil(H/2) border
     w = torch.randn(32, 3, 3, 3, generator=g) * 0.5
@@ -144,7 +142,7 @@ def test_stem_32_channels_matches_fp64():
     out = torch.full((2, 17, 24, 32), 7.0, device="cuda", dtype=torch.bfloat16)
     frames = torch.from_numpy(img).cuda()
     w_dev, b_dev = w.permute(0, 2, 3, 1).contiguous().cuda(), b.cuda()          # (out, ky, kx, in); kept alive over the launch
-    _lib.call("sam6d_yolo_stem_c", _p(frames), 2, 33, 47, 32, _p(w_dev), _p(b_dev), _p(out), _s())
+    _lib.call("sam6d_yolo_stem_c", frames, 2, 33, 47, 32, w_dev, b_dev, out)
     torch.cuda.synchronize()
     x = torch.from_numpy(np.ascontiguousarray(img[..., ::-1])).double().permute(0, 3, 1, 2) / 255.0
     pre = F.conv2d(x, w.double(), b.double(), 2, 1)
@@ -156,15 +154,14 @@ def test_stem_32_channels_matches_fp64():
     assert (err <= bound).all(), f"worst err/bound {(err / bound).max().item():.3g}"
 
 
-def test_stem_rejects_bad_width():
+def test_stem_rejects_bad_width_tensor_args():
     from sam6d_b200 import _lib
-    from sam6d_b200.fast_sam import _p, _s
     img = torch.zeros(1, 4, 4, 3, dtype=torch.uint8, device="cuda")
     w, b = torch.zeros(40, 27, device="cuda"), torch.zeros(40, device="cuda")
     out = torch.zeros(1, 2, 2, 40, device="cuda", dtype=torch.bfloat16)
     for C in (40, 96):
         with pytest.raises(_lib.Sam6dError, match="invalid argument"):
-            _lib.call("sam6d_yolo_stem_c", _p(img), 1, 4, 4, C, _p(w), _p(b), _p(out), _s())
+            _lib.call("sam6d_yolo_stem_c", img, 1, 4, 4, C, w, b, out)
 
 
 def _decode_all(head, sizes):
@@ -172,9 +169,9 @@ def _decode_all(head, sizes):
     return d(head, sizes)
 
 
-def test_s_network_matches_oracle(sd, frames, oracle_out):
+def test_s_network_matches_oracle_tensor_args(sd, frames, oracle_out):
     """whole s network, two frames in one batch, bf16 activations vs the fp32 oracle; the error model of
-    test_gpu_fastsam.test_network_matches_oracle (s has fewer layers on its longest path than x): 5 % of the rms spread"""
+    test_gpu_fastsam.test_network_matches_oracle_tensor_args (s has fewer layers on its longest path than x): 5 % of the rms spread"""
     from oracle import fastsam_oracle as fo
     from sam6d_b200.fast_sam import YOLOv8Seg
     net = YOLOv8Seg("s").cuda().eval()

@@ -7,7 +7,6 @@ fp32 roundings.  A tensor-core (wgmma) fp32 accumulation is charged 2u per added
 than round.  CUDA's documented accuracy of the math functions used: __expf(x) 2 + floor(|1.173 x|) ulp, sinf / cosf / erff /
 rsqrtf 2 ulp, __logf 3 ulp (an ulp of a result in [1, 2) is 2u).  Each check prints its largest error / bound ratio; where a
 bound is loose enough to leave doubt, a deliberately wrong answer computed in torch must fail the same bound."""
-import ctypes
 import itertools
 import math
 import os
@@ -42,14 +41,6 @@ def ops(lib):
 
 def _g(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _ratio(err, bound):
@@ -88,7 +79,7 @@ def test_sam_mask_dot_every_subpixel(lib, B, G):
     hyper[:, 0] = float("nan")                   # mask token 0 (the single-mask output) must never reach the multimask slice
     up_d, hyper_d = up.cuda(), hyper.cuda()
     masks = torch.full((B, 3, 4 * G, 4 * G), float("nan"), device="cuda")
-    lib.call("sam6d_sam_mask_dot", _p(up_d), _p(hyper_d), B, G, _p(masks), _s())
+    lib.call("sam6d_sam_mask_dot", up_d, hyper_d, B, G, masks)
     got = masks.double()
     assert torch.isfinite(got).all(), "a pixel was not written or mask token 0 leaked in"
     # up rows (b, y, x, i, j), columns (i', j', o) -> pixel (4y + 2i + i', 4x + 2j + j')
@@ -179,7 +170,7 @@ def _run_tok2img(lib, B, T, L, shared, seed):
     K = torch.randn(Bk, L, 128, generator=g).bfloat16().cuda()
     V = torch.randn(Bk, L, 128, generator=g).bfloat16().cuda()
     out = torch.full((B, T, 128), float("nan"), device="cuda")
-    lib.call("sam6d_sam_tok2img_attn", _p(Q), _p(K), _p(V), ctypes.c_longlong(0 if shared else L * 128), B, T, L, _p(out), _s())
+    lib.call("sam6d_sam_tok2img_attn", Q, K, V, 0 if shared else L * 128, B, T, L, out)
     return out, _tok2img_ref(Q, K, V, B, T, L, shared)
 
 
@@ -199,7 +190,7 @@ def test_sam_tok2img_attn_smem_limit(lib):
     Q = torch.zeros(1, 8, 128, device="cuda")
     KV = torch.zeros(6401, 128, dtype=torch.bfloat16, device="cuda")
     with pytest.raises(lib.Sam6dError, match="invalid argument"):
-        lib.call("sam6d_sam_tok2img_attn", _p(Q), _p(KV), _p(KV), ctypes.c_longlong(0), 1, 8, 6401, _p(Q), _s())
+        lib.call("sam6d_sam_tok2img_attn", Q, KV, KV, 0, 1, 8, 6401, Q)
 
 
 @pytest.mark.parametrize("shared", [True, False])
@@ -214,7 +205,7 @@ def test_sam_img2tok_attn(lib, T, L, shared):
     Kt = (torch.randn(B, T, 128, generator=g) * 5).cuda()
     Vt = torch.randn(B, T, 128, generator=g).cuda()
     out = torch.full((B, L, 128), float("nan"), dtype=torch.bfloat16, device="cuda")
-    lib.call("sam6d_sam_img2tok_attn", _p(Q), ctypes.c_longlong(0 if shared else L * 128), _p(Kt), _p(Vt), B, T, L, _p(out), _s())
+    lib.call("sam6d_sam_img2tok_attn", Q, 0 if shared else L * 128, Kt, Vt, B, T, L, out)
     qh = Q.double().view(Bq, L, 8, 16).permute(0, 2, 1, 3)
     kh = Kt.double().view(B, T, 8, 16).permute(0, 2, 1, 3)
     vh = Vt.double().view(B, T, 8, 16).permute(0, 2, 1, 3)
@@ -235,7 +226,7 @@ def test_sam_self_attn(lib, B, T):
     g = _g(3000 + 10 * B + T)
     q, k, v = ((torch.randn(B, T, 256, generator=g) * 1.5).cuda() for _ in range(3))
     out = torch.full((B, T, 256), float("nan"), device="cuda")
-    lib.call("sam6d_sam_self_attn", _p(q), _p(k), _p(v), B, T, _p(out), _s())
+    lib.call("sam6d_sam_self_attn", q, k, v, B, T, out)
     sep = lambda t: t.double().view(B, T, 8, 32).permute(0, 2, 1, 3)      # noqa: E731
     qh, kh, vh = sep(q), sep(k), sep(v)
     scale = 1 / math.sqrt(32)
@@ -257,7 +248,7 @@ def test_sam_ln2d_gelu(lib, rows, mean, std):
     gam = (1 + 0.2 * torch.randn(64, generator=g)).cuda()
     bet = (0.3 * torch.randn(64, generator=g)).cuda()
     y = torch.full((rows, 64), float("nan"), dtype=torch.bfloat16, device="cuda")
-    lib.call("sam6d_sam_ln2d_gelu", _p(x), _p(gam), _p(bet), ctypes.c_longlong(rows), _p(y), _s())
+    lib.call("sam6d_sam_ln2d_gelu", x, gam, bet, rows, y)
     xd, gd, bd = x.double(), gam.double(), bet.double()
     mu = xd.mean(1, keepdim=True)
     dv = xd - mu
@@ -290,7 +281,7 @@ def test_sam_pe_encode(lib, rows):
     c[:min(rows, 4)] = corners[:min(rows, 4)]
     c_d, G_d = c.cuda(), Gm.cuda()
     out = torch.full((rows, 256), float("nan"), device="cuda")
-    lib.call("sam6d_sam_pe_encode", _p(c_d), _p(G_d), rows, _p(out), _s())
+    lib.call("sam6d_sam_pe_encode", c_d, G_d, rows, out)
     cd = 2 * c.double() - 1
     v = 2 * math.pi * (cd @ Gm.double())
     ref = torch.cat([torch.sin(v), torch.cos(v)], dim=1)
@@ -358,7 +349,7 @@ def test_gemm_tma_epilogue_matrix(ops, M, N, K, act, has_bias, has_res, odt):
 
 
 @pytest.mark.parametrize("B,M,shared_res", [(1, 4096, True), (3, 4096, True), (3, 4096, False), (3, 1000, True), (2, 1000, False)])
-def test_gemm_tma_batched_img_proj(ops, B, M, shared_res):
+def test_gemm_tma_batched_img_proj_views(ops, B, M, shared_res):
     """sam6d_gemm_tma_batched as the decoder's _img_proj calls it: one W shared by every problem (w_rpb = 0), a bias and a bf16
     residual shared by every problem (r_bs = 0) or per problem, bf16 out.  At M = 1000 a 128-row tile straddles two problems.
     C has 8 padding columns and one padding row per problem, which must keep their sentinel."""
@@ -369,7 +360,7 @@ def test_gemm_tma_batched_img_proj(ops, B, M, shared_res):
     bias = torch.randn(N, generator=g).cuda()
     R = torch.randn(*((M, N) if shared_res else (B, M, N)), generator=g).bfloat16().cuda()
     out = torch.full((B, M + 1, ldc), 7.0, dtype=torch.bfloat16, device="cuda")
-    ops.gemm_tma_batched(A, W, out, M, N, ldc, (M + 1) * ldc, bias=bias, residual=R, ldr=N, r_bs=0 if shared_res else M * N)
+    ops.gemm_tma_batched(A, W, out[:, :M, :N], bias=bias, residual=R.expand(B, M, N))
     Ad, Wd = A.double(), W.double()
     x = Ad @ Wd.t() + bias.double()
     o = x + R.double()
@@ -379,7 +370,7 @@ def test_gemm_tma_batched_img_proj(ops, B, M, shared_res):
 
 
 @pytest.mark.parametrize("C", [384, 768, 1024, 1536])
-def test_gemm_bf16_dinov2_patch_embedding(ops, C):
+def test_gemm_bf16_dinov2_patch_embedding_views(ops, C):
     """sam6d_gemm_bf16 as DINOv2's patch embedding calls it: fp32 patches (K = 588 zero-padded to 592, rounded to bf16 in the
     kernel), bf16 W shared by the batch (sW = 0), a positional residual shared by the batch (sR = 0), C written from row 1 of a
     (B, 257, C) token buffer (sC = 257 C); row 0 (the class token) keeps its sentinel"""
@@ -392,8 +383,7 @@ def test_gemm_bf16_dinov2_patch_embedding(ops, C):
     a, w = patches.cuda(), pw.bfloat16().cuda()
     pb, pos = torch.randn(C, generator=g).cuda(), torch.randn(L, C, generator=g).cuda()
     tok = torch.full((B, L + 1, C), 3.25, device="cuda")
-    ops.gemm_tc_raw(a.data_ptr(), 0, w.data_ptr(), 1, pb, pos.data_ptr(), tok.data_ptr() + C * 4, 0, L, C, Kp, Kp, Kp, C, C, batch=B,
-                    sA=L * Kp, sW=0, sC=(L + 1) * C, sR=0)
+    ops.gemm_tc(a.view(B, L, Kp), w, pb, residual=pos.expand(B, L, C), out=tok[:, 1:, :])
     Ad, Wd = a.bfloat16().double().view(B, L, Kp), w.double()
     x = Ad @ Wd.t() + pb.double()
     o = x + pos.double()
@@ -539,13 +529,13 @@ def test_masked_patch_normalize(lib, C):
     # the square root halves the relative error of the sum
     e32 = ref.abs() * (((C / 32 + 5) / 2 + 3) * U) * 1.01
     tok_d, pm_d = tok.cuda(), pmask.cuda()
-    base = ctypes.c_void_p(tok_d.data_ptr() + C * 4)
+    base = tok_d[:, 1:]
     for want_f32, want_bf16, want_valid in itertools.product([True, False], repeat=3):
         f32 = torch.full((P, G * G, C), float("nan"), device="cuda") if want_f32 else None
         b16 = torch.full((P, G * G, C), float("nan"), dtype=torch.bfloat16, device="cuda") if want_bf16 else None
         val = torch.full((P, G * G), 7, dtype=torch.uint8, device="cuda") if want_valid else None
-        args = (base, ctypes.c_longlong(C), ctypes.c_longlong(S * C), _p(pm_d), P, G, patch, C, ctypes.c_float(0.5), _p(f32), _p(b16),
-                _p(val), _s())
+        args = (base, C, S * C, pm_d, P, G, patch, C, 0.5, f32, b16,
+                val)
         if not (want_f32 or want_bf16):
             with pytest.raises(lib.Sam6dError, match="invalid argument"):
                 lib.call("sam6d_masked_patch_normalize", *args)
@@ -608,8 +598,7 @@ def test_appearance_reduce(lib, N):
     sim_d, qv_d = sim.cuda(), qvalid.cuda()
     appe = torch.full((P,), float("nan"), device="cuda")
     vis = torch.full((P,), float("nan"), device="cuda")
-    lib.call("sam6d_appearance_reduce", _p(sim_d), ctypes.c_longlong(ld), ctypes.c_longlong((N + 3) * ld), P, N, _p(qv_d),
-             ctypes.c_float(thred), _p(appe), _p(vis), _s())
+    lib.call("sam6d_appearance_reduce", sim_d, ld, (N + 3) * ld, P, N, qv_d, thred, appe, vis)
     a_ref, v_ref, abs_sum, Q = _appearance_ref(body.double(), qvalid, thred)
     # appe: one row max per thread (exact), a 5-level warp tree and 8 partials (gamma_13), + 1e-6, one division; clamp is
     # 1-Lipschitz.  vis: integer counts, + 1e-6 and one division

@@ -109,18 +109,17 @@ def test_gemm(ops, M, N, K):
     torch.testing.assert_close(got.double(), ref, atol=2e-5, rtol=1e-5)     # fp32 accumulate over K <= 512
 
 
-def test_gemm_batched_strided(ops):
+def test_gemm_batched_strided_views(ops):
     B, N, M, C = 3, 65, 70, 256
     f1 = torch.randn(B, N, C, generator=G(1))
     f2 = torch.randn(B, M, C, generator=G(2))
     out = torch.empty(B, N, M).cuda()
     a, w = f1.cuda(), f2.cuda()
-    ops.gemm_raw(a.data_ptr(), w.data_ptr(), None, 0, out.data_ptr(), N, M, C, C, C, M, 0, batch=B, sA=N * C, sW=M * C,
-                 sC=N * M, alpha=10.0)
+    ops.gemm(a, w, out=out, alpha=10.0)
     torch.testing.assert_close(out.cpu(), 10.0 * f1 @ f2.transpose(1, 2), atol=2e-4, rtol=1e-5)
 
 
-def test_row_ops(ops):
+def test_row_ops_views(ops):
     x = torch.randn(500, 256, generator=G(1)) * 3 + 0.5
     g, b = torch.randn(256, generator=G(2)), torch.randn(256, generator=G(3))
     torch.testing.assert_close(ops.layernorm(x.cuda(), g.cuda(), b.cuda()).cpu(),
@@ -137,7 +136,7 @@ def test_row_ops(ops):
     ref = q / q.norm(dim=-1, keepdim=True) * qn
     xc = x.cuda()
     out = torch.empty_like(xc)
-    ops.focus_rows_raw(xc.data_ptr(), (500, 0, 256), out.data_ptr(), (500, 0, 256), scale.cuda(), 500, 256)
+    ops.focus_rows(xc, scale.cuda(), out=out)
     torch.testing.assert_close(out.cpu(), ref, atol=1e-5, rtol=2e-5)
     # rigid warp, radius
     p = torch.randn(2, 100, 3, generator=G(6))
@@ -183,7 +182,7 @@ def test_geo_embed(ops):
 
 
 # ------------------------------------------------------------------------------------------------- attention
-def test_rpe_scores_and_mha(ops):
+def test_rpe_scores_and_mha_views(ops):
     B, S, C, H = 2, 197, 256, 4
     E = torch.randn(B, S, S, C, generator=G(1))
     U = torch.randn(B, S, H, C, generator=G(2))
@@ -202,8 +201,7 @@ def test_rpe_scores_and_mha(ops):
     ref = (att @ vh).permute(0, 2, 1, 3).reshape(B, S, C)
     qc, kc, vc = q.cuda(), k.cuda(), v.cuda()
     out = torch.empty(B, S, C).cuda()
-    ops.mha_raw(qc.data_ptr(), C, S * C, kc.data_ptr(), C, 150 * C, vc.data_ptr(), C, 150 * C, bias.cuda(), B, H, S, 150, 0.125,
-                out.data_ptr(), C, S * C)
+    ops.mha(qc, kc, vc, bias.cuda(), 0.125, out)
     torch.testing.assert_close(out.cpu(), ref, atol=2e-5, rtol=1e-4)
 
 
@@ -275,7 +273,7 @@ def test_transformer_tail_fused(ops, M):
     assert err.max().item() < 6e-2 and err.mean().item() < 4e-3, (err.max().item(), err.mean().item())
 
 
-def test_linear_attention(ops):
+def test_linear_attention_views(ops):
     sd = po.make_state_dict(seed=4)
     p = "fine_point_matching.transformers.0.dense_layer.attention.attention"
     B, N, J, C = 2, 300, 50, 256
@@ -286,18 +284,18 @@ def test_linear_attention(ops):
     k = torch.nn.functional.linear(xkv, sd[p + ".proj_k.weight"], sd[p + ".proj_k.bias"]).cuda().contiguous()
     v = torch.nn.functional.linear(xkv, sd[p + ".proj_v.weight"], sd[p + ".proj_v.bias"]).cuda().contiguous()
     sp = torch.nn.functional.softplus(sd[p + ".scale"]).reshape(-1).cuda()
-    ops.focus_rows_raw(q.data_ptr(), (B * N, 0, C), q.data_ptr(), (B * N, 0, C), sp, B * N, C)
-    ops.focus_rows_raw(k.data_ptr(), (B * J, 0, C), k.data_ptr(), (B * J, 0, C), sp, B * J, C)
+    ops.focus_rows(q.view(B * N, C), sp, out=q.view(B * N, C))
+    ops.focus_rows(k.view(B * J, C), sp, out=k.view(B * J, C))
     KV = torch.empty(B, 4, 64, 64).cuda()
     KS = torch.empty(B, 4, 64).cuda()
-    ops.linattn_kv_raw(k.data_ptr(), C, J * C, v.data_ptr(), C, J * C, B, 4, J, KV, KS)
+    ops.linattn_kv(k, v, KV, KS)
     x = torch.empty(B, N, C).cuda()
-    ops.linattn_apply_raw(q.data_ptr(), N, N * C, C, KV, KS, B, 4, x.data_ptr(), N * C, C)
+    ops.linattn_apply(q, KV, KS, x)
     torch.testing.assert_close(x.cpu(), ref, atol=1e-4, rtol=1e-3)
 
 
 @pytest.mark.parametrize("B,N,J", [(2, 300, 50), (3, 2048, 196), (1, 129, 7)])
-def test_linear_attention_tensor_core(ops, B, N, J):
+def test_linear_attention_tensor_core_views(ops, B, N, J):
     """bf16 dense tokens: feature map + per-head (q' KV)/(q' . ksum) in one wgmma kernel, against fp64 math on the same
     bf16-rounded query projection.  The token rows sit behind a bg row (the (B,N+1,C) layout of the fine stage)."""
     C = 256
@@ -320,12 +318,12 @@ def test_linear_attention_tensor_core(ops, B, N, J):
     ref = ((qh @ (kh.transpose(-1, -2) @ vh)) * z).permute(0, 2, 1, 3).reshape(B, N, C)
 
     kd, vd, spd = k.cuda().contiguous(), v.cuda().contiguous(), sp.cuda()
-    ops.focus_rows_raw(kd.data_ptr(), (B * J, 0, C), kd.data_ptr(), (B * J, 0, C), spd, B * J, C)
-    blob, KS = ops.linattn_kv_pack_raw(kd.data_ptr(), C, J * C, vd.data_ptr(), C, J * C, B, J, kd.device)
+    ops.focus_rows(kd.view(B * J, C), spd, out=kd.view(B * J, C))
+    blob, KS = ops.linattn_kv_pack(kd, vd)
     torch.testing.assert_close(KS.cpu().double(), kh.sum(dim=2), atol=1e-4, rtol=1e-4)
     qd = q.cuda()
     x = torch.full((B, N + 1, C), 7.0, dtype=torch.bfloat16, device="cuda")
-    ops.linattn_tc_raw(qd.data_ptr() + C * 2, C, (N + 1) * C, blob, KS, spd, B, N, x.data_ptr() + C * 2, C, (N + 1) * C)
+    ops.linattn_tc(qd[:, 1:, :], blob, KS, spd, x[:, 1:, :])
     x = x.cpu()
     assert (x[:, 0] == 7.0).all()                                     # rows outside the view are untouched
     torch.testing.assert_close(x[:, 1:].double(), ref, atol=2e-2 * ref.abs().max().item(), rtol=3e-2)
@@ -555,14 +553,13 @@ def test_gemm_tc(ops, M, N, K, adt, wdt, odt):
     torch.testing.assert_close(got.double(), ref, atol=tol, rtol=1e-5 if odt == torch.float32 else 1e-2)
 
 
-def test_gemm_tc_batched_strided(ops):
+def test_gemm_tc_batched_strided_views(ops):
     B, N, M, C = 3, 300, 257, 256
     f1 = torch.randn(B, N, C, generator=G(1))
     f2 = torch.randn(B, M, C, generator=G(2))
     out = torch.empty(B, N, M).cuda()
     a, w = f1.cuda(), f2.cuda()
-    ops.gemm_tc_raw(a.data_ptr(), 0, w.data_ptr(), 0, None, 0, out.data_ptr(), 0, N, M, C, C, C, M, 0, batch=B, sA=N * C, sW=M * C,
-                    sC=N * M, alpha=10.0)
+    ops.gemm_tc(a, w, out=out, alpha=10.0)
     ref = 10.0 * f1.bfloat16().double() @ f2.bfloat16().double().transpose(1, 2)
     torch.testing.assert_close(out.cpu().double(), ref, atol=2e-4, rtol=1e-5)
 
@@ -771,7 +768,7 @@ def test_attn_global_tensor_core(ops):
 
 
 @pytest.mark.parametrize("B,S,T", [(3, 197, 197), (2, 2049, 2049), (4, 130, 77)])
-def test_gemm_tma_batched_scores(ops, B, S, T):
+def test_gemm_tma_batched_scores_view(ops, B, S, T):
     """stacked per-proposal score matrices: tiles that run into the next proposal's rows must not leak into the output"""
     C = 256
     a = torch.randn(B, S, C, generator=G(1))
@@ -779,7 +776,7 @@ def test_gemm_tma_batched_scores(ops, B, S, T):
     ld = (T + 3) // 4 * 4
     out = torch.full((B, S, ld), 7.0, device="cuda")
     an, wn = ops.l2norm_rows_bf16(a.cuda()), ops.l2norm_rows_bf16(w.cuda())
-    ops.gemm_tma_batched(an, wn, out, S, T, ld, S * ld, alpha=10.0)
+    ops.gemm_tma_batched(an, wn, out[:, :, :T], alpha=10.0)
     ref = 10.0 * an.float().cpu().double() @ wn.float().cpu().double().transpose(1, 2)
     torch.testing.assert_close(out.cpu()[:, :, :T].double(), ref, atol=2e-4, rtol=1e-5)
     assert (out.cpu()[:, :, T:] == 7.0).all()

@@ -16,7 +16,6 @@ does (`_spread`).  That difference is carried through the rest of the chain with
 
 Each check prints its largest error / bound ratio; where a bound is loose enough to leave doubt, a deliberately wrong answer
 computed in torch must fail the same bound."""
-import ctypes
 import math
 
 import numpy as np
@@ -50,14 +49,6 @@ def _g(seed):
 
 def _gc(seed):
     return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _ratio(err, bound):
@@ -255,11 +246,11 @@ def test_fine_assignment_passes(lib, B, S):
     pts2 = torch.randn(B, S - 1, 3, generator=g).cuda()
     ld = (S + 3) // 4 * 4
     dev = "cuda"
-    a, sh = ctypes.c_float(alpha), ctypes.c_float(alpha)
+    a, sh = alpha, alpha
     rinv = torch.full((B, ld), float("nan"), device=dev)
     cinv = torch.full((B, ld), float("nan"), device=dev)
-    lib.call("sam6d_fine_pass_tc", _p(F1), _p(F2), B, S, a, sh, 0, None, None, ld, None, _p(rinv), None, None, None, _s())
-    lib.call("sam6d_fine_pass_tc", _p(F2), _p(F1), B, S, a, sh, 0, None, None, ld, None, _p(cinv), None, None, None, _s())
+    lib.call("sam6d_fine_pass_tc", F1, F2, B, S, a, sh, 0, None, None, ld, None, rinv, None, None, None)
+    lib.call("sam6d_fine_pass_tc", F2, F1, B, S, a, sh, 0, None, None, ld, None, cinv, None, None, None)
 
     # ---- ROWSUM: inv_i = 1 / sum_j e_ij.  Per row 64 columns of every 256-column tile in one thread's chain, then 2 quad levels
     e, eta = _fine_e(F1, F2, alpha)
@@ -285,7 +276,7 @@ def test_fine_assignment_passes(lib, B, S):
 
     # ---- ARGMAX (F2, F1): column labels.  P = (e rf) (e cf): two ex2 errors, three roundings
     lab2 = torch.full((B, S), -7, dtype=torch.int32, device=dev)
-    lib.call("sam6d_fine_pass_tc", _p(F2), _p(F1), B, S, a, sh, 1, _p(cf), _p(rf), ld, None, None, _p(lab2), None, None, _s())
+    lib.call("sam6d_fine_pass_tc", F2, F1, B, S, a, sh, 1, cf, rf, ld, None, None, lab2, None, None)
     eT, etaT = _fine_e(F2, F1, alpha)
     P2 = eT * eT * cf[:, :S, None].to(F64) * rf[:, None, :S].to(F64)
     a2, ok2 = _first_argmax_with_gap(P2, 2 * etaT + 3 * U, torch.arange(S, device=dev))
@@ -298,7 +289,7 @@ def test_fine_assignment_passes(lib, B, S):
 
     # ---- masked points: q4[b,j] = (pts2[b,j-1], 1) where column j >= 1 carries a non-background label, else 0 (also j >= S)
     q4 = torch.full((B, ld, 4), float("nan"), device=dev)
-    lib.call("sam6d_fine_masked_points", _p(lab2), _p(pts2), B, S, ld, _p(q4), _s())
+    lib.call("sam6d_fine_masked_points", lab2, pts2, B, S, ld, q4)
     want = torch.zeros(B, ld, 4, device=dev)
     keep = (lab2[:, 1:] > 0)[..., None]
     want[:, 1:S, :3] = torch.where(keep, pts2, torch.zeros_like(pts2))
@@ -309,7 +300,7 @@ def test_fine_assignment_passes(lib, B, S):
     lab1 = torch.full((B, S), -7, dtype=torch.int32, device=dev)
     wts = torch.full((B, S - 1), float("nan"), device=dev)
     pred = torch.full((B, S - 1, 3), float("nan"), device=dev)
-    lib.call("sam6d_fine_pass_tc", _p(F1), _p(F2), B, S, a, sh, 2, _p(rf), _p(cf), ld, _p(q4), None, _p(lab1), _p(wts), _p(pred), _s())
+    lib.call("sam6d_fine_pass_tc", F1, F2, B, S, a, sh, 2, rf, cf, ld, q4, None, lab1, wts, pred)
     e, eta = _fine_e(F1, F2, alpha)
     P = e * e * rf[:, :S, None].to(F64) * cf[:, None, :S].to(F64)
     del e
@@ -398,8 +389,8 @@ def _pe_ref(pts, idx, w, drop_b3=False):
 def _run_pe(lib, pts, idx, w, out, off):
     B, N, _ = pts.shape
     W1, B1, W2, B2, W3, B3 = w
-    lib.call("sam6d_pe_mlp_max_tc", _p(pts), _p(idx), B, N, idx.shape[2], _p(W1), _p(B1), _p(W2), _p(B2), _p(W3), _p(B3), _p(out),
-             int(out.dtype == torch.bfloat16), out.shape[-1], off, _s())
+    lib.call("sam6d_pe_mlp_max_tc", pts, idx, B, N, idx.shape[2], W1, B1, W2, B2, W3, B3, out, int(out.dtype == torch.bfloat16),
+             out.shape[-1], off)
 
 
 def _pe_check(lib, name, pts, idx, w, odt, off):
@@ -486,8 +477,7 @@ def test_linear_attention(lib, J, N):
     V = torch.randn(B, J, C, generator=g, device=dev)
     blob = torch.empty(B, 4 * 64 * 64, dtype=torch.bfloat16, device=dev)
     KS = torch.empty(B, 4, 64, device=dev)
-    lib.call("sam6d_linattn_kv_pack", _p(Kf), ctypes.c_longlong(C), ctypes.c_longlong(J * C), _p(V), ctypes.c_longlong(C),
-             ctypes.c_longlong(J * C), B, J, _p(blob), _p(KS), _s())
+    lib.call("sam6d_linattn_kv_pack", Kf, C, J * C, V, C, J * C, B, J, blob, KS)
     kh = Kf.to(F64).view(B, J, 4, 64)
     vh = V.to(F64).view(B, J, 4, 64)
     # ksum: one fp32 chain of J terms
@@ -503,8 +493,7 @@ def test_linear_attention(lib, J, N):
     q[:, 1::5] = -q[:, 1::5].abs() - 0.01
     q = q.bfloat16()
     x = torch.full((B, N + 1, C), 7.0, dtype=torch.bfloat16, device=dev)
-    lib.call("sam6d_linattn_tc", ctypes.c_void_p(q.data_ptr() + C * 2), ctypes.c_longlong(C), ctypes.c_longlong((N + 1) * C), _p(blob),
-             _p(KS), _p(sp), B, N, ctypes.c_void_p(x.data_ptr() + C * 2), ctypes.c_longlong(C), ctypes.c_longlong((N + 1) * C), _s())
+    lib.call("sam6d_linattn_tc", q[:, 1:], C, (N + 1) * C, blob, KS, sp, B, N, x[:, 1:], C, (N + 1) * C)
     assert (x[:, 0] == 7.0).all(), "a row outside the view was written"
     qf = _focus64(q[:, 1:].to(F64), sp.to(F64))
     # feature map in fp32: t = (q+ + 1e-6) / s (3u), sums of t^2 and t^6 (8-term chains + a 5-level warp tree: gamma_13),

@@ -15,7 +15,6 @@ Discrete outputs (labels, k-NN sets, sample indices, hits, the picked hypothesis
 the derived error the kernel must match exactly; elsewhere its choice must be one the bound allows, and the count of such
 undecided elements is printed (~0 on random data).  Planted exact ties must go to the first index.  Each check prints its
 largest error / bound ratio; where a bound could hide a mistake, a plausible wrong answer computed in torch must fail it."""
-import ctypes
 import math
 
 import numpy as np
@@ -669,14 +668,13 @@ def test_fine_assign_edges(ops, refused):
     assert (lab1[:, 400:430] == 0).all()
     # S = 96 (three 32-row tiles) through the C ABI itself, with every buffer sized for it
     from sam6d_b200 import _lib
-    S, ld, p = 96, 96, lambda x: ctypes.c_void_p(x.data_ptr())
+    S, ld = 96, 96
     A96, pts96 = _score_matrix(1, S, g), _ball(1, S - 1, g)
     f = lambda *s: torch.zeros(*s, device=DEV)              # noqa: E731
     i = lambda *s: torch.zeros(*s, dtype=torch.int32, device=DEV)   # noqa: E731
     bufs = [f(1, ld), f(1, ld), f(1, 3, ld), i(1, 3, ld), i(1, S), i(1, S), f(1, S - 1), f(1, S - 1, 3)]
     with pytest.raises(refused, match="invalid argument"):
-        _lib.call("sam6d_fine_assign", p(A96), 1, S, ld, ctypes.c_float(10.0), p(pts96), *[p(x) for x in bufs],
-                  ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        _lib.call("sam6d_fine_assign", A96, 1, S, ld, 10.0, pts96, *bufs)
 
 
 # ================================================================================================== 8. weighted_procrustes

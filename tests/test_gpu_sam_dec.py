@@ -67,7 +67,6 @@ def test_mask_decoder_matches_reference(gold, amg):
 def test_postprocess_stats_and_binarize_against_oracle(amg):
     """Sam.postprocess_masks + stability counts + boxes + binarisation evaluated per output pixel, on smooth synthetic low-res
     logits, against the reference formulation (two F.interpolate calls, utils.amg helpers restated in the oracle)"""
-    import ctypes
     from sam6d_b200 import _lib
     g = torch.Generator().manual_seed(4)
     n = 12
@@ -76,10 +75,8 @@ def test_postprocess_stats_and_binarize_against_oracle(amg):
     low[3] = -5.0                                                  # an empty mask
     ref = so.postprocess_masks(low[None], (768, 1024), (480, 640))[0]
     stats = torch.empty(n, 8, dtype=torch.int32, device="cuda")
-    p = lambda t: ctypes.c_void_p(t.data_ptr())                    # noqa: E731
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     low_d = low.cuda()
-    _lib.call("sam6d_sam_mask_stats", p(low_d), n, 256, 1024, 768, 1024, 480, 640, ctypes.c_float(0.0), ctypes.c_float(1.0), p(stats), st)
+    _lib.call("sam6d_sam_mask_stats", low_d, n, 256, 1024, 768, 1024, 480, 640, 0.0, 1.0, stats)
     s = stats.cpu()
     hi, lo = (ref > 1.0).flatten(1).sum(1), (ref > -1.0).flatten(1).sum(1)
     print("count(>1) gpu/ref", s[:, 0].tolist(), hi.tolist())
@@ -90,7 +87,7 @@ def test_postprocess_stats_and_binarize_against_oracle(amg):
     assert (mine - boxes).abs().max() <= 1
     sel = torch.arange(n, dtype=torch.int32, device="cuda")
     out = torch.empty(n, 480, 640, dtype=torch.uint8, device="cuda")
-    _lib.call("sam6d_sam_mask_binarize", p(low_d), p(sel), n, 256, 1024, 768, 1024, 480, 640, ctypes.c_float(0.0), p(out), st)
+    _lib.call("sam6d_sam_mask_binarize", low_d, sel, n, 256, 1024, 768, 1024, 480, 640, 0.0, out)
     mism = (out.cpu().bool() != (ref > 0.0)).float().mean().item()
     assert mism < 2e-5, mism
 

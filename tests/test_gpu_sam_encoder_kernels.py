@@ -14,7 +14,6 @@ sensitivity: a relative error eps_j on each weight p_j moves the output by at mo
 and a relative error on every product of the P V sum by that error times pv.  A logit error ds_j is a relative weight error
 of ds_j + max ds, which is the `2 * dlog` in every eta below.  Each check prints its largest error / bound ratio; where a bound
 could hide a mistake, a deliberately wrong answer computed in torch must fail the same bound."""
-import ctypes
 import math
 import types
 from functools import partial
@@ -54,18 +53,6 @@ def ops(lib):
 
 def _gc(seed):
     return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ll(v):
-    return ctypes.c_longlong(int(v))
 
 
 def _f32(x):
@@ -240,8 +227,8 @@ def test_attn_global_tc(ops, lib, D, H, B):
     for odt in (torch.float32, torch.bfloat16):
         got[odt] = ops.attn_global_tc(qk, vt, blob, B, H, GRID, scale, out_dtype=odt, D=D)
         wide = torch.full((B * L, C + 16), SENT, dtype=odt, device="cuda")
-        lib.call("sam6d_attn_global_tc_ex", _p(qk_wide), _ll(ld), _p(vt), _ll(vt.shape[1]), _p(blob), B, H, GRID, D,
-                 ctypes.c_float(scale), _p(wide), int(odt == torch.bfloat16), _ll(C + 16), _s())
+        lib.call("sam6d_attn_global_tc_ex", qk_wide, ld, vt, vt.shape[1], blob, B, H, GRID, D, scale, wide, int(odt == torch.bfloat16),
+                 C + 16)
         assert (wide[:, C:] == SENT).all(), "columns past H*D of the output were written"
         assert torch.equal(wide[:, :C], got[odt]), "spare q|k columns changed the result"
     worst = {odt: _Worst(f"attn_global_tc D={D} H={H} B={B} {str(odt)[6:]}") for odt in got}
@@ -320,9 +307,8 @@ def _attn_tc_call(lib, qk, vt, blob, nW, H, D, Hs, Ws, scale, odt, extra_rows=64
     """sam6d_attn_tc (BIAS_MODE 2) into an output with sentinel columns past H*D and `extra_rows` sentinel rows past the end"""
     C, L = H * D, Hs * Ws
     out = torch.full((nW * L + extra_rows, C + 8), SENT, dtype=odt, device="cuda")
-    lib.call("sam6d_attn_tc", _p(qk), _ll(qk.shape[1]), 0, _p(qk), _ll(qk.shape[1]), C, _p(vt), _ll(vt.shape[1]), nW, H, L, L, D, 2,
-             ctypes.c_void_p(0), _p(blob), ctypes.c_void_p(0), Hs, Ws, ctypes.c_void_p(0), ctypes.c_float(scale), _p(out),
-             int(odt == torch.bfloat16), _ll(C + 8), _s())
+    lib.call("sam6d_attn_tc", qk, qk.shape[1], 0, qk, qk.shape[1], C, vt, vt.shape[1], nW, H, L, L, D, 2, 0, blob, 0, Hs, Ws, 0, scale, out,
+             int(odt == torch.bfloat16), C + 8)
     assert (out[:, C:] == SENT).all(), "columns past H*D were written"
     assert (out[nW * L:] == SENT).all(), "rows past the last window were written (a query tile ran past m_lim)"
     return out[:nW * L, :C]
@@ -547,8 +533,7 @@ def test_layernorm_bf16_generic(lib):
     gam = 1.0 + 0.2 * torch.randn(C, generator=g, device="cuda")
     bet = 0.2 * torch.randn(C, generator=g, device="cuda")
     y = torch.empty(rows, C, dtype=torch.bfloat16, device="cuda")
-    lib.call("sam6d_layernorm_bf16", _p(xb), _ll(rows), _ll(0), _ll(ld), _p(y), _ll(rows), _ll(0), _ll(C), _p(gam), _p(bet),
-             _ll(rows), C, ctypes.c_float(1e-6), _s())
+    lib.call("sam6d_layernorm_bf16", xb, rows, 0, ld, y, rows, 0, C, gam, bet, rows, C, 1e-6)
     ref, bound = _ln_bound(x.to(F64), gam.to(F64), bet.to(F64), EPS6, C // 32, torch.bfloat16)
     _check("layernorm_bf16 generic C=1280", (y.to(F64) - ref).abs(), bound)
 
@@ -582,7 +567,7 @@ def _bf_bound(ref, e):
 
 
 @pytest.mark.parametrize("name", ["vit_h", "vit_l", "vit_b"])
-def test_encoder_wiring(ops, name):
+def test_encoder_wiring_views(ops, name):
     """ImageEncoderViT (bf16) with one windowed and one global block: the module's forward replayed stage by stage with the
     same ops calls must give the same bits, and every stage is held to the reference formula (image_encoder.py) evaluated in
     float64 on the kernel's own output of the previous stage"""
@@ -615,8 +600,7 @@ def test_encoder_wiring(ops, name):
 
     patches = img.float().reshape(1, 3, GRID, P, GRID, P).permute(0, 2, 4, 1, 3, 5).reshape(L, 3 * P * P).contiguous()
     tok = torch.empty(L, C, dtype=torch.float32, device="cuda")
-    ops.gemm_tc_raw(patches.data_ptr(), 0, w["pe_w"].bf16.data_ptr(), 1, w["pe_b"], w["pos"].data_ptr(), tok.data_ptr(), 0, L, C,
-                    3 * P * P, 3 * P * P, 3 * P * P, C, C, batch=1, sA=L * 3 * P * P, sW=0, sC=L * C, sR=0)
+    ops.gemm_tc(patches, w["pe_w"].bf16, w["pe_b"], residual=w["pos"], out=tok)
     # patch embed + pos: conv 16 x 16 / 16 == a 768-term GEMM over bf16 patches and weights; + bias, + pos one rounding each.
     # (The float64 conv itself is exact to within 768 * 2^-53 mag, 2^29 times below the charged 2 * 768 u mag.)
     pe_w = wbf("patch_embed.proj.weight")

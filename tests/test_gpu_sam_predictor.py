@@ -4,7 +4,6 @@ float64 evaluation; then every case of tests/golden/sam_predictor.pt (outputs of
 predictor against the automatic mask generator on the shapes they share.
 
 Notation as tests/test_gpu_ism_kernels.py: u = 2^-24, ub = 2^-8, a chain of n fp32 roundings is charged n u."""
-import ctypes
 import math
 import os
 
@@ -27,14 +26,6 @@ def lib():
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     from sam6d_b200 import _lib
     return _lib
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _check(name, err, bound):
@@ -134,7 +125,7 @@ def test_sam_tok2img_attn_up_to_32_tokens(lib, T, shared):
     K = torch.randn(Bk, L, 128, generator=g).bfloat16().cuda()
     V = torch.randn(Bk, L, 128, generator=g).bfloat16().cuda()
     out = torch.full((B, T, 128), float("nan"), device="cuda")
-    lib.call("sam6d_sam_tok2img_attn", _p(Q), _p(K), _p(V), ctypes.c_longlong(0 if shared else L * 128), B, T, L, _p(out), _s())
+    lib.call("sam6d_sam_tok2img_attn", Q, K, V, 0 if shared else L * 128, B, T, L, out)
     qh = Q.double().view(B, T, 8, 16).permute(0, 2, 1, 3)
     kh = K.double().view(Bk, L, 8, 16).permute(0, 2, 1, 3)
     vh = V.double().view(Bk, L, 8, 16).permute(0, 2, 1, 3)
@@ -155,7 +146,7 @@ def test_sam_img2tok_attn_up_to_32_tokens(lib, T):
     Kt = (torch.randn(B, T, 128, generator=g) * 5).cuda()
     Vt = torch.randn(B, T, 128, generator=g).cuda()
     out = torch.full((B, L, 128), float("nan"), dtype=torch.bfloat16, device="cuda")
-    lib.call("sam6d_sam_img2tok_attn", _p(Q), ctypes.c_longlong(L * 128), _p(Kt), _p(Vt), B, T, L, _p(out), _s())
+    lib.call("sam6d_sam_img2tok_attn", Q, L * 128, Kt, Vt, B, T, L, out)
     qh = Q.double().view(B, L, 8, 16).permute(0, 2, 1, 3)
     kh = Kt.double().view(B, T, 8, 16).permute(0, 2, 1, 3)
     vh = Vt.double().view(B, T, 8, 16).permute(0, 2, 1, 3)
@@ -174,7 +165,7 @@ def test_sam_self_attn_up_to_32_tokens(lib, T):
     g = torch.Generator().manual_seed(700 + T)
     q, k, v = ((torch.randn(B, T, 256, generator=g) * 1.5).cuda() for _ in range(3))
     out = torch.full((B, T, 256), float("nan"), device="cuda")
-    lib.call("sam6d_sam_self_attn", _p(q), _p(k), _p(v), B, T, _p(out), _s())
+    lib.call("sam6d_sam_self_attn", q, k, v, B, T, out)
     sep = lambda t: t.double().view(B, T, 8, 32).permute(0, 2, 1, 3)      # noqa: E731
     qh, kh, vh = sep(q), sep(k), sep(v)
     scale = 1 / math.sqrt(32)
@@ -189,12 +180,12 @@ def test_sam_self_attn_up_to_32_tokens(lib, T):
 def test_attention_kernels_refuse_more_than_32_tokens(lib):
     q = torch.zeros(1, 33, 256, device="cuda")
     with pytest.raises(lib.Sam6dError, match="invalid argument"):
-        lib.call("sam6d_sam_self_attn", _p(q), _p(q), _p(q), 1, 33, _p(q), _s())
+        lib.call("sam6d_sam_self_attn", q, q, q, 1, 33, q)
     K = torch.zeros(4096, 128, dtype=torch.bfloat16, device="cuda")
     with pytest.raises(lib.Sam6dError, match="invalid argument"):
-        lib.call("sam6d_sam_tok2img_attn", _p(q), _p(K), _p(K), ctypes.c_longlong(0), 1, 33, 4096, _p(q), _s())
+        lib.call("sam6d_sam_tok2img_attn", q, K, K, 0, 1, 33, 4096, q)
     with pytest.raises(lib.Sam6dError, match="invalid argument"):
-        lib.call("sam6d_sam_img2tok_attn", _p(K), ctypes.c_longlong(0), _p(q), _p(q), 1, 33, 4096, _p(K), _s())
+        lib.call("sam6d_sam_img2tok_attn", K, 0, q, q, 1, 33, 4096, K)
 
 
 # ================================================================================================== mask-token range, upscaling
@@ -205,18 +196,18 @@ def test_mask_dot_range_bit_identical(lib):
     hyper = torch.randn(B, 4, 32, generator=g).cuda()
     S = 4 * G
     m3 = torch.empty(B, 3, S, S, device="cuda")
-    lib.call("sam6d_sam_mask_dot", _p(up), _p(hyper), B, G, _p(m3), _s())
+    lib.call("sam6d_sam_mask_dot", up, hyper, B, G, m3)
     r13 = torch.empty(B, 3, S, S, device="cuda")
-    lib.call("sam6d_sam_mask_dot_range", _p(up), _p(hyper), B, G, 1, 3, _p(r13), _s())
+    lib.call("sam6d_sam_mask_dot_range", up, hyper, B, G, 1, 3, r13)
     assert torch.equal(m3, r13)
     r04 = torch.empty(B, 4, S, S, device="cuda")
-    lib.call("sam6d_sam_mask_dot_range", _p(up), _p(hyper), B, G, 0, 4, _p(r04), _s())
+    lib.call("sam6d_sam_mask_dot_range", up, hyper, B, G, 0, 4, r04)
     r01 = torch.empty(B, 1, S, S, device="cuda")
-    lib.call("sam6d_sam_mask_dot_range", _p(up), _p(hyper), B, G, 0, 1, _p(r01), _s())
+    lib.call("sam6d_sam_mask_dot_range", up, hyper, B, G, 0, 1, r01)
     assert torch.equal(r01[:, 0], r04[:, 0]) and torch.equal(r13, r04[:, 1:])
     for m0, nm in ((0, 5), (3, 2), (-1, 1), (0, 0)):
         with pytest.raises(lib.Sam6dError, match="invalid argument"):
-            lib.call("sam6d_sam_mask_dot_range", _p(up), _p(hyper), B, G, m0, nm, _p(r04), _s())
+            lib.call("sam6d_sam_mask_dot_range", up, hyper, B, G, m0, nm, r04)
 
 
 @pytest.mark.parametrize("size", [(480, 640), (640, 480), (37, 1000)])

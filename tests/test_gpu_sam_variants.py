@@ -2,7 +2,6 @@
 kernels against the reference formula (image_encoder.py:224-240, 325-361), the full ViT-B / ViT-L encoders against the vendored
 reference module's CPU output (tests/golden/sam_vit{b,l}.pt, tools/make_golden.py), batch independence, and the ISM CLI with
 --sam_model_type vit_b chained into the PEM CLI."""
-import ctypes
 import json
 import os
 
@@ -72,16 +71,12 @@ def test_attn_global_tc_ex_head_dim_80_is_the_old_entry_point():
     qd = qkv.cuda()
     vt = ops.transpose_tokens(qd, 2 * H * D, H * D, B, L)
     blob = ops.pack_rel_pos(rel_h.cuda(), rel_w.cuda(), slab_rows=128)
-    p = lambda t: ctypes.c_void_p(t.data_ptr())                              # noqa: E731
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     for odt in (torch.float32, torch.bfloat16):
         a = torch.full((B * L, H * D), float("nan"), dtype=odt, device="cuda")
         b = torch.full_like(a, float("nan"))
         bf = int(odt == torch.bfloat16)
-        _lib.call("sam6d_attn_global_tc", p(qd), ctypes.c_longlong(qd.shape[1]), p(vt), ctypes.c_longlong(vt.shape[1]), p(blob), B, H, S,
-                  ctypes.c_float(D ** -0.5), p(a), bf, ctypes.c_longlong(H * D), st)
-        _lib.call("sam6d_attn_global_tc_ex", p(qd), ctypes.c_longlong(qd.shape[1]), p(vt), ctypes.c_longlong(vt.shape[1]), p(blob), B, H, S,
-                  80, ctypes.c_float(D ** -0.5), p(b), bf, ctypes.c_longlong(H * D), st)
+        _lib.call("sam6d_attn_global_tc", qd, qd.shape[1], vt, vt.shape[1], blob, B, H, S, D ** -0.5, a, bf, H * D)
+        _lib.call("sam6d_attn_global_tc_ex", qd, qd.shape[1], vt, vt.shape[1], blob, B, H, S, 80, D ** -0.5, b, bf, H * D)
         assert torch.isfinite(a).all()
         assert torch.equal(a, b)
         torch.testing.assert_close(ops.attn_global_tc(qd, vt, blob, B, H, S, D ** -0.5, out_dtype=odt), a, atol=0, rtol=0)

@@ -95,13 +95,12 @@ def main():
     pobj = dev(np.array([g["obj_id"] - 1 for _, g in pairs]), torch.int32)
     Kp = dev(np.tile([600.0, 600.0, 319.5, 240.25], (len(pairs), 1)))
     verts = [dev(meshes[o][0]) for o in (1, 2, 3)]
-    from sam6d_b200.render import _p, _stream
     V, S = torch.cat(verts).contiguous(), torch.cat(syms).contiguous()
     voff = dev(np.cumsum([0] + [len(meshes[o][0]) for o in (1, 2, 3)]), torch.int32)
     soff = dev(np.cumsum([0] + [len(s) for s in syms]), torch.int32)
     res_d = torch.empty(len(pairs), 2, dtype=torch.float32, device="cuda")
-    ms_mssd = events(lambda: _lib.call("sam6d_bop_mssd_mspd", _p(est), _p(gtp), _p(pobj), _p(Kp), len(pairs), _p(V), _p(voff), _p(S), _p(soff),
-                                       3, max(len(s) for s in syms), _p(res_d), _stream()), 10)
+    ms_mssd = events(lambda: _lib.call("sam6d_bop_mssd_mspd", est, gtp, pobj, Kp, len(pairs), V, voff, S, soff, 3,
+                                       max(len(s) for s in syms), res_d), 10)
     ref = bop_eval.mssd_mspd(est, gtp, pobj, Kp, verts, syms)
     assert torch.equal(ref, res_d)
     n_eval = sum(len(meshes[g["obj_id"]][0]) * len(syms[g["obj_id"] - 1]) for _, g in pairs)
@@ -122,8 +121,8 @@ def main():
     img = torch.zeros(len(sel), dtype=torch.int32, device="cuda")
     taus = torch.from_numpy(bop_eval.VSD_TAUS.astype(np.float32)).cuda()
     out = torch.empty(len(sel), 12, dtype=torch.int32, device="cuda")
-    ms_vsd = events(lambda: _lib.call("sam6d_bop_vsd_counts", _p(de), _p(dg), _p(dt), _p(img), len(sel), 480, 640, 600.0, 600.0, 319.5,
-                                      240.25, 15.0, 80.0, _p(taus), _p(out), _stream()), 20)
+    ms_vsd = events(lambda: _lib.call("sam6d_bop_vsd_counts", de, dg, dt, img, len(sel), 480, 640, 600.0, 600.0, 319.5, 240.25, 15.0, 80.0,
+                                      taus, out), 20)
     vsd_bytes = 2 * len(sel) * 480 * 640 * 4 + 480 * 640 * 4
     ms_render = events(lambda: render.render([mesh], torch.from_numpy(poses).cuda(), K, 480, 640), 3)
 

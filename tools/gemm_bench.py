@@ -23,8 +23,8 @@ for (M, N, K) in [(6304, 1792, 256), (6304, 256, 256), (6304, 512, 256), (6304, 
 # batched score matrix 32 x (2049 x 2049 x 256)
 B, S, C = 32, 2049, 256
 f1 = torch.randn(B, S, C, device="cuda"); f2 = torch.randn(B, S, C, device="cuda"); out = torch.empty(B, S, S, device="cuda")
-t0 = timeit(lambda: ops.gemm_raw(f1.data_ptr(), f2.data_ptr(), None, 0, out.data_ptr(), S, S, C, C, C, S, 0, batch=B, sA=S*C, sW=S*C, sC=S*S, alpha=10.0), n=5)
-t1 = timeit(lambda: ops.gemm_tc_raw(f1.data_ptr(), 0, f2.data_ptr(), 0, None, 0, out.data_ptr(), 0, S, S, C, C, C, S, 0, batch=B, sA=S*C, sW=S*C, sC=S*S, alpha=10.0), n=5)
+t0 = timeit(lambda: ops.gemm(f1, f2, out=out, alpha=10.0), n=5)
+t1 = timeit(lambda: ops.gemm_tc(f1, f2, out=out, alpha=10.0), n=5)
 fl = 2.0 * B * S * S * C
 print(f"fine score 32x2049x2049x256: simt {t0:.3f} ms ({fl/t0/1e9:.1f} TF)  tc {t1:.3f} ms ({fl/t1/1e9:.1f} TF; output write {B*S*S*4/t1/1e6:.0f} GB/s)")
 

@@ -15,8 +15,7 @@ bias = torch.randn(256, device="cuda")
 for dt in (torch.bfloat16, torch.float32):
     E = torch.empty(npairs, 256, device="cuda", dtype=dt)
     def run():
-        _lib.call("sam6d_geo_embed_tc", T.data_ptr(), npairs, div.data_ptr(), Wa.data_ptr(), Wd.data_ptr(), bias.data_ptr(),
-                  E.data_ptr(), 1 if dt == torch.bfloat16 else 0, None)
+        _lib.call("sam6d_geo_embed_tc", T, npairs, div, Wa, Wd, bias, E, 1 if dt == torch.bfloat16 else 0)
     for _ in range(3): run()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -10,7 +10,6 @@ with nvidia-smi in the same run.
 
     python tools/sam_predictor_bench.py [--iters 10] [--types vit_b,vit_h]"""
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -112,9 +111,7 @@ def main():
             for T in (8, 32):
                 Q = torch.randn(B, T, 128, device=dev)
                 O = torch.empty_like(Q)
-                call = lambda: _lib.call("sam6d_sam_tok2img_attn", ctypes.c_void_p(Q.data_ptr()), ctypes.c_void_p(K.data_ptr()),  # noqa: E731
-                                         ctypes.c_void_p(V.data_ptr()), ctypes.c_longlong(L * 128), B, T, L, ctypes.c_void_p(O.data_ptr()),
-                                         ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+                call = lambda: _lib.call("sam6d_sam_tok2img_attn", Q, K, V, L * 128, B, T, L, O)  # noqa: E731
                 r[f"tok2img_b64_T{T}_us"] = round(_kernel_us(_lib, "sam6d_sam_tok2img_attn", call, args.iters), 1)
             del K, V, m
         amg = CustomSamAutomaticMaskGenerator(sam, points_per_batch=64, stability_score_thresh=0.97, box_nms_thresh=0.7,
