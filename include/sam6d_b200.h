@@ -384,6 +384,29 @@ int sam6d_attn_global_tc(const void* qkv, long long ld, const void* Vt, long lon
 int sam6d_attn_global_tc_ex(const void* qkv, long long ld, const void* Vt, long long vt_ld, const void* rel_blob, int B, int H, int grid,
                             int head_dim, float scale, void* out, int out_is_bf16, long long out_ld, void* stream);
 
+/* ---- depth refinement of PEM poses: point-to-plane ICP (not in the reference; csrc/icp.cu, oracle/icp_oracle.py) ------------ */
+/* B instances, each a pose R (B,3,3) row-major and t (B,3) f32 (object -> camera, metres), observed points pts (B,N,3) f32
+ * (camera frame, metres), object obj[b] in [0,O) with samples (O,M,3) and unit normals (O,M,3) f32 (object frame, metres) and
+ * radius (B) f32 > 0 (the object's max |model point|).  All contiguous.  The pose is kept in fp64; iteration k = 0 .. iters-1:
+ * y_i = R^T (p_i - t) in fp32 with the pose rounded to fp32; j(i) = argmin_j |y_i - q_j|^2 in fp32, an exact tie to the lowest j;
+ * inliers |y_i - q_j(i)|^2 < tau_k^2, tau_k = radius * max(0.3 * 2^-k, 0.05); over the inliers, in fp64 with coordinates / radius,
+ * e_i = n_j . (y_i - q_j), J_i = [(y_i x n_j)^T, n_j^T], (sum J^T J + lambda I) delta = sum J^T e with lambda = 1e-4 trace / 6,
+ * solved by Cholesky; delta = (w, v): R <- R Exp(w), t <- t + R_old (radius v).  An instance stops with fewer than 32 inliers
+ * (the pose of that iteration's start is kept, so at k = 0 the input comes back bit for bit) or after applying a step with
+ * |w| < 1e-7 and |v| < 1e-7.  Outputs: R_out (B,3,3), t_out (B,3) f32; inliers (B) i32 and rms (B) f32 (metres, the
+ * point-to-plane RMS before the update) of the last iteration evaluated; iters_run (B) i32, the pose updates applied.  An
+ * instance whose obj is out of range or whose radius is not a positive finite number comes back unrefined with inliers -1.
+ * Optional (NULL: not written), of the last iteration evaluated: corr (B,N) i32 = j(i) for an inlier, -1 - j(i) for an outlier;
+ * sums (B,29) f64 = the upper triangle of sum J^T J row by row (21), sum J^T e (6), the inlier count, sum e^2.
+ * Results are bit-reproducible.  -22: B < 0, N < 1, O < 1, M < 1, iters < 0, a NULL pointer with B > 0, or M above
+ * sam6d_icp_max_samples(). */
+int sam6d_icp_refine(const float* R, const float* t, const float* pts, int B, int N, const float* samples, const float* normals,
+                     int O, int M, const int* obj, const float* radius, int iters, float* R_out, float* t_out, int* inliers,
+                     float* rms, int* iters_run, int* corr, double* sums, void* stream);
+/* the largest M sam6d_icp_refine accepts on the current device (its samples and normals fill the opt-in shared memory of one
+ * CTA); a negative value is minus a CUDA error.  Not a status code: call it directly, not through the status-checking wrapper. */
+int sam6d_icp_max_samples(void);
+
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):
  * 0 mean, 1 median (torch.median's lower median), 2 max, 3 avg_5.  sim_out (P,O,T) optional; obj_score (P,O) f32 and obj_tmpl

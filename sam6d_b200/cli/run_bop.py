@@ -45,6 +45,8 @@ def get_parser():
     ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
+    # not in the reference: refine each PEM pose against the observed depth (pipeline.icp_refine_out)
+    ap.add_argument("--icp_iters", default=0, type=int, help="point-to-plane ICP iterations per PEM pose (0: off)")
     return ap
 
 
@@ -70,7 +72,8 @@ def main(argv=None):
                   pred_iou_thresh=args.pred_iou_thresh, points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
                   precision=args.precision, level_templates=args.level_templates, pose_distribution=args.pose_distribution,
                   aggregation_function=args.aggregation_function, rendering_type=args.rendering_type,
-                  pbr_root=dataset_root if args.rendering_type == "pbr" else None, pbr_split=args.pbr_split)
+                  pbr_root=dataset_root if args.rendering_type == "pbr" else None, pbr_split=args.pbr_split,
+                  icp_iters=args.icp_iters)
     os.makedirs(args.output_dir, exist_ok=True)
     if args.stage in ("ism", "both"):
         objects = sam6d.onboard_bop(args.bop_root, args.dataset_name, template_size=args.template_size)

@@ -67,6 +67,8 @@ def get_parser():
     ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth (default: the PEM CLI's)")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
+    # not in the reference: refine each PEM pose against the observed depth (pipeline.icp_refine_out)
+    ap.add_argument("--icp_iters", default=0, type=int, help="point-to-plane ICP iterations per PEM pose (0: off)")
     return ap
 
 
@@ -83,7 +85,8 @@ def main(argv=None):
                   points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
                   det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
                   pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
-                  rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split)
+                  rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split,
+                  icp_iters=args.icp_iters)
     multi = isinstance(args.cad_path, list)
     n_cad = len(args.cad_path) if multi else 1
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:

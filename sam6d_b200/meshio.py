@@ -122,16 +122,26 @@ def load_ply_mesh(path, read_texture: bool = True) -> Mesh:
     return Mesh(verts, faces, _colors(cols), uv, texture, tex_file)
 
 
-def sample_surface(verts, faces, n, rng=None):
-    """area-weighted random points on the triangles (trimesh.sample.sample_surface semantics); vertices when there are no faces"""
+def sample_surface(verts, faces, n, rng=None, return_normals: bool = False):
+    """area-weighted random points on the triangles (trimesh.sample.sample_surface semantics); vertices when there are no faces.
+    rng: numpy's global RNG (default), a RandomState or a Generator.  return_normals: also the unit normal of each point's
+    face, (b - a) x (c - a) normalised (float32), from the same draws; a mesh without faces has none (ValueError)."""
     rng = rng if rng is not None else np.random
+    uniform = rng.random if isinstance(rng, np.random.Generator) else rng.random_sample
     if len(faces) == 0:
+        if return_normals:
+            raise ValueError("sample_surface: a mesh without faces has no normals")
         return verts[rng.choice(len(verts), n, replace=len(verts) < n)].astype(np.float32)
     a, b, c = verts[faces[:, 0]].astype(np.float64), verts[faces[:, 1]].astype(np.float64), verts[faces[:, 2]].astype(np.float64)
-    area = 0.5 * np.linalg.norm(np.cross(b - a, c - a), axis=1)
-    f = np.searchsorted(np.cumsum(area), rng.random_sample(n) * area.sum())
+    cross = np.cross(b - a, c - a)
+    area = 0.5 * np.linalg.norm(cross, axis=1)
+    f = np.searchsorted(np.cumsum(area), uniform(n) * area.sum())
     f = np.minimum(f, len(faces) - 1)
-    u = rng.random_sample((n, 2))
+    u = uniform((n, 2))
     flip = u.sum(axis=1) > 1.0
     u[flip] = 1.0 - u[flip]
-    return (a[f] + u[:, :1] * (b[f] - a[f]) + u[:, 1:] * (c[f] - a[f])).astype(np.float32)
+    pts = (a[f] + u[:, :1] * (b[f] - a[f]) + u[:, 1:] * (c[f] - a[f])).astype(np.float32)
+    if not return_normals:
+        return pts
+    nrm = cross[f] / np.maximum(2.0 * area[f], np.finfo(np.float64).tiny)[:, None]
+    return pts, nrm.astype(np.float32)

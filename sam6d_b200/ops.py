@@ -795,6 +795,53 @@ def pose_score(pts1: Tensor, lab1: Tensor, R: Tensor, t: Tensor, model: Tensor, 
     return score, ts
 
 
+# ---------------------------------------------------------------------------------------------- depth refinement
+def icp_max_samples() -> int:
+    """the largest number of samples per object icp_refine accepts on the current device"""
+    m = _lib.lib().sam6d_icp_max_samples()
+    if m < 0:
+        raise _lib.Sam6dError(f"sam6d_icp_max_samples: CUDA error {-m}")
+    return m
+
+
+def icp_refine(R: Tensor, t: Tensor, pts: Tensor, samples: Tensor, normals: Tensor, obj: Tensor, radius: Tensor, iters: int,
+               system: bool = False):
+    """point-to-plane ICP of B poses against their observed points (the algorithm: include/sam6d_b200.h, sam6d_icp_refine).
+    R (B,3,3), t (B,3), pts (B,N,3) f32 camera frame, metres; samples, normals (O,M,3) f32 object frame; obj (B) i32 object of
+    each instance; radius (B) f32 -> (R, t refined, inliers (B) i32, rms (B) f32 metres, iters_run (B) i32).  An instance with
+    an out-of-range obj or a non-positive radius comes back unrefined with inliers -1.  system=True also returns, of the last
+    iteration evaluated, corr (B,N) i32 (j(i) of an inlier, -1 - j(i) of an outlier) and sums (B,29) f64 (the normal
+    equations' upper triangle of A, b, the inlier count and sum e^2)."""
+    _check(R, torch.float32, "R", 3)
+    _check(t, torch.float32, "t", 2)
+    _check(pts, torch.float32, "pts", 3)
+    _check(samples, torch.float32, "samples", 3)
+    _check(normals, torch.float32, "normals", 3)
+    _check(obj, torch.int32, "obj", 1)
+    _check(radius, torch.float32, "radius", 1)
+    B, N, c = pts.shape
+    O, M, cs = samples.shape
+    if c != 3 or cs != 3 or normals.shape != samples.shape:
+        raise RuntimeError(f"icp_refine: pts must be (B,N,3) and samples, normals (O,M,3), got {tuple(pts.shape)}, "
+                           f"{tuple(samples.shape)}, {tuple(normals.shape)}")
+    if R.shape != (B, 3, 3) or t.shape != (B, 3) or obj.shape != (B,) or radius.shape != (B,):
+        raise RuntimeError(f"icp_refine: R (B,3,3), t (B,3), obj (B), radius (B) with B = {B}, got {tuple(R.shape)}, "
+                           f"{tuple(t.shape)}, {tuple(obj.shape)}, {tuple(radius.shape)}")
+    dev = pts.device
+    R_out = torch.empty_like(R)
+    t_out = torch.empty_like(t)
+    inliers = torch.empty(B, dtype=torch.int32, device=dev)
+    rms = torch.empty(B, dtype=torch.float32, device=dev)
+    iters_run = torch.empty(B, dtype=torch.int32, device=dev)
+    corr = torch.empty(B, N, dtype=torch.int32, device=dev) if system else None
+    sums = torch.empty(B, 29, dtype=torch.float64, device=dev) if system else None
+    _lib.call("sam6d_icp_refine", R, t, pts, B, N, samples, normals, O, M, obj, radius, int(iters), R_out, t_out, inliers, rms,
+              iters_run, corr, sums)
+    if system:
+        return R_out, t_out, inliers, rms, iters_run, corr, sums
+    return R_out, t_out, inliers, rms, iters_run
+
+
 # ---------------------------------------------------------------------------------------------- SAM encoder attention
 def attn_relpos(qkv: Tensor, nW: int, Hs: int, Ws: int, nH: int, rel_h: Tensor, rel_w: Tensor, scale: float,
                 out_dtype=torch.float32) -> Tensor:

@@ -33,6 +33,8 @@ from .cli import pem_run_inference_custom as pem_cli
 from .cli import render_custom_templates as render_cli
 
 N_ISM_CLOUD = 2048                     # points of the geometric score's template cloud (ISM/run_inference_custom.py:196)
+ICP_SAMPLES = 4096                     # surface samples per object for the ICP refinement (icp_iters > 0; not in the reference)
+ICP_SEED = 6                           # their draws come from this seed, never from the caller's rng
 RENDERING_TYPES = ("pyrender", "pbr")  # onboarding_config.rendering_type: the ISM references are renders, or BOP PBR frames
 
 
@@ -188,14 +190,15 @@ def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
 
 # ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
 def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
-              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None):
+              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None, icp=None, icp_iters: int = 0):
     """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
     enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
     model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
     else from torch's global CUDA generator (the reference's torch.rand).  mark(stage) after the inputs and after the forward.
     Several objects: bank (O,2048,3), (O,2048,256), model_points_m (O,n,3) and det_obj the object index of every record; each
     detection gets its object's radius filter, model points and template bank, and all run as one batch.  The frame then also
-    holds obj (P) int64, choose_idx (P,2048) and rand, the coarse stage's uniforms."""
+    holds obj (P) int64, choose_idx (P,2048) and rand, the coarse stage's uniforms.  icp_iters > 0: after the forward the poses
+    are refined by icp_refine_out against the observed points with icp = (samples, normals) (O,M,3) on the device."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
     input_data, img, _, model_points, kept = inputs.get_test_data(
@@ -215,6 +218,9 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
             if generator is not None:
                 rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
             out = model(input_data, rand=rand)
+            if icp_iters > 0:
+                obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int32, device=input_data["pts"].device)
+                icp_refine_out(out, input_data["pts"], input_data["model"], obj, icp, icp_iters)
     mark("forward")
     frame = SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
     if det_obj is not None:
@@ -239,16 +245,48 @@ def pem_records(frame):
     return records
 
 
+# ---- depth refinement of the PEM poses (not in the reference) ---------------------------------------------------------------
+def icp_model(verts_mm: np.ndarray, faces: np.ndarray):
+    """a CAD model in mm -> (ICP_SAMPLES surface points (M,3) f32 in metres, their unit face normals (M,3) f32), drawn from
+    np.random.default_rng(ICP_SEED): the same samples for the same mesh, and no draw from any caller's RNG"""
+    pts, nrm = meshio.sample_surface(verts_mm, faces, ICP_SAMPLES, np.random.default_rng(ICP_SEED), return_normals=True)
+    return pts / np.float32(1000.0), nrm
+
+
+def icp_tensors(points_m, normals, device):
+    """icp_model arrays of one object (M,3) or of O objects (O,M,3) -> (samples, normals) (O,M,3) f32 on the device"""
+    if points_m is None or normals is None:
+        raise ValueError("ICP refinement needs the objects' ICP samples: onboard them with SAM6D(..., icp_iters > 0)")
+    m = np.asarray(points_m).shape[-2]
+    return tuple(torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.float32).reshape(-1, m, 3))).to(device)
+                 for a in (points_m, normals))
+
+
+def icp_refine_out(out: dict, pts: torch.Tensor, model: torch.Tensor, obj: torch.Tensor, icp, iters: int):
+    """refine Net.forward's poses against the observed points pts (P,N,3) in place: out["pred_R"], out["pred_t"] become the
+    refined pose, the PEM's stays in out["pem_R"], out["pem_t"]; out["icp_inliers"] (P) i32 and out["icp_rms"] (P) f32 (metres)
+    are the last iteration's inlier count and point-to-plane RMS.  model (P,n,3): each instance's model points, whose max norm
+    is its object radius; obj (P): its object index into icp = (samples, normals) (O,M,3)."""
+    radius = model.norm(dim=2).amax(dim=1).contiguous()
+    R, t, inliers, rms, _ = ops.icp_refine(out["pred_R"].contiguous(), out["pred_t"].contiguous(), pts.contiguous(), icp[0], icp[1],
+                                           obj.to(torch.int32).contiguous(), radius, iters)
+    out.update(pem_R=out["pred_R"], pem_t=out["pred_t"], pred_R=R, pred_t=t, icp_inliers=inliers, icp_rms=rms)
+    return out
+
+
 # ---- the whole pipeline ----------------------------------------------------------------------------------------------------
 @dataclass
 class Onboarded:
-    """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank, model points"""
+    """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank, model points;
+    with icp_iters > 0 also the ICP samples (M,3) in metres and their unit normals (icp_model), else None"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
     cloud_m: np.ndarray
     bank: tuple
     model_points_m: np.ndarray
+    icp_points_m: Optional[np.ndarray] = None
+    icp_normals: Optional[np.ndarray] = None
 
 
 class SAM6D:
@@ -265,7 +303,10 @@ class SAM6D:
     frames of the BOP split pbr_root/pbr_split (sam6d_b200/pbr.py: for each view the frame whose object pose is nearest it,
     cut out with its visible mask), which needs each object's BOP id and pose_distribution "all".  The split is scanned once,
     at the first onboarding.  The geometric-score poses, the template cloud, the PEM bank and the model points come from the
-    mesh either way."""
+    mesh either way.
+
+    icp_iters (not in the reference; default 0, off): refine every PEM pose with that many point-to-plane ICP iterations
+    against the frame's observed points (icp_refine_out).  Records then carry the refined R and t; scores are unchanged."""
     rendering_type = "pyrender"
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
@@ -274,7 +315,7 @@ class SAM6D:
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
                  device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5",
                  fastsam_model: str = "FastSAM-x", rendering_type: str = "pyrender", pbr_root: Optional[str] = None,
-                 pbr_split: str = "train_pbr"):
+                 pbr_split: str = "train_pbr", icp_iters: int = 0):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
         if fastsam_model not in ism_cli.FASTSAM_MODELS:
@@ -290,6 +331,9 @@ class SAM6D:
             if pose_distribution != "all":
                 raise NotImplementedError(f'rendering_type "pbr" selects references for pose_distribution "all" only, got {pose_distribution!r}')
             pbr.list_scenes(pbr_root, pbr_split)                              # FileNotFoundError without the split
+        if int(icp_iters) < 0:
+            raise ValueError(f"icp_iters must be >= 0, got {icp_iters}")
+        self.icp_iters = int(icp_iters)
         self.rendering_type, self.pbr_root, self.pbr_split, self._pbr_rows = rendering_type, pbr_root, pbr_split, None
         self.level_templates, self.pose_distribution = int(level_templates), pose_distribution
         self.aggregation_function = aggregation_function
@@ -349,7 +393,8 @@ class SAM6D:
         bank = pem_template_bank(self.pem, list(rgbs[:n0]), list(masks[:n0]), [x.astype(np.float32) for x in xyzs[:n0]], rng=rng,
                                  device=self.device)
         model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
-        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points)
+        icp_pts, icp_nrm = icp_model(verts, faces) if self.icp_iters > 0 else (None, None)
+        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points, icp_pts, icp_nrm)
 
     def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
         """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
@@ -438,7 +483,7 @@ class SAM6D:
         chunk of 16).  Random draws from `rng` (default numpy's global RNG): the model points of every object, each object's
         42 template samples, then the observed points in detection order.  An image none of whose detections survives is
         skipped (the reference fails there).  Writes the CSV lines to out_path and returns them.  mark(stage) after
-        "onboard", and per image after "decode", "pem_inputs" and "forward"."""
+        "onboard", and per image after "decode", "pem_inputs" and "forward".  icp_iters > 0: each image's poses are refined (icp_refine_out) before its rows are built."""
         mark = mark or (lambda stage: None)
         rng = rng if rng is not None else np.random
         cfg = pem_cli.TEST_DATASET
@@ -450,6 +495,9 @@ class SAM6D:
                                    device=self.device) for i in objs.ids]
         bank = tuple(torch.stack([b[k].reshape(b[k].shape[-2:]) for b in banks]) for k in range(2))
         del banks
+        icp = None
+        if self.icp_iters > 0:
+            icp = icp_tensors(*(np.stack(a) for a in zip(*[icp_model(m.vertices, m.faces) for m in meshes])), self.device)
         mark("onboard")
         with open(detections_path) as fh:
             groups = bop.group_detections(json.load(fh))
@@ -473,6 +521,8 @@ class SAM6D:
             rand = bop.pem_rand(g, n, n_rand, self.device)
             with torch.no_grad():
                 out = self.pem(data, rand=rand)
+                if icp is not None:
+                    icp_refine_out(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters)
             scores = (out["pred_pose_score"] * data["score"]).cpu().numpy()
             R = out["pred_R"].reshape(-1, 9).cpu().numpy()
             t = out["pred_t"].cpu().numpy() * 1000
@@ -514,8 +564,9 @@ class SAM6D:
                                    n_proposals=det.n_proposals, reason=None, ism_time=ism_time, **({"obj": det.obj} if multi else {}))
         g = torch.Generator(device=self.device)
         g.manual_seed(pem_cli.RD_SEED)
+        icp = icp_tensors(obj.icp_points_m, obj.icp_normals, self.device) if self.icp_iters > 0 else None
         frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
-                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj)
+                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj, icp=icp, icp_iters=self.icp_iters)
         pem_recs = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
@@ -529,7 +580,8 @@ class ObjectSet:
     """several objects after SAM6D.onboard_objects, stacked along a leading object axis O: ISM references ref_cls (O,T,C) and
     ref_patch (O,T,256,C), template poses poses_m (O,T,4,4) (the framing distance depends on the mesh), geometric-score clouds
     cloud_m (O,2048,3), PEM template banks (O,2048,3) and (O,2048,256), model points model_points_m (O,Nm,3), each object's
-    radius (O,) (the PEM's max |model point|) and category ids obj_ids"""
+    radius (O,) (the PEM's max |model point|) and category ids obj_ids; with icp_iters > 0 the ICP samples icp_points_m (O,M,3)
+    and their normals icp_normals (O,M,3), else None"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
@@ -538,12 +590,17 @@ class ObjectSet:
     model_points_m: np.ndarray
     radii: np.ndarray
     obj_ids: list
+    icp_points_m: Optional[np.ndarray] = None
+    icp_normals: Optional[np.ndarray] = None
 
     @staticmethod
     def stack(parts, ref_patch, obj_ids) -> "ObjectSet":
         """Onboarded objects (their ref_patch already stacked into `ref_patch`) -> ObjectSet"""
         mp = np.stack([np.asarray(p.model_points_m, dtype=np.float32) for p in parts])
+        icp = parts[0].icp_points_m is not None
         return ObjectSet(ref_cls=torch.stack([p.ref_cls for p in parts]), ref_patch=ref_patch,
                          poses_m=np.stack([p.poses_m for p in parts]), cloud_m=np.stack([p.cloud_m for p in parts]),
                          bank=tuple(torch.stack([p.bank[i].reshape(p.bank[i].shape[-2:]) for p in parts]) for i in range(2)),
-                         model_points_m=mp, radii=np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp]), obj_ids=list(obj_ids))
+                         model_points_m=mp, radii=np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp]), obj_ids=list(obj_ids),
+                         icp_points_m=np.stack([p.icp_points_m for p in parts]) if icp else None,
+                         icp_normals=np.stack([p.icp_normals for p in parts]) if icp else None)
