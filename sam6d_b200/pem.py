@@ -118,27 +118,30 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
     return t.detach().to(torch.float32).contiguous()
 
 
-def _stack2(a: torch.Tensor, b: torch.Tensor) -> Optional[torch.Tensor]:
-    """The scene cloud and the template cloud go through the same weights in most layers.  When their tensors are the two
-    halves of one allocation (Net.forward builds them that way) return the (2B, ...) view so one launch serves both clouds;
-    otherwise None and the caller makes two calls (the reference API passes them as separate arguments)."""
-    if (a.shape == b.shape and a.dtype == b.dtype and a.is_contiguous() and b.is_contiguous() and a.device == b.device
+def _pair(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """The scene cloud and the template cloud go through the same weights in most layers, so the modules run them as one
+    (2B, ...) batch [a ; b].  That is a view when a and b are the two halves of one allocation (Net.forward builds them that
+    way) and a concatenated copy otherwise (the reference API passes them as separate arguments): the kernels see the same
+    batch either way, so results do not depend on how the caller allocated the clouds."""
+    if a.shape != b.shape or a.dtype != b.dtype:
+        raise ValueError(f"the two clouds must have equal shapes and dtypes: {tuple(a.shape)} {a.dtype}, {tuple(b.shape)} {b.dtype}")
+    if (a.is_contiguous() and b.is_contiguous() and a.device == b.device
             and a.untyped_storage().data_ptr() == b.untyped_storage().data_ptr()
             and b.storage_offset() == a.storage_offset() + a.numel()):
-        return torch.as_strided(a, (2 * a.shape[0],) + tuple(a.shape[1:]), a.stride(), a.storage_offset())
-    return None
+        return torch.as_strided(a, (2 * a.numel(),), (1,), a.storage_offset()).view(2 * a.shape[0], *a.shape[1:])
+    return torch.cat([a, b])
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # shared token-layer math
 # ---------------------------------------------------------------------------------------------------------------------
-def _attn_tail(prec, x2d: torch.Tensor, hid: torch.Tensor, lw) -> torch.Tensor:
-    """AttentionLayer / RPEAttentionLayer tail + AttentionOutput (transformer.py:176-197, 435-438):
+def _attn_tail(x2d: torch.Tensor, hid: torch.Tensor, lw) -> torch.Tensor:
+    """AttentionLayer / RPEAttentionLayer tail + AttentionOutput (transformer.py:176-197, 435-438), fp32:
        y = LN(linear(hid) + x);  out = LN(y + squeeze(relu(expand(y))))"""
-    y = _gemm(prec, hid, lw["wo"], lw["bo"], residual=x2d)
+    y = ops.gemm(hid, lw["wo"].f32, lw["bo"], residual=x2d)
     y = ops.layernorm(y, lw["g1"], lw["b1"])
-    h = _gemm(prec, y, lw["we"], lw["be"], relu=True)
-    z = _gemm(prec, h, lw["ws"], lw["bs"], residual=y)
+    h = ops.gemm(y, lw["we"].f32, lw["be"], relu=True)
+    z = ops.gemm(h, lw["ws"].f32, lw["bs"], residual=y)
     return ops.layernorm(z, lw["g2"], lw["b2"])
 
 
@@ -190,7 +193,8 @@ class GeometricTransformer(nn.Module):
             ca = self.layers[1].attention.attention
             self._packed.w = dict(
                 w_self=_W(w_self), b_self=b_self.contiguous(), tail_self=_pack_tail(self.layers[0]),
-                # tensor-core attention path: q|k|v as one bf16 GEMM, the folded rel-pos queries u as a second (fp32) one
+                # bf16 self-attention outside rpe_tc's reach (_self_bf16): q|k|v as one bf16 GEMM, the folded rel-pos queries u
+                # as a second (fp32) one
                 w_qkv=_W(w_self[:3 * C]), b_qkv=b_self[:3 * C].contiguous(), w_u=_W(w_self[3 * C:]), b_u=b_self[3 * C:].contiguous(),
                 wq_c=_W(ca.proj_q.weight), bq_c=_f32(ca.proj_q.bias),
                 wkv_c=_W(torch.cat([_f32(ca.proj_k.weight), _f32(ca.proj_v.weight)], dim=0)),
@@ -202,43 +206,29 @@ class GeometricTransformer(nn.Module):
             self._packed.key = key
         return self._packed.w
 
+    # ---- fp32 (precision="fp32"): CUDA-core kernels, fp32 storage
     def _self_layer(self, x: torch.Tensor, emb: torch.Tensor, w) -> torch.Tensor:
         B, S, C = x.shape
         x2d = x.reshape(B * S, C)
-        if self.precision == "bf16" and S <= 256:
-            d = C // NUM_HEADS
-            qkv = ops.gemm_tc(x2d, w["w_qkv"].bf16, w["b_qkv"], out_dtype=torch.bfloat16)          # (B*S, q|k|v) bf16
-            u = ops.gemm_tc(x2d, w["w_u"].bf16, w["b_u"])                                            # (B*S, 4*C) fp32
-            sp = ops.rpe_scores(emb, u)
-            vt = ops.transpose_tokens(qkv, 2 * C, C, B, S)
-            hid = ops.attn_tc(qkv, 0, qkv, C, vt, B, NUM_HEADS, S, S, d, 1.0 / math.sqrt(d), bias=sp)
-            return _attn_tail(self.precision, x2d, hid, w["tail_self"]).view(B, S, C)
-        qkvu = _gemm(self.precision, x2d, w["w_self"], w["b_self"])              # (B*S, q|k|v|u0..u3)
+        qkvu = ops.gemm(x2d, w["w_self"].f32, w["b_self"])                       # (B*S, q|k|v|u0..u3)
         sp = ops.rpe_scores(emb, qkvu[:, 3 * C:])                                  # (B,H,S,S)
         hid = torch.empty(B * S, C, dtype=torch.float32, device=x.device)
         qkv = qkvu.view(B, S, -1)
         ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:3 * C], sp, 1.0 / math.sqrt(C // NUM_HEADS), hid.view(B, S, C))
-        return _attn_tail(self.precision, x2d, hid, w["tail_self"]).view(B, S, C)
+        return _attn_tail(x2d, hid, w["tail_self"]).view(B, S, C)
 
     def _cross_layer(self, x: torch.Tensor, mem: torch.Tensor, w) -> torch.Tensor:
         B, S, C = x.shape
         Sm = mem.shape[1]
         x2d = x.reshape(B * S, C)
-        if self.precision == "bf16" and Sm <= 256:
-            d = C // NUM_HEADS
-            q = ops.gemm_tc(x2d, w["wq_c"].bf16, w["bq_c"], out_dtype=torch.bfloat16)
-            kv = ops.gemm_tc(mem.reshape(B * Sm, C), w["wkv_c"].bf16, w["bkv_c"], out_dtype=torch.bfloat16)
-            vt = ops.transpose_tokens(kv, C, C, B, Sm)
-            hid = ops.attn_tc(q, 0, kv, 0, vt, B, NUM_HEADS, S, Sm, d, 1.0 / math.sqrt(d))
-            return _attn_tail(self.precision, x2d, hid, w["tail_cross"]).view(B, S, C)
-        q = _gemm(self.precision, x2d, w["wq_c"], w["bq_c"])
-        kv = _gemm(self.precision, mem.reshape(B * Sm, C), w["wkv_c"], w["bkv_c"]).view(B, Sm, 2 * C)
+        q = ops.gemm(x2d, w["wq_c"].f32, w["bq_c"])
+        kv = ops.gemm(mem.reshape(B * Sm, C), w["wkv_c"].f32, w["bkv_c"]).view(B, Sm, 2 * C)
         hid = torch.empty(B * S, C, dtype=torch.float32, device=x.device)
         ops.mha(q.view(B, S, C), kv[..., :C], kv[..., C:], None, 1.0 / math.sqrt(C // NUM_HEADS), hid.view(B, S, C))
-        return _attn_tail(self.precision, x2d, hid, w["tail_cross"]).view(B, S, C)
+        return _attn_tail(x2d, hid, w["tail_cross"]).view(B, S, C)
 
-    # ---- bf16 token stream (precision="bf16", both clouds in one allocation): every Linear is the persistent TMA GEMM, the
-    # residual stream, LayerNorm inputs/outputs and the attention output are bf16, accumulation and statistics fp32.
+    # ---- bf16 token stream (precision="bf16"): every Linear is the persistent TMA GEMM, the residual stream, LayerNorm
+    # inputs/outputs and the attention output are bf16, accumulation and statistics fp32.
     def _self_bf16(self, x, emb, w):
         B, S, C = x.shape
         d = C // NUM_HEADS
@@ -282,23 +272,14 @@ class GeometricTransformer(nn.Module):
         if masks0 is not None or masks1 is not None:
             raise NotImplementedError("key masks are never used on the SAM-6D inference path")
         w = self._weights()
-        emb = _stack2(embeddings0, embeddings1) if feats0.shape == feats1.shape else None
-        if emb is not None and self.precision == "bf16" and feats0.shape[1] <= 256:
-            B = feats0.shape[0]
-            f = _stack2(feats0, feats1)
-            if f is None:
-                f = torch.cat([feats0, feats1], dim=0)
+        B = feats0.shape[0]
+        # both clouds share the self-attention weights: one batch of 2B through every kernel of the layer
+        f, emb = _pair(feats0, feats1), _pair(embeddings0, embeddings1)
+        if self.precision == "bf16":
             f = self._forward_bf16(f.to(torch.bfloat16).contiguous(), emb, w)
             return f[:B], f[B:]
-        if emb is not None:
-            # both clouds share the self-attention weights: one batch of 2B through every kernel of the layer
-            B = feats0.shape[0]
-            f = _stack2(feats0, feats1)
-            f = self._self_layer(f if f is not None else torch.cat([feats0, feats1], dim=0), emb, w)
-            feats0, feats1 = f[:B], f[B:]
-        else:
-            feats0 = self._self_layer(feats0.contiguous(), embeddings0, w)
-            feats1 = self._self_layer(feats1.contiguous(), embeddings1, w)
+        f = self._self_layer(f, emb, w)
+        feats0, feats1 = f[:B], f[B:]
         feats0 = self._cross_layer(feats0, feats1, w)
         feats1 = self._cross_layer(feats1, feats0, w)      # sequential: sees the updated feats0 (transformer.py:505-507)
         return feats0, feats1
@@ -488,24 +469,15 @@ class CoarsePointMatching(nn.Module):
     def forward(self, p1, f1, geo1, p2, f2, geo2, radius, end_points, rand=None):
         if self.training:
             raise NotImplementedError("sam6d_b200 implements the inference path (model.eval())")
-        f12 = _stack2(f1, f2)
-        if f12 is not None:
-            e = self._embed(f12)
-            f1, f2 = e[:f1.shape[0]], e[f1.shape[0]:]
-        else:
-            f1 = self._embed(f1.contiguous())
-            f2 = self._embed(f2.contiguous())
+        B = f1.shape[0]
+        e = self._embed(_pair(f1, f2))
+        f1, f2 = e[:B], e[B:]
         for blk in self.transformers:
             f1, f2 = blk(f1, geo1, f2, geo2)
-        B, S, H = f1.shape
+        S, H = f1.shape[1:]
         w = self._weights()
-        f12 = _stack2(f1, f2)
-        if f12 is not None:                                     # both clouds: one out_proj launch
-            o = _gemm(self.precision, f12.reshape(2 * B * S, H), w["w_out"], w["b_out"]).view(2 * B, S, -1)
-            o1, o2 = o[:B], o[B:]
-        else:
-            o1 = _gemm(self.precision, f1.reshape(B * S, H), w["w_out"], w["b_out"]).view(B, S, -1)
-            o2 = _gemm(self.precision, f2.reshape(B * S, H), w["w_out"], w["b_out"]).view(B, S, -1)
+        o = _gemm(self.precision, _pair(f1, f2).reshape(2 * B * S, H), w["w_out"], w["b_out"]).view(2 * B, S, -1)
+        o1, o2 = o[:B], o[B:]
         atten = compute_feature_similarity(o1, o2, self.cfg.sim_type, self.cfg.temp, self.cfg.normalize_feat, self.precision)
         model = ops.scale_by_radius(end_points['model'].contiguous(), radius.contiguous())
         init_R, init_t, self.last_select_scores = compute_coarse_Rt(atten, p1, p2, model, self.cfg.nproposal1,
@@ -585,12 +557,11 @@ class PositionalEncoding(nn.Module):
         pts = pts.contiguous()
         B, N, _ = pts.shape
         feat = torch.empty(B, N, 256, dtype=torch.bfloat16 if self.precision == "bf16" else torch.float32, device=pts.device)
-        pair = ops.ball_query_pair(pts, pts, self.r1, self.ns1, self.r2, self.ns2) if self.r1 <= self.r2 else None
-        for r, ns, name, off in ((self.r1, self.ns1, "m1", 0), (self.r2, self.ns2, "m2", 128)):
-            if pair is not None:
-                idx, cnt = pair[:2] if off == 0 else pair[2:]
-            else:
-                idx, cnt = ops.ball_query(pts, pts, r, ns, return_count=True)
+        # ball_query_pair takes the smaller radius first; its outputs are those of two ball_query calls
+        (ra, nsa, name_a, off_a), (rb, nsb, name_b, off_b) = sorted(
+            ((self.r1, self.ns1, "m1", 0), (self.r2, self.ns2, "m2", 128)), key=lambda s: s[0])
+        ia, ca, ib, cb = ops.ball_query_pair(pts, pts, ra, nsa, rb, nsb)
+        for name, off, idx, cnt in ((name_a, off_a, ia, ca), (name_b, off_b, ib, cb)):
             if self.precision == "bf16":
                 ops.pe_mlp_max_tc(pts, idx, w[name + "_tc"], feat, off)
             else:
@@ -668,7 +639,7 @@ class SparseToDenseTransformer(nn.Module):
         return ops.gather_rows(dense_feats, idx_ext)
 
     def _dense_layer_bf16(self, dense, sparse, w):
-        """_dense_layer for the bf16 token stream: dense (B,N+1,C) bf16, sparse (B,J+1,C) fp32.  Every GEMM is the persistent
+        """_dense_layer for the bf16 token stream: dense (B,N+1,C) bf16, sparse (B,J+1,C) bf16.  Every GEMM is the persistent
         TMA kernel over all B*(N+1) rows (the bg row rides along and is overwritten at the end), the feature map and the
         per-head (q' KV) / (q' . ksum) run in one wgmma kernel, LayerNorms read and write bf16."""
         B, N1, C = dense.shape
@@ -722,24 +693,24 @@ class SparseToDenseTransformer(nn.Module):
     @torch.no_grad()
     def forward(self, dense_feats0, embeddings0, fps_idx0, dense_feats1, embeddings1, fps_idx1, masks0=None, masks1=None):
         w = self._weights()
-        ext0 = torch.cat([torch.zeros_like(fps_idx0[:, :1]), fps_idx0], dim=1).contiguous()
-        ext1 = torch.cat([torch.zeros_like(fps_idx1[:, :1]), fps_idx1], dim=1).contiguous()
-        dense = _stack2(dense_feats0, dense_feats1)
-        if dense is not None:
-            # one batch of 2B clouds through the gather, the (shared-weight) dense linear-attention layer and its FFN
-            B = dense_feats0.shape[0]
-            feats = self._sample_feats(dense, torch.cat([ext0, ext1], dim=0))
-            feats0, feats1 = self.sparse_layer(feats[:B], embeddings0, feats[B:], embeddings1, masks0, masks1)
-            layer = self._dense_layer_bf16 if dense.dtype == torch.bfloat16 else self._dense_layer
-            out = layer(dense, torch.cat([feats0, feats1], dim=0), w)
-            return out[:B], out[B:]
-        feats0 = self._sample_feats(dense_feats0.contiguous(), ext0)
-        feats1 = self._sample_feats(dense_feats1.contiguous(), ext1)
-        feats0, feats1 = self.sparse_layer(feats0, embeddings0, feats1, embeddings1, masks0, masks1)
+        B = dense_feats0.shape[0]
+        idx = torch.cat([fps_idx0, fps_idx1], dim=0)
+        ext = torch.cat([torch.zeros_like(idx[:, :1]), idx], dim=1)
         layer = self._dense_layer_bf16 if dense_feats0.dtype == torch.bfloat16 else self._dense_layer
-        dense_feats0 = layer(dense_feats0.contiguous(), feats0, w)
-        dense_feats1 = layer(dense_feats1.contiguous(), feats1, w)
-        return dense_feats0, dense_feats1
+        stacked = dense_feats0.shape == dense_feats1.shape
+        if stacked:
+            # one batch of 2B clouds through the gather, the (shared-weight) dense linear-attention layer and its FFN
+            dense = _pair(dense_feats0, dense_feats1)
+            feats = self._sample_feats(dense, ext)
+        else:
+            # unequal point counts: the gather and the dense layer run per cloud; the sparse clouds have equal sizes
+            feats = torch.cat([self._sample_feats(dense_feats0.contiguous(), ext[:B]),
+                               self._sample_feats(dense_feats1.contiguous(), ext[B:])])
+        feats0, feats1 = self.sparse_layer(feats[:B], embeddings0, feats[B:], embeddings1, masks0, masks1)
+        if not stacked:
+            return layer(dense_feats0.contiguous(), feats0, w), layer(dense_feats1.contiguous(), feats1, w)
+        out = layer(dense, _pair(feats0, feats1), w)
+        return out[:B], out[B:]
 
 
 class FinePointMatching(nn.Module):
@@ -799,9 +770,8 @@ class FinePointMatching(nn.Module):
             raise NotImplementedError("sam6d_b200 implements the inference path (model.eval())")
         p1, p2 = p1.contiguous(), p2.contiguous()
         p1_ = ops.rigid_warp(p1, end_points['init_R'].contiguous(), end_points['init_t'].contiguous())
-        f12 = _stack2(f1, f2) if p1.shape == p2.shape else None
-        if f12 is not None:
-            e = self._embed(f12, torch.cat([p1_, p2], dim=0))              # both clouds: one PE pass, one in_proj GEMM
+        if p1.shape == p2.shape:
+            e = self._embed(_pair(f1, f2), torch.cat([p1_, p2], dim=0))    # both clouds: one PE pass, one in_proj GEMM
             f1, f2 = e[:p1.shape[0]], e[p1.shape[0]:]
         else:
             f1 = self._embed(f1.contiguous(), p1_)
@@ -810,9 +780,8 @@ class FinePointMatching(nn.Module):
             f1, f2 = blk(f1, geo1, fps_idx1, f2, geo2, fps_idx2)
         B, S, H = f1.shape
         w = self._weights()
-        f12 = _stack2(f1, f2)
-        if f12 is not None:
-            o = _gemm(self.precision, f12.reshape(2 * B * S, H), w["w_out"], w["b_out"]).view(2 * B, S, -1)
+        if f1.shape == f2.shape:
+            o = _gemm(self.precision, _pair(f1, f2).reshape(2 * B * S, H), w["w_out"], w["b_out"]).view(2 * B, S, -1)
             o1, o2 = o[:B], o[B:]
         else:
             o1 = _gemm(self.precision, f1.reshape(B * S, H), w["w_out"], w["b_out"]).view(B, S, -1)
@@ -952,16 +921,16 @@ class Net(nn.Module):
                 fts2 = torch.cat([dense_fm, dense_fo], dim=0)
             dense_pm, dense_po, dense_fm, dense_fo = pts2[:B], pts2[B:], fts2[:B], fts2[B:]
             sp, sf, idx = sample_pts_feats(pts2, fts2, self.coarse_npoint, return_index=True)
-            bg_point = torch.ones(2 * B, 1, 3, dtype=torch.float32, device=pts2.device) * 100
-            geo = self.geo_embedding(torch.cat([bg_point, sp], dim=1))
-            sparse_pm, sparse_po, sparse_fm, sparse_fo = sp[:B], sp[B:], sf[:B], sf[B:]
-            fps_idx_m, fps_idx_o, geo_embedding_m, geo_embedding_o = idx[:B], idx[B:], geo[:B], geo[B:]
         else:
-            bg_point = torch.ones(B, 1, 3, dtype=torch.float32, device=dense_pm.device) * 100
-            sparse_pm, sparse_fm, fps_idx_m = sample_pts_feats(dense_pm, dense_fm, self.coarse_npoint, return_index=True)
-            geo_embedding_m = self.geo_embedding(torch.cat([bg_point, sparse_pm], dim=1))
-            sparse_po, sparse_fo, fps_idx_o = sample_pts_feats(dense_po, dense_fo, self.coarse_npoint, return_index=True)
-            geo_embedding_o = self.geo_embedding(torch.cat([bg_point, sparse_po], dim=1))
+            # unequal point counts: FPS, PE and the dense layers run per cloud; both clouds come down to coarse_npoint points,
+            # so the geometric embedding and the sparse stage still run on 2B clouds
+            m = sample_pts_feats(dense_pm, dense_fm, self.coarse_npoint, return_index=True)
+            o = sample_pts_feats(dense_po, dense_fo, self.coarse_npoint, return_index=True)
+            sp, sf, idx = (torch.cat(z) for z in zip(m, o))
+        bg_point = torch.ones(2 * B, 1, 3, dtype=torch.float32, device=sp.device) * 100
+        geo = self.geo_embedding(torch.cat([bg_point, sp], dim=1))
+        sparse_pm, sparse_po, sparse_fm, sparse_fo = sp[:B], sp[B:], sf[:B], sf[B:]
+        fps_idx_m, fps_idx_o, geo_embedding_m, geo_embedding_o = idx[:B], idx[B:], geo[:B], geo[B:]
         end_points = self.coarse_point_matching(sparse_pm, sparse_fm, geo_embedding_m, sparse_po, sparse_fo, geo_embedding_o,
                                                 radius, end_points, rand=rand)
         if init_pose is not None:
