@@ -407,6 +407,24 @@ int sam6d_icp_refine(const float* R, const float* t, const float* pts, int B, in
  * CTA); a negative value is minus a CUDA error.  Not a status code: call it directly, not through the status-checking wrapper. */
 int sam6d_icp_max_samples(void);
 
+/* ---- observed points of tracked objects (not in the reference; csrc/track.cu, oracle/track_oracle.py) ----------------------- */
+/* O objects of one H x W frame.  rdepth (O,H,W) f32: each object's rendered depth at its predicted pose (> 0 = silhouette, as
+ * render.render returns it); depth (H,W) u16 raw; depth_scale and the pinhole fx, fy, cx, cy as fp32; centre (O,3) and
+ * radius (O) f32 in metres, each object's gate; margin >= 0 pixels; N >= 1.  A pixel (y, x) is a candidate of object o when
+ *   1. some silhouette pixel of o lies within max(|dy|, |dx|) <= margin of it (two separable max passes),
+ *   2. its observed depth z = (float(raw) * depth_scale) / 1000 is > 0, and
+ *   3. its point p = ((x - cx) * z / fx, (y - cy) * z / fy, z) satisfies (dx^2 + dy^2) + dz^2 <= radius^2 with d = p - centre
+ *      (and radius > 0);
+ * every operation of 2 and 3 in fp32, rounded to nearest, in the order written (inputs.py's depth and inputs.cu's
+ * back-projection, in fp32).  The candidates, in raster order, have ranks k = 0 .. count-1; output i takes rank
+ * floor(i count / N) when count >= N, i mod count when 0 < count < N; with count 0 every point is 0.  Outputs: pts (O,N,3) f32
+ * metres, count (O) i32, optional index (O,N) i32 (y W + x of each output's pixel, -1 when count is 0; NULL: not written) and
+ * cand (O,H,W) u8, the candidate mask.  Scratch: hmask (O,H,W) u8, rows (O,H) i32.  No randomness; results are exact.
+ * -22: O < 0, H < 1, W < 1, W > 49152, H or O > 65535, margin < 0, N < 1, or a NULL pointer other than index with O > 0. */
+int sam6d_track_points(const float* rdepth, const unsigned short* depth, int O, int H, int W, float depth_scale, float fx, float fy,
+                       float cx, float cy, const float* centre, const float* radius, int margin, int N, unsigned char* hmask,
+                       unsigned char* cand, int* rows, float* pts, int* count, int* index, void* stream);
+
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):
  * 0 mean, 1 median (torch.median's lower median), 2 max, 3 avg_5.  sim_out (P,O,T) optional; obj_score (P,O) f32 and obj_tmpl

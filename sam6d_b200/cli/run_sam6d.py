@@ -77,16 +77,7 @@ def main(argv=None):
     args = ap.parse_args(argv)
     if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
         ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
-    from ..pipeline import SAM6D
-    sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
-                  dinov2_model=args.dinov2_model,
-                  checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
-                  stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
-                  points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
-                  det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
-                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
-                  rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split,
-                  icp_iters=args.icp_iters)
+    sam6d = build_sam6d(args)
     multi = isinstance(args.cad_path, list)
     n_cad = len(args.cad_path) if multi else 1
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:
@@ -111,6 +102,20 @@ def main(argv=None):
     if res.pem:
         (write_vis_objects if multi else pem_cli.write_vis)(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
     return 0
+
+
+def build_sam6d(args):
+    """the SAM6D of the parsed model options"""
+    from ..pipeline import SAM6D
+    return SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
+                 dinov2_model=args.dinov2_model,
+                 checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
+                 stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
+                 points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
+                 det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
+                 pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
+                 rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split,
+                 icp_iters=args.icp_iters)
 
 
 def write_vis_objects(path, frame, cam_K):

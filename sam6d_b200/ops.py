@@ -10,6 +10,7 @@ stride of 0 (expand) shares one matrix across the batch.
 """
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -840,6 +841,37 @@ def icp_refine(R: Tensor, t: Tensor, pts: Tensor, samples: Tensor, normals: Tens
     if system:
         return R_out, t_out, inliers, rms, iters_run, corr, sums
     return R_out, t_out, inliers, rms, iters_run
+
+
+def track_points(rdepth: Tensor, depth: Tensor, depth_scale: float, K, centre: Tensor, radius: Tensor, margin: int, n: int,
+                 return_index: bool = False):
+    """observed points of O tracked objects (the rule: include/sam6d_b200.h, sam6d_track_points).  rdepth (O,H,W) f32 rendered
+    depth (> 0 = silhouette), depth (H,W) u16 raw, depth_scale and K (3,3) host values (rounded to fp32), centre (O,3) and
+    radius (O) f32 gate in metres, margin pixels -> (pts (O,n,3) f32 metres, count (O) i32, cand (O,H,W) u8 candidate mask),
+    plus index (O,n) i32 (the pixel y W + x of every point, -1 for an object with no candidate) when return_index."""
+    _check(rdepth, torch.float32, "rdepth", 3)
+    _check(depth, torch.uint16, "depth", 2)
+    _check(centre, torch.float32, "centre", 2)
+    _check(radius, torch.float32, "radius", 1)
+    O, H, W = rdepth.shape
+    if tuple(depth.shape) != (H, W) or tuple(centre.shape) != (O, 3) or tuple(radius.shape) != (O,):
+        raise RuntimeError(f"track_points: rdepth (O,H,W), depth (H,W), centre (O,3), radius (O) with (O,H,W) = {(O, H, W)}, got "
+                           f"{tuple(depth.shape)}, {tuple(centre.shape)}, {tuple(radius.shape)}")
+    if int(margin) < 0 or int(n) < 1:
+        raise RuntimeError(f"track_points: margin must be >= 0 and n >= 1, got {margin}, {n}")
+    k = np.asarray(K.cpu() if isinstance(K, torch.Tensor) else K, dtype=np.float64).reshape(3, 3).astype(np.float32)
+    dev = rdepth.device
+    hmask = torch.empty(O, H, W, dtype=torch.uint8, device=dev)
+    cand = torch.empty(O, H, W, dtype=torch.uint8, device=dev)
+    rows = torch.empty(O, H, dtype=torch.int32, device=dev)
+    pts = torch.empty(O, int(n), 3, dtype=torch.float32, device=dev)
+    count = torch.empty(O, dtype=torch.int32, device=dev)
+    index = torch.empty(O, int(n), dtype=torch.int32, device=dev) if return_index else None
+    _lib.call("sam6d_track_points", rdepth, depth, O, H, W, float(np.float32(depth_scale)), float(k[0, 0]), float(k[1, 1]), float(k[0, 2]),
+              float(k[1, 2]), centre, radius, int(margin), int(n), hmask, cand, rows, pts, count, index)
+    if return_index:
+        return pts, count, cand, index
+    return pts, count, cand
 
 
 # ---------------------------------------------------------------------------------------------- SAM encoder attention
