@@ -424,6 +424,21 @@ int sam6d_icp_max_samples(void);
 int sam6d_track_points(const float* rdepth, const unsigned short* depth, int O, int H, int W, float depth_scale, float fx, float fy,
                        float cx, float cy, const float* centre, const float* radius, int margin, int N, unsigned char* hmask,
                        unsigned char* cand, int* rows, float* pts, int* count, int* index, void* stream);
+/* sam6d_track_points over L live tracks of one scene (several may follow copies of one mesh), with every pixel given to at most
+ * one track.  Inputs, outputs and scratch as sam6d_track_points with O = L, plus scratch dmask (L,H,W) u8 (the dilated
+ * silhouettes).  Track j is eligible at pixel (y, x) when conditions 1-3 of sam6d_track_points hold for j, with the same fp32
+ * operations in the same order.  The pixel is a candidate of
+ *   - the eligible j with the least rdepth[j,y,x] when some eligible j has rdepth[j,y,x] > 0 (the rendered scene's front
+ *     surface), else
+ *   - the eligible j with the least d2_j / (radius_j * radius_j), d2_j the squared distance of condition 3 (each operation
+ *     in fp32, rounded to nearest);
+ * exact ties go to the lowest j, and a pixel with no eligible track is no candidate.  Ranks, selection, the zero output of
+ * count 0 and index as sam6d_track_points.  With L = 1 the candidates, and so every output, are sam6d_track_points'.
+ * No randomness; results are exact.  -22: as sam6d_track_points with O = L, or dmask NULL with L > 0. */
+int sam6d_track_points_scene(const float* rdepth, const unsigned short* depth, int L, int H, int W, float depth_scale, float fx,
+                             float fy, float cx, float cy, const float* centre, const float* radius, int margin, int N,
+                             unsigned char* hmask, unsigned char* dmask, unsigned char* cand, int* rows, float* pts, int* count,
+                             int* index, void* stream);
 
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):

@@ -6,7 +6,8 @@ first frame, then follow each object's pose with depth and ICP, detecting again 
 
 Frames are the file names present in both --rgb_dir and --depth_dir, in sorted order; one camera.json (cam_K, depth_scale)
 serves every frame.  Writes $OUT/sam6d_results/track_pem.json: a list with one {"frame": name, "records": [...]} per frame,
-the records as Tracker returns them (detection_pem.json's keys plus "track" and "frames_tracked")."""
+the records as Tracker returns them (detection_pem.json's keys plus "track" and "frames_tracked", and "track_id" with
+--max_instances above 1)."""
 import argparse
 import json
 import os
@@ -37,6 +38,10 @@ def get_parser():
     ap.add_argument("--min_inlier_fraction", default=0.5, type=float, help="a track with fewer ICP inliers is lost")
     ap.add_argument("--max_rms_m", default=0.005, type=float, help="a track with a larger ICP RMS (metres) is lost")
     ap.add_argument("--redetect_interval", default=30, type=int, help="frames without detection before detecting again")
+    ap.add_argument("--max_instances", default=1, type=int, help="tracks per object (copies of one object in the scene)")
+    ap.add_argument("--start_score", default=0.3, type=float, help="least PEM score that starts an object's second and later tracks")
+    ap.add_argument("--assoc_scale", default=0.5, type=float,
+                    help="centroid distance, over the object's radius, within which two tracks of one object are one copy")
     return ap
 
 
@@ -60,7 +65,8 @@ def main(argv=None):
     objs = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size)
     tracker = Tracker(sam6d, objs, args.cad_path, track_icp_iters=args.track_icp_iters, margin_px=args.margin_px,
                       gate_scale=args.gate_scale, min_inlier_fraction=args.min_inlier_fraction, max_rms_m=args.max_rms_m,
-                      redetect_interval=args.redetect_interval)
+                      redetect_interval=args.redetect_interval, max_instances=args.max_instances, start_score=args.start_score,
+                      assoc_scale=args.assoc_scale)
     cam = json.load(open(args.cam_path))
     out = []
     for name in names:

@@ -12,6 +12,11 @@
 //      for every i that selects k (count >= N: floor(i count / N) = k; 0 < count < N: i = k mod count).
 // Every fp32 operation that decides membership is an explicit round-to-nearest intrinsic, so nothing is contracted into an FMA
 // and the oracle reproduces the candidate set exactly.
+//
+// sam6d_track_points_scene gives every pixel to at most one of L live tracks (the rule: include/sam6d_b200.h).  Five launches:
+// trk_dilate_rows; trk_dilate_cols (the same running column window, written out as the dilated mask); trk_assign (one thread
+// per pixel over the L tracks: the eligible track rendered in front, else the eligible track nearest its gate centre relative
+// to its radius); trk_scan; trk_select.
 #include "common.cuh"
 
 namespace {
@@ -29,10 +34,14 @@ __device__ __forceinline__ float3 trk_point(const TrkCam& c, unsigned short raw,
   return make_float3(__fdiv_rn(__fmul_rn(__fsub_rn((float)x, c.cx), z), c.fx), __fdiv_rn(__fmul_rn(__fsub_rn((float)y, c.cy), z), c.fy), z);
 }
 
-__device__ __forceinline__ bool trk_in_gate(float3 p, const float* centre, float radius) {
+// (dx^2 + dy^2) + dz^2 with d = p - centre
+__device__ __forceinline__ float trk_gate_d2(float3 p, const float* centre) {
   const float dx = __fsub_rn(p.x, centre[0]), dy = __fsub_rn(p.y, centre[1]), dz = __fsub_rn(p.z, centre[2]);
-  const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-  return radius > 0.f && d2 <= __fmul_rn(radius, radius);
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+
+__device__ __forceinline__ bool trk_in_gate(float3 p, const float* centre, float radius) {
+  return radius > 0.f && trk_gate_d2(p, centre) <= __fmul_rn(radius, radius);
 }
 
 // exclusive scan of one int per thread over a TRK_THREADS block; the block total in *total.  warp_sums: TRK_THREADS / 32 ints.
@@ -106,6 +115,60 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_candidates(const unsigned cha
   }
   __syncthreads();
   if (threadIdx.x < y1 - y0 && srows[threadIdx.x]) atomicAdd(&rows[(size_t)o * H + y0 + threadIdx.x], srows[threadIdx.x]);
+}
+
+// sam6d_track_points_scene's vertical pass: the (2m+1)-row window of hmask down each column, as trk_candidates counts it
+__global__ void __launch_bounds__(TRK_THREADS) trk_dilate_cols(const unsigned char* __restrict__ hmask, int H, int W, int m,
+                                                              unsigned char* __restrict__ dmask) {
+  const int x = blockIdx.x * TRK_THREADS + threadIdx.x, y0 = blockIdx.y * TRK_ROWS, j = blockIdx.z;
+  if (x >= W) return;
+  const int y1 = min(y0 + TRK_ROWS, H);
+  const unsigned char* hm = hmask + (size_t)j * H * W;
+  unsigned char* dm = dmask + (size_t)j * H * W;
+  int win = 0;
+  for (int yy = max(y0 - m, 0); yy < min(y0 + m, H); ++yy) win += hm[(size_t)yy * W + x];
+  for (int y = y0; y < y1; ++y) {
+    if (y + m < H) win += hm[(size_t)(y + m) * W + x];
+    dm[(size_t)y * W + x] = win > 0;
+    if (y - m >= 0) win -= hm[(size_t)(y - m) * W + x];
+  }
+}
+
+// sam6d_track_points_scene's assignment: one thread per pixel walks the L tracks in order, keeps the eligible track with the
+// least rendered depth and the eligible track with the least d2 / r^2 (strict <: exact ties stay with the lower j), writes
+// every track's candidate byte and adds one to the winner's row count (warp-aggregated integer atomics: exact)
+__global__ void __launch_bounds__(TRK_THREADS) trk_assign(const float* __restrict__ rdepth, const unsigned char* __restrict__ dmask,
+                                                         const unsigned short* __restrict__ depth, TrkCam cam,
+                                                         const float* __restrict__ centre, const float* __restrict__ radius, int L,
+                                                         int H, int W, unsigned char* __restrict__ cand, int* __restrict__ rows) {
+  const int x = blockIdx.x * TRK_THREADS + threadIdx.x, y = blockIdx.y;
+  const bool col = x < W;
+  int win = -1;
+  if (col) {
+    const size_t px = (size_t)y * W + x, plane = (size_t)H * W;
+    const float3 p = trk_point(cam, depth[px], y, x);
+    int front = -1, band = -1;
+    float front_z = 0.f, band_q = 0.f;
+    if (p.z > 0.f)
+      for (int j = 0; j < L; ++j) {
+        if (!dmask[j * plane + px]) continue;
+        const float r = radius[j];
+        if (!(r > 0.f)) continue;
+        const float d2 = trk_gate_d2(p, centre + 3 * j), r2 = __fmul_rn(r, r);
+        if (!(d2 <= r2)) continue;
+        const float rz = rdepth[j * plane + px];
+        if (rz > 0.f) {
+          if (front < 0 || rz < front_z) front = j, front_z = rz;
+        } else if (front < 0) {
+          const float q = __fdiv_rn(d2, r2);
+          if (band < 0 || q < band_q) band = j, band_q = q;
+        }
+      }
+    win = front >= 0 ? front : band;
+    for (int j = 0; j < L; ++j) cand[j * plane + px] = j == win;
+  }
+  const unsigned same = __match_any_sync(0xffffffffu, win);
+  if (win >= 0 && (threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&rows[(size_t)win * H + y], __popc(same));
 }
 
 // rows (O,H): counts in, exclusive offsets out; count (O) the totals.  An object with no candidate gets zeros (and index -1).
@@ -184,6 +247,30 @@ S6_API int sam6d_track_points(const float* rdepth, const unsigned short* depth, 
   trk_scan<<<O, TRK_THREADS, 0, st>>>(rows, H, N, count, pts, index);
   S6_LAUNCH_CHECK();
   trk_select<<<dim3(H, O), TRK_THREADS, 0, st>>>(cand, depth, cam, rows, count, H, W, N, pts, index);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+S6_API int sam6d_track_points_scene(const float* rdepth, const unsigned short* depth, int L, int H, int W, float depth_scale, float fx,
+                                    float fy, float cx, float cy, const float* centre, const float* radius, int margin, int N,
+                                    unsigned char* hmask, unsigned char* dmask, unsigned char* cand, int* rows, float* pts, int* count,
+                                    int* index, void* stream) {
+  S6_REQUIRE(L >= 0 && H >= 1 && W >= 1 && margin >= 0 && N >= 1 && (long long)H * W <= 0x7fffffffLL);
+  if (L == 0) return 0;
+  S6_REQUIRE(rdepth && depth && centre && radius && hmask && dmask && cand && rows && pts && count);
+  S6_REQUIRE(W <= 48 * 1024 && L <= 65535 && H <= 65535);
+  cudaStream_t st = s6_stream(stream);
+  const TrkCam cam{depth_scale, fx, fy, cx, cy};
+  const int m = margin < (H > W ? H : W) ? margin : (H > W ? H : W);
+  trk_dilate_rows<<<dim3(H, L), TRK_THREADS, W, st>>>(rdepth, H, W, m, hmask, rows);
+  S6_LAUNCH_CHECK();
+  trk_dilate_cols<<<dim3(s6_cdiv(W, TRK_THREADS), s6_cdiv(H, TRK_ROWS), L), TRK_THREADS, 0, st>>>(hmask, H, W, m, dmask);
+  S6_LAUNCH_CHECK();
+  trk_assign<<<dim3(s6_cdiv(W, TRK_THREADS), H), TRK_THREADS, 0, st>>>(rdepth, dmask, depth, cam, centre, radius, L, H, W, cand, rows);
+  S6_LAUNCH_CHECK();
+  trk_scan<<<L, TRK_THREADS, 0, st>>>(rows, H, N, count, pts, index);
+  S6_LAUNCH_CHECK();
+  trk_select<<<dim3(H, L), TRK_THREADS, 0, st>>>(cand, depth, cam, rows, count, H, W, N, pts, index);
   S6_LAUNCH_CHECK();
   return 0;
 }

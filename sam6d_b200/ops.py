@@ -874,6 +874,37 @@ def track_points(rdepth: Tensor, depth: Tensor, depth_scale: float, K, centre: T
     return pts, count, cand
 
 
+def track_points_scene(rdepth: Tensor, depth: Tensor, depth_scale: float, K, centre: Tensor, radius: Tensor, margin: int, n: int,
+                       return_index: bool = False):
+    """track_points over L live tracks of one scene, every pixel given to at most one track: the eligible track rendered in
+    front, else the one nearest its gate centre relative to its radius (the rule: include/sam6d_b200.h,
+    sam6d_track_points_scene).  Arguments and returns as track_points with O = L; with L = 1 the outputs are track_points'."""
+    _check(rdepth, torch.float32, "rdepth", 3)
+    _check(depth, torch.uint16, "depth", 2)
+    _check(centre, torch.float32, "centre", 2)
+    _check(radius, torch.float32, "radius", 1)
+    L, H, W = rdepth.shape
+    if tuple(depth.shape) != (H, W) or tuple(centre.shape) != (L, 3) or tuple(radius.shape) != (L,):
+        raise RuntimeError(f"track_points_scene: rdepth (L,H,W), depth (H,W), centre (L,3), radius (L) with (L,H,W) = {(L, H, W)}, "
+                           f"got {tuple(depth.shape)}, {tuple(centre.shape)}, {tuple(radius.shape)}")
+    if int(margin) < 0 or int(n) < 1:
+        raise RuntimeError(f"track_points_scene: margin must be >= 0 and n >= 1, got {margin}, {n}")
+    k = np.asarray(K.cpu() if isinstance(K, torch.Tensor) else K, dtype=np.float64).reshape(3, 3).astype(np.float32)
+    dev = rdepth.device
+    hmask = torch.empty(L, H, W, dtype=torch.uint8, device=dev)
+    dmask = torch.empty(L, H, W, dtype=torch.uint8, device=dev)
+    cand = torch.empty(L, H, W, dtype=torch.uint8, device=dev)
+    rows = torch.empty(L, H, dtype=torch.int32, device=dev)
+    pts = torch.empty(L, int(n), 3, dtype=torch.float32, device=dev)
+    count = torch.empty(L, dtype=torch.int32, device=dev)
+    index = torch.empty(L, int(n), dtype=torch.int32, device=dev) if return_index else None
+    _lib.call("sam6d_track_points_scene", rdepth, depth, L, H, W, float(np.float32(depth_scale)), float(k[0, 0]), float(k[1, 1]),
+              float(k[0, 2]), float(k[1, 2]), centre, radius, int(margin), int(n), hmask, dmask, cand, rows, pts, count, index)
+    if return_index:
+        return pts, count, cand, index
+    return pts, count, cand
+
+
 # ---------------------------------------------------------------------------------------------- SAM encoder attention
 def attn_relpos(qkv: Tensor, nW: int, Hs: int, Ws: int, nH: int, rel_h: Tensor, rel_w: Tensor, scale: float,
                 out_dtype=torch.float32) -> Tensor:

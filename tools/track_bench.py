@@ -1,7 +1,7 @@
 """Time a tracked frame (sam6d_b200/track.py: Tracker) at O = 1 / 8 / 21 objects, split into its render, point selection
 (csrc/track.cu) and ICP (csrc/icp.cu), beside a SAM6D.detect_objects frame of the same objects, on the GPU.
 
-    python tools/track_bench.py [--objects 1 8 21] [--reps 50] [--segmentor fastsam]
+    python tools/track_bench.py [--objects 1 8 21] [--reps 50] [--segmentor fastsam] [--max_instances 1]
 
 The scene is tests/test_gpu_track.py's: a 480 x 640 frame, K with f = 600, the 1.6 k-face hull mesh (radius 110 mm) as every
 object, O copies spread over the frame at 0.6 - 0.9 m with 1 mm depth noise.  Each object is seeded at its true pose, so every
@@ -10,7 +10,11 @@ M = 4096 ICP samples, 10 ICP iterations); the tracked frame is the host clock ar
 selection, the ICP, the loss rule's device-to-host copy and the records), averaged over --reps frames after a warm-up.  The
 detect_objects frame (FastSAM-x or SAM ViT-H and DINOv2 ViT-L with seeded random weights: its proposal count, and so its
 time, is not that of trained weights) is the host clock over 5 frames after 2 warm-up frames.  Prints the card's name and
-power limit, then one JSON line."""
+power limit, then one JSON line.
+
+With --max_instances I > 1 every object is placed I times (L = O x I tracks, each copy seeded at its true pose), the tracker
+runs with max_instances I, and point selection is timed both ways at the same L: the shared rule (ops.track_points) and the
+exclusive one the tracker uses (ops.track_points_scene).  The detect_objects frame is not timed then."""
 import argparse
 import json
 import os
@@ -73,6 +77,7 @@ def main():
     ap.add_argument("--objects", type=int, nargs="+", default=[1, 8, 21])
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--segmentor", default="fastsam", choices=("fastsam", "sam"))
+    ap.add_argument("--max_instances", type=int, default=1, help="copies of each object, and tracks per object")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     import test_gpu_track as tt
@@ -87,40 +92,56 @@ def main():
     sam6d = SAM6D(segmentor=args.segmentor, random_weights=True)
     rgb_bg = np.full((tt.H, tt.W, 3), 90, np.uint8)
     rows = []
+    I = args.max_instances
     for O in args.objects:
         rng = np.random.RandomState(O)
-        poses, raw = scene(O, up[0], rng)
+        L = O * I
+        poses, raw = scene(L, up[0], rng)
         rgb = rgb_bg.copy()
         rgb[raw > 0] = (200, 120, 40)
         objs = sam6d.onboard_objects([mesh] * O, template_size=256, rng=np.random.RandomState(0))
-        # no loss and no re-detection: every timed frame is a tracked frame of all O objects (the first call detects)
-        tr = Tracker(sam6d, objs, [mesh] * O, redetect_interval=10 ** 9, min_inlier_fraction=0.0, max_rms_m=float("inf"))
-        for o, (R, t) in enumerate(poses):
-            tr.start(o, R, t)
+        # no loss and no re-detection: every timed frame is a tracked frame of all L tracks (the first call detects)
+        tr = Tracker(sam6d, objs, [mesh] * O, redetect_interval=10 ** 9, min_inlier_fraction=0.0, max_rms_m=float("inf"),
+                     max_instances=I, assoc_scale=0.0)
+        for i, (R, t) in enumerate(poses):
+            tr.start(i // I, R, t)
         tr(rgb, raw, tt.K.ravel(), tt.DEPTH_SCALE)
         live = tr.live.sum()
         # the stages at the tracker's shapes, from the tracker's own state
-        idx = torch.arange(O, device="cuda")
         R, t = tr.R.contiguous(), tr.t.contiguous()
-        P = torch.zeros(O, 1, 4, 4, device="cuda")
+        P = torch.zeros(L, 1, 4, 4, device="cuda")
         P[:, 0, :3, :3], P[:, 0, :3, 3], P[:, 0, 3, 3] = R, t * 1000.0, 1.0
-        rd = render.render(tr.meshes, P, tt.K, tt.H, tt.W)["depth"][:, 0].contiguous()
+        meshes = [tr.meshes[o] for o in tr.obj]
+        rd = render.render(meshes, P, tt.K, tt.H, tt.W)["depth"][:, 0].contiguous()
         depth_d = torch.from_numpy(raw).cuda()
-        centre = (torch.einsum("lij,lj->li", R, tr.centroid) + t).contiguous()
-        pts, _, _ = ops.track_points(rd, depth_d, tt.DEPTH_SCALE, tt.K, centre, tr.gate_radius, tr.margin_px, tr.n_points)
-        obj = idx.to(torch.int32)
-        ms_render = events(lambda: render.render(tr.meshes, P, tt.K, tt.H, tt.W), args.reps)
-        ms_select = events(lambda: ops.track_points(rd, depth_d, tt.DEPTH_SCALE, tt.K, centre, tr.gate_radius, tr.margin_px,
-                                                    tr.n_points), args.reps)
-        ms_icp = events(lambda: ops.icp_refine(R, t, pts, tr.icp[0], tr.icp[1], obj, tr.icp_radius, tr.track_icp_iters), args.reps)
+        obj = torch.from_numpy(tr.obj).cuda()
+        centre = (torch.einsum("lij,lj->li", R, tr.centroid[obj]) + t).contiguous()
+        gate = tr.gate_radius[obj].contiguous()
+        pts, _, _ = ops.track_points(rd, depth_d, tt.DEPTH_SCALE, tt.K, centre, gate, tr.margin_px, tr.n_points)
+        icp_radius, obj = tr.icp_radius[obj].contiguous(), obj.to(torch.int32)
+        ms_render = events(lambda: render.render(meshes, P, tt.K, tt.H, tt.W), args.reps)
+        ms_select = events(lambda: ops.track_points(rd, depth_d, tt.DEPTH_SCALE, tt.K, centre, gate, tr.margin_px, tr.n_points),
+                           args.reps)
+        ms_icp = events(lambda: ops.icp_refine(R, t, pts, tr.icp[0], tr.icp[1], obj, icp_radius, tr.track_icp_iters),
+                        args.reps)
         ms_frame = wall(lambda: tr(rgb, raw, tt.K.ravel(), tt.DEPTH_SCALE), args.reps, 3)
         states = tr(rgb, raw, tt.K.ravel(), tt.DEPTH_SCALE).state
-        ms_detect = wall(lambda: sam6d.detect_objects(rgb, raw, tt.K.ravel(), tt.DEPTH_SCALE, objs), 5, 2)
-        row = dict(objects=O, live_after=int(live), tracked=states.count("tracked"), render_ms=round(ms_render, 3),
-                   select_ms=round(ms_select, 3), icp_ms=round(ms_icp, 3), tracked_frame_ms=round(ms_frame, 3),
-                   detect_frame_ms=round(ms_detect, 2), detect_over_tracked=round(ms_detect / ms_frame, 1))
-        print(f"[track_bench] O={O}: render {ms_render:.3f} ms, select {ms_select:.3f} ms, ICP {ms_icp:.3f} ms; tracked frame "
-              f"{ms_frame:.3f} ms ({row['tracked']} of {O} tracked), detect_objects frame ({args.segmentor}) {ms_detect:.1f} ms")
+        if I == 1:
+            ms_detect = wall(lambda: sam6d.detect_objects(rgb, raw, tt.K.ravel(), tt.DEPTH_SCALE, objs), 5, 2)
+            row = dict(objects=O, live_after=int(live), tracked=states.count("tracked"), render_ms=round(ms_render, 3),
+                       select_ms=round(ms_select, 3), icp_ms=round(ms_icp, 3), tracked_frame_ms=round(ms_frame, 3),
+                       detect_frame_ms=round(ms_detect, 2), detect_over_tracked=round(ms_detect / ms_frame, 1))
+            print(f"[track_bench] O={O}: render {ms_render:.3f} ms, select {ms_select:.3f} ms, ICP {ms_icp:.3f} ms; tracked frame "
+                  f"{ms_frame:.3f} ms ({row['tracked']} of {O} tracked), detect_objects frame ({args.segmentor}) {ms_detect:.1f} ms")
+        else:
+            ms_scene = events(lambda: ops.track_points_scene(rd, depth_d, tt.DEPTH_SCALE, tt.K, centre, gate, tr.margin_px,
+                                                             tr.n_points), args.reps)
+            row = dict(objects=O, instances=I, tracks=L, live_after=int(live), tracked=states.count("tracked"),
+                       render_ms=round(ms_render, 3), select_shared_ms=round(ms_select, 3), select_scene_ms=round(ms_scene, 3),
+                       icp_ms=round(ms_icp, 3), tracked_frame_ms=round(ms_frame, 3))
+            print(f"[track_bench] O={O} x {I} (L={L}): render {ms_render:.3f} ms, select track_points {ms_select:.3f} ms, "
+                  f"track_points_scene {ms_scene:.3f} ms, ICP {ms_icp:.3f} ms; tracked frame {ms_frame:.3f} ms "
+                  f"({row['tracked']} of {L} tracked)")
         rows.append(row)
         del tr, objs
         torch.cuda.empty_cache()
