@@ -440,6 +440,21 @@ int sam6d_track_points_scene(const float* rdepth, const unsigned short* depth, i
                              unsigned char* hmask, unsigned char* dmask, unsigned char* cand, int* rows, float* pts, int* count,
                              int* index, void* stream);
 
+/* ---- depth agreement of pose hypotheses (not in the reference; csrc/verify.cu, oracle/verify_oracle.py) -------------------- */
+/* P hypotheses of one H x W frame.  rdepth (P,H,W) f32: each hypothesis's rendered depth in render units (0 = empty), rscale
+ * (finite, > 0) the factor to metres (1e-3 for meshes in mm); depth (H,W) f32 the observed depth in metres (0 = invalid);
+ * mask (M,H,W) u8 detection masks.  mrow (P) i32 and tau (P) f32 are HOST arrays, read before the call returns: hypothesis p
+ * reads mask row mrow[p] in [0, M) and has tolerance tau[p] (finite, > 0) in metres.  At pixel i of hypothesis p, each in fp32
+ * rounded to nearest: dr = rdepth[p,i] * rscale, do = depth[i], e = do - dr.  Classes:
+ *   silhouette dr > 0;  occluded: silhouette, do > 0 and e < -tau (something in front of the model: neutral);
+ *   fit: silhouette, do > 0 and |e| <= tau;  violation: silhouette, do > 0 and e > tau (the sensor sees behind the surface);
+ *   mask: mask[mrow[p], i] != 0;  mask_fit: mask and fit.
+ * counts (P,6) i32 = n_sil, n_occ, n_fit, n_viol, n_mask, n_mask_fit.  Integer block sums and one atomic per CTA and counter:
+ * results are exact and deterministic.  -22 (nothing launched): P < 0, H < 1, W < 1, a NULL pointer with P > 0, M < 1, an
+ * mrow outside [0, M), a tau or rscale that is not finite or is <= 0. */
+int sam6d_pose_verify(const float* rdepth, const float* depth, const unsigned char* mask, const int* mrow, const float* tau, int P,
+                      int M, int H, int W, float rscale, int* counts, void* stream);
+
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):
  * 0 mean, 1 median (torch.median's lower median), 2 max, 3 avg_5.  sim_out (P,O,T) optional; obj_score (P,O) f32 and obj_tmpl

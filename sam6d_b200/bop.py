@@ -248,13 +248,14 @@ def csv_rows(scene_id: int, image_id: int, obj_ids, scores: np.ndarray, R: np.nd
 
 def pem_instances(dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, objects: BopObjects,
                   model_points: np.ndarray, rng=None, choose_idx: Optional[np.ndarray] = None, n_sample: int = 2048, img_size: int = 224,
-                  device=None):
+                  device=None, frame_rows: bool = False):
     """BOPTestset.__getitem__ / get_instance for the detections of one image, on the device (inputs.FrameInputs): the detections
     with score > 0.25; the mask is the RLE AND depth > 0 with pem_depth's depth; a detection is kept with more than 8 mask pixels
     and at least 8 points within diameter * 0.6 (float64) of their centroid; observed-point samples drawn from `rng` in
     detection order (or choose_idx (Q,n_sample)).  model_points (O,n,3) f32 in metres, O in objects' order.
     -> (dict of pts (Q,n_sample,3), rgb (Q,3,S,S) (BGR crop, as get_bop_image), rgb_choose (Q,n_sample) i64, model (Q,n,3),
-    score (Q) f32, obj (Q) i64 object index; the kept detections; choose_idx)"""
+    score (Q) f32, obj (Q) i64 object index; the kept detections; choose_idx), and with frame_rows=True a fourth item,
+    inputs.FrameInputs.rows of the kept detections (the device depth and masks pose verification reads)"""
     from . import inputs
     sel = [d for d in dets if d["score"] > SEG_FILTER_SCORE]
     obj = np.array([objects.index(d["category_id"]) for d in sel], dtype=np.int64)
@@ -269,4 +270,6 @@ def pem_instances(dets, image_u8: np.ndarray, depth_raw: np.ndarray, cam_K, dept
     o = torch.from_numpy(obj[keep]).to(dev)
     data = dict(pts=pts, rgb=rgb, rgb_choose=rgb_choose, model=torch.from_numpy(np.asarray(model_points, dtype=np.float32)).to(dev)[o],
                 score=torch.tensor([sel[i]["score"] for i in keep], dtype=torch.float32, device=dev), obj=o)
+    if frame_rows:
+        return data, [sel[i] for i in keep], np.asarray(choose_idx), frame.rows(keep)
     return data, [sel[i] for i in keep], np.asarray(choose_idx)

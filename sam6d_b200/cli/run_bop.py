@@ -47,6 +47,9 @@ def get_parser():
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
     # not in the reference: refine each PEM pose against the observed depth (pipeline.icp_refine_out)
     ap.add_argument("--icp_iters", default=0, type=int, help="point-to-plane ICP iterations per PEM pose (0: off)")
+    # not in the reference: rescore each reported pose by its agreement with the observed depth (pipeline.verify_out)
+    ap.add_argument("--verify", action="store_true", help="render every pose and multiply its score by its depth agreement")
+    ap.add_argument("--verify_tau", default=0.1, type=float, help="--verify's depth tolerance over the object's radius")
     return ap
 
 
@@ -73,7 +76,7 @@ def main(argv=None):
                   precision=args.precision, level_templates=args.level_templates, pose_distribution=args.pose_distribution,
                   aggregation_function=args.aggregation_function, rendering_type=args.rendering_type,
                   pbr_root=dataset_root if args.rendering_type == "pbr" else None, pbr_split=args.pbr_split,
-                  icp_iters=args.icp_iters)
+                  icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau)
     os.makedirs(args.output_dir, exist_ok=True)
     if args.stage in ("ism", "both"):
         objects = sam6d.onboard_bop(args.bop_root, args.dataset_name, template_size=args.template_size)

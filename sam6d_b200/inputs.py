@@ -6,6 +6,7 @@ come back in between so that the host can draw the sample indices with numpy's R
     ret_dict, whole_image, whole_pts, model_points, all_dets = get_test_data(dets, image, depth, cam_K, depth_scale, model_points, ...)
 
 ret_dict carries the reference's keys: pts (P,2048,3), rgb (P,3,224,224), rgb_choose (P,2048) int64, score (P), model, K."""
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -109,6 +110,11 @@ class FrameInputs:
                       self.image, self.mask, int(rgb_mask_flag), pts, rgb_choose, rgb, u8)
         return pts, rgb_choose, rgb, u8
 
+    def rows(self, keep: np.ndarray) -> SimpleNamespace:
+        """the device state pose verification reads, without a copy: depth (H,W) f32 metres, mask (P,H,W) u8 (the RLE AND
+        depth > 0) and mrow (Q,) int64, the mask row of each kept detection"""
+        return SimpleNamespace(depth=self.depth, mask=self.mask, mrow=np.asarray(keep, dtype=np.int64))
+
     def whole_points(self) -> torch.Tensor:
         """get_point_cloud_from_depth of the frame, (H*W, 3) float32 (visualisation only in the reference)"""
         ys, xs = torch.meshgrid(torch.arange(self.H, device=self.device), torch.arange(self.W, device=self.device), indexing="ij")
@@ -129,13 +135,15 @@ def draw_choose_idx(n_valid: Sequence[int], n_sample: int, rng=None) -> np.ndarr
 
 def get_test_data(dets: List[Dict], whole_image: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale: float, model_points: np.ndarray,
                   det_score_thresh: float = 0.2, n_sample_observed_point: int = 2048, img_size: int = 224, rgb_mask_flag: bool = True,
-                  choose_idx: Optional[np.ndarray] = None, rng=None, device=None, det_obj: Optional[Sequence[int]] = None):
+                  choose_idx: Optional[np.ndarray] = None, rng=None, device=None, det_obj: Optional[Sequence[int]] = None,
+                  frame_rows: bool = False):
     """The reference's get_test_data after its file reads (the caller loads rgb / depth / camera / detections / CAD samples).
     model_points: (n,3) float32 CAD samples in metres (the reference draws them with trimesh, :182-184).
     -> (ret_dict, whole_image, whole_pts (H*W,3), model_points, all_dets) like the reference.
     Several objects: model_points (O,n,3) and det_obj the object index of every detection in `dets`.  Each detection then gets
     its object's radius filter and `model` rows; ret_dict["obj"] (P) int64 holds the object index of every kept one and
-    ret_dict["choose_idx"] the sample indices drawn for it."""
+    ret_dict["choose_idx"] the sample indices drawn for it.
+    frame_rows=True appends frame_rows(), the frame's device depth and decoded masks with the kept detections' rows."""
     sel = [i for i, d in enumerate(dets) if d["score"] > det_score_thresh]           # :168-171
     dets = [dets[i] for i in sel]
     model_points = np.asarray(model_points, dtype=np.float32)
@@ -161,6 +169,8 @@ def get_test_data(dets: List[Dict], whole_image: np.ndarray, depth_raw: np.ndarr
                K=torch.tensor(np.asarray(cam_K, dtype=np.float64).reshape(3, 3), dtype=torch.float32, device=dev).unsqueeze(0).repeat(n, 1, 1))
     if det_obj is not None:
         ret["obj"], ret["choose_idx"] = obj, np.asarray(choose_idx)
+    if frame_rows:
+        return ret, whole_image, frame.whole_points(), model_points, [dets[i] for i in keep], frame.rows(keep)
     return ret, whole_image, frame.whole_points(), model_points, [dets[i] for i in keep]
 
 

@@ -905,6 +905,94 @@ def track_points_scene(rdepth: Tensor, depth: Tensor, depth_scale: float, K, cen
     return pts, count, cand
 
 
+# ---------------------------------------------------------------------------------------------- pose verification
+VERIFY_COUNTS = ("n_sil", "n_occ", "n_fit", "n_viol", "n_mask", "n_mask_fit")
+VERIFY_RENDER_BYTES = 1 << 28          # render outputs per chunk of hypotheses in verify_poses, at about 26 B per pixel
+
+
+def verify_rows(mrow, tau, P: int, M: int):
+    """mrow (P) and tau (P, or one number) as sam6d_pose_verify reads them -> host int32 and float32 arrays.  ValueError for an
+    mrow outside [0, M) or a tau (after rounding to fp32) that is not finite or is <= 0."""
+    mrow = np.asarray(mrow.cpu() if isinstance(mrow, Tensor) else mrow).reshape(-1)
+    tau = np.asarray(tau.cpu() if isinstance(tau, Tensor) else tau, dtype=np.float64)
+    tau = np.ascontiguousarray(np.broadcast_to(tau.reshape(-1) if tau.ndim else tau, (P,)), dtype=np.float32)
+    if mrow.shape != (P,) or (P and not np.issubdtype(mrow.dtype, np.integer)):
+        raise ValueError(f"verify: mrow must hold {P} integer mask rows, got {mrow.dtype} {mrow.shape}")
+    if P and (mrow.min() < 0 or mrow.max() >= M):
+        raise ValueError(f"verify: mrow must lie in [0, {M}), got [{mrow.min()}, {mrow.max()}]")
+    if P and not (np.isfinite(tau).all() and (tau > 0).all()):
+        raise ValueError("verify: every tau must be finite and > 0 in fp32")
+    return np.ascontiguousarray(mrow, dtype=np.int32), tau
+
+
+def _pose_verify(rdepth: Tensor, depth: Tensor, mask: Tensor, mrow: np.ndarray, tau: np.ndarray, rscale: float, counts: Tensor):
+    P, H, W = rdepth.shape
+    _lib.call("sam6d_pose_verify", rdepth, depth, mask, mrow.ctypes.data, tau.ctypes.data, P, mask.shape[0], H, W,
+              float(np.float32(rscale)), counts)
+
+
+def verify_counts(rdepth: Tensor, depth: Tensor, mask: Tensor, mrow, tau, rscale: float = 1e-3) -> Tensor:
+    """depth agreement of P rendered hypotheses (the rule: include/sam6d_b200.h, sam6d_pose_verify).  rdepth (P,H,W) f32 in
+    render units, rscale their factor to metres (rounded to fp32); depth (H,W) f32 metres; mask (M,H,W) u8; mrow (P) each
+    hypothesis's mask row; tau (P) metres -> counts (P,6) i32 in the order of VERIFY_COUNTS"""
+    _check(rdepth, torch.float32, "rdepth", 3)
+    _check(depth, torch.float32, "depth", 2)
+    _check(mask, torch.uint8, "mask", 3)
+    P, H, W = rdepth.shape
+    if tuple(depth.shape) != (H, W) or tuple(mask.shape[1:]) != (H, W):
+        raise RuntimeError(f"verify_counts: rdepth (P,H,W), depth (H,W), mask (M,H,W) with (H,W) = {(H, W)}, got "
+                           f"{tuple(depth.shape)}, {tuple(mask.shape)}")
+    mrow, tau = verify_rows(mrow, tau, P, mask.shape[0])
+    counts = torch.empty(P, 6, dtype=torch.int32, device=rdepth.device)
+    _pose_verify(rdepth, depth, mask, mrow, tau, rscale, counts)
+    return counts
+
+
+def verify_score(counts: Tensor) -> Tensor:
+    """counts (P,6) -> verify (P,) f32 = fit_frac x cover, fit_frac = n_fit / (n_fit + n_viol) and cover = n_mask_fit / n_mask,
+    each 0 when its denominator is 0 (fp32; the counts are exact in fp32 up to 2^24 pixels)"""
+    c = counts.to(torch.float32)
+    seen, n_mask = c[:, 2] + c[:, 3], c[:, 4]
+    fit_frac = torch.where(seen > 0, c[:, 2] / seen.clamp_min(1.0), torch.zeros_like(seen))
+    cover = torch.where(n_mask > 0, c[:, 5] / n_mask.clamp_min(1.0), torch.zeros_like(n_mask))
+    return fit_frac * cover
+
+
+def verify_poses(R: Tensor, t: Tensor, obj, meshes, depth_m: Tensor, mask: Tensor, mrow, K, tau):
+    """render every pose and count its depth agreement with the frame.  R (P,3,3), t (P,3) f32 metres object -> camera; obj (P)
+    each hypothesis's index into meshes, CUDA meshes in mm (render.upload); depth_m (H,W) f32 metres (0 = invalid); mask
+    (M,H,W) u8 and mrow (P) each hypothesis's mask row; K (3,3) host values; tau (P) tolerances in metres.  Each pose is one
+    mesh entry with one view of render.render, translation t x 1000, in chunks that keep the render's outputs under
+    VERIFY_RENDER_BYTES.  -> (counts (P,6) i32 as verify_counts, verify (P,) f32 = verify_score(counts))"""
+    from . import render
+    _check(R, torch.float32, "R", 3)
+    _check(t, torch.float32, "t", 2)
+    _check(depth_m, torch.float32, "depth_m", 2)
+    _check(mask, torch.uint8, "mask", 3)
+    P = R.shape[0]
+    H, W = depth_m.shape
+    if tuple(R.shape) != (P, 3, 3) or tuple(t.shape) != (P, 3) or tuple(mask.shape[1:]) != (H, W):
+        raise RuntimeError(f"verify_poses: R (P,3,3), t (P,3), depth_m (H,W), mask (M,H,W), got {tuple(R.shape)}, {tuple(t.shape)}, "
+                           f"{tuple(depth_m.shape)}, {tuple(mask.shape)}")
+    obj = np.asarray(obj.cpu() if isinstance(obj, Tensor) else obj, dtype=np.int64).reshape(-1)
+    if obj.shape != (P,) or (P and (obj.min() < 0 or obj.max() >= len(meshes))):
+        raise ValueError(f"verify_poses: obj must hold {P} indices into {len(meshes)} meshes")
+    mrow, tau = verify_rows(mrow, tau, P, mask.shape[0])
+    dev = R.device
+    counts = torch.empty(P, 6, dtype=torch.int32, device=dev)
+    step = max(1, VERIFY_RENDER_BYTES // (26 * H * W))
+    for p0 in range(0, P, step):
+        p1 = min(P, p0 + step)
+        poses = torch.zeros(p1 - p0, 1, 4, 4, dtype=torch.float32, device=dev)
+        poses[:, 0, :3, :3] = R[p0:p1]
+        poses[:, 0, :3, 3] = t[p0:p1] * 1000.0                                          # the meshes are in mm
+        poses[:, 0, 3, 3] = 1.0
+        rdepth = render.render([meshes[o] for o in obj[p0:p1]], poses, K, H, W)["depth"][:, 0].contiguous()
+        _pose_verify(rdepth, depth_m, mask, mrow[p0:p1], tau[p0:p1], 1e-3, counts[p0:p1])
+        del rdepth
+    return counts, verify_score(counts)
+
+
 # ---------------------------------------------------------------------------------------------- SAM encoder attention
 def attn_relpos(qkv: Tensor, nW: int, Hs: int, Ws: int, nH: int, rel_h: Tensor, rel_w: Tensor, scale: float,
                 out_dtype=torch.float32) -> Tensor:

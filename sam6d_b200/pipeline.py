@@ -190,7 +190,8 @@ def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
 
 # ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
 def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
-              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None, icp=None, icp_iters: int = 0):
+              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None, icp=None, icp_iters: int = 0,
+              verify=None, verify_tau: float = 0.1):
     """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
     enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
     model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
@@ -198,12 +199,17 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
     Several objects: bank (O,2048,3), (O,2048,256), model_points_m (O,n,3) and det_obj the object index of every record; each
     detection gets its object's radius filter, model points and template bank, and all run as one batch.  The frame then also
     holds obj (P) int64, choose_idx (P,2048) and rand, the coarse stage's uniforms.  icp_iters > 0: after the forward the poses
-    are refined by icp_refine_out against the observed points with icp = (samples, normals) (O,M,3) on the device."""
+    are refined by icp_refine_out against the observed points with icp = (samples, normals) (O,M,3) on the device.
+    verify, the device meshes in mm of the objects (one per object, in model_points_m's order; verify_mesh): after the forward
+    and any ICP, verify_out checks every reported pose against the frame's depth and its detection's mask with tolerance
+    verify_tau x its object's radius."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
-    input_data, img, _, model_points, kept = inputs.get_test_data(
+    got = inputs.get_test_data(
         [dict(d) for d in dets], rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh,
-        cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device, det_obj=det_obj)
+        cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device, det_obj=det_obj,
+        frame_rows=verify is not None)
+    input_data, img, _, model_points, kept = got[:5]
     n = input_data["pts"].size(0)
     mark("pem_inputs")
     out = rand = None
@@ -221,6 +227,9 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
             if icp_iters > 0:
                 obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int32, device=input_data["pts"].device)
                 icp_refine_out(out, input_data["pts"], input_data["model"], obj, icp, icp_iters)
+            if verify is not None:
+                obj = input_data["obj"].cpu().numpy() if det_obj is not None else np.zeros(n, np.int64)
+                verify_out(out, verify, obj, object_radii(model_points_m), got[5], cam_K, verify_tau)
     mark("forward")
     frame = SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
     if det_obj is not None:
@@ -230,11 +239,17 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
 
 def pem_records(frame):
     """pem_frame's result -> the PEM CLI's records: the kept ISM records with the pose score, R and t (mm).  The host arrays
-    behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation."""
+    behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation.  When the poses were
+    verified (verify_out), the score is pred_pose_score x ISM score x verify and each record also carries "verify"."""
     if frame.out is None:
         return []
     out = frame.out
-    frame.pose_scores = (out["pred_pose_score"] * out["score"]).detach().cpu().numpy()
+    verified = "verify" in out
+    if verified:
+        frame.pose_scores = (out["pred_pose_score"] * out["score"] * out["verify"]).detach().cpu().numpy()
+        verify = out["verify"].cpu().numpy()
+    else:
+        frame.pose_scores = (out["pred_pose_score"] * out["score"]).detach().cpu().numpy()
     frame.pred_rot = out["pred_R"].detach().cpu().numpy()
     frame.pred_trans = out["pred_t"].detach().cpu().numpy() * 1000
     records = frame.dets
@@ -242,6 +257,8 @@ def pem_records(frame):
         records[idx]["score"] = float(frame.pose_scores[idx])
         records[idx]["R"] = list(frame.pred_rot[idx].tolist())
         records[idx]["t"] = list(frame.pred_trans[idx].tolist())
+        if verified:
+            records[idx]["verify"] = float(verify[idx])
     return records
 
 
@@ -274,11 +291,39 @@ def icp_refine_out(out: dict, pts: torch.Tensor, model: torch.Tensor, obj: torch
     return out
 
 
+# ---- depth verification of the reported poses (not in the reference) ----------------------------------------------------------
+def verify_mesh(verts_mm: np.ndarray, faces: np.ndarray, device) -> meshio.Mesh:
+    """a CAD model in mm -> its vertices and faces on the device, the mesh ops.verify_poses renders (no colours)"""
+    faces = np.asarray(faces)
+    if faces.ndim != 2 or faces.shape[0] == 0:
+        raise ValueError("pose verification renders the object: its mesh needs faces")
+    return render.upload(meshio.Mesh(vertices=np.asarray(verts_mm, np.float32), faces=faces), device)
+
+
+def object_radii(model_points_m) -> np.ndarray:
+    """model points (n,3) or (O,n,3) -> (O,) each object's max |model point| in metres, as ObjectSet.radii"""
+    mp = np.asarray(model_points_m, dtype=np.float32)
+    return np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp.reshape((-1,) + mp.shape[-2:])])
+
+
+def verify_out(out: dict, meshes, obj: np.ndarray, radii: np.ndarray, rows, cam_K, verify_tau: float):
+    """check Net.forward's (or the ICP's) poses against the frame in place: out["verify_counts"] (P,6) i32 and out["verify"]
+    (P,) f32 of ops.verify_poses.  meshes: the objects' device meshes in mm; obj (P) each pose's object; radii (O,) metres;
+    rows: inputs.FrameInputs.rows of the kept detections (depth, mask, mrow); tau = verify_tau x the object's radius."""
+    obj = np.asarray(obj, dtype=np.int64)
+    tau = float(verify_tau) * np.asarray(radii, dtype=np.float64)[obj]
+    counts, v = ops.verify_poses(out["pred_R"].contiguous(), out["pred_t"].contiguous(), obj, meshes, rows.depth, rows.mask, rows.mrow,
+                                 np.asarray(cam_K, dtype=np.float64).reshape(3, 3), tau)
+    out.update(verify_counts=counts, verify=v)
+    return out
+
+
 # ---- the whole pipeline ----------------------------------------------------------------------------------------------------
 @dataclass
 class Onboarded:
     """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank, model points;
-    with icp_iters > 0 also the ICP samples (M,3) in metres and their unit normals (icp_model), else None"""
+    with icp_iters > 0 also the ICP samples (M,3) in metres and their unit normals (icp_model), else None; with verify the
+    device mesh in mm that pose verification renders (verify_mesh), else None"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
@@ -287,6 +332,7 @@ class Onboarded:
     model_points_m: np.ndarray
     icp_points_m: Optional[np.ndarray] = None
     icp_normals: Optional[np.ndarray] = None
+    verify_mesh: Optional[meshio.Mesh] = None
 
 
 class SAM6D:
@@ -306,7 +352,12 @@ class SAM6D:
     mesh either way.
 
     icp_iters (not in the reference; default 0, off): refine every PEM pose with that many point-to-plane ICP iterations
-    against the frame's observed points (icp_refine_out).  Records then carry the refined R and t; scores are unchanged."""
+    against the frame's observed points (icp_refine_out).  Records then carry the refined R and t; scores are unchanged.
+
+    verify (not in the reference; default False, off): render every reported pose, after any ICP, and count its agreement with
+    the frame's depth and its detection's mask (verify_out, with tolerance verify_tau x the object's radius).  Each record's
+    score is then pred_pose_score x ISM score x verify, and the record carries "verify"; R and t are unchanged.  Onboarding
+    keeps each object's mesh on the device for it."""
     rendering_type = "pyrender"
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
@@ -315,7 +366,7 @@ class SAM6D:
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
                  device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5",
                  fastsam_model: str = "FastSAM-x", rendering_type: str = "pyrender", pbr_root: Optional[str] = None,
-                 pbr_split: str = "train_pbr", icp_iters: int = 0):
+                 pbr_split: str = "train_pbr", icp_iters: int = 0, verify: bool = False, verify_tau: float = 0.1):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
         if fastsam_model not in ism_cli.FASTSAM_MODELS:
@@ -334,6 +385,9 @@ class SAM6D:
         if int(icp_iters) < 0:
             raise ValueError(f"icp_iters must be >= 0, got {icp_iters}")
         self.icp_iters = int(icp_iters)
+        if not (np.isfinite(verify_tau) and verify_tau > 0):
+            raise ValueError(f"verify_tau must be a finite number > 0, got {verify_tau}")
+        self.verify, self.verify_tau = bool(verify), float(verify_tau)
         self.rendering_type, self.pbr_root, self.pbr_split, self._pbr_rows = rendering_type, pbr_root, pbr_split, None
         self.level_templates, self.pose_distribution = int(level_templates), pose_distribution
         self.aggregation_function = aggregation_function
@@ -394,7 +448,8 @@ class SAM6D:
                                  device=self.device)
         model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
         icp_pts, icp_nrm = icp_model(verts, faces) if self.icp_iters > 0 else (None, None)
-        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points, icp_pts, icp_nrm)
+        vmesh = verify_mesh(verts, faces, self.device) if self.verify else None
+        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points, icp_pts, icp_nrm, vmesh)
 
     def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
         """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
@@ -483,7 +538,9 @@ class SAM6D:
         chunk of 16).  Random draws from `rng` (default numpy's global RNG): the model points of every object, each object's
         42 template samples, then the observed points in detection order.  An image none of whose detections survives is
         skipped (the reference fails there).  Writes the CSV lines to out_path and returns them.  mark(stage) after
-        "onboard", and per image after "decode", "pem_inputs" and "forward".  icp_iters > 0: each image's poses are refined (icp_refine_out) before its rows are built."""
+        "onboard", and per image after "decode", "pem_inputs" and "forward".  icp_iters > 0: each image's poses are refined (icp_refine_out) before its rows are built.
+        verify: each image's poses are then verified (verify_out, the dataset's meshes) and each row's score is
+        pred_pose_score x detection score x verify."""
         mark = mark or (lambda stage: None)
         rng = rng if rng is not None else np.random
         cfg = pem_cli.TEST_DATASET
@@ -498,6 +555,9 @@ class SAM6D:
         icp = None
         if self.icp_iters > 0:
             icp = icp_tensors(*(np.stack(a) for a in zip(*[icp_model(m.vertices, m.faces) for m in meshes])), self.device)
+        vmeshes, radii = None, None
+        if self.verify:
+            vmeshes, radii = [verify_mesh(m.vertices, m.faces, self.device) for m in meshes], object_radii(model_points)
         mark("onboard")
         with open(detections_path) as fh:
             groups = bop.group_detections(json.load(fh))
@@ -511,8 +571,9 @@ class SAM6D:
             mark("decode")
             torch.cuda.synchronize(self.device)
             t0 = time.time()
-            data, kept, _ = bop.pem_instances(dets, image, raw, cam_K, depth_scale, objs, model_points, rng=rng,
-                                              n_sample=cfg["n_sample_observed_point"], img_size=cfg["img_size"], device=self.device)
+            got = bop.pem_instances(dets, image, raw, cam_K, depth_scale, objs, model_points, rng=rng, n_sample=cfg["n_sample_observed_point"],
+                                    img_size=cfg["img_size"], device=self.device, frame_rows=vmeshes is not None)
+            data, kept = got[:2]
             mark("pem_inputs")
             n = len(kept)
             if n == 0:
@@ -523,7 +584,12 @@ class SAM6D:
                 out = self.pem(data, rand=rand)
                 if icp is not None:
                     icp_refine_out(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters)
-            scores = (out["pred_pose_score"] * data["score"]).cpu().numpy()
+                if vmeshes is not None:
+                    verify_out(out, vmeshes, data["obj"].cpu().numpy(), radii, got[3], cam_K, self.verify_tau)
+            if vmeshes is not None:
+                scores = (out["pred_pose_score"] * data["score"] * out["verify"]).cpu().numpy()
+            else:
+                scores = (out["pred_pose_score"] * data["score"]).cpu().numpy()
             R = out["pred_R"].reshape(-1, 9).cpu().numpy()
             t = out["pred_t"].cpu().numpy() * 1000
             image_time = time.time() - t0 + float(np.float32(dets[0]["time"]))
@@ -565,8 +631,14 @@ class SAM6D:
         g = torch.Generator(device=self.device)
         g.manual_seed(pem_cli.RD_SEED)
         icp = icp_tensors(obj.icp_points_m, obj.icp_normals, self.device) if self.icp_iters > 0 else None
+        vmeshes = None
+        if self.verify:
+            vmeshes = obj.verify_meshes if multi else ([obj.verify_mesh] if obj.verify_mesh is not None else None)
+            if vmeshes is None:
+                raise ValueError("pose verification needs the objects' device meshes: onboard them with SAM6D(..., verify=True)")
         frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
-                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj, icp=icp, icp_iters=self.icp_iters)
+                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj, icp=icp, icp_iters=self.icp_iters,
+                          verify=vmeshes, verify_tau=self.verify_tau)
         pem_recs = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
@@ -581,7 +653,7 @@ class ObjectSet:
     ref_patch (O,T,256,C), template poses poses_m (O,T,4,4) (the framing distance depends on the mesh), geometric-score clouds
     cloud_m (O,2048,3), PEM template banks (O,2048,3) and (O,2048,256), model points model_points_m (O,Nm,3), each object's
     radius (O,) (the PEM's max |model point|) and category ids obj_ids; with icp_iters > 0 the ICP samples icp_points_m (O,M,3)
-    and their normals icp_normals (O,M,3), else None"""
+    and their normals icp_normals (O,M,3), else None; with verify the O device meshes verify_meshes (verify_mesh), else None"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
@@ -592,6 +664,7 @@ class ObjectSet:
     obj_ids: list
     icp_points_m: Optional[np.ndarray] = None
     icp_normals: Optional[np.ndarray] = None
+    verify_meshes: Optional[list] = None
 
     @staticmethod
     def stack(parts, ref_patch, obj_ids) -> "ObjectSet":
@@ -603,4 +676,5 @@ class ObjectSet:
                          bank=tuple(torch.stack([p.bank[i].reshape(p.bank[i].shape[-2:]) for p in parts]) for i in range(2)),
                          model_points_m=mp, radii=np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp]), obj_ids=list(obj_ids),
                          icp_points_m=np.stack([p.icp_points_m for p in parts]) if icp else None,
-                         icp_normals=np.stack([p.icp_normals for p in parts]) if icp else None)
+                         icp_normals=np.stack([p.icp_normals for p in parts]) if icp else None,
+                         verify_meshes=[p.verify_mesh for p in parts] if parts[0].verify_mesh is not None else None)
