@@ -332,6 +332,23 @@ int sam6d_coarse_hypotheses(const int* idx, const float* pts1, const float* pts2
 int sam6d_topk_smallest(const float* v, int B, int n, int k, int* out, void* stream);
 int sam6d_coarse_select(const float* Rt, const int* top, int B, int n1, int n2, const float* pts1, const float* w1, int n,
                         const float* model, int nm, float* scores, float* R, float* t, void* stream);
+/* K mutually distinct hypotheses per proposal (not in the reference), from the Rt (B,n1,12), top (B,n2) and scores (B,n2) of
+ * sam6d_coarse_select.  One CTA per proposal, K greedy rounds over the n2 retained hypotheses (all live at the start):
+ *   1. pick i = the first argmax of the live scores, coarse_pick_kernel's rule: a NaN score is never picked; an all-NaN row
+ *      picks hypothesis 0 in round 0; a later round with no pickable live hypothesis ends the selection;
+ *   2. slot r = (R_i, t_i, score_i), valid 1; i is no longer live;
+ *   3. every live j that is not distinct from i is no longer live.  j is distinct from i when tr < cos_thr or d2 >= d2_min,
+ *      in fp32 rounded to nearest, no fused multiply-add, in this order:
+ *        tr = R_i[0] R_j[0];  tr = tr + R_i[e] R_j[e] for e = 1..8      (trace(R_i^T R_j), R row-major)
+ *        dx, dy, dz = t_i - t_j;  d2 = (dx dx + dy dy) + dz dz
+ *      with cos_thr = 1 + 2 cos(min_angle) and d2_min = min_dist^2 (the t are the coarse stage's radius-normalised units).
+ * R_out (B,K,3,3), t_out (B,K,3), score_out (B,K) f32, valid (B,K) u8, count (B) i32 = the number of rounds that picked; the
+ * slots from count on are copies of slot 0 with valid 0.  Slot 0 is sam6d_coarse_select's R, t bit for bit.
+ * -22 (nothing launched): B < 0, n1 < 1, n2 < 1, n2 > 2048 (the shared-memory staging), K < 1, K > n2, a non-finite
+ * threshold, a NULL pointer. */
+int sam6d_coarse_pick_distinct(const float* Rt, const int* top, const float* scores, int B, int n1, int n2, int K, float cos_thr,
+                               float d2_min, float* R_out, float* t_out, float* score_out, unsigned char* valid, int* count,
+                               void* stream);
 
 /* ---- fine stage ---------------------------------------------------------------------------------------------------- */
 

@@ -14,6 +14,7 @@ import os
 import sys
 
 from . import ism_run_inference_custom as ism_cli
+from . import pem_run_inference_custom as pem_cli
 from .. import bop
 
 
@@ -50,12 +51,14 @@ def get_parser():
     # not in the reference: rescore each reported pose by its agreement with the observed depth (pipeline.verify_out)
     ap.add_argument("--verify", action="store_true", help="render every pose and multiply its score by its depth agreement")
     ap.add_argument("--verify_tau", default=0.1, type=float, help="--verify's depth tolerance over the object's radius")
+    pem_cli.add_hypothesis_args(ap)
     return ap
 
 
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
+    pem_cli.check_hypothesis_args(ap, args)
     if args.stage in ("pem", "both") and args.template_dir is None:
         ap.error(f"--stage {args.stage} needs --template_dir (the PEM's template views)")
     if args.stage == "both" and args.detections is not None:
@@ -76,7 +79,8 @@ def main(argv=None):
                   precision=args.precision, level_templates=args.level_templates, pose_distribution=args.pose_distribution,
                   aggregation_function=args.aggregation_function, rendering_type=args.rendering_type,
                   pbr_root=dataset_root if args.rendering_type == "pbr" else None, pbr_split=args.pbr_split,
-                  icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau)
+                  icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau, pem_hypotheses=args.pem_hypotheses,
+                  hyp_min_angle=args.hyp_min_angle, hyp_min_dist=args.hyp_min_dist)
     os.makedirs(args.output_dir, exist_ok=True)
     if args.stage in ("ism", "both"):
         objects = sam6d.onboard_bop(args.bop_root, args.dataset_name, template_size=args.template_size)

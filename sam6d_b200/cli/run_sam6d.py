@@ -72,12 +72,14 @@ def get_parser():
     # not in the reference: rescore each reported pose by its agreement with the observed depth (pipeline.verify_out)
     ap.add_argument("--verify", action="store_true", help="render every pose and multiply its score by its depth agreement")
     ap.add_argument("--verify_tau", default=0.1, type=float, help="--verify's depth tolerance over the object's radius")
+    pem_cli.add_hypothesis_args(ap)
     return ap
 
 
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
+    pem_cli.check_hypothesis_args(ap, args)
     if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
         ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
     sam6d = build_sam6d(args)
@@ -118,7 +120,8 @@ def build_sam6d(args):
                  det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
                  rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split,
-                 icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau)
+                 icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau, pem_hypotheses=args.pem_hypotheses,
+                 hyp_min_angle=args.hyp_min_angle, hyp_min_dist=args.hyp_min_dist)
 
 
 def write_vis_objects(path, frame, cam_K):

@@ -53,6 +53,7 @@ def frame_pairs(rgb_dir: str, depth_dir: str):
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
+    run_sam6d.pem_cli.check_hypothesis_args(ap, args)
     if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
         ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
     if args.obj_ids is not None and len(args.obj_ids) != len(args.cad_path):

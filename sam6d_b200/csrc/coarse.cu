@@ -8,6 +8,7 @@
 //   3. coarse_hypotheses : 3-point Procrustes per hypothesis + mean residual                      -> Rt (b,n1,12), resid
 //   4. coarse_topk    : the n2 smallest residuals (value, then index)                              -> top (b,n2)
 //   5. coarse_select  : score = sum(w1) / (sum_i w1_i min_m ||(p_i - t) R - model_m|| + 1e-8); argmax -> init_R, init_t
+//   6. coarse_pick_distinct (opt-in, not in the reference): K mutually distinct hypotheses of the n2 scored ones
 #include "common.cuh"
 #include "svd3.cuh"
 
@@ -324,6 +325,75 @@ __global__ void coarse_pick_kernel(const float* __restrict__ scores, const int* 
   if (lane < 3) t[(size_t)b * 3 + lane] = rt[9 + lane];
 }
 
+// ---- 6. K mutually distinct hypotheses (not in the reference) ---------------------------------------------------
+// one CTA per proposal; the n2 retained hypotheses sit in shared memory as R (9), t (3), score and a live flag.  K greedy rounds:
+// block argmax of the live scores (coarse_pick_kernel's rule), write the pick, drop every live hypothesis that is not distinct
+// from it (the rule and its fp32 order: include/sam6d_b200.h, sam6d_coarse_pick_distinct)
+constexpr int PICK_THREADS = 256, PICK_MAX_N2 = 2048;
+__global__ void __launch_bounds__(PICK_THREADS) coarse_pick_distinct_kernel(const float* __restrict__ Rt, const int* __restrict__ top,
+                                                                            const float* __restrict__ scores, int n1, int n2, int K,
+                                                                            float cos_thr, float d2_min, float* __restrict__ R_out,
+                                                                            float* __restrict__ t_out, float* __restrict__ score_out,
+                                                                            unsigned char* __restrict__ valid, int* __restrict__ count) {
+  extern __shared__ float hs[];
+  float* hr = hs;                    // n2 x 12: R row-major, t
+  float* sc = hr + (size_t)n2 * 12;  // n2
+  unsigned char* live = reinterpret_cast<unsigned char*>(sc + n2);
+  __shared__ float rv[PICK_THREADS / 32];
+  __shared__ int ri[PICK_THREADS / 32];
+  __shared__ int pick;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int e = tid; e < n2 * 12; e += PICK_THREADS) {
+    const int j = e / 12, c = e - j * 12;
+    hr[e] = Rt[((size_t)b * n1 + top[(size_t)b * n2 + j]) * 12 + c];
+  }
+  for (int j = tid; j < n2; j += PICK_THREADS) { sc[j] = scores[(size_t)b * n2 + j]; live[j] = 1; }
+  __syncthreads();
+  int found = 0;
+  for (int r = 0; r < K; ++r) {
+    float bv = -INFINITY; int bi = 0x7fffffff;
+    for (int j = tid; j < n2; j += PICK_THREADS)
+      if (live[j]) argmax_first(bv, bi, sc[j], j);
+    warp_argmax_first(bv, bi);
+    if (lane == 0) { rv[warp] = bv; ri[warp] = bi; }
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < PICK_THREADS / 32; ++w) argmax_first(bv, bi, rv[w], ri[w]);
+      if (bi == 0x7fffffff && r == 0) bi = 0;   // all-NaN row: keep the first hypothesis, as coarse_pick_kernel
+      pick = bi;
+    }
+    __syncthreads();
+    const int i = pick;
+    if (i == 0x7fffffff) break;                 // no live hypothesis left (or only NaN scores)
+    const float* hi = hr + (size_t)i * 12;
+    if (tid < 9) R_out[((size_t)b * K + r) * 9 + tid] = hi[tid];
+    if (tid < 3) t_out[((size_t)b * K + r) * 3 + tid] = hi[9 + tid];
+    if (tid == 0) { score_out[(size_t)b * K + r] = sc[i]; valid[(size_t)b * K + r] = 1; }
+    for (int j = tid; j < n2; j += PICK_THREADS) {
+      if (!live[j]) continue;
+      const float* hj = hr + (size_t)j * 12;
+      float tr = __fmul_rn(hi[0], hj[0]);
+#pragma unroll
+      for (int e = 1; e < 9; ++e) tr = __fadd_rn(tr, __fmul_rn(hi[e], hj[e]));
+      const float dx = __fsub_rn(hi[9], hj[9]), dy = __fsub_rn(hi[10], hj[10]), dz = __fsub_rn(hi[11], hj[11]);
+      const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+      if (j == i || !(tr < cos_thr || d2 >= d2_min)) live[j] = 0;
+    }
+    found = r + 1;
+    __syncthreads();
+  }
+  // slots past the last pick: copies of slot 0, not valid
+  for (int e = tid; e < (K - found) * 14; e += PICK_THREADS) {
+    const int r = found + e / 14, c = e - (e / 14) * 14;
+    const size_t s0 = (size_t)b * K, s = s0 + r;
+    if (c < 9) R_out[s * 9 + c] = R_out[s0 * 9 + c];
+    else if (c < 12) t_out[s * 3 + c - 9] = t_out[s0 * 3 + c - 9];
+    else if (c == 12) score_out[s] = score_out[s0];
+    else valid[s] = 0;
+  }
+  if (tid == 0) count[b] = found;
+}
+
 }  // namespace
 
 // A (B,S,S) f32 -> W (B,(S-1)^2) masked soft assignment ^1.5, w1 (B,S-1)      (model_utils.py:206-216)
@@ -390,6 +460,22 @@ S6_API int sam6d_coarse_select(const float* Rt, const int* top, int B, int n1, i
   coarse_select_kernel<<<grid, SEL_THREADS, smem, s6_stream(stream)>>>(Rt, top, n1, n2, pts1, w1, n, model, nm, scores);
   S6_LAUNCH_CHECK();
   coarse_pick_kernel<<<B, 32, 0, s6_stream(stream)>>>(scores, top, Rt, n1, n2, R, t);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+// K mutually distinct hypotheses of the n2 that sam6d_coarse_select scored (the rule: include/sam6d_b200.h)
+S6_API int sam6d_coarse_pick_distinct(const float* Rt, const int* top, const float* scores, int B, int n1, int n2, int K, float cos_thr,
+                                      float d2_min, float* R_out, float* t_out, float* score_out, unsigned char* valid, int* count,
+                                      void* stream) {
+  S6_REQUIRE(B >= 0 && n1 > 0 && n2 > 0 && n2 <= PICK_MAX_N2 && K >= 1 && K <= n2);
+  S6_REQUIRE(isfinite(cos_thr) && isfinite(d2_min));
+  S6_REQUIRE(Rt && top && scores && R_out && t_out && score_out && valid && count);
+  if (B == 0) return 0;
+  const size_t smem = (size_t)n2 * 13 * sizeof(float) + n2;
+  S6_CHECK(cudaFuncSetAttribute(coarse_pick_distinct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  coarse_pick_distinct_kernel<<<B, PICK_THREADS, smem, s6_stream(stream)>>>(Rt, top, scores, n1, n2, K, cos_thr, d2_min, R_out, t_out,
+                                                                          score_out, valid, count);
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -693,6 +693,37 @@ def coarse_select(Rt: Tensor, top: Tensor, pts1: Tensor, w1: Tensor, model: Tens
     return R, t, scores
 
 
+def hypothesis_thresholds(min_angle: float, min_dist: float) -> Tuple[float, float]:
+    """min_angle (degrees), min_dist (radius-normalised) -> (cos_thr, d2_min) as sam6d_coarse_pick_distinct receives them: 1 + 2
+    cos(min_angle) and min_dist^2, each evaluated in float64 and rounded to fp32"""
+    return (float(np.float32(1.0 + 2.0 * np.cos(np.radians(float(min_angle))))),
+            float(np.float32(float(min_dist) * float(min_dist))))
+
+
+def coarse_pick_distinct(Rt: Tensor, top: Tensor, scores: Tensor, K: int, min_angle: float, min_dist: float):
+    """K mutually distinct hypotheses of the coarse stage per proposal (the rule: include/sam6d_b200.h,
+    sam6d_coarse_pick_distinct).  Rt (B,n1,12), top (B,n2), scores (B,n2) of coarse_select -> R (B,K,3,3), t (B,K,3), score (B,K)
+    f32, valid (B,K) u8, count (B) i32; slot 0 is coarse_select's pose, slots from count on are copies of it with valid 0."""
+    _check(Rt, torch.float32, "Rt", 3)
+    _check(top, torch.int32, "top", 2)
+    _check(scores, torch.float32, "scores", 2)
+    B, n1, _ = Rt.shape
+    n2 = top.shape[1]
+    if tuple(scores.shape) != (B, n2) or top.shape[0] != B:
+        raise RuntimeError(f"coarse_pick_distinct: Rt (B,n1,12), top and scores (B,n2), got {tuple(Rt.shape)}, {tuple(top.shape)}, "
+                           f"{tuple(scores.shape)}")
+    cos_thr, d2_min = hypothesis_thresholds(min_angle, min_dist)
+    dev = Rt.device
+    K = int(K)
+    R = torch.empty(B, max(K, 0), 3, 3, dtype=torch.float32, device=dev)
+    t = torch.empty(B, max(K, 0), 3, dtype=torch.float32, device=dev)
+    score = torch.empty(B, max(K, 0), dtype=torch.float32, device=dev)
+    valid = torch.empty(B, max(K, 0), dtype=torch.uint8, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    _lib.call("sam6d_coarse_pick_distinct", Rt, top, scores, B, n1, n2, K, cos_thr, d2_min, R, t, score, valid, count)
+    return R, t, score, valid, count
+
+
 # ---------------------------------------------------------------------------------------------- fine stage
 def pe_mlp_max(pts: Tensor, idx: Tensor, cnt: Tensor, weights, out: Tensor, out_off: int):
     _check(pts, torch.float32, "pts", 3)

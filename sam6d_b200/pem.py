@@ -386,10 +386,14 @@ def compute_feature_similarity(feat1, feat2, type='cosine', temp=1.0, normalize_
     return store[:, :, :M]                     # (B,N,M) like the reference; dense rows, row stride ld
 
 
-def compute_coarse_Rt(atten, pts1, pts2, model_pts=None, n_proposal1=6000, n_proposal2=300, rand=None, return_scores=False):
+def compute_coarse_Rt(atten, pts1, pts2, model_pts=None, n_proposal1=6000, n_proposal2=300, rand=None, return_scores=False,
+                      n_hypotheses=1, min_angle=30.0, min_dist=0.2):
     """model_utils.py:187-246.  `rand` (B, 3*n_proposal1) overrides the torch.rand draw (used by the parity tests to feed the
     reference and this implementation the same uniforms); by default the call is the reference's own
-    torch.rand(B, n_proposal1*3, device=device), so the Philox stream position matches."""
+    torch.rand(B, n_proposal1*3, device=device), so the Philox stream position matches.
+    n_hypotheses = K > 1 (not in the reference) appends the K mutually distinct hypotheses of ops.coarse_pick_distinct (at least
+    min_angle degrees or min_dist radius-normalised units apart) to the return values: R (B,K,3,3), t (B,K,3), score (B,K),
+    valid (B,K) u8, count (B) i32, slot 0 being the returned R, t."""
     B = pts1.shape[0]
     if model_pts is None:
         model_pts = pts2
@@ -400,9 +404,10 @@ def compute_coarse_Rt(atten, pts1, pts2, model_pts=None, n_proposal1=6000, n_pro
     Rt, resid = ops.coarse_hypotheses(idx, pts1.contiguous(), pts2.contiguous())
     top = ops.topk_smallest(resid, n_proposal2)
     R, t, scores = ops.coarse_select(Rt, top, pts1.contiguous(), w1, model_pts.contiguous())
+    hyp = ops.coarse_pick_distinct(Rt, top, scores, n_hypotheses, min_angle, min_dist) if n_hypotheses > 1 else ()
     if return_scores:
-        return R, t, scores          # (B, n_proposal2) selection scores of the retained hypotheses
-    return R, t
+        return (R, t, scores) + hyp  # (B, n_proposal2) selection scores of the retained hypotheses
+    return (R, t) + hyp
 
 
 def compute_fine_Rt(atten, pts1, pts2, model_pts=None, dis_thres=0.15, temp=0.1, radius=None, check_bound=True):
@@ -466,7 +471,9 @@ class CoarsePointMatching(nn.Module):
         return out
 
     @torch.no_grad()
-    def forward(self, p1, f1, geo1, p2, f2, geo2, radius, end_points, rand=None):
+    def forward(self, p1, f1, geo1, p2, f2, geo2, radius, end_points, rand=None, hypotheses=(1, 30.0, 0.2)):
+        """hypotheses = (K, min_angle, min_dist): with K > 1 end_points also gets hyp_init_R (B,K,3,3), hyp_init_t (B,K,3) and
+        hyp_valid (B,K) u8 of compute_coarse_Rt's distinct hypotheses"""
         if self.training:
             raise NotImplementedError("sam6d_b200 implements the inference path (model.eval())")
         B = f1.shape[0]
@@ -480,8 +487,12 @@ class CoarsePointMatching(nn.Module):
         o1, o2 = o[:B], o[B:]
         atten = compute_feature_similarity(o1, o2, self.cfg.sim_type, self.cfg.temp, self.cfg.normalize_feat, self.precision)
         model = ops.scale_by_radius(end_points['model'].contiguous(), radius.contiguous())
-        init_R, init_t, self.last_select_scores = compute_coarse_Rt(atten, p1, p2, model, self.cfg.nproposal1,
-                                                                    self.cfg.nproposal2, rand=rand, return_scores=True)
+        K, min_angle, min_dist = hypotheses
+        res = compute_coarse_Rt(atten, p1, p2, model, self.cfg.nproposal1, self.cfg.nproposal2, rand=rand, return_scores=True,
+                                n_hypotheses=K, min_angle=min_angle, min_dist=min_dist)
+        init_R, init_t, self.last_select_scores = res[:3]
+        if K > 1:
+            end_points['hyp_init_R'], end_points['hyp_init_t'], _, end_points['hyp_valid'], _ = res[3:]
         end_points['init_R'] = init_R
         end_points['init_t'] = init_t
         if self.return_feat:
@@ -820,6 +831,29 @@ DEFAULT_MODEL_CFG = dict(
                              focusing_factor=3, temp=0.1, sim_type='cosine', normalize_feat=True, loss_dis_thres=0.15),
 )  # PEM/config/base.yaml:17-54
 
+MAX_HYPOTHESES = 16            # Net.set_hypotheses: fine-stage passes per forward
+# the outputs a forward with K > 1 hypotheses adds (Net.set_hypotheses), as graph.StepGraphs copies them out of a replay
+HYP_KEYS = ("hyp_init_R", "hyp_init_t", "hyp_R", "hyp_t", "hyp_pose_score", "hyp_valid", "hyp_index")
+
+
+def check_hypotheses(k, min_angle, min_dist):
+    """-> (k, min_angle, min_dist) as int, float, float; ValueError unless 1 <= k <= MAX_HYPOTHESES, 0 < min_angle <= 180
+    (degrees) and min_dist >= 0, both finite"""
+    if isinstance(k, bool) or int(k) != k or not 1 <= int(k) <= MAX_HYPOTHESES:
+        raise ValueError(f"the number of hypotheses must be an integer in [1, {MAX_HYPOTHESES}], got {k}")
+    if not (math.isfinite(min_angle) and 0.0 < min_angle <= 180.0):
+        raise ValueError(f"min_angle must lie in (0, 180] degrees, got {min_angle}")
+    if not (math.isfinite(min_dist) and min_dist >= 0.0):
+        raise ValueError(f"min_dist must be a finite number >= 0, got {min_dist}")
+    return int(k), float(min_angle), float(min_dist)
+
+
+def first_best(score: torch.Tensor, valid: torch.Tensor) -> torch.Tensor:
+    """(B,K) scores and valid flags -> (B) i64 the first k with the largest score among the valid slots; a NaN score never
+    wins, and a row with nothing to choose gives 0"""
+    ok = valid.bool() & ~torch.isnan(score)
+    return torch.where(ok, score, torch.full_like(score, -math.inf)).argmax(dim=1)
+
 
 class Net(nn.Module):
     """Pose_Estimation_Model `Net` (pose_estimation_model.py:11-53).
@@ -847,6 +881,7 @@ class Net(nn.Module):
         self.coarse_point_matching = CoarsePointMatching(cfg.coarse_point_matching)
         self.fine_point_matching = FinePointMatching(cfg.fine_point_matching)
         self._graphs = None
+        self.hypotheses = (1, 30.0, 0.2)
         self.set_precision(precision)
 
     def enable_graphs(self, max_graphs: int = 8):
@@ -871,6 +906,17 @@ class Net(nn.Module):
                 m.precision = precision
         return self
 
+    def set_hypotheses(self, k: int = 1, min_angle: float = 30.0, min_dist: float = 0.2):
+        """run the fine stage from k mutually distinct coarse hypotheses and keep the best (not in the reference).  Two
+        hypotheses are distinct when their rotations differ by at least min_angle degrees or their translations by at least
+        min_dist object radii (ops.coarse_pick_distinct).  forward() then runs the coarse stage once and the fine stage once per
+        hypothesis on the same batch, and reports, per proposal, the pass with the largest pred_pose_score among the valid
+        ones (the first on a tie), plus hyp_init_R (B,k,3,3), hyp_init_t (B,k,3), hyp_R, hyp_t, hyp_pose_score (B,k), hyp_valid
+        (B,k) u8 and hyp_index (B) i64; init_R and init_t stay the coarse stage's pick.  k = 1 (default): the reference's
+        forward, with no hyp_* output."""
+        self.hypotheses = check_hypotheses(k, min_angle, min_dist)
+        return self
+
     def _features(self, end_points):
         """ViTEncoder.forward, inference branch (feature_extraction.py:128-142)"""
         if 'dense_fm' in end_points:
@@ -892,13 +938,14 @@ class Net(nn.Module):
         """rand: the (B, 3*nproposal1) uniforms of compute_coarse_Rt (default: drawn like the reference).  init_pose = (R, t):
         the fine stage starts from this pose instead of the coarse stage's (the coarse stage still runs and reports init_R /
         init_t); used by the parity tests to hold the fine stage to the 1e-3 bar independently of the coarse stage's discrete
-        hypothesis selection."""
+        hypothesis selection.  A call with init_pose runs one fine pass whatever set_hypotheses chose."""
         if self.training:
             raise NotImplementedError("sam6d_b200 implements the inference path: call model.eval()")
         if self._graphs is not None and init_pose is None and 'pts' in end_points:
             n_rand = self.coarse_point_matching.cfg.nproposal1 * 3
             out = self._graphs.run(lambda ep, r: self._forward(ep, r, None), end_points, rand, n_rand,
-                                   extra=(self.precision, hash(_param_key(self))))
+                                   extra=(self.precision, hash(_param_key(self)), self.hypotheses),
+                                   keys=HYP_KEYS if self.hypotheses[0] > 1 else ())
             if out is not None:
                 return out
         return self._forward(end_points, rand, init_pose)
@@ -931,8 +978,25 @@ class Net(nn.Module):
         geo = self.geo_embedding(torch.cat([bg_point, sp], dim=1))
         sparse_pm, sparse_po, sparse_fm, sparse_fo = sp[:B], sp[B:], sf[:B], sf[B:]
         fps_idx_m, fps_idx_o, geo_embedding_m, geo_embedding_o = idx[:B], idx[B:], geo[:B], geo[B:]
+        K = self.hypotheses[0] if init_pose is None else 1
         end_points = self.coarse_point_matching(sparse_pm, sparse_fm, geo_embedding_m, sparse_po, sparse_fo, geo_embedding_o,
-                                                radius, end_points, rand=rand)
+                                                radius, end_points, rand=rand, hypotheses=(K,) + self.hypotheses[1:])
+        if K > 1:
+            # one fine pass per hypothesis over the same B proposals: every pass reuses the clouds, features and geometric
+            # embeddings above (a (B K)-batch would copy the ~20 MB per-cloud embedding K times)
+            passes = []
+            for k in range(K):
+                ep = dict(end_points, init_R=end_points['hyp_init_R'][:, k].contiguous(),
+                          init_t=end_points['hyp_init_t'][:, k].contiguous())
+                ep = self.fine_point_matching(dense_pm, dense_fm, geo_embedding_m, fps_idx_m, dense_po, dense_fo, geo_embedding_o,
+                                              fps_idx_o, radius, ep)
+                passes.append((ep['pred_R'], ep['pred_t'], ep['pred_pose_score']))
+            hyp_R, hyp_t, hyp_s = (torch.stack(z, dim=1) for z in zip(*passes))
+            idx = first_best(hyp_s, end_points['hyp_valid'])
+            rows = torch.arange(B, device=idx.device)
+            end_points.update(hyp_R=hyp_R, hyp_t=hyp_t, hyp_pose_score=hyp_s, hyp_index=idx, pred_R=hyp_R[rows, idx],
+                              pred_t=hyp_t[rows, idx], pred_pose_score=hyp_s[rows, idx])
+            return end_points
         if init_pose is not None:
             coarse_R, coarse_t = end_points['init_R'], end_points['init_t']
             end_points['init_R'], end_points['init_t'] = init_pose[0].contiguous(), init_pose[1].contiguous()

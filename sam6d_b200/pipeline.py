@@ -31,6 +31,7 @@ from . import bop, inputs, ism, meshio, ops, pbr, render
 from .cli import ism_run_inference_custom as ism_cli
 from .cli import pem_run_inference_custom as pem_cli
 from .cli import render_custom_templates as render_cli
+from .pem import check_hypotheses, first_best
 
 N_ISM_CLOUD = 2048                     # points of the geometric score's template cloud (ISM/run_inference_custom.py:196)
 ICP_SAMPLES = 4096                     # surface samples per object for the ICP refinement (icp_iters > 0; not in the reference)
@@ -202,7 +203,8 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
     are refined by icp_refine_out against the observed points with icp = (samples, normals) (O,M,3) on the device.
     verify, the device meshes in mm of the objects (one per object, in model_points_m's order; verify_mesh): after the forward
     and any ICP, verify_out checks every reported pose against the frame's depth and its detection's mask with tolerance
-    verify_tau x its object's radius."""
+    verify_tau x its object's radius.  With several PEM hypotheses (Net.set_hypotheses) finish_poses picks each detection's
+    pose."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
     got = inputs.get_test_data(
@@ -224,12 +226,11 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
             if generator is not None:
                 rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
             out = model(input_data, rand=rand)
-            if icp_iters > 0:
-                obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int32, device=input_data["pts"].device)
-                icp_refine_out(out, input_data["pts"], input_data["model"], obj, icp, icp_iters)
-            if verify is not None:
-                obj = input_data["obj"].cpu().numpy() if det_obj is not None else np.zeros(n, np.int64)
-                verify_out(out, verify, obj, object_radii(model_points_m), got[5], cam_K, verify_tau)
+            if icp_iters > 0 or verify is not None:
+                obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int64, device=input_data["pts"].device)
+                finish_poses(out, input_data["pts"], input_data["model"], obj, icp, icp_iters, verify,
+                             object_radii(model_points_m) if verify is not None else None, got[5] if verify is not None else None,
+                             cam_K, verify_tau)
     mark("forward")
     frame = SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
     if det_obj is not None:
@@ -240,7 +241,8 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
 def pem_records(frame):
     """pem_frame's result -> the PEM CLI's records: the kept ISM records with the pose score, R and t (mm).  The host arrays
     behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation.  When the poses were
-    verified (verify_out), the score is pred_pose_score x ISM score x verify and each record also carries "verify"."""
+    verified (verify_out), the score is pred_pose_score x ISM score x verify and each record also carries "verify".  With
+    several PEM hypotheses each record also carries "hypothesis", the index of the one it reports."""
     if frame.out is None:
         return []
     out = frame.out
@@ -252,6 +254,7 @@ def pem_records(frame):
         frame.pose_scores = (out["pred_pose_score"] * out["score"]).detach().cpu().numpy()
     frame.pred_rot = out["pred_R"].detach().cpu().numpy()
     frame.pred_trans = out["pred_t"].detach().cpu().numpy() * 1000
+    hyp = out["hyp_index"].cpu().numpy() if "hyp_index" in out else None
     records = frame.dets
     for idx in range(len(records)):
         records[idx]["score"] = float(frame.pose_scores[idx])
@@ -259,6 +262,8 @@ def pem_records(frame):
         records[idx]["t"] = list(frame.pred_trans[idx].tolist())
         if verified:
             records[idx]["verify"] = float(verify[idx])
+        if hyp is not None:
+            records[idx]["hypothesis"] = int(hyp[idx])
     return records
 
 
@@ -318,6 +323,42 @@ def verify_out(out: dict, meshes, obj: np.ndarray, radii: np.ndarray, rows, cam_
     return out
 
 
+# ---- several PEM hypotheses per detection (not in the reference) ----------------------------------------------------------------
+def finish_poses(out: dict, pts: torch.Tensor, model: torch.Tensor, obj: torch.Tensor, icp=None, icp_iters: int = 0, verify=None,
+                 radii=None, rows=None, cam_K=None, verify_tau: float = 0.1):
+    """the steps after Net.forward, in place: ICP (icp_iters > 0, icp_refine_out), then verification (verify, the objects'
+    device meshes: verify_out with radii (O,) and the frame's rows), and with several hypotheses (out["hyp_R"] (B,K,3,3),
+    Net.set_hypotheses) the choice of each detection's pose.  pts (B,N,3) observed points, model (B,n,3) model points, obj (B)
+    object index of each detection.
+    - One hypothesis, or verification off: Net's choice stands; ICP refines the reported poses only.
+    - Several hypotheses and verification on: ICP refines all B K poses and verify_out checks all of them, each against its
+      detection's mask row; the reported pose is the first valid k with the largest hyp_pose_score x verify.  out then also
+      holds hyp_verify (B,K) and, with ICP, hyp_icp_R (B,K,3,3), hyp_icp_t (B,K,3); pred_*, verify, verify_counts, pem_*,
+      icp_* and hyp_index are the chosen hypothesis's."""
+    K = out["hyp_R"].shape[1] if "hyp_R" in out else 1
+    if K == 1 or verify is None:
+        if icp_iters > 0:
+            icp_refine_out(out, pts, model, obj, icp, icp_iters)
+        if verify is not None:
+            verify_out(out, verify, obj.cpu().numpy(), radii, rows, cam_K, verify_tau)
+        return out
+    B = out["hyp_R"].shape[0]
+    hyp = dict(pred_R=out["hyp_R"].reshape(B * K, 3, 3), pred_t=out["hyp_t"].reshape(B * K, 3))
+    if icp_iters > 0:
+        icp_refine_out(hyp, *(x.repeat_interleave(K, dim=0) for x in (pts, model, obj)), icp, icp_iters)
+    verify_out(hyp, verify, np.repeat(obj.cpu().numpy(), K), radii,
+               SimpleNamespace(depth=rows.depth, mask=rows.mask, mrow=np.repeat(np.asarray(rows.mrow), K)), cam_K, verify_tau)
+    v = hyp["verify"].view(B, K)
+    idx = first_best(out["hyp_pose_score"] * v, out["hyp_valid"])
+    sel = idx + torch.arange(B, device=idx.device) * K
+    keys = ("pred_R", "pred_t", "verify", "verify_counts") + (("pem_R", "pem_t", "icp_inliers", "icp_rms") if icp_iters > 0 else ())
+    out.update({k: hyp[k][sel] for k in keys})
+    out.update(hyp_index=idx, pred_pose_score=out["hyp_pose_score"].reshape(-1)[sel], hyp_verify=v)
+    if icp_iters > 0:
+        out.update(hyp_icp_R=hyp["pred_R"].view(B, K, 3, 3), hyp_icp_t=hyp["pred_t"].view(B, K, 3))
+    return out
+
+
 # ---- the whole pipeline ----------------------------------------------------------------------------------------------------
 @dataclass
 class Onboarded:
@@ -357,7 +398,12 @@ class SAM6D:
     verify (not in the reference; default False, off): render every reported pose, after any ICP, and count its agreement with
     the frame's depth and its detection's mask (verify_out, with tolerance verify_tau x the object's radius).  Each record's
     score is then pred_pose_score x ISM score x verify, and the record carries "verify"; R and t are unchanged.  Onboarding
-    keeps each object's mesh on the device for it."""
+    keeps each object's mesh on the device for it.
+
+    pem_hypotheses (not in the reference; default 1, off): run the PEM's fine stage from that many mutually distinct coarse
+    hypotheses, at least hyp_min_angle degrees or hyp_min_dist object radii apart (Net.set_hypotheses), and report one pose
+    per detection: the one with the best pose score, or with verify on the best pose score x verify over all of them
+    (finish_poses; with ICP every hypothesis is refined before it is verified).  Records then carry "hypothesis"."""
     rendering_type = "pyrender"
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
@@ -366,7 +412,8 @@ class SAM6D:
                  confidence_thresh: float = ism_cli.CONFIDENCE_THRESH, det_score_thresh: float = 0.2, precision: str = "bf16",
                  device=None, level_templates: int = 0, pose_distribution: str = "all", aggregation_function: str = "avg_5",
                  fastsam_model: str = "FastSAM-x", rendering_type: str = "pyrender", pbr_root: Optional[str] = None,
-                 pbr_split: str = "train_pbr", icp_iters: int = 0, verify: bool = False, verify_tau: float = 0.1):
+                 pbr_split: str = "train_pbr", icp_iters: int = 0, verify: bool = False, verify_tau: float = 0.1,
+                 pem_hypotheses: int = 1, hyp_min_angle: float = 30.0, hyp_min_dist: float = 0.2):
         if segmentor not in ("sam", "fastsam"):
             raise ValueError(f"The segmentor_model {segmentor} is not supported")
         if fastsam_model not in ism_cli.FASTSAM_MODELS:
@@ -388,6 +435,7 @@ class SAM6D:
         if not (np.isfinite(verify_tau) and verify_tau > 0):
             raise ValueError(f"verify_tau must be a finite number > 0, got {verify_tau}")
         self.verify, self.verify_tau = bool(verify), float(verify_tau)
+        hypotheses = check_hypotheses(pem_hypotheses, hyp_min_angle, hyp_min_dist)
         self.rendering_type, self.pbr_root, self.pbr_split, self._pbr_rows = rendering_type, pbr_root, pbr_split, None
         self.level_templates, self.pose_distribution = int(level_templates), pose_distribution
         self.aggregation_function = aggregation_function
@@ -400,6 +448,8 @@ class SAM6D:
                                    points_per_side=points_per_side)
         self.seg, self.desc = ism_cli.build_models(ism_args, self.device)
         self.pem = pem_cli.build_model(SimpleNamespace(precision=precision, checkpoint=checkpoint, random_weights=random_weights), self.device)
+        if hypotheses[0] > 1:
+            self.pem.set_hypotheses(*hypotheses)
 
     def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None, obj_id: Optional[int] = None) -> Onboarded:
         """render the templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates' framing
@@ -582,10 +632,8 @@ class SAM6D:
             rand = bop.pem_rand(g, n, n_rand, self.device)
             with torch.no_grad():
                 out = self.pem(data, rand=rand)
-                if icp is not None:
-                    icp_refine_out(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters)
-                if vmeshes is not None:
-                    verify_out(out, vmeshes, data["obj"].cpu().numpy(), radii, got[3], cam_K, self.verify_tau)
+                finish_poses(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters, vmeshes, radii,
+                             got[3] if vmeshes is not None else None, cam_K, self.verify_tau)
             if vmeshes is not None:
                 scores = (out["pred_pose_score"] * data["score"] * out["verify"]).cpu().numpy()
             else:
