@@ -349,6 +349,23 @@ int sam6d_coarse_select(const float* Rt, const int* top, int B, int n1, int n2, 
 int sam6d_coarse_pick_distinct(const float* Rt, const int* top, const float* scores, int B, int n1, int n2, int K, float cos_thr,
                                float d2_min, float* R_out, float* t_out, float* score_out, unsigned char* valid, int* count,
                                void* stream);
+/* sam6d_coarse_pick_distinct with "distinct" read up to the object's symmetries (not in the reference).  Same inputs, rounds
+ * and outputs, plus symR (S,9) (row-major) and symt (S,3) in metres, sym_range (B,2) i32 = (offset, count) of proposal b's
+ * symmetry set in them (the identity first), radius (B) the forward's radius (finite, > 0), which the coarse t are in units of.
+ * After pick i, with s = offset..offset+count-1, in fp32 rounded to nearest, no fused multiply-add, in this order:
+ *   A[y][x] = (R_i[y][0] R_s[0][x] + R_i[y][1] R_s[1][x]) + R_i[y][2] R_s[2][x]           (A = R_i R_s)
+ *   u[y]    = (R_i[y][0] t_s[0] + R_i[y][1] t_s[1]) + R_i[y][2] t_s[2];  w[y] = u[y] / radius + t_i[y]
+ *   tr = A[0] R_j[0];  tr = tr + A[e] R_j[e] for e = 1..8;  dx, dy, dz = w - t_j;  d2 = (dx dx + dy dy) + dz dz
+ * a live j is dropped when j == i or, for some s, !(tr < cos_thr || d2 >= d2_min).  With a range holding only the identity
+ * (exact 1 and 0 entries, t_s = 0), A and w equal R_i and t_i up to the sign of zeros, so for finite R_i, t_i every decision,
+ * and so every output, is bit for bit that of sam6d_coarse_pick_distinct.  max_count (1..2048, host): the largest count of
+ * any range, which sizes the shared-memory staging; a range with offset < 0, count < 1, count > max_count or offset + count
+ * > S is read as empty (only the pick itself is dropped).  -22 (nothing launched): sam6d_coarse_pick_distinct's cases, S < 1,
+ * max_count outside [1, 2048]. */
+int sam6d_coarse_pick_distinct_sym(const float* Rt, const int* top, const float* scores, int B, int n1, int n2, int K, float cos_thr,
+                                   float d2_min, const float* symR, const float* symt, int S, const int* sym_range, int max_count,
+                                   const float* radius, float* R_out, float* t_out, float* score_out, unsigned char* valid,
+                                   int* count, void* stream);
 
 /* ---- fine stage ---------------------------------------------------------------------------------------------------- */
 
@@ -471,6 +488,23 @@ int sam6d_track_points_scene(const float* rdepth, const unsigned short* depth, i
  * mrow outside [0, M), a tau or rscale that is not finite or is <= 0. */
 int sam6d_pose_verify(const float* rdepth, const float* depth, const unsigned char* mask, const int* mrow, const float* tau, int P,
                       int M, int H, int W, float rscale, int* counts, void* stream);
+
+/* ---- object symmetries and diameter (not in the reference; csrc/symmetry.cu, sam6d_b200/symmetry.py, oracle/symmetry_oracle.py) */
+/* Agreement of C candidate rigid transforms Rt (C,12) (R row-major, t) f32 with a sampled surface: queries q (Nq,3), targets
+ * tg (M,3) from an independent draw, optional colours qc (Nq,3) and tc (M,3) in [0, 1] (both or neither).  For candidate c and
+ * query x: y = R x + t, and the nearest target n(x) = the first index with the smallest d2 = |tg_j - y|^2 (fp32, fused
+ * multiply-add allowed).  x agrees when d2 <= geo_tol^2 (fp32) and, with colours, max_k |qc_x[k] - tc_n(x)[k]| <= color_tol.
+ * count (C) i32 = the agreeing queries; sumsq (C) f32 = the sum of d2 over all queries, summed in a fixed order (per CTA of 1024
+ * queries, then over CTAs), so results do not depend on scheduling.  work: scratch of C * ceil(Nq / 1024) * 8 bytes.
+ * -22 (nothing launched): C < 0, C > 65535, Nq < 1, M < 1, a tolerance that is not finite or is < 0, only one of qc / tc, a
+ * NULL pointer. */
+int sam6d_symmetry_agreement(const float* Rt, int C, const float* q, const float* qc, int Nq, const float* tg, const float* tc, int M,
+                             float geo_tol, float color_tol, int* count, float* sumsq, void* work, void* stream);
+/* d2 (1) f32 = the largest squared distance between two of the V points pts (V,3) f32 (models_info's diameter is its square
+ * root): every pair by tiled brute force, d2 = (dx dx + dy dy) + dz dz in fp32 rounded to nearest without fused multiply-add,
+ * the maximum through an atomic on the bits (exact and deterministic).  -22 (nothing launched): V < 1, V > 65535 * 1024, a
+ * NULL pointer. */
+int sam6d_point_diameter(const float* pts, int V, float* d2, void* stream);
 
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):

@@ -58,7 +58,7 @@ def get_parser():
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
-    pem_cli.check_hypothesis_args(ap, args)
+    pem_cli.check_hypothesis_args(ap, args, models_info=True)
     if args.stage in ("pem", "both") and args.template_dir is None:
         ap.error(f"--stage {args.stage} needs --template_dir (the PEM's template views)")
     if args.stage == "both" and args.detections is not None:
@@ -89,7 +89,8 @@ def main(argv=None):
         print(f"=> {len(recs)} detections written to {detections}")
     if args.stage in ("pem", "both"):
         out = os.path.join(args.output_dir, f"result_{args.dataset_name}.csv")
-        lines = sam6d.run_bop_pem(detections, args.bop_root, args.dataset_name, args.template_dir, out, max_frames=args.max_frames)
+        lines = sam6d.run_bop_pem(detections, args.bop_root, args.dataset_name, args.template_dir, out, max_frames=args.max_frames,
+                                  symmetries=pem_cli.symmetry_option(args))
         print(f"=> {len(lines)} poses written to {out}")
     return 0
 

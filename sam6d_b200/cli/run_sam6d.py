@@ -88,10 +88,11 @@ def main(argv=None):
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:
         raise SystemExit(f"--obj_ids: {len(args.obj_ids)} ids for {n_cad} CAD models")
     if multi:
-        obj = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size)
+        obj = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size,
+                                    symmetries=pem_cli.symmetry_option(args))
     else:
         obj = sam6d.onboard(args.cad_path, template_size=args.template_size,
-                            obj_id=args.obj_ids[0] if args.rendering_type == "pbr" else None)
+                            obj_id=args.obj_ids[0] if args.rendering_type == "pbr" else None, symmetries=pem_cli.symmetry_option(args))
     cam = json.load(open(args.cam_path))
     rgb = pem_cli.load_im(args.rgb_path).astype("uint8")
     run = sam6d.detect_objects if multi else sam6d

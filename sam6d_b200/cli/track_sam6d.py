@@ -63,7 +63,8 @@ def main(argv=None):
         raise SystemExit(f"no frame is named the same in {args.rgb_dir} and {args.depth_dir}")
     from ..track import Tracker
     sam6d = run_sam6d.build_sam6d(args)
-    objs = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size)
+    objs = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size,
+                                 symmetries=run_sam6d.pem_cli.symmetry_option(args))
     tracker = Tracker(sam6d, objs, args.cad_path, track_icp_iters=args.track_icp_iters, margin_px=args.margin_px,
                       gate_scale=args.gate_scale, min_inlier_fraction=args.min_inlier_fraction, max_rms_m=args.max_rms_m,
                       redetect_interval=args.redetect_interval, max_instances=args.max_instances, start_score=args.start_score,

@@ -9,6 +9,7 @@
 //   4. coarse_topk    : the n2 smallest residuals (value, then index)                              -> top (b,n2)
 //   5. coarse_select  : score = sum(w1) / (sum_i w1_i min_m ||(p_i - t) R - model_m|| + 1e-8); argmax -> init_R, init_t
 //   6. coarse_pick_distinct (opt-in, not in the reference): K mutually distinct hypotheses of the n2 scored ones
+//   7. coarse_pick_distinct_sym (opt-in, not in the reference): the same, distinct up to the object's symmetries
 #include "common.cuh"
 #include "svd3.cuh"
 
@@ -394,6 +395,98 @@ __global__ void __launch_bounds__(PICK_THREADS) coarse_pick_distinct_kernel(cons
   if (tid == 0) count[b] = found;
 }
 
+// ---- 7. K hypotheses distinct up to the object's symmetries (not in the reference) -----------------------------------------
+// coarse_pick_distinct_kernel with one more shared-memory stage: after each pick i, the cnt transforms of i's symmetric copies,
+// A_s = R_i R_s and w_s = R_i t_s / radius + t_i, then j is dropped when it is near any copy (the rule and its fp32 order:
+// include/sam6d_b200.h, sam6d_coarse_pick_distinct_sym)
+constexpr int PICK_MAX_SYM = 2048;
+__global__ void __launch_bounds__(PICK_THREADS) coarse_pick_distinct_sym_kernel(
+    const float* __restrict__ Rt, const int* __restrict__ top, const float* __restrict__ scores, int n1, int n2, int K, float cos_thr,
+    float d2_min, const float* __restrict__ symR, const float* __restrict__ symt, int S, const int* __restrict__ sym_range, int max_count,
+    const float* __restrict__ radius, float* __restrict__ R_out, float* __restrict__ t_out, float* __restrict__ score_out,
+    unsigned char* __restrict__ valid, int* __restrict__ count) {
+  extern __shared__ float hs[];
+  float* hr = hs;                            // n2 x 12: R row-major, t
+  float* sc = hr + (size_t)n2 * 12;          // n2
+  float* cp = sc + n2;                       // max_count x 12: A_s row-major, w_s
+  unsigned char* live = reinterpret_cast<unsigned char*>(cp + (size_t)max_count * 12);
+  __shared__ float rv[PICK_THREADS / 32];
+  __shared__ int ri[PICK_THREADS / 32];
+  __shared__ int pick;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int off = sym_range[(size_t)b * 2], cnt0 = sym_range[(size_t)b * 2 + 1];
+  // a range outside the set: only the pick itself is dropped
+  const int cnt = (off < 0 || cnt0 < 1 || cnt0 > max_count || off > S - cnt0) ? 0 : cnt0;
+  const float rad = radius[b];
+  for (int e = tid; e < n2 * 12; e += PICK_THREADS) {
+    const int j = e / 12, c = e - j * 12;
+    hr[e] = Rt[((size_t)b * n1 + top[(size_t)b * n2 + j]) * 12 + c];
+  }
+  for (int j = tid; j < n2; j += PICK_THREADS) { sc[j] = scores[(size_t)b * n2 + j]; live[j] = 1; }
+  __syncthreads();
+  int found = 0;
+  for (int r = 0; r < K; ++r) {
+    float bv = -INFINITY; int bi = 0x7fffffff;
+    for (int j = tid; j < n2; j += PICK_THREADS)
+      if (live[j]) argmax_first(bv, bi, sc[j], j);
+    warp_argmax_first(bv, bi);
+    if (lane == 0) { rv[warp] = bv; ri[warp] = bi; }
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < PICK_THREADS / 32; ++w) argmax_first(bv, bi, rv[w], ri[w]);
+      if (bi == 0x7fffffff && r == 0) bi = 0;   // all-NaN row: keep the first hypothesis, as coarse_pick_kernel
+      pick = bi;
+    }
+    __syncthreads();
+    const int i = pick;
+    if (i == 0x7fffffff) break;                 // no live hypothesis left (or only NaN scores)
+    const float* hi = hr + (size_t)i * 12;
+    if (tid < 9) R_out[((size_t)b * K + r) * 9 + tid] = hi[tid];
+    if (tid < 3) t_out[((size_t)b * K + r) * 3 + tid] = hi[9 + tid];
+    if (tid == 0) { score_out[(size_t)b * K + r] = sc[i]; valid[(size_t)b * K + r] = 1; }
+    for (int s = tid; s < cnt; s += PICK_THREADS) {
+      const float* Rs = symR + (size_t)(off + s) * 9;
+      const float* ts = symt + (size_t)(off + s) * 3;
+      float* o = cp + (size_t)s * 12;
+#pragma unroll
+      for (int y = 0; y < 3; ++y) {
+#pragma unroll
+        for (int x = 0; x < 3; ++x)
+          o[y * 3 + x] = __fadd_rn(__fadd_rn(__fmul_rn(hi[y * 3], Rs[x]), __fmul_rn(hi[y * 3 + 1], Rs[3 + x])), __fmul_rn(hi[y * 3 + 2], Rs[6 + x]));
+        const float u = __fadd_rn(__fadd_rn(__fmul_rn(hi[y * 3], ts[0]), __fmul_rn(hi[y * 3 + 1], ts[1])), __fmul_rn(hi[y * 3 + 2], ts[2]));
+        o[9 + y] = __fadd_rn(__fdiv_rn(u, rad), hi[9 + y]);
+      }
+    }
+    __syncthreads();
+    for (int j = tid; j < n2; j += PICK_THREADS) {
+      if (!live[j]) continue;
+      const float* hj = hr + (size_t)j * 12;
+      bool drop = j == i;
+      for (int s = 0; s < cnt && !drop; ++s) {
+        const float* a = cp + (size_t)s * 12;
+        float tr = __fmul_rn(a[0], hj[0]);
+#pragma unroll
+        for (int e = 1; e < 9; ++e) tr = __fadd_rn(tr, __fmul_rn(a[e], hj[e]));
+        const float dx = __fsub_rn(a[9], hj[9]), dy = __fsub_rn(a[10], hj[10]), dz = __fsub_rn(a[11], hj[11]);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+        drop = !(tr < cos_thr || d2 >= d2_min);
+      }
+      if (drop) live[j] = 0;
+    }
+    found = r + 1;
+    __syncthreads();
+  }
+  for (int e = tid; e < (K - found) * 14; e += PICK_THREADS) {
+    const int r = found + e / 14, c = e - (e / 14) * 14;
+    const size_t s0 = (size_t)b * K, s = s0 + r;
+    if (c < 9) R_out[s * 9 + c] = R_out[s0 * 9 + c];
+    else if (c < 12) t_out[s * 3 + c - 9] = t_out[s0 * 3 + c - 9];
+    else if (c == 12) score_out[s] = score_out[s0];
+    else valid[s] = 0;
+  }
+  if (tid == 0) count[b] = found;
+}
+
 }  // namespace
 
 // A (B,S,S) f32 -> W (B,(S-1)^2) masked soft assignment ^1.5, w1 (B,S-1)      (model_utils.py:206-216)
@@ -476,6 +569,25 @@ S6_API int sam6d_coarse_pick_distinct(const float* Rt, const int* top, const flo
   S6_CHECK(cudaFuncSetAttribute(coarse_pick_distinct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   coarse_pick_distinct_kernel<<<B, PICK_THREADS, smem, s6_stream(stream)>>>(Rt, top, scores, n1, n2, K, cos_thr, d2_min, R_out, t_out,
                                                                           score_out, valid, count);
+  S6_LAUNCH_CHECK();
+  return 0;
+}
+
+// sam6d_coarse_pick_distinct with "distinct" read up to each proposal's symmetry set (the rule: include/sam6d_b200.h)
+S6_API int sam6d_coarse_pick_distinct_sym(const float* Rt, const int* top, const float* scores, int B, int n1, int n2, int K,
+                                          float cos_thr, float d2_min, const float* symR, const float* symt, int S, const int* sym_range,
+                                          int max_count, const float* radius, float* R_out, float* t_out, float* score_out,
+                                          unsigned char* valid, int* count, void* stream) {
+  S6_REQUIRE(B >= 0 && n1 > 0 && n2 > 0 && n2 <= PICK_MAX_N2 && K >= 1 && K <= n2);
+  S6_REQUIRE(S >= 1 && max_count >= 1 && max_count <= PICK_MAX_SYM);
+  S6_REQUIRE(isfinite(cos_thr) && isfinite(d2_min));
+  S6_REQUIRE(Rt && top && scores && symR && symt && sym_range && radius && R_out && t_out && score_out && valid && count);
+  if (B == 0) return 0;
+  const size_t smem = ((size_t)n2 * 13 + (size_t)max_count * 12) * sizeof(float) + n2;
+  S6_CHECK(cudaFuncSetAttribute(coarse_pick_distinct_sym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  coarse_pick_distinct_sym_kernel<<<B, PICK_THREADS, smem, s6_stream(stream)>>>(Rt, top, scores, n1, n2, K, cos_thr, d2_min, symR, symt, S,
+                                                                              sym_range, max_count, radius, R_out, t_out, score_out,
+                                                                              valid, count);
   S6_LAUNCH_CHECK();
   return 0;
 }

@@ -724,6 +724,46 @@ def coarse_pick_distinct(Rt: Tensor, top: Tensor, scores: Tensor, K: int, min_an
     return R, t, score, valid, count
 
 
+PICK_MAX_SYM = 2048             # symmetries per object that sam6d_coarse_pick_distinct_sym stages
+
+
+def coarse_pick_distinct_sym(Rt: Tensor, top: Tensor, scores: Tensor, K: int, min_angle: float, min_dist: float, symR: Tensor,
+                             symt: Tensor, sym_range: Tensor, radius: Tensor, max_count: Optional[int] = None):
+    """coarse_pick_distinct with "distinct" read up to each proposal's symmetry set (the rule: include/sam6d_b200.h,
+    sam6d_coarse_pick_distinct_sym).  symR (S,3,3) or (S,9), symt (S,3) f32 in metres, sym_range (B,2) i32 (offset, count) of
+    each proposal's set, identity first; radius (B) f32 the forward's radius.  max_count: the largest count of any range
+    (default min(S, PICK_MAX_SYM), enough for every set symmetry.pack_sets builds).  Same outputs as coarse_pick_distinct;
+    with identity-only ranges they are its outputs bit for bit."""
+    _check(Rt, torch.float32, "Rt", 3)
+    _check(top, torch.int32, "top", 2)
+    _check(scores, torch.float32, "scores", 2)
+    _check(symR, torch.float32, "symR")
+    _check(symt, torch.float32, "symt", 2)
+    _check(sym_range, torch.int32, "sym_range", 2)
+    _check(radius, torch.float32, "radius", 1)
+    B, n1, _ = Rt.shape
+    n2 = top.shape[1]
+    S = symt.shape[0]
+    if tuple(scores.shape) != (B, n2) or top.shape[0] != B:
+        raise RuntimeError(f"coarse_pick_distinct_sym: Rt (B,n1,12), top and scores (B,n2), got {tuple(Rt.shape)}, {tuple(top.shape)}, "
+                           f"{tuple(scores.shape)}")
+    if symR.numel() != S * 9 or symt.shape[1] != 3 or tuple(sym_range.shape) != (B, 2) or tuple(radius.shape) != (B,):
+        raise RuntimeError(f"coarse_pick_distinct_sym: symR (S,3,3), symt (S,3), sym_range (B,2), radius (B), got {tuple(symR.shape)}, "
+                           f"{tuple(symt.shape)}, {tuple(sym_range.shape)}, {tuple(radius.shape)}")
+    cos_thr, d2_min = hypothesis_thresholds(min_angle, min_dist)
+    max_count = min(S, PICK_MAX_SYM) if max_count is None else int(max_count)
+    dev = Rt.device
+    K = int(K)
+    R = torch.empty(B, max(K, 0), 3, 3, dtype=torch.float32, device=dev)
+    t = torch.empty(B, max(K, 0), 3, dtype=torch.float32, device=dev)
+    score = torch.empty(B, max(K, 0), dtype=torch.float32, device=dev)
+    valid = torch.empty(B, max(K, 0), dtype=torch.uint8, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    _lib.call("sam6d_coarse_pick_distinct_sym", Rt, top, scores, B, n1, n2, K, cos_thr, d2_min, symR, symt, S, sym_range, max_count,
+              radius, R, t, score, valid, count)
+    return R, t, score, valid, count
+
+
 # ---------------------------------------------------------------------------------------------- fine stage
 def pe_mlp_max(pts: Tensor, idx: Tensor, cnt: Tensor, weights, out: Tensor, out_off: int):
     _check(pts, torch.float32, "pts", 3)
@@ -1096,3 +1136,45 @@ def mask_rle(masks: Tensor) -> Tuple[Tensor, Tensor]:
     rle_cum = torch.empty(int(rle_off[n]), dtype=torch.int32, device=dev)
     _lib.call("sam6d_mask_rle_write", masks, n, H, W, col_cnt, band_off, rle_off, rle_cum)
     return rle_cum, rle_off
+
+
+# ---------------------------------------------------------------------------------------------- object symmetries (symmetry.py)
+SYM_QUERY_CHUNK = 1024          # queries per CTA of sam6d_symmetry_agreement: its scratch holds one int and one float per chunk
+
+
+def symmetry_agreement(Rt: Tensor, q: Tensor, tg: Tensor, geo_tol: float, color_tol: float = 0.0, qc: Optional[Tensor] = None,
+                       tc: Optional[Tensor] = None):
+    """C candidate transforms Rt (C,12) (R row-major, t) against query samples q (Nq,3) and target samples tg (M,3), with optional
+    colours qc (Nq,3) and tc (M,3) in [0, 1] (the rule: include/sam6d_b200.h, sam6d_symmetry_agreement) -> count (C) i32, the
+    queries whose nearest target is within geo_tol (and color_tol in colour), and sumsq (C) f32, their summed squared
+    nearest-neighbour distances over all queries"""
+    _check(Rt, torch.float32, "Rt", 2)
+    _check(q, torch.float32, "q", 2)
+    _check(tg, torch.float32, "tg", 2)
+    if (qc is None) != (tc is None):
+        raise RuntimeError("symmetry_agreement: colours for both sample sets or for neither")
+    C, Nq, M = Rt.shape[0], q.shape[0], tg.shape[0]
+    if Rt.shape[1] != 12 or q.shape[1] != 3 or tg.shape[1] != 3:
+        raise RuntimeError(f"symmetry_agreement: Rt (C,12), q (Nq,3), tg (M,3), got {tuple(Rt.shape)}, {tuple(q.shape)}, {tuple(tg.shape)}")
+    if qc is not None:
+        _check(qc, torch.float32, "qc", 2)
+        _check(tc, torch.float32, "tc", 2)
+        if tuple(qc.shape) != (Nq, 3) or tuple(tc.shape) != (M, 3):
+            raise RuntimeError(f"symmetry_agreement: qc (Nq,3), tc (M,3), got {tuple(qc.shape)}, {tuple(tc.shape)}")
+    dev = Rt.device
+    count = torch.empty(C, dtype=torch.int32, device=dev)
+    sumsq = torch.empty(C, dtype=torch.float32, device=dev)
+    work = torch.empty(max(C, 1) * ((Nq + SYM_QUERY_CHUNK - 1) // SYM_QUERY_CHUNK) * 2, dtype=torch.int32, device=dev)
+    _lib.call("sam6d_symmetry_agreement", Rt, C, q, qc, Nq, tg, tc, M, float(geo_tol), float(color_tol), count, sumsq, work)
+    return count, sumsq
+
+
+def point_diameter(pts: Tensor) -> Tensor:
+    """pts (V,3) f32 -> (1,) f32 the largest squared distance between two of them (sam6d_point_diameter; its square root is
+    models_info's diameter)"""
+    _check(pts, torch.float32, "pts", 2)
+    if pts.shape[1] != 3:
+        raise RuntimeError(f"point_diameter: pts (V,3), got {tuple(pts.shape)}")
+    d2 = torch.empty(1, dtype=torch.float32, device=pts.device)
+    _lib.call("sam6d_point_diameter", pts, pts.shape[0], d2)
+    return d2

@@ -387,13 +387,15 @@ def compute_feature_similarity(feat1, feat2, type='cosine', temp=1.0, normalize_
 
 
 def compute_coarse_Rt(atten, pts1, pts2, model_pts=None, n_proposal1=6000, n_proposal2=300, rand=None, return_scores=False,
-                      n_hypotheses=1, min_angle=30.0, min_dist=0.2):
+                      n_hypotheses=1, min_angle=30.0, min_dist=0.2, symmetries=None):
     """model_utils.py:187-246.  `rand` (B, 3*n_proposal1) overrides the torch.rand draw (used by the parity tests to feed the
     reference and this implementation the same uniforms); by default the call is the reference's own
     torch.rand(B, n_proposal1*3, device=device), so the Philox stream position matches.
     n_hypotheses = K > 1 (not in the reference) appends the K mutually distinct hypotheses of ops.coarse_pick_distinct (at least
     min_angle degrees or min_dist radius-normalised units apart) to the return values: R (B,K,3,3), t (B,K,3), score (B,K),
-    valid (B,K) u8, count (B) i32, slot 0 being the returned R, t."""
+    valid (B,K) u8, count (B) i32, slot 0 being the returned R, t.  symmetries = (symR (S,3,3), symt (S,3) metres, sym_range (B,2)
+    i32, radius (B)): with K > 1 two hypotheses are then distinct only when they are so from every symmetric copy of each other
+    (ops.coarse_pick_distinct_sym)."""
     B = pts1.shape[0]
     if model_pts is None:
         model_pts = pts2
@@ -404,7 +406,10 @@ def compute_coarse_Rt(atten, pts1, pts2, model_pts=None, n_proposal1=6000, n_pro
     Rt, resid = ops.coarse_hypotheses(idx, pts1.contiguous(), pts2.contiguous())
     top = ops.topk_smallest(resid, n_proposal2)
     R, t, scores = ops.coarse_select(Rt, top, pts1.contiguous(), w1, model_pts.contiguous())
-    hyp = ops.coarse_pick_distinct(Rt, top, scores, n_hypotheses, min_angle, min_dist) if n_hypotheses > 1 else ()
+    if n_hypotheses > 1 and symmetries is not None:
+        hyp = ops.coarse_pick_distinct_sym(Rt, top, scores, n_hypotheses, min_angle, min_dist, *symmetries)
+    else:
+        hyp = ops.coarse_pick_distinct(Rt, top, scores, n_hypotheses, min_angle, min_dist) if n_hypotheses > 1 else ()
     if return_scores:
         return (R, t, scores) + hyp  # (B, n_proposal2) selection scores of the retained hypotheses
     return (R, t) + hyp
@@ -473,7 +478,8 @@ class CoarsePointMatching(nn.Module):
     @torch.no_grad()
     def forward(self, p1, f1, geo1, p2, f2, geo2, radius, end_points, rand=None, hypotheses=(1, 30.0, 0.2)):
         """hypotheses = (K, min_angle, min_dist): with K > 1 end_points also gets hyp_init_R (B,K,3,3), hyp_init_t (B,K,3) and
-        hyp_valid (B,K) u8 of compute_coarse_Rt's distinct hypotheses"""
+        hyp_valid (B,K) u8 of compute_coarse_Rt's distinct hypotheses; when end_points also holds hyp_sym_R (S,3,3), hyp_sym_t
+        (S,3) and hyp_sym_range (B,2) (symmetry.pack_sets), distinct up to each proposal's symmetries"""
         if self.training:
             raise NotImplementedError("sam6d_b200 implements the inference path (model.eval())")
         B = f1.shape[0]
@@ -488,8 +494,11 @@ class CoarsePointMatching(nn.Module):
         atten = compute_feature_similarity(o1, o2, self.cfg.sim_type, self.cfg.temp, self.cfg.normalize_feat, self.precision)
         model = ops.scale_by_radius(end_points['model'].contiguous(), radius.contiguous())
         K, min_angle, min_dist = hypotheses
+        sym = None
+        if K > 1 and all(k in end_points for k in SYM_KEYS):
+            sym = tuple(end_points[k].contiguous() for k in SYM_KEYS) + (radius.contiguous(),)
         res = compute_coarse_Rt(atten, p1, p2, model, self.cfg.nproposal1, self.cfg.nproposal2, rand=rand, return_scores=True,
-                                n_hypotheses=K, min_angle=min_angle, min_dist=min_dist)
+                                n_hypotheses=K, min_angle=min_angle, min_dist=min_dist, symmetries=sym)
         init_R, init_t, self.last_select_scores = res[:3]
         if K > 1:
             end_points['hyp_init_R'], end_points['hyp_init_t'], _, end_points['hyp_valid'], _ = res[3:]
@@ -834,6 +843,8 @@ DEFAULT_MODEL_CFG = dict(
 MAX_HYPOTHESES = 16            # Net.set_hypotheses: fine-stage passes per forward
 # the outputs a forward with K > 1 hypotheses adds (Net.set_hypotheses), as graph.StepGraphs copies them out of a replay
 HYP_KEYS = ("hyp_init_R", "hyp_init_t", "hyp_R", "hyp_t", "hyp_pose_score", "hyp_valid", "hyp_index")
+# inputs that make the K > 1 pick distinct up to the objects' symmetries (symmetry.pack_sets; CoarsePointMatching.forward)
+SYM_KEYS = ("hyp_sym_R", "hyp_sym_t", "hyp_sym_range")
 
 
 def check_hypotheses(k, min_angle, min_dist):

@@ -19,6 +19,7 @@ the same stage functions, so one `SAM6D` frame computes what the chained CLIs co
 the ISM and the PEM the proposal masks stay on the device: their RLE is built by a kernel (ops.mask_rle) and only the run
 ends come to the host, instead of every (H,W) float mask."""
 import json
+import os
 import time
 from dataclasses import dataclass
 from types import SimpleNamespace
@@ -27,7 +28,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import bop, inputs, ism, meshio, ops, pbr, render
+from . import bop, bop_eval, inputs, ism, meshio, ops, pbr, render, symmetry
 from .cli import ism_run_inference_custom as ism_cli
 from .cli import pem_run_inference_custom as pem_cli
 from .cli import render_custom_templates as render_cli
@@ -192,7 +193,7 @@ def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
 # ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
 def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
               generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None, icp=None, icp_iters: int = 0,
-              verify=None, verify_tau: float = 0.1):
+              verify=None, verify_tau: float = 0.1, symmetries=None):
     """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
     enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
     model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
@@ -204,7 +205,8 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
     verify, the device meshes in mm of the objects (one per object, in model_points_m's order; verify_mesh): after the forward
     and any ICP, verify_out checks every reported pose against the frame's depth and its detection's mask with tolerance
     verify_tau x its object's radius.  With several PEM hypotheses (Net.set_hypotheses) finish_poses picks each detection's
-    pose."""
+    pose, and symmetries (a symmetry.SymmetrySet of the objects, in model_points_m's order) makes the hypotheses distinct up to
+    each object's symmetries (symmetry_inputs)."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
     got = inputs.get_test_data(
@@ -225,6 +227,8 @@ def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_po
                 input_data["dense_fo"] = bank[1][input_data["obj"]]
             if generator is not None:
                 rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
+            if symmetries is not None and model.hypotheses[0] > 1:
+                symmetry_inputs(input_data, symmetries, input_data["obj"] if det_obj is not None else None)
             out = model(input_data, rand=rand)
             if icp_iters > 0 or verify is not None:
                 obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int64, device=input_data["pts"].device)
@@ -359,6 +363,47 @@ def finish_poses(out: dict, pts: torch.Tensor, model: torch.Tensor, obj: torch.T
     return out
 
 
+# ---- hypotheses distinct up to the objects' symmetries (not in the reference) ---------------------------------------------------
+SYMMETRY_SOURCES = ("auto",)           # besides None and {obj_id: models_info entry}; run_bop_pem also takes "models_info"
+
+
+def symmetry_inputs(data: dict, symmetries: "symmetry.SymmetrySet", obj: Optional[torch.Tensor] = None) -> dict:
+    """fill Net.forward's hyp_sym_R, hyp_sym_t and hyp_sym_range (pem.SYM_KEYS) in place: every object's packed set, and each
+    detection's range in it by its object index obj (B) (None: all object 0)"""
+    B = data["pts"].shape[0]
+    obj = torch.zeros(B, dtype=torch.int64, device=symmetries.range.device) if obj is None else obj.to(symmetries.range.device)
+    data.update(hyp_sym_R=symmetries.R, hyp_sym_t=symmetries.t, hyp_sym_range=symmetries.range[obj].contiguous())
+    return data
+
+
+def check_symmetries(symmetries, obj_ids, sources=SYMMETRY_SOURCES):
+    """ValueError unless symmetries is None, one of `sources`, or a dict holding a models_info entry for every id of obj_ids"""
+    if symmetries is None or (isinstance(symmetries, str) and symmetries in sources):
+        return
+    if isinstance(symmetries, dict):
+        missing = [i for i in obj_ids if int(i) not in symmetries]
+        if missing:
+            raise ValueError(f"symmetries: no models_info entry for obj_ids {missing}")
+        bad = [i for i in obj_ids if not isinstance(symmetries[int(i)], dict)]
+        if bad:
+            raise ValueError(f"symmetries: the entries of obj_ids {bad} are not models_info dicts")
+        return
+    raise ValueError(f"symmetries must be None, one of {sources} or {{obj_id: models_info entry}}, got {symmetries!r}")
+
+
+def object_symmetries(symmetries, meshes, obj_ids, device) -> Optional["symmetry.SymmetrySet"]:
+    """a checked `symmetries` value -> the objects' packed symmetry sets (symmetry.pack_sets), or None.  "auto":
+    symmetry.find_symmetries of every mesh (meshio.Mesh or PLY path)"""
+    if symmetries is None:
+        return None
+    if isinstance(symmetries, str):
+        meshes = [meshio.load_ply_mesh(m) if isinstance(m, str) else m for m in meshes]
+        infos = [symmetry.find_symmetries(m, backend=symmetry.GpuBackend(device)) for m in meshes]
+    else:
+        infos = [symmetries[int(i)] for i in obj_ids]
+    return symmetry.pack_sets(infos, device)
+
+
 # ---- the whole pipeline ----------------------------------------------------------------------------------------------------
 @dataclass
 class Onboarded:
@@ -374,6 +419,7 @@ class Onboarded:
     icp_points_m: Optional[np.ndarray] = None
     icp_normals: Optional[np.ndarray] = None
     verify_mesh: Optional[meshio.Mesh] = None
+    symmetries: Optional["symmetry.SymmetrySet"] = None
 
 
 class SAM6D:
@@ -403,7 +449,8 @@ class SAM6D:
     pem_hypotheses (not in the reference; default 1, off): run the PEM's fine stage from that many mutually distinct coarse
     hypotheses, at least hyp_min_angle degrees or hyp_min_dist object radii apart (Net.set_hypotheses), and report one pose
     per detection: the one with the best pose score, or with verify on the best pose score x verify over all of them
-    (finish_poses; with ICP every hypothesis is refined before it is verified).  Records then carry "hypothesis"."""
+    (finish_poses; with ICP every hypothesis is refined before it is verified).  Records then carry "hypothesis".  Objects
+    onboarded with symmetries (onboard_objects) get hypotheses that are distinct up to their symmetries."""
     rendering_type = "pyrender"
 
     def __init__(self, segmentor: str = "sam", sam_model_type: str = "vit_h", dinov2_model: str = "dinov2_vitl14",
@@ -451,7 +498,7 @@ class SAM6D:
         if hypotheses[0] > 1:
             self.pem.set_hypotheses(*hypotheses)
 
-    def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None, obj_id: Optional[int] = None) -> Onboarded:
+    def onboard(self, mesh_or_ply_path, template_size: int = 512, rng=None, obj_id: Optional[int] = None, symmetries=None) -> Onboarded:
         """render the templates of a CAD model in mm (a PLY path or a numpy meshio.Mesh) with render_custom_templates' framing
         and colours, and build everything a frame needs from them without touching a file: every view of
         render.template_view_set(level_templates, pose_distribution) is rendered once; the ISM references and the
@@ -460,13 +507,23 @@ class SAM6D:
         samples, the PEM model points.
 
         rendering_type "pbr": obj_id, the object's BOP id, is required; the ISM references are the split's frames chosen by
-        pbr.select_references, whose draws come first from `rng`, then the draws above; only the 42 level-0 views are rendered."""
+        pbr.select_references, whose draws come first from `rng`, then the draws above; only the 42 level-0 views are rendered.
+
+        symmetries (not in the reference; used with pem_hypotheses > 1): None, "auto" or the object's models_info entry, kept
+        as Onboarded.symmetries (onboard_objects)."""
+        if isinstance(symmetries, dict):
+            symmetries = {0: symmetries}
+        check_symmetries(symmetries, [0])
         if self.rendering_type == "pbr":
             if obj_id is None:
                 raise ValueError('rendering_type "pbr" needs the BOP object id: onboard(..., obj_id=)')
             ref_cls, ref_patch = self._pbr_references([obj_id], rng)
-            return self._onboard_mesh(mesh_or_ply_path, template_size, rng, (ref_cls[0], ref_patch[0]))
-        return self._onboard_mesh(mesh_or_ply_path, template_size, rng)
+            ob = self._onboard_mesh(mesh_or_ply_path, template_size, rng, (ref_cls[0], ref_patch[0]))
+        else:
+            ob = self._onboard_mesh(mesh_or_ply_path, template_size, rng)
+        if symmetries is not None:
+            ob.symmetries = object_symmetries(symmetries, [mesh_or_ply_path], [0], self.device)
+        return ob
 
     def _pbr_references(self, obj_ids, rng):
         """the PBR references of every object of obj_ids -> (ref_cls (O,T,C), ref_patch (O,T,256,C)) for the ISM's views"""
@@ -501,14 +558,18 @@ class SAM6D:
         vmesh = verify_mesh(verts, faces, self.device) if self.verify else None
         return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points, icp_pts, icp_nrm, vmesh)
 
-    def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None) -> "ObjectSet":
+    def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None, symmetries=None) -> "ObjectSet":
         """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
         obj_ids: the category id of every object (distinct ints), default 1..O.  The fp32 patch tokens (44 MB per object at
         C = 1024) are copied into the stack as each object is built, so only one object's extra copy is alive at a time.
 
         rendering_type "pbr": obj_ids are required and are the objects' BOP ids.  The references of all objects are selected
         first (pbr.select_references' draws, object after object, as the reference's load_processed_metaData makes them), then
-        built in one pass over the split's frames straight into the stacks; then each mesh is onboarded with its draws."""
+        built in one pass over the split's frames straight into the stacks; then each mesh is onboarded with its draws.
+
+        symmetries (not in the reference; used with pem_hypotheses > 1): None (default), "auto" (symmetry.find_symmetries of
+        every mesh, whose samples draw from their own seed, not from `rng`) or {obj_id: models_info entry}; kept packed on the
+        device as ObjectSet.symmetries (symmetry.pack_sets), so that detect_objects' hypotheses are distinct up to them."""
         meshes = list(meshes)
         n = len(meshes)
         if self.rendering_type == "pbr" and obj_ids is None:
@@ -516,10 +577,14 @@ class SAM6D:
         obj_ids = list(range(1, n + 1)) if obj_ids is None else [int(i) for i in obj_ids]
         if n == 0 or len(obj_ids) != n or len(set(obj_ids)) != n:
             raise ValueError(f"onboard_objects: {n} meshes need {n} distinct obj_ids, got {obj_ids}")
+        check_symmetries(symmetries, obj_ids)
         if self.rendering_type == "pbr":
             ref_cls, ref_patch = self._pbr_references(obj_ids, rng)
             parts = [self._onboard_mesh(mesh, template_size, rng, (ref_cls[o], None)) for o, mesh in enumerate(meshes)]
-            return ObjectSet.stack(parts, ref_patch, obj_ids)
+            objs = ObjectSet.stack(parts, ref_patch, obj_ids)
+            if symmetries is not None:
+                objs.symmetries = object_symmetries(symmetries, meshes, obj_ids, self.device)
+            return objs
         parts, ref_patch = [], None
         for o, mesh in enumerate(meshes):
             ob = self.onboard(mesh, template_size, rng)
@@ -528,7 +593,10 @@ class SAM6D:
             ref_patch[o] = ob.ref_patch
             ob.ref_patch = None
             parts.append(ob)
-        return ObjectSet.stack(parts, ref_patch, obj_ids)
+        objs = ObjectSet.stack(parts, ref_patch, obj_ids)
+        if symmetries is not None:
+            objs.symmetries = object_symmetries(symmetries, meshes, obj_ids, self.device)
+        return objs
 
     def __call__(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, obj: Onboarded, rng=None, mark=None):
         """one RGB-D frame: rgb (H,W,3) u8, depth (H,W) raw u16, cam_K (9 values) and depth_scale as camera.json holds them.
@@ -581,7 +649,7 @@ class SAM6D:
         return records
 
     def run_bop_pem(self, detections_path: str, bop_root: str, dataset_name: str, template_dir: str, out_path: Optional[str] = None,
-                    rng=None, max_frames: Optional[int] = None, mark=None):
+                    rng=None, max_frames: Optional[int] = None, mark=None, symmetries=None):
         """test_bop.py over a detection file (ours or the reference ISM's; uncompressed RLE): per image of the file (bop.
         group_detections, the first max_frames), bop.pem_instances, then Net.forward on all of the image's instances with the
         coarse-stage uniforms of test_bop.py (bop.pem_rand: one CUDA generator seeded RD_SEED for the run, one torch.rand per
@@ -590,11 +658,16 @@ class SAM6D:
         skipped (the reference fails there).  Writes the CSV lines to out_path and returns them.  mark(stage) after
         "onboard", and per image after "decode", "pem_inputs" and "forward".  icp_iters > 0: each image's poses are refined (icp_refine_out) before its rows are built.
         verify: each image's poses are then verified (verify_out, the dataset's meshes) and each row's score is
-        pred_pose_score x detection score x verify."""
+        pred_pose_score x detection score x verify.  symmetries, with pem_hypotheses > 1: as onboard_objects', or "models_info",
+        the dataset's own models_info.json next to its models."""
         mark = mark or (lambda stage: None)
         rng = rng if rng is not None else np.random
         cfg = pem_cli.TEST_DATASET
         objs = bop.load_objects(bop_root, dataset_name)
+        check_symmetries(symmetries, objs.ids, SYMMETRY_SOURCES + ("models_info",))
+        if symmetries == "models_info":
+            symmetries = bop_eval.load_models_info(os.path.join(bop_root, dataset_name, bop.model_dir(dataset_name), "models_info.json"))
+            check_symmetries(symmetries, objs.ids)
         meshes = [meshio.load_ply_mesh(p) for p in objs.ply_paths]
         model_points = np.stack([meshio.sample_surface(m.vertices, m.faces, bop.N_SAMPLE_MODEL_POINT, rng) / 1000.0 for m in meshes])
         model_points = model_points.astype(np.float32)
@@ -608,6 +681,9 @@ class SAM6D:
         vmeshes, radii = None, None
         if self.verify:
             vmeshes, radii = [verify_mesh(m.vertices, m.faces, self.device) for m in meshes], object_radii(model_points)
+        syms = None
+        if symmetries is not None and self.pem.hypotheses[0] > 1:
+            syms = object_symmetries(symmetries, meshes, objs.ids, self.device)
         mark("onboard")
         with open(detections_path) as fh:
             groups = bop.group_detections(json.load(fh))
@@ -630,6 +706,8 @@ class SAM6D:
                 continue
             data["dense_po"], data["dense_fo"] = bank[0][data["obj"]], bank[1][data["obj"]]
             rand = bop.pem_rand(g, n, n_rand, self.device)
+            if syms is not None:
+                symmetry_inputs(data, syms, data["obj"])
             with torch.no_grad():
                 out = self.pem(data, rand=rand)
                 finish_poses(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters, vmeshes, radii,
@@ -686,7 +764,7 @@ class SAM6D:
                 raise ValueError("pose verification needs the objects' device meshes: onboard them with SAM6D(..., verify=True)")
         frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
                           rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj, icp=icp, icp_iters=self.icp_iters,
-                          verify=vmeshes, verify_tau=self.verify_tau)
+                          verify=vmeshes, verify_tau=self.verify_tau, symmetries=getattr(obj, "symmetries", None))
         pem_recs = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
@@ -713,6 +791,7 @@ class ObjectSet:
     icp_points_m: Optional[np.ndarray] = None
     icp_normals: Optional[np.ndarray] = None
     verify_meshes: Optional[list] = None
+    symmetries: Optional["symmetry.SymmetrySet"] = None
 
     @staticmethod
     def stack(parts, ref_patch, obj_ids) -> "ObjectSet":
