@@ -114,7 +114,8 @@ int sam6d_l2norm_rows_bf16(const float* x, long long x_rpb, long long x_bstride,
 /* focused-linear-attention feature map (PEM/model/transformer.py:541-550); softplus_scale (C) = softplus(scale) */
 int sam6d_focus_rows(const float* x, long long x_rpb, long long x_bstride, long long x_ld, float* y, long long y_rpb,
                      long long y_bstride, long long y_ld, const float* softplus_scale, long long rows, int C, void* stream);
-/* out = (p - t) @ R per proposal (PEM/model/fine_point_matching.py:44) */
+/* out = (p - t) @ R per proposal (PEM/model/fine_point_matching.py:44).  Here and in the next two, an empty batch returns 0
+ * without launching, whatever its array addresses */
 int sam6d_rigid_warp(const float* p, const float* R, const float* t, int b, int n, float* out, void* stream);
 /* radius[b] = max_i ||po[b,i]|| and x / (radius + 1e-6) (PEM/model/feature_extraction.py:139-142) */
 int sam6d_cloud_radius(const float* po, int b, int n, float* radius, void* stream);
@@ -274,13 +275,15 @@ int sam6d_transformer_tail_bf16(const void* hid, long long ld_hid, const void* x
 /* ---- attention ---------------------------------------------------------------------------------------------------- */
 
 /* relative-position score term of RPEMultiHeadAttention (PEM/model/transformer.py:389-394) with proj_p folded into
- * the query: E (B,S,S,256) f32 or bf16, U (B*S rows of 4x256, row stride u_ld) = W_p,h^T q_h  ->  SP (B,4,S,S) */
+ * the query: E (B,S,S,256) f32 or bf16, U (B*S rows of 4x256, row stride u_ld) = W_p,h^T q_h  ->  SP (B,4,S,S);
+ * u_ld % 4 == 0 and 16-byte aligned E and U */
 int sam6d_rpe_scores(const void* E, int e_is_bf16, const float* U, long long u_ld, int B, int S, float* SP, void* stream);
 /* the same term on TMA + wgmma (bf16 path, the HBM-bound stream over E): E (B,S,S,256) bf16, U (B*S, 4*256) bf16
  * contiguous, S <= 200  ->  SP (B,4,S,sp_ld) f32 with padded score rows, sp_ld >= S (columns [S, sp_ld) are not written);
  * with sp_ld a multiple of 4 sam6d_attn_tc_bias_ld streams it */
 int sam6d_rpe_scores_tc_ld(const void* E, const void* U, int B, int S, float* SP, int sp_ld, void* stream);
-/* softmax((Q K^T + bias) * scale) V, head dim 64, Sk <= 256 (MultiHeadAttention :109-148, RPEMultiHeadAttention :369-406) */
+/* softmax((Q K^T + bias) * scale) V, head dim 64, Sk <= 256 (MultiHeadAttention :109-148, RPEMultiHeadAttention :369-406);
+ * bias contiguous (B,H,Sq,Sk) or NULL; k_ld, v_ld, k_bs, v_bs multiples of 4, K and V 16-byte aligned, B*H <= 65535 */
 int sam6d_mha(const float* Q, long long q_ld, long long q_bs, const float* K, long long k_ld, long long k_bs, const float* V,
               long long v_ld, long long v_bs, const float* bias, int B, int H, int Sq, int Sk, float scale, float* O,
               long long o_ld, long long o_bs, void* stream);

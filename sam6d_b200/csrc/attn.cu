@@ -286,6 +286,8 @@ __global__ void __launch_bounds__(256) linattn_apply_kernel(const float* __restr
 // E (B,S,S,256) [f32 or bf16], U (B,S,4,256) f32 -> SP (B,4,S,S) f32
 S6_API int sam6d_rpe_scores(const void* E, int e_is_bf16, const float* U, long long u_ld, int B, int S, float* SP, void* stream) {
   S6_REQUIRE(E && U && SP && B >= 0 && S > 0 && u_ld >= 1024 && (u_ld % 4) == 0);
+  // U and E rows are read with 16-byte loads
+  S6_REQUIRE(((reinterpret_cast<uintptr_t>(U) | reinterpret_cast<uintptr_t>(E)) & 15) == 0);
   if (B == 0) return 0;
   if (e_is_bf16)
     S6_CHECK(s6_launch_pdl(rpe_scores_kernel<__nv_bfloat16>, dim3(B * S), dim3(256), 0, s6_stream(stream), (const __nv_bfloat16*)E, U,
@@ -302,6 +304,9 @@ S6_API int sam6d_mha(const float* Q, long long q_ld, long long q_bs, const float
                      float scale, float* O, long long o_ld, long long o_bs, void* stream) {
   S6_REQUIRE(Q && K && V && O && B >= 0 && H > 0 && Sq > 0 && Sk > 0 && Sk <= MHA_MAXK);
   S6_REQUIRE((k_ld % 4 == 0) && (v_ld % 4 == 0) && (k_bs % 4 == 0) && (v_bs % 4 == 0));
+  // K and V are staged with 16-byte loads; B*H is grid.y
+  S6_REQUIRE(((reinterpret_cast<uintptr_t>(K) | reinterpret_cast<uintptr_t>(V)) & 15) == 0);
+  S6_REQUIRE((long long)B * H <= 65535);
   if (B == 0) return 0;
   size_t smem = ((size_t)Sk * (MHA_KP + 64) + 8 * 64 * 4 + 8 * MHA_MAXK * 4) * sizeof(float);
   S6_CHECK(cudaFuncSetAttribute(mha_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -335,26 +335,30 @@ S6_API int sam6d_focus_rows(const float* x, long long x_rpb, long long x_bstride
 }
 
 S6_API int sam6d_rigid_warp(const float* p, const float* R, const float* t, int b, int n, float* out, void* stream) {
-  S6_REQUIRE(p && R && t && out && b >= 0 && n >= 0);
+  // an empty batch is nothing to do, whatever the (possibly null) addresses of its empty arrays
+  S6_REQUIRE(b >= 0 && n >= 0);
   long long total = (long long)b * n;
   if (total == 0) return 0;
+  S6_REQUIRE(p && R && t && out);
   rigid_warp_kernel<<<s6_cdiv(total, 256), 256, 0, s6_stream(stream)>>>(p, R, t, n, total, out);
   S6_LAUNCH_CHECK();
   return 0;
 }
 
 S6_API int sam6d_cloud_radius(const float* po, int b, int n, float* radius, void* stream) {
-  S6_REQUIRE(po && radius && b >= 0 && n > 0);
+  S6_REQUIRE(b >= 0 && n > 0);
   if (b == 0) return 0;
+  S6_REQUIRE(po && radius);
   radius_kernel<<<b, 256, 0, s6_stream(stream)>>>(po, n, radius);
   S6_LAUNCH_CHECK();
   return 0;
 }
 
 S6_API int sam6d_scale_by_radius(const float* src, const float* radius, int b, long long per_batch, float* dst, void* stream) {
-  S6_REQUIRE(src && radius && dst && b >= 0 && per_batch >= 0);
+  S6_REQUIRE(b >= 0 && per_batch >= 0);
   long long total = (long long)b * per_batch;
   if (total == 0) return 0;
+  S6_REQUIRE(src && radius && dst);
   scale_by_radius_kernel<<<s6_cdiv(total, 256), 256, 0, s6_stream(stream)>>>(src, radius, per_batch, total, dst);
   S6_LAUNCH_CHECK();
   return 0;

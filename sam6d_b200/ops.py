@@ -454,7 +454,7 @@ def geo_embed_lut(T: Tensor, tabA: Tensor, inv_ha: float, tabD: Tensor, inv_hd: 
 # ---------------------------------------------------------------------------------------------- attention
 def rpe_scores(E: Tensor, U: Tensor) -> Tensor:
     """E (B,S,S,256) f32|bf16, U (B,S,4,256) f32 contiguous or a (B*S, 4*256) f32 row view (e.g. the u columns of a fused
-    projection) -> (B,4,S,S) f32."""
+    projection; 16-byte aligned, with a row stride that is a multiple of 4) -> (B,4,S,S) f32."""
     if E.dtype not in (torch.float32, torch.bfloat16):
         raise RuntimeError("E must be float32 or bfloat16")
     _check(E, E.dtype, "E", 4)
@@ -506,13 +506,25 @@ def attn_tc_padded_bias(Q: Tensor, q_col0: int, K: Tensor, k_col0: int, Vt: Tens
 
 def mha(q: Tensor, k: Tensor, v: Tensor, bias: Optional[Tensor], scale: float, out: Tensor) -> Tensor:
     """softmax((q k^T + bias) * scale) v per head of 64 channels: q, out (B,Sq,H*64), k, v (B,Sk,H*64) f32 row views (e.g.
-    column slices of a fused qkv projection); bias (B,H,Sq,Sk) f32 or None"""
+    column slices of a fused qkv projection); bias (B,H,Sq,Sk) f32 contiguous or None"""
+    for t, name in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
+        if t.dtype != torch.float32 or t.dim() != 3:
+            raise RuntimeError(f"mha: {name} must be a 3-D float32 row view, got {t.dtype} with shape {tuple(t.shape)}")
     B, Sq, HD = q.shape
+    Sk = k.shape[1]
+    if HD % 64 or k.shape != (B, Sk, HD) or v.shape != (B, Sk, HD) or out.shape != (B, Sq, HD):
+        raise RuntimeError(f"mha: q, out (B,Sq,H*64) and k, v (B,Sk,H*64), got q {tuple(q.shape)} k {tuple(k.shape)} "
+                           f"v {tuple(v.shape)} out {tuple(out.shape)}")
+    H = HD // 64
+    if bias is not None:
+        _check(bias, torch.float32, "bias", 4)
+        if bias.shape != (B, H, Sq, Sk):
+            raise RuntimeError(f"mha: bias must be (B,H,Sq,Sk) = {(B, H, Sq, Sk)}, got {tuple(bias.shape)}")
     _, q_bs, q_ld = _rows(q)
     _, k_bs, k_ld = _rows(k)
     _, v_bs, v_ld = _rows(v)
     _, o_bs, o_ld = _rows(out)
-    _lib.call("sam6d_mha", q, q_ld, q_bs, k, k_ld, k_bs, v, v_ld, v_bs, bias, B, HD // 64, Sq, k.shape[1], scale, out, o_ld, o_bs)
+    _lib.call("sam6d_mha", q, q_ld, q_bs, k, k_ld, k_bs, v, v_ld, v_bs, bias, B, H, Sq, Sk, scale, out, o_ld, o_bs)
     return out
 
 
