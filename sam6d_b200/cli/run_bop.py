@@ -13,8 +13,8 @@ import argparse
 import os
 import sys
 
-from . import ism_run_inference_custom as ism_cli
 from . import pem_run_inference_custom as pem_cli
+from . import run_sam6d
 from .. import bop
 
 
@@ -27,38 +27,14 @@ def get_parser():
     ap.add_argument("--stage", default="both", choices=("ism", "pem", "both"))
     ap.add_argument("--detections", default=None, help="--stage pem: the detection JSON (default OUT/result_<dataset_name>.json)")
     ap.add_argument("--max_frames", default=None, type=int, help="only the first N frames (ISM) / images (PEM)")
-    ap.add_argument("--template_size", default=512, type=int, help="ISM onboarding render size in pixels")
-    ap.add_argument("--segmentor_model", default="sam", choices=("sam", "fastsam"), help="The segmentor model in ISM")
-    ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
-    ap.add_argument("--checkpoint_dir", default=None, help="the ISM's checkpoints (SAM / FastSAM and DINOv2 weights)")
-    ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"))
-    ap.add_argument("--fastsam_model", default="FastSAM-x", choices=tuple(ism_cli.FASTSAM_MODELS))
-    ap.add_argument("--dinov2_model", default="dinov2_vitl14", choices=("dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"))
-    ap.add_argument("--points_per_side", default=32, type=int)
-    ap.add_argument("--pred_iou_thresh", default=0.88, type=float)
-    ap.add_argument("--confidence_thresh", default=ism_cli.CONFIDENCE_THRESH, type=float, help="semantic-score threshold")
-    ap.add_argument("--aggregation_function", default="avg_5", choices=("mean", "median", "max", "avg_5"))
-    ap.add_argument("--level_templates", default=0, type=int, choices=(0, 1, 2))
-    ap.add_argument("--pose_distribution", default="all", choices=("all", "upper"))
-    ap.add_argument("--rendering_type", default="pyrender", choices=("pyrender", "pbr"),
-                    help="ISM references rendered from the CAD models, or frames of the dataset's own --pbr_split")
-    ap.add_argument("--pbr_split", default="train_pbr", help="with --rendering_type pbr: the split whose frames become the references")
-    ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth")
-    ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
-    ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
-    # not in the reference: refine each PEM pose against the observed depth (pipeline.icp_refine_out)
-    ap.add_argument("--icp_iters", default=0, type=int, help="point-to-plane ICP iterations per PEM pose (0: off)")
-    # not in the reference: rescore each reported pose by its agreement with the observed depth (pipeline.verify_out)
-    ap.add_argument("--verify", action="store_true", help="render every pose and multiply its score by its depth agreement")
-    ap.add_argument("--verify_tau", default=0.1, type=float, help="--verify's depth tolerance over the object's radius")
-    pem_cli.add_hypothesis_args(ap)
+    run_sam6d.add_model_args(ap, frames=False)
     return ap
 
 
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
-    pem_cli.check_hypothesis_args(ap, args, models_info=True)
+    pem_cli.check_pose_args(ap, args, models_info=True)
     if args.stage in ("pem", "both") and args.template_dir is None:
         ap.error(f"--stage {args.stage} needs --template_dir (the PEM's template views)")
     if args.stage == "both" and args.detections is not None:
@@ -71,16 +47,7 @@ def main(argv=None):
     detections = args.detections or os.path.join(args.output_dir, f"result_{args.dataset_name}.json")
     if args.stage == "pem" and not os.path.isfile(detections):
         ap.error(f"--stage pem: no detection file {detections}")
-    from ..pipeline import SAM6D
-    sam6d = SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
-                  dinov2_model=args.dinov2_model, checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint,
-                  random_weights=args.random_weights, stability_score_thresh=args.stability_score_thresh,
-                  pred_iou_thresh=args.pred_iou_thresh, points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
-                  precision=args.precision, level_templates=args.level_templates, pose_distribution=args.pose_distribution,
-                  aggregation_function=args.aggregation_function, rendering_type=args.rendering_type,
-                  pbr_root=dataset_root if args.rendering_type == "pbr" else None, pbr_split=args.pbr_split,
-                  icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau, pem_hypotheses=args.pem_hypotheses,
-                  hyp_min_angle=args.hyp_min_angle, hyp_min_dist=args.hyp_min_dist)
+    sam6d = run_sam6d.build_sam6d(args, pbr_root=dataset_root if args.rendering_type == "pbr" else None)
     os.makedirs(args.output_dir, exist_ok=True)
     if args.stage in ("ism", "both"):
         objects = sam6d.onboard_bop(args.bop_root, args.dataset_name, template_size=args.template_size)

@@ -35,15 +35,22 @@ class _OneOrSeveral(argparse.Action):
 
 def get_parser():
     ap = argparse.ArgumentParser(description="SAM-6D: templates -> ISM -> PEM in one process")
-    ap.add_argument("--segmentor_model", default="sam", choices=("sam", "fastsam"), help="The segmentor model in ISM")
     ap.add_argument("--output_dir", required=True, help="Path to root directory of the output")
     ap.add_argument("--cad_path", required=True, nargs="+", action=_OneOrSeveral, help="Path to CAD(mm); several for several objects")
     ap.add_argument("--obj_ids", type=int, nargs="+", default=None, help="category ids of the CAD models (default 1..O)")
     ap.add_argument("--rgb_path", required=True, help="Path to RGB image")
     ap.add_argument("--depth_path", required=True, help="Path to Depth image(mm)")
     ap.add_argument("--cam_path", required=True, help="Path to camera information")
+    add_model_args(ap)
+    return ap
+
+
+def add_model_args(ap, frames: bool = True):
+    """the model and pose options of run_sam6d, track_sam6d and run_bop.  frames=False leaves out --det_score_thresh and
+    --pbr_root: run_bop filters detections by the BOP rule and takes the PBR split from its dataset"""
     ap.add_argument("--template_size", default=512, type=int, help="template width and height in pixels (render_custom_templates --size)")
     # the ISM CLI's options
+    ap.add_argument("--segmentor_model", default="sam", choices=("sam", "fastsam"), help="The segmentor model in ISM")
     ap.add_argument("--stability_score_thresh", default=0.97, type=float, help="stability_score_thresh of SAM")
     ap.add_argument("--checkpoint_dir", default=None, help="the ISM CLI's --checkpoint_dir (SAM / FastSAM and DINOv2 weights)")
     ap.add_argument("--sam_model_type", default="vit_h", choices=("vit_h", "vit_l", "vit_b"))
@@ -59,30 +66,25 @@ def get_parser():
     ap.add_argument("--pose_distribution", default="all", choices=("all", "upper"),
                     help="onboarding_config.pose_distribution: all, or upper (cameras with z >= 0)")
     ap.add_argument("--rendering_type", default="pyrender", choices=("pyrender", "pbr"),
-                    help="onboarding_config.rendering_type: ISM references rendered from the CAD model, or frames of a BOP PBR split")
-    ap.add_argument("--pbr_root", default=None, help="with --rendering_type pbr: the BOP dataset directory (holding --pbr_split)")
+                    help="onboarding_config.rendering_type: ISM references rendered from the CAD models, or frames of a BOP PBR split")
     ap.add_argument("--pbr_split", default="train_pbr", help="with --rendering_type pbr: the split whose frames become the references")
     # the PEM CLI's options
-    ap.add_argument("--det_score_thresh", default=0.2, type=float, help="The score threshold of detection")
     ap.add_argument("--checkpoint", default=None, help="sam-6d-pem-base.pth (default: the PEM CLI's)")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--random_weights", action="store_true", help="seeded random weights when no checkpoints exist (plumbing runs)")
-    # not in the reference: refine each PEM pose against the observed depth (pipeline.icp_refine_out)
-    ap.add_argument("--icp_iters", default=0, type=int, help="point-to-plane ICP iterations per PEM pose (0: off)")
-    # not in the reference: rescore each reported pose by its agreement with the observed depth (pipeline.verify_out)
-    ap.add_argument("--verify", action="store_true", help="render every pose and multiply its score by its depth agreement")
-    ap.add_argument("--verify_tau", default=0.1, type=float, help="--verify's depth tolerance over the object's radius")
-    pem_cli.add_hypothesis_args(ap)
-    return ap
+    pem_cli.add_pose_args(ap)
+    if frames:
+        ap.add_argument("--pbr_root", default=None, help="with --rendering_type pbr: the BOP dataset directory (holding --pbr_split)")
+        ap.add_argument("--det_score_thresh", default=0.2, type=float, help="The score threshold of detection")
 
 
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
-    pem_cli.check_hypothesis_args(ap, args)
+    pem_cli.check_pose_args(ap, args)
     if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
         ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
-    sam6d = build_sam6d(args)
+    sam6d = build_sam6d(args, pbr_root=args.pbr_root, det_score_thresh=args.det_score_thresh)
     multi = isinstance(args.cad_path, list)
     n_cad = len(args.cad_path) if multi else 1
     if args.obj_ids is not None and len(args.obj_ids) != n_cad:
@@ -106,41 +108,23 @@ def main(argv=None):
         print(f"=> {res.reason}")
     print(f"=> {len(res.ism)} ISM detections, {len(res.pem)} poses written to {out_dir}")
     if res.pem:
-        (write_vis_objects if multi else pem_cli.write_vis)(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
+        pem_cli.write_vis(os.path.join(out_dir, "vis_pem.png"), res.frame, cam["cam_K"])
     return 0
 
 
-def build_sam6d(args):
-    """the SAM6D of the parsed model options"""
+def build_sam6d(args, pbr_root=None, **kw):
+    """the SAM6D of add_model_args' options; pbr_root: the BOP dataset of --rendering_type pbr; kw: SAM6D's other arguments"""
     from ..pipeline import SAM6D
     return SAM6D(segmentor=args.segmentor_model, sam_model_type=args.sam_model_type, fastsam_model=args.fastsam_model,
                  dinov2_model=args.dinov2_model,
                  checkpoint_dir=args.checkpoint_dir, checkpoint=args.checkpoint, random_weights=args.random_weights,
                  stability_score_thresh=args.stability_score_thresh, pred_iou_thresh=args.pred_iou_thresh,
                  points_per_side=args.points_per_side, confidence_thresh=args.confidence_thresh,
-                 det_score_thresh=args.det_score_thresh, precision=args.precision, level_templates=args.level_templates,
+                 precision=args.precision, level_templates=args.level_templates,
                  pose_distribution=args.pose_distribution, aggregation_function=args.aggregation_function,
-                 rendering_type=args.rendering_type, pbr_root=args.pbr_root, pbr_split=args.pbr_split,
+                 rendering_type=args.rendering_type, pbr_root=pbr_root, pbr_split=args.pbr_split,
                  icp_iters=args.icp_iters, verify=args.verify, verify_tau=args.verify_tau, pem_hypotheses=args.pem_hypotheses,
-                 hyp_min_angle=args.hyp_min_angle, hyp_min_dist=args.hyp_min_dist)
-
-
-def write_vis_objects(path, frame, cam_K):
-    """vis_pem.png of a multi-object frame: the frame beside the projected box and points of each object's best-scoring poses,
-    drawn with that object's model points"""
-    print("=> visualizating ...")
-    try:
-        import cv2
-        import numpy as np
-        K = np.asarray(cam_K, dtype=np.float64).reshape(3, 3)
-        vis = frame.img
-        for o in np.unique(frame.obj):
-            rows = np.flatnonzero(frame.obj == o)
-            best = rows[frame.pose_scores[rows] == frame.pose_scores[rows].max()]
-            vis = pem_cli.draw_detections(vis, frame.pred_rot[best], frame.pred_trans[best], frame.model_points[o] * 1000, K)
-        cv2.imwrite(path, np.concatenate([frame.img, vis], axis=1)[:, :, ::-1])
-    except Exception as e:                                            # the visualisation is not part of the result
-        print(f"=> visualisation skipped: {e}", file=sys.stderr)
+                 hyp_min_angle=args.hyp_min_angle, hyp_min_dist=args.hyp_min_dist, **kw)
 
 
 if __name__ == "__main__":

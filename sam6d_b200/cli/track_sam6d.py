@@ -16,9 +16,6 @@ import sys
 from . import pem_run_inference_custom as pem_cli
 from . import run_sam6d
 
-# run_sam6d's options that name its one frame and its objects; the rest (the model options) are shared
-_FRAME_OPTIONS = {"help", "cad_path", "obj_ids", "rgb_path", "depth_path", "cam_path", "output_dir"}
-
 
 def get_parser():
     ap = argparse.ArgumentParser(description="SAM-6D tracking: detect, then follow each object's pose with depth")
@@ -28,9 +25,7 @@ def get_parser():
     ap.add_argument("--depth_dir", required=True, help="directory of the depth frames (mm), named as the RGB frames")
     ap.add_argument("--cam_path", required=True, help="Path to camera information")
     ap.add_argument("--output_dir", required=True, help="Path to root directory of the output")
-    for action in run_sam6d.get_parser()._actions:
-        if action.dest not in _FRAME_OPTIONS:
-            ap._add_action(action)
+    run_sam6d.add_model_args(ap)
     # the tracker's parameters (sam6d_b200/track.py; not tuned on real video)
     ap.add_argument("--track_icp_iters", default=10, type=int, help="ICP iterations per tracked frame")
     ap.add_argument("--margin_px", default=16, type=int, help="dilation of the rendered silhouette in pixels")
@@ -53,7 +48,7 @@ def frame_pairs(rgb_dir: str, depth_dir: str):
 def main(argv=None):
     ap = get_parser()
     args = ap.parse_args(argv)
-    run_sam6d.pem_cli.check_hypothesis_args(ap, args)
+    pem_cli.check_pose_args(ap, args)
     if args.rendering_type == "pbr" and (args.obj_ids is None or args.pbr_root is None):
         ap.error("--rendering_type pbr needs --pbr_root and --obj_ids (the BOP ids of the CAD models)")
     if args.obj_ids is not None and len(args.obj_ids) != len(args.cad_path):
@@ -62,9 +57,9 @@ def main(argv=None):
     if not names:
         raise SystemExit(f"no frame is named the same in {args.rgb_dir} and {args.depth_dir}")
     from ..track import Tracker
-    sam6d = run_sam6d.build_sam6d(args)
+    sam6d = run_sam6d.build_sam6d(args, pbr_root=args.pbr_root, det_score_thresh=args.det_score_thresh)
     objs = sam6d.onboard_objects(args.cad_path, obj_ids=args.obj_ids, template_size=args.template_size,
-                                 symmetries=run_sam6d.pem_cli.symmetry_option(args))
+                                 symmetries=pem_cli.symmetry_option(args))
     tracker = Tracker(sam6d, objs, args.cad_path, track_icp_iters=args.track_icp_iters, margin_px=args.margin_px,
                       gate_scale=args.gate_scale, min_inlier_fraction=args.min_inlier_fraction, max_rms_m=args.max_rms_m,
                       redetect_interval=args.redetect_interval, max_instances=args.max_instances, start_score=args.start_score,

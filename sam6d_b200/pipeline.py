@@ -23,7 +23,7 @@ import os
 import time
 from dataclasses import dataclass
 from types import SimpleNamespace
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -190,72 +190,93 @@ def pem_template_bank(model, rgbs, masks, xyzs_mm, rng=None, device=None):
         return model.feature_extraction.get_obj_feats(all_tem, all_tem_pts, all_tem_choose)
 
 
+# ---- the per-object inputs of the steps after Net.forward (not in the reference) ----------------------------------------------
+class PoseInputs(NamedTuple):
+    """what finish_poses and symmetry_inputs need of O objects, each None when its step is off: icp (samples, normals) (O,M,3)
+    f32 on the device (icp_model), meshes the O device meshes in mm that verification renders (verify_mesh), radii (O,) each
+    object's max |model point| in metres (object_radii), symmetries their packed symmetry.SymmetrySet (object_symmetries)"""
+    icp: Optional[tuple] = None
+    meshes: Optional[list] = None
+    radii: Optional[np.ndarray] = None
+    symmetries: Optional["symmetry.SymmetrySet"] = None
+
+
+def build_pose_inputs(meshes, model_points_m, device, icp: bool = False, verify: bool = False, symmetries=None,
+                      obj_ids=None) -> PoseInputs:
+    """O numpy meshes in mm (meshio.Mesh) and their model points (O,n,3) -> their PoseInputs: the ICP samples with icp, the
+    device meshes and radii with verify, and unless None the packed symmetries of a check_symmetries value for obj_ids.  No
+    draw from any caller's RNG: the ICP samples and "auto" symmetries draw from their own seeds, mesh by mesh."""
+    samples = icp_tensors(*(np.stack(a) for a in zip(*[icp_model(m.vertices, m.faces) for m in meshes])), device) if icp else None
+    return PoseInputs(icp=samples, meshes=[verify_mesh(m.vertices, m.faces, device) for m in meshes] if verify else None,
+                      radii=object_radii(model_points_m) if verify else None,
+                      symmetries=object_symmetries(symmetries, meshes, obj_ids, device))
+
+
 # ---- PEM inputs + Net.forward (PEM/run_inference_custom.py:165-307) -------------------------------------------------------------
-def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh: float, rng=None,
-              generator: Optional[torch.Generator] = None, device=None, mark=None, det_obj=None, icp=None, icp_iters: int = 0,
-              verify=None, verify_tau: float = 0.1, symmetries=None):
-    """ISM records -> SimpleNamespace(dets, out, img, model_points): the detections the PEM keeps (above det_score_thresh with
-    enough valid depth) as copies of their records, Net.forward's outputs (None when none is kept), and the frame image and
-    model points as get_test_data returns them.  The coarse stage's uniforms are drawn from `generator` when one is given,
-    else from torch's global CUDA generator (the reference's torch.rand).  mark(stage) after the inputs and after the forward.
-    Several objects: bank (O,2048,3), (O,2048,256), model_points_m (O,n,3) and det_obj the object index of every record; each
-    detection gets its object's radius filter, model points and template bank, and all run as one batch.  The frame then also
-    holds obj (P) int64, choose_idx (P,2048) and rand, the coarse stage's uniforms.  icp_iters > 0: after the forward the poses
-    are refined by icp_refine_out against the observed points with icp = (samples, normals) (O,M,3) on the device.
-    verify, the device meshes in mm of the objects (one per object, in model_points_m's order; verify_mesh): after the forward
-    and any ICP, verify_out checks every reported pose against the frame's depth and its detection's mask with tolerance
-    verify_tau x its object's radius.  With several PEM hypotheses (Net.set_hypotheses) finish_poses picks each detection's
-    pose, and symmetries (a symmetry.SymmetrySet of the objects, in model_points_m's order) makes the hypotheses distinct up to
-    each object's symmetries (symmetry_inputs)."""
+def pem_step(model, data: dict, bank, pose: PoseInputs, rand, rows, cam_K, icp_iters: int = 0, verify_tau: float = 0.1) -> dict:
+    """Net.forward on the instances of `data` (get_test_data's or bop.pem_instances' dict; data["obj"] (P) the object index of
+    each) and the steps after it -> Net.forward's outputs.  Each instance gets its object's template bank (O,2048,3),
+    (O,2048,256); with several PEM hypotheses (Net.set_hypotheses) and pose.symmetries, hypotheses distinct up to its
+    object's symmetries (symmetry_inputs).  rand: the coarse stage's uniforms (None: torch's global CUDA generator, the
+    reference's torch.rand).  Then finish_poses with pose's ICP samples (icp_iters > 0), and with pose.meshes verification
+    against rows, the frame's device depth and masks (inputs.FrameInputs.rows), with tolerance verify_tau x the object's radius."""
+    data["dense_po"], data["dense_fo"] = bank[0][data["obj"]], bank[1][data["obj"]]
+    if pose.symmetries is not None and model.hypotheses[0] > 1:
+        symmetry_inputs(data, pose.symmetries, data["obj"])
+    with torch.no_grad():
+        out = model(data, rand=rand)
+        return finish_poses(out, data["pts"], data["model"], data["obj"], pose.icp, icp_iters, pose.meshes, pose.radii, rows, cam_K,
+                            verify_tau)
+
+
+def pem_frame(model, bank, dets, rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_obj, det_score_thresh: float, rng=None,
+              generator: Optional[torch.Generator] = None, device=None, mark=None, pose: PoseInputs = PoseInputs(), icp_iters: int = 0,
+              verify_tau: float = 0.1):
+    """ISM records of O objects -> SimpleNamespace(dets, out, img, model_points, obj, choose_idx, rand): the detections the PEM
+    keeps (above det_score_thresh with enough valid depth) as copies of their records, Net.forward's outputs (None when none is
+    kept), the frame image and the model points (O,n,3) as get_test_data returns them, the object index obj (P) int64 and the
+    sample indices choose_idx (P,2048) of every kept detection, and rand, the coarse stage's uniforms.  bank (O,2048,3),
+    (O,2048,256), model_points_m (O,n,3) and det_obj the object index of every record (one object: model_points_m[None] and
+    zeros); each detection gets its object's radius filter, model points and template bank, and all run as one batch
+    (pem_step, with the objects' PoseInputs `pose`, default none).  The coarse stage's uniforms are drawn from `generator` when
+    one is given, else from torch's global CUDA generator.  mark(stage) after the inputs and after the forward."""
     cfg = pem_cli.TEST_DATASET
     mark = mark or (lambda stage: None)
     got = inputs.get_test_data(
         [dict(d) for d in dets], rgb_u8, depth_raw, cam_K, depth_scale, model_points_m, det_score_thresh,
         cfg["n_sample_observed_point"], cfg["img_size"], cfg["rgb_mask_flag"], rng=rng, device=device, det_obj=det_obj,
-        frame_rows=verify is not None)
-    input_data, img, _, model_points, kept = got[:5]
-    n = input_data["pts"].size(0)
+        frame_rows=pose.meshes is not None)
+    data, img, _, model_points, kept = got[:5]
+    n = data["pts"].size(0)
     mark("pem_inputs")
     out = rand = None
     if n:
-        with torch.no_grad():
-            if det_obj is None:
-                input_data["dense_po"] = bank[0].repeat(n, 1, 1)
-                input_data["dense_fo"] = bank[1].repeat(n, 1, 1)
-            else:
-                input_data["dense_po"] = bank[0][input_data["obj"]]
-                input_data["dense_fo"] = bank[1][input_data["obj"]]
-            if generator is not None:
-                rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=input_data["pts"].device, generator=generator)
-            if symmetries is not None and model.hypotheses[0] > 1:
-                symmetry_inputs(input_data, symmetries, input_data["obj"] if det_obj is not None else None)
-            out = model(input_data, rand=rand)
-            if icp_iters > 0 or verify is not None:
-                obj = input_data["obj"] if det_obj is not None else torch.zeros(n, dtype=torch.int64, device=input_data["pts"].device)
-                finish_poses(out, input_data["pts"], input_data["model"], obj, icp, icp_iters, verify,
-                             object_radii(model_points_m) if verify is not None else None, got[5] if verify is not None else None,
-                             cam_K, verify_tau)
+        if generator is not None:
+            rand = torch.rand(n, model.coarse_point_matching.cfg.nproposal1 * 3, device=data["pts"].device, generator=generator)
+        out = pem_step(model, data, bank, pose, rand, got[5] if pose.meshes is not None else None, cam_K, icp_iters, verify_tau)
     mark("forward")
-    frame = SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points)
-    if det_obj is not None:
-        frame.obj, frame.choose_idx, frame.rand = input_data["obj"].cpu().numpy(), input_data["choose_idx"], rand
-    return frame
+    return SimpleNamespace(dets=kept, out=out, img=img, model_points=model_points, obj=data["obj"].cpu().numpy(),
+                           choose_idx=data["choose_idx"], rand=rand)
+
+
+def reported_scores(out: dict, det_score: torch.Tensor) -> torch.Tensor:
+    """the score a pose is reported with: pred_pose_score x its detection's score, x verify when the poses were verified"""
+    score = out["pred_pose_score"] * det_score
+    return score * out["verify"] if "verify" in out else score
 
 
 def pem_records(frame):
-    """pem_frame's result -> the PEM CLI's records: the kept ISM records with the pose score, R and t (mm).  The host arrays
-    behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation.  When the poses were
-    verified (verify_out), the score is pred_pose_score x ISM score x verify and each record also carries "verify".  With
-    several PEM hypotheses each record also carries "hypothesis", the index of the one it reports."""
+    """pem_frame's result -> the PEM CLI's records: the kept ISM records with the pose score (reported_scores), R and t (mm).
+    The host arrays behind them are kept on `frame` as pose_scores, pred_rot, pred_trans (mm) for the visualisation.  When the
+    poses were verified (verify_out) each record also carries "verify".  With several PEM hypotheses each record also carries
+    "hypothesis", the index of the one it reports."""
     if frame.out is None:
         return []
     out = frame.out
     verified = "verify" in out
+    frame.pose_scores = reported_scores(out, out["score"]).detach().cpu().numpy()
     if verified:
-        frame.pose_scores = (out["pred_pose_score"] * out["score"] * out["verify"]).detach().cpu().numpy()
         verify = out["verify"].cpu().numpy()
-    else:
-        frame.pose_scores = (out["pred_pose_score"] * out["score"]).detach().cpu().numpy()
     frame.pred_rot = out["pred_R"].detach().cpu().numpy()
     frame.pred_trans = out["pred_t"].detach().cpu().numpy() * 1000
     hyp = out["hyp_index"].cpu().numpy() if "hyp_index" in out else None
@@ -281,8 +302,6 @@ def icp_model(verts_mm: np.ndarray, faces: np.ndarray):
 
 def icp_tensors(points_m, normals, device):
     """icp_model arrays of one object (M,3) or of O objects (O,M,3) -> (samples, normals) (O,M,3) f32 on the device"""
-    if points_m is None or normals is None:
-        raise ValueError("ICP refinement needs the objects' ICP samples: onboard them with SAM6D(..., icp_iters > 0)")
     m = np.asarray(points_m).shape[-2]
     return tuple(torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.float32).reshape(-1, m, 3))).to(device)
                  for a in (points_m, normals))
@@ -367,11 +386,10 @@ def finish_poses(out: dict, pts: torch.Tensor, model: torch.Tensor, obj: torch.T
 SYMMETRY_SOURCES = ("auto",)           # besides None and {obj_id: models_info entry}; run_bop_pem also takes "models_info"
 
 
-def symmetry_inputs(data: dict, symmetries: "symmetry.SymmetrySet", obj: Optional[torch.Tensor] = None) -> dict:
+def symmetry_inputs(data: dict, symmetries: "symmetry.SymmetrySet", obj: torch.Tensor) -> dict:
     """fill Net.forward's hyp_sym_R, hyp_sym_t and hyp_sym_range (pem.SYM_KEYS) in place: every object's packed set, and each
-    detection's range in it by its object index obj (B) (None: all object 0)"""
-    B = data["pts"].shape[0]
-    obj = torch.zeros(B, dtype=torch.int64, device=symmetries.range.device) if obj is None else obj.to(symmetries.range.device)
+    detection's range in it by its object index obj (B)"""
+    obj = obj.to(symmetries.range.device)
     data.update(hyp_sym_R=symmetries.R, hyp_sym_t=symmetries.t, hyp_sym_range=symmetries.range[obj].contiguous())
     return data
 
@@ -393,11 +411,10 @@ def check_symmetries(symmetries, obj_ids, sources=SYMMETRY_SOURCES):
 
 def object_symmetries(symmetries, meshes, obj_ids, device) -> Optional["symmetry.SymmetrySet"]:
     """a checked `symmetries` value -> the objects' packed symmetry sets (symmetry.pack_sets), or None.  "auto":
-    symmetry.find_symmetries of every mesh (meshio.Mesh or PLY path)"""
+    symmetry.find_symmetries of every meshio.Mesh"""
     if symmetries is None:
         return None
     if isinstance(symmetries, str):
-        meshes = [meshio.load_ply_mesh(m) if isinstance(m, str) else m for m in meshes]
         infos = [symmetry.find_symmetries(m, backend=symmetry.GpuBackend(device)) for m in meshes]
     else:
         infos = [symmetries[int(i)] for i in obj_ids]
@@ -407,19 +424,16 @@ def object_symmetries(symmetries, meshes, obj_ids, device) -> Optional["symmetry
 # ---- the whole pipeline ----------------------------------------------------------------------------------------------------
 @dataclass
 class Onboarded:
-    """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank, model points;
-    with icp_iters > 0 also the ICP samples (M,3) in metres and their unit normals (icp_model), else None; with verify the
-    device mesh in mm that pose verification renders (verify_mesh), else None"""
+    """one object after SAM6D.onboard: ISM references, template poses, geometric-score cloud, PEM template bank (1,2048,3),
+    (1,2048,256), model points; pose_inputs, the object's PoseInputs (O = 1) for the SAM6D's icp_iters and verify and the
+    symmetries it was onboarded with"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
     cloud_m: np.ndarray
     bank: tuple
     model_points_m: np.ndarray
-    icp_points_m: Optional[np.ndarray] = None
-    icp_normals: Optional[np.ndarray] = None
-    verify_mesh: Optional[meshio.Mesh] = None
-    symmetries: Optional["symmetry.SymmetrySet"] = None
+    pose_inputs: PoseInputs = PoseInputs()
 
 
 class SAM6D:
@@ -510,19 +524,20 @@ class SAM6D:
         pbr.select_references, whose draws come first from `rng`, then the draws above; only the 42 level-0 views are rendered.
 
         symmetries (not in the reference; used with pem_hypotheses > 1): None, "auto" or the object's models_info entry, kept
-        as Onboarded.symmetries (onboard_objects)."""
+        in Onboarded.pose_inputs (onboard_objects)."""
         if isinstance(symmetries, dict):
             symmetries = {0: symmetries}
         check_symmetries(symmetries, [0])
+        refs = None
         if self.rendering_type == "pbr":
             if obj_id is None:
                 raise ValueError('rendering_type "pbr" needs the BOP object id: onboard(..., obj_id=)')
             ref_cls, ref_patch = self._pbr_references([obj_id], rng)
-            ob = self._onboard_mesh(mesh_or_ply_path, template_size, rng, (ref_cls[0], ref_patch[0]))
-        else:
-            ob = self._onboard_mesh(mesh_or_ply_path, template_size, rng)
-        if symmetries is not None:
-            ob.symmetries = object_symmetries(symmetries, [mesh_or_ply_path], [0], self.device)
+            refs = (ref_cls[0], ref_patch[0])
+        mesh = meshio.load_ply_mesh(mesh_or_ply_path) if isinstance(mesh_or_ply_path, str) else mesh_or_ply_path
+        ob = self._onboard_mesh(mesh, template_size, rng, refs)
+        ob.pose_inputs = build_pose_inputs([mesh], ob.model_points_m, self.device, icp=self.icp_iters > 0, verify=self.verify,
+                                           symmetries=symmetries, obj_ids=[0])
         return ob
 
     def _pbr_references(self, obj_ids, rng):
@@ -533,9 +548,9 @@ class SAM6D:
         sel = pbr.select_references(self._pbr_rows, obj_ids, union[index], rng)
         return pbr.reference_features(self.desc, self._pbr_rows, sel, self.device)
 
-    def _onboard_mesh(self, mesh_or_ply_path, template_size, rng, refs=None) -> Onboarded:
-        """onboard() from the mesh, with the ISM references `refs` (ref_cls, ref_patch) when they are given"""
-        mesh = meshio.load_ply_mesh(mesh_or_ply_path) if isinstance(mesh_or_ply_path, str) else mesh_or_ply_path
+    def _onboard_mesh(self, mesh: meshio.Mesh, template_size, rng, refs=None) -> Onboarded:
+        """onboard() from the numpy mesh but for its pose inputs, with the ISM references `refs` (ref_cls, ref_patch) when they
+        are given"""
         verts, faces = mesh.vertices, mesh.faces
         if refs is None:
             out, poses = render_templates(mesh, template_size, level_templates=self.level_templates, pose_distribution=self.pose_distribution)
@@ -554,14 +569,13 @@ class SAM6D:
         bank = pem_template_bank(self.pem, list(rgbs[:n0]), list(masks[:n0]), [x.astype(np.float32) for x in xyzs[:n0]], rng=rng,
                                  device=self.device)
         model_points = meshio.sample_surface(verts, faces, pem_cli.TEST_DATASET["n_sample_model_point"], rng) / 1000.0
-        icp_pts, icp_nrm = icp_model(verts, faces) if self.icp_iters > 0 else (None, None)
-        vmesh = verify_mesh(verts, faces, self.device) if self.verify else None
-        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points, icp_pts, icp_nrm, vmesh)
+        return Onboarded(ref_cls, ref_patch, render_cli.to_metres(poses[ism_index]), cloud, bank, model_points)
 
     def onboard_objects(self, meshes, obj_ids=None, template_size: int = 512, rng=None, symmetries=None) -> "ObjectSet":
-        """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet.
-        obj_ids: the category id of every object (distinct ints), default 1..O.  The fp32 patch tokens (44 MB per object at
-        C = 1024) are copied into the stack as each object is built, so only one object's extra copy is alive at a time.
+        """onboard() every mesh in turn (random draws from `rng`, object after object) and stack the results into an ObjectSet,
+        whose pose inputs are built once for all of them.  obj_ids: the category id of every object (distinct ints), default
+        1..O.  The fp32 patch tokens (44 MB per object at C = 1024) are copied into the stack as each object is built, so only
+        one object's extra copy is alive at a time.
 
         rendering_type "pbr": obj_ids are required and are the objects' BOP ids.  The references of all objects are selected
         first (pbr.select_references' draws, object after object, as the reference's load_processed_metaData makes them), then
@@ -569,7 +583,7 @@ class SAM6D:
 
         symmetries (not in the reference; used with pem_hypotheses > 1): None (default), "auto" (symmetry.find_symmetries of
         every mesh, whose samples draw from their own seed, not from `rng`) or {obj_id: models_info entry}; kept packed on the
-        device as ObjectSet.symmetries (symmetry.pack_sets), so that detect_objects' hypotheses are distinct up to them."""
+        device in ObjectSet.pose_inputs (symmetry.pack_sets), so that detect_objects' hypotheses are distinct up to them."""
         meshes = list(meshes)
         n = len(meshes)
         if self.rendering_type == "pbr" and obj_ids is None:
@@ -578,24 +592,22 @@ class SAM6D:
         if n == 0 or len(obj_ids) != n or len(set(obj_ids)) != n:
             raise ValueError(f"onboard_objects: {n} meshes need {n} distinct obj_ids, got {obj_ids}")
         check_symmetries(symmetries, obj_ids)
+        meshes = [meshio.load_ply_mesh(m) if isinstance(m, str) else m for m in meshes]
         if self.rendering_type == "pbr":
             ref_cls, ref_patch = self._pbr_references(obj_ids, rng)
             parts = [self._onboard_mesh(mesh, template_size, rng, (ref_cls[o], None)) for o, mesh in enumerate(meshes)]
-            objs = ObjectSet.stack(parts, ref_patch, obj_ids)
-            if symmetries is not None:
-                objs.symmetries = object_symmetries(symmetries, meshes, obj_ids, self.device)
-            return objs
-        parts, ref_patch = [], None
-        for o, mesh in enumerate(meshes):
-            ob = self.onboard(mesh, template_size, rng)
-            if ref_patch is None:
-                ref_patch = ob.ref_patch.new_empty((n,) + tuple(ob.ref_patch.shape))
-            ref_patch[o] = ob.ref_patch
-            ob.ref_patch = None
-            parts.append(ob)
+        else:
+            parts, ref_patch = [], None
+            for o, mesh in enumerate(meshes):
+                ob = self._onboard_mesh(mesh, template_size, rng)
+                if ref_patch is None:
+                    ref_patch = ob.ref_patch.new_empty((n,) + tuple(ob.ref_patch.shape))
+                ref_patch[o] = ob.ref_patch
+                ob.ref_patch = None
+                parts.append(ob)
         objs = ObjectSet.stack(parts, ref_patch, obj_ids)
-        if symmetries is not None:
-            objs.symmetries = object_symmetries(symmetries, meshes, obj_ids, self.device)
+        objs.pose_inputs = build_pose_inputs(meshes, objs.model_points_m, self.device, icp=self.icp_iters > 0, verify=self.verify,
+                                             symmetries=symmetries, obj_ids=obj_ids)
         return objs
 
     def __call__(self, rgb_u8: np.ndarray, depth_raw: np.ndarray, cam_K, depth_scale, obj: Onboarded, rng=None, mark=None):
@@ -675,15 +687,8 @@ class SAM6D:
                                    device=self.device) for i in objs.ids]
         bank = tuple(torch.stack([b[k].reshape(b[k].shape[-2:]) for b in banks]) for k in range(2))
         del banks
-        icp = None
-        if self.icp_iters > 0:
-            icp = icp_tensors(*(np.stack(a) for a in zip(*[icp_model(m.vertices, m.faces) for m in meshes])), self.device)
-        vmeshes, radii = None, None
-        if self.verify:
-            vmeshes, radii = [verify_mesh(m.vertices, m.faces, self.device) for m in meshes], object_radii(model_points)
-        syms = None
-        if symmetries is not None and self.pem.hypotheses[0] > 1:
-            syms = object_symmetries(symmetries, meshes, objs.ids, self.device)
+        pose = build_pose_inputs(meshes, model_points, self.device, icp=self.icp_iters > 0, verify=self.verify,
+                                 symmetries=symmetries if self.pem.hypotheses[0] > 1 else None, obj_ids=objs.ids)
         mark("onboard")
         with open(detections_path) as fh:
             groups = bop.group_detections(json.load(fh))
@@ -698,24 +703,15 @@ class SAM6D:
             torch.cuda.synchronize(self.device)
             t0 = time.time()
             got = bop.pem_instances(dets, image, raw, cam_K, depth_scale, objs, model_points, rng=rng, n_sample=cfg["n_sample_observed_point"],
-                                    img_size=cfg["img_size"], device=self.device, frame_rows=vmeshes is not None)
+                                    img_size=cfg["img_size"], device=self.device, frame_rows=self.verify)
             data, kept = got[:2]
             mark("pem_inputs")
             n = len(kept)
             if n == 0:
                 continue
-            data["dense_po"], data["dense_fo"] = bank[0][data["obj"]], bank[1][data["obj"]]
             rand = bop.pem_rand(g, n, n_rand, self.device)
-            if syms is not None:
-                symmetry_inputs(data, syms, data["obj"])
-            with torch.no_grad():
-                out = self.pem(data, rand=rand)
-                finish_poses(out, data["pts"], data["model"], data["obj"], icp, self.icp_iters, vmeshes, radii,
-                             got[3] if vmeshes is not None else None, cam_K, self.verify_tau)
-            if vmeshes is not None:
-                scores = (out["pred_pose_score"] * data["score"] * out["verify"]).cpu().numpy()
-            else:
-                scores = (out["pred_pose_score"] * data["score"]).cpu().numpy()
+            out = pem_step(self.pem, data, bank, pose, rand, got[3] if self.verify else None, cam_K, self.icp_iters, self.verify_tau)
+            scores = reported_scores(out, data["score"]).cpu().numpy()
             R = out["pred_R"].reshape(-1, 9).cpu().numpy()
             t = out["pred_t"].cpu().numpy() * 1000
             image_time = time.time() - t0 + float(np.float32(dets[0]["time"]))
@@ -747,24 +743,23 @@ class SAM6D:
         cum, off = ops.mask_rle(det.masks.contiguous())
         mark("rle")
         counts = rle_counts(cum.cpu().numpy(), off.cpu().numpy())
-        det_obj = det.obj.cpu().numpy() if multi else None
+        det_obj = det.obj.cpu().numpy()
         records = ism_records(det.boxes.cpu().numpy(), det.scores.cpu().numpy(), counts, det.masks.shape[1:], time.time() - t0,
                               category_ids=np.asarray(obj_ids)[det_obj] if multi else None)
         mark("ism_records")
         if not pem:
             return SimpleNamespace(ism=records, pem=[], masks=det.masks, boxes=det.boxes, scores=det.scores, R=None, t=None, frame=None,
                                    n_proposals=det.n_proposals, reason=None, ism_time=ism_time, **({"obj": det.obj} if multi else {}))
+        pose = obj.pose_inputs if self.verify else obj.pose_inputs._replace(meshes=None)       # pem_step verifies given meshes
+        if (self.icp_iters > 0 and pose.icp is None) or (self.verify and pose.meshes is None):
+            raise ValueError("ICP and pose verification need the objects' ICP samples and device meshes: onboard them with a SAM6D "
+                             "of this icp_iters and verify")
         g = torch.Generator(device=self.device)
         g.manual_seed(pem_cli.RD_SEED)
-        icp = icp_tensors(obj.icp_points_m, obj.icp_normals, self.device) if self.icp_iters > 0 else None
-        vmeshes = None
-        if self.verify:
-            vmeshes = obj.verify_meshes if multi else ([obj.verify_mesh] if obj.verify_mesh is not None else None)
-            if vmeshes is None:
-                raise ValueError("pose verification needs the objects' device meshes: onboard them with SAM6D(..., verify=True)")
-        frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, obj.model_points_m, self.det_score_thresh,
-                          rng=rng, generator=g, device=self.device, mark=mark, det_obj=det_obj, icp=icp, icp_iters=self.icp_iters,
-                          verify=vmeshes, verify_tau=self.verify_tau, symmetries=getattr(obj, "symmetries", None))
+        mp = np.asarray(obj.model_points_m)
+        frame = pem_frame(self.pem, obj.bank, records, rgb_u8, depth_raw, cam_K, depth_scale, mp.reshape((-1,) + mp.shape[-2:]), det_obj,
+                          self.det_score_thresh, rng=rng, generator=g, device=self.device, mark=mark, pose=pose, icp_iters=self.icp_iters,
+                          verify_tau=self.verify_tau)
         pem_recs = pem_records(frame)
         mark("pem_records")
         R = frame.out["pred_R"] if frame.out is not None else None
@@ -778,8 +773,8 @@ class ObjectSet:
     """several objects after SAM6D.onboard_objects, stacked along a leading object axis O: ISM references ref_cls (O,T,C) and
     ref_patch (O,T,256,C), template poses poses_m (O,T,4,4) (the framing distance depends on the mesh), geometric-score clouds
     cloud_m (O,2048,3), PEM template banks (O,2048,3) and (O,2048,256), model points model_points_m (O,Nm,3), each object's
-    radius (O,) (the PEM's max |model point|) and category ids obj_ids; with icp_iters > 0 the ICP samples icp_points_m (O,M,3)
-    and their normals icp_normals (O,M,3), else None; with verify the O device meshes verify_meshes (verify_mesh), else None"""
+    radius (O,) (the PEM's max |model point|) and category ids obj_ids; pose_inputs, the objects' PoseInputs for the SAM6D's
+    icp_iters and verify and the symmetries they were onboarded with"""
     ref_cls: torch.Tensor
     ref_patch: torch.Tensor
     poses_m: np.ndarray
@@ -788,20 +783,13 @@ class ObjectSet:
     model_points_m: np.ndarray
     radii: np.ndarray
     obj_ids: list
-    icp_points_m: Optional[np.ndarray] = None
-    icp_normals: Optional[np.ndarray] = None
-    verify_meshes: Optional[list] = None
-    symmetries: Optional["symmetry.SymmetrySet"] = None
+    pose_inputs: PoseInputs = PoseInputs()
 
     @staticmethod
     def stack(parts, ref_patch, obj_ids) -> "ObjectSet":
-        """Onboarded objects (their ref_patch already stacked into `ref_patch`) -> ObjectSet"""
+        """Onboarded objects (their ref_patch already stacked into `ref_patch`) -> ObjectSet, without pose inputs"""
         mp = np.stack([np.asarray(p.model_points_m, dtype=np.float32) for p in parts])
-        icp = parts[0].icp_points_m is not None
         return ObjectSet(ref_cls=torch.stack([p.ref_cls for p in parts]), ref_patch=ref_patch,
                          poses_m=np.stack([p.poses_m for p in parts]), cloud_m=np.stack([p.cloud_m for p in parts]),
                          bank=tuple(torch.stack([p.bank[i].reshape(p.bank[i].shape[-2:]) for p in parts]) for i in range(2)),
-                         model_points_m=mp, radii=np.asarray([np.max(np.linalg.norm(m, axis=1)) for m in mp]), obj_ids=list(obj_ids),
-                         icp_points_m=np.stack([p.icp_points_m for p in parts]) if icp else None,
-                         icp_normals=np.stack([p.icp_normals for p in parts]) if icp else None,
-                         verify_meshes=[p.verify_mesh for p in parts] if parts[0].verify_mesh is not None else None)
+                         model_points_m=mp, radii=object_radii(mp), obj_ids=list(obj_ids))

@@ -38,9 +38,9 @@ TRACKED, DETECTED, ABSENT = "tracked", "detected", "absent"
 class Tracker:
     """up to max_instances tracks per object of `objects` (an ObjectSet of `sam6d`).  meshes: the numpy meshes in mm passed
     to onboard_objects, in the same order (meshio.Mesh or PLY paths); they are uploaded once for rendering, and the ICP
-    samples and normals come from pipeline.icp_model, whatever icp_iters sam6d has.  Parameters (defaults not tuned on real
-    video): track_icp_iters ICP iterations per tracked frame; margin_px the silhouette dilation in pixels; gate_scale the gate
-    radius over the object's radius about its model-point centroid; min_inlier_fraction and max_rms_m the loss rule;
+    samples and normals come from pipeline.build_pose_inputs, whatever icp_iters sam6d has.  Parameters (defaults not tuned
+    on real video): track_icp_iters ICP iterations per tracked frame; margin_px the silhouette dilation in pixels; gate_scale
+    the gate radius over the object's radius about its model-point centroid; min_inlier_fraction and max_rms_m the loss rule;
     redetect_interval the frames after which detection runs again to pick up objects not yet found; max_instances I the
     tracks per object, start_score the least PEM score that starts an object's second and later tracks, assoc_scale the
     centroid distance, over the object's radius about its centroid, within which two tracks of one object are one copy.
@@ -67,7 +67,7 @@ class Tracker:
         self.n_points = pem_cli.TEST_DATASET["n_sample_observed_point"]
         dev = self.device = torch.device(sam6d.device)
         self.meshes = [render.upload(meshio.Mesh(vertices=m.vertices, faces=m.faces), dev) for m in meshes]
-        self.icp = pipeline.icp_tensors(*(np.stack(a) for a in zip(*[pipeline.icp_model(m.vertices, m.faces) for m in meshes])), dev)
+        self.icp = pipeline.build_pose_inputs(meshes, objects.model_points_m, dev, icp=True).icp
         mp = torch.from_numpy(np.ascontiguousarray(objects.model_points_m, dtype=np.float32)).to(dev)
         self.icp_radius = mp.norm(dim=2).amax(dim=1).contiguous()                       # as pipeline.icp_refine_out
         mp64 = np.asarray(objects.model_points_m, np.float64)

@@ -370,7 +370,8 @@ def test_pipeline_frame_with_icp(golden_dir):
         a, b = getattr(objs0, k), getattr(objs1, k)
         for x, y in (zip(a, b) if k == "bank" else [(a, b)]):
             assert (torch.equal(x, y) if isinstance(x, torch.Tensor) else np.array_equal(x, y)), k
-    assert objs0.icp_points_m is None and objs1.icp_points_m.shape == (2, 4096, 3) and objs1.icp_normals.shape == (2, 4096, 3)
+    icp = objs1.pose_inputs.icp
+    assert objs0.pose_inputs.icp is None and icp[0].shape == (2, 4096, 3) and icp[1].shape == (2, 4096, 3)
     # the frame: the same records and scores, only R and t refined (time is the host clock)
     drop = lambda recs, keys: [{k: v for k, v in r.items() if k not in keys} for r in recs]          # noqa: E731
     assert drop(res0.ism, ("time",)) == drop(res1.ism, ("time",)) and len(res1.pem) == len(res0.pem) > 0

@@ -211,8 +211,8 @@ def test_one_object_against_test_step(golden_dir, tmp_path):
     assert strip(res.ism) == strip(recs)
     g = torch.Generator(device=model.device)
     g.manual_seed(pem_cli.RD_SEED)
-    frame = pem_frame(model.pem, one.bank, recs, rgb, depth, K, scale, one.model_points_m, model.det_score_thresh,
-                      rng=np.random.RandomState(5), generator=g, device=model.device)
+    frame = pem_frame(model.pem, one.bank, recs, rgb, depth, K, scale, one.model_points_m[None], np.zeros(len(recs), np.int64),
+                      model.det_score_thresh, rng=np.random.RandomState(5), generator=g, device=model.device)
     assert torch.equal(res.R, frame.out["pred_R"]) and torch.equal(res.t, frame.out["pred_t"])
 
 

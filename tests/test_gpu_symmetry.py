@@ -209,15 +209,16 @@ def test_end_to_end_with_symmetries(golden_dir):
         model.pem.set_hypotheses(4)
         base = model.onboard_objects(meshes, obj_ids=[3, 7], template_size=192, rng=np.random.RandomState(0))
         none = model.onboard_objects(meshes, obj_ids=[3, 7], template_size=192, rng=np.random.RandomState(0), symmetries=None)
-        assert base.symmetries is None and none.symmetries is None
+        assert base.pose_inputs.symmetries is None and none.pose_inputs.symmetries is None
         res0 = model.detect_objects(*frame, base, rng=np.random.RandomState(5))
         res1 = model.detect_objects(*frame, none, rng=np.random.RandomState(5))
         assert res0.pem and strip(res0.pem) == strip(res1.pem)
         auto = model.onboard_objects(meshes, obj_ids=[3, 7], template_size=192, rng=np.random.RandomState(0), symmetries="auto")
-        assert auto.symmetries is not None and tuple(auto.symmetries.range.shape) == (2, 2)
+        syms = auto.pose_inputs.symmetries
+        assert syms is not None and tuple(syms.range.shape) == (2, 2)
         res = model.detect_objects(*frame, auto, rng=np.random.RandomState(5))
         assert len(res.pem) == len(res0.pem) and all(0 <= r["hypothesis"] < 4 for r in res.pem)
-        print(f"auto symmetries: ranges {auto.symmetries.range.tolist()}, hypotheses {[r['hypothesis'] for r in res.pem]}")
+        print(f"auto symmetries: ranges {syms.range.tolist()}, hypotheses {[r['hypothesis'] for r in res.pem]}")
     finally:
         model.pem.set_hypotheses(1)
 

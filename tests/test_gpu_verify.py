@@ -232,7 +232,7 @@ def _expected(ops, res, objs, frame_in):
     fi = inputs.FrameInputs(res.pem, rgb, depth, cam_K, scale, 1.0)
     P = len(res.pem)
     tau = 0.1 * np.asarray(objs.radii, np.float64)[res.frame.obj]
-    return ops.verify_poses(res.R.contiguous(), res.t.contiguous(), res.frame.obj, objs.verify_meshes, fi.depth, fi.mask, np.arange(P),
+    return ops.verify_poses(res.R.contiguous(), res.t.contiguous(), res.frame.obj, objs.pose_inputs.meshes, fi.depth, fi.mask, np.arange(P),
                             cam_K, tau)
 
 
@@ -243,7 +243,7 @@ def test_pipeline_frame_with_verification(ops, golden_dir):
         objs_plain = model.onboard_objects(meshes, obj_ids=[3, 7], template_size=192, rng=np.random.RandomState(0))
         model.verify, model.icp_iters = True, 10
         objs = model.onboard_objects(meshes, obj_ids=[3, 7], template_size=192, rng=np.random.RandomState(0))
-        assert objs_plain.verify_meshes is None and len(objs.verify_meshes) == 2
+        assert objs_plain.pose_inputs.meshes is None and len(objs.pose_inputs.meshes) == 2
         assert torch.equal(objs.bank[1], objs_plain.bank[1]) and np.array_equal(objs.model_points_m, objs_plain.model_points_m)
         for icp_iters in (0, 10):
             model.icp_iters = icp_iters

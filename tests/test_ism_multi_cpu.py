@@ -79,11 +79,11 @@ def test_oracle_nms_per_object(gold, tag):
 
 # ---- host side of onboard_objects / detect_objects ----------------------------------------------------------------------------
 def _fake_sam6d(T=4, C=8, Nm=16):
-    """a SAM6D without models whose onboard() draws from rng in onboard's order (cloud, PEM samples, model points) and builds
-    arrays from the draws"""
+    """a SAM6D without models, ICP or verification whose onboarding of one mesh draws from rng in onboard's order (cloud, PEM
+    samples, model points) and builds arrays from the draws"""
     from sam6d_b200.pipeline import SAM6D, Onboarded
 
-    def onboard(mesh, template_size=512, rng=None):
+    def onboard(mesh, template_size=512, rng=None, refs=None):
         rng = rng if rng is not None else np.random
         cloud = rng.rand(2048, 3)
         tem = rng.rand(3)
@@ -93,7 +93,8 @@ def _fake_sam6d(T=4, C=8, Nm=16):
                                                                                              torch.full((1, 2048, 256), tem[2])),
                          model_points_m=mp)
     m = SAM6D.__new__(SAM6D)
-    m.onboard = onboard
+    m._onboard_mesh = onboard
+    m.icp_iters, m.verify, m.device = 0, False, torch.device("cpu")
     return m
 
 
@@ -105,10 +106,10 @@ def test_onboard_objects_stacks_in_draw_order():
     assert objs.poses_m.shape == (3, 4, 4, 4) and objs.cloud_m.shape == (3, 2048, 3)
     assert objs.bank[0].shape == (3, 2048, 3) and objs.bank[1].shape == (3, 2048, 256)
     assert objs.model_points_m.shape == (3, 16, 3) and objs.model_points_m.dtype == np.float32 and objs.radii.shape == (3,)
-    # object after object from one generator: the same draws as three onboard() calls in a row
+    # object after object from one generator: the same draws as onboarding the three meshes in a row
     rng = np.random.RandomState(7)
     for o, mesh in enumerate([1.0, 2.0, 3.0]):
-        one = m.onboard(mesh, rng=rng)
+        one = m._onboard_mesh(mesh, rng=rng)
         assert torch.equal(objs.ref_cls[o], one.ref_cls) and torch.equal(objs.ref_patch[o], one.ref_patch)
         assert np.array_equal(objs.cloud_m[o], one.cloud_m) and np.array_equal(objs.poses_m[o], one.poses_m)
         assert torch.equal(objs.bank[0][o], one.bank[0][0]) and torch.equal(objs.bank[1][o], one.bank[1][0])

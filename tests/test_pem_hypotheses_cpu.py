@@ -142,7 +142,8 @@ def test_cli_options():
         a = parser.parse_args(base + ["--pem_hypotheses", "4", "--hyp_min_angle", "45", "--hyp_min_dist", "0.1"])
         assert (a.pem_hypotheses, a.hyp_min_angle, a.hyp_min_dist) == (4, 45.0, 0.1)
     for main, base in ((pem_cli.main, []), (run_sam6d.main, req), (run_bop.main, bop), (track_sam6d.main, trk)):
-        for bad in (["--pem_hypotheses", "0"], ["--pem_hypotheses", "17"], ["--hyp_min_angle", "0"], ["--hyp_min_dist", "-1"]):
+        for bad in (["--pem_hypotheses", "0"], ["--pem_hypotheses", "17"], ["--hyp_min_angle", "0"], ["--hyp_min_dist", "-1"],
+                    ["--verify_tau", "0"], ["--verify_tau", "inf"], ["--icp_iters", "-1"]):
             with pytest.raises(SystemExit):
                 main(base + bad)
 

@@ -136,9 +136,12 @@ def test_defaults_leave_verification_off():
     from sam6d_b200.cli import pem_run_inference_custom as pem_cli, run_bop, run_sam6d, track_sam6d
     p = inspect.signature(pipeline.SAM6D.__init__).parameters
     assert p["verify"].default is False and p["verify_tau"].default == 0.1
-    assert inspect.signature(pipeline.pem_frame).parameters["verify"].default is None
-    assert pipeline.Onboarded.__dataclass_fields__["verify_mesh"].default is None
-    assert pipeline.ObjectSet.__dataclass_fields__["verify_meshes"].default is None
+    # verification, ICP and symmetries are off and hold nothing unless asked for
+    assert all(x is None for x in pipeline.PoseInputs()) and pipeline.PoseInputs._fields == ("icp", "meshes", "radii", "symmetries")
+    assert inspect.signature(pipeline.pem_frame).parameters["pose"].default == pipeline.PoseInputs()
+    assert pipeline.Onboarded.__dataclass_fields__["pose_inputs"].default == pipeline.PoseInputs()
+    assert pipeline.ObjectSet.__dataclass_fields__["pose_inputs"].default == pipeline.PoseInputs()
+    assert pipeline.build_pose_inputs([None], np.ones((1, 4, 3)), "cpu") == pipeline.PoseInputs()
     req = ["--cad_path", "o.ply", "--rgb_path", "r.png", "--depth_path", "d.png", "--cam_path", "c.json", "--output_dir", "out"]
     bop = ["--bop_root", "b", "--dataset_name", "ycbv", "--output_dir", "out"]
     trk = ["--cad_path", "o.ply", "--rgb_dir", "r", "--depth_dir", "d", "--cam_path", "c.json", "--output_dir", "out"]
