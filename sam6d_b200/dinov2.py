@@ -26,29 +26,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib, ops
-from .pem import _W, _f32, _Packed, _param_key
-
-_ACT_GELU = 2
-
-
-class _PatchEmbed(nn.Module):
-    def __init__(self, patch, in_chans, dim):
-        super().__init__()
-        self.proj = nn.Conv2d(in_chans, dim, kernel_size=patch, stride=patch)
-
-
-class _Attention(nn.Module):
-    def __init__(self, dim):
-        super().__init__()
-        self.qkv = nn.Linear(dim, dim * 3, bias=True)
-        self.proj = nn.Linear(dim, dim, bias=True)
-
-
-class _Mlp(nn.Module):
-    def __init__(self, dim, hidden):
-        super().__init__()
-        self.fc1 = nn.Linear(dim, hidden)
-        self.fc2 = nn.Linear(hidden, dim)
+from .layers import _W, _f32, _Packed, _PatchEmbed, _Attention, _Mlp, block, pack_block, patch_embed, patch_rows
 
 
 class _SwiGLUFFNFused(nn.Module):
@@ -108,33 +86,31 @@ class DinoVisionTransformer(nn.Module):
 
     # ---- weights in kernel form ------------------------------------------------------------------------------------
     def _weights(self):
-        key = _param_key(self)
-        if self._packed.key != key:
-            C, P = self.embed_dim, self.patch_size
-            K = 3 * P * P
-            Kp = (K + 7) // 8 * 8                                 # 588 -> 592: the GEMM wants K % 8 == 0 (zero columns)
-            pw = torch.zeros(C, Kp, dtype=torch.float32, device=self.cls_token.device)
-            pw[:, :K] = _f32(self.patch_embed.proj.weight).reshape(C, K)
-            w = dict(pe_w=_W(pw), pe_b=_f32(self.patch_embed.proj.bias), K=K, Kp=Kp, nw=_f32(self.norm.weight), nb=_f32(self.norm.bias),
-                     blocks=[])
-            for blk in self.blocks:
-                g1, g2 = _f32(blk.ls1.gamma).double(), _f32(blk.ls2.gamma).double()
-                # x + gamma * (W y + b) = x + (diag(gamma) W) y + gamma * b : LayerScale folded into the projection
-                # Mlp: f1 / f2 = fc1 / fc2.  SwiGLU: f1 = w12 with its gate and up rows interleaved for gemm_tma(act=3), f2 = w3
-                if self.ffn_layer == "swiglufused":
-                    f1, f1b = _W(ops.pack_swiglu_rows(_f32(blk.mlp.w12.weight))), ops.pack_swiglu_rows(_f32(blk.mlp.w12.bias))
-                    f2w, f2b = blk.mlp.w3.weight, blk.mlp.w3.bias
-                else:
-                    f1, f1b = _W(blk.mlp.fc1.weight), _f32(blk.mlp.fc1.bias)
-                    f2w, f2b = blk.mlp.fc2.weight, blk.mlp.fc2.bias
-                w["blocks"].append(dict(
-                    n1w=_f32(blk.norm1.weight), n1b=_f32(blk.norm1.bias), qkv=_W(blk.attn.qkv.weight), qkv_b=_f32(blk.attn.qkv.bias),
-                    proj=_W((_f32(blk.attn.proj.weight).double() * g1[:, None]).float()), proj_b=(_f32(blk.attn.proj.bias).double() * g1).float().contiguous(),
-                    n2w=_f32(blk.norm2.weight), n2b=_f32(blk.norm2.bias), f1=f1, f1b=f1b,
-                    f2=_W((_f32(f2w).double() * g2[:, None]).float()), f2b=(_f32(f2b).double() * g2).float().contiguous()))
-            self._packed.w, self._packed.key = w, key
-            self._pos_cache = {}
-        return self._packed.w
+        return self._packed.get(self._pack, self)
+
+    def _pack(self):
+        C, P = self.embed_dim, self.patch_size
+        K = 3 * P * P
+        Kp = (K + 7) // 8 * 8                                 # 588 -> 592: the GEMM wants K % 8 == 0 (zero columns)
+        pw = torch.zeros(C, Kp, dtype=torch.float32, device=self.cls_token.device)
+        pw[:, :K] = _f32(self.patch_embed.proj.weight).reshape(C, K)
+        w = dict(pe_w=_W(pw), pe_b=_f32(self.patch_embed.proj.bias), Kp=Kp, nw=_f32(self.norm.weight), nb=_f32(self.norm.bias),
+                 blocks=[])
+        for blk in self.blocks:
+            g1, g2 = _f32(blk.ls1.gamma).double(), _f32(blk.ls2.gamma).double()
+            # x + gamma * (W y + b) = x + (diag(gamma) W) y + gamma * b : LayerScale folded into the projection
+            # Mlp: l1 / l2 = fc1 / fc2.  SwiGLU: l1 = w12 with its gate and up rows interleaved for gemm_tma(act=3), l2 = w3
+            if self.ffn_layer == "swiglufused":
+                f1w, f1b = ops.pack_swiglu_rows(_f32(blk.mlp.w12.weight)), ops.pack_swiglu_rows(_f32(blk.mlp.w12.bias))
+                f2w, f2b = blk.mlp.w3.weight, blk.mlp.w3.bias
+            else:
+                f1w, f1b = blk.mlp.fc1.weight, blk.mlp.fc1.bias
+                f2w, f2b = blk.mlp.fc2.weight, blk.mlp.fc2.bias
+            w["blocks"].append(pack_block(
+                blk.norm1, blk.attn.qkv.weight, blk.attn.qkv.bias,
+                (_f32(blk.attn.proj.weight).double() * g1[:, None]).float(), (_f32(blk.attn.proj.bias).double() * g1).float(),
+                blk.norm2, f1w, f1b, (_f32(f2w).double() * g2[:, None]).float(), (_f32(f2b).double() * g2).float()))
+        return w
 
     def _pos(self, npatch, w, h):
         """interpolate_pos_encoding (vision_transformer.py:179-207) -> (cls row (C,), patch rows (npatch, C)) with cls_token added"""
@@ -178,22 +154,17 @@ class DinoVisionTransformer(nn.Module):
         if Himg % P or Wimg % P or L > 256:
             raise RuntimeError("input must be a multiple of the patch size with at most 256 patches")
         cls, pos = self._pos(L, Himg, Wimg)
-        K, Kp = w["K"], w["Kp"]
-        patches = torch.zeros(B * L, Kp, dtype=torch.float32, device=x.device)
-        patches[:, :K] = x.float().reshape(B, Cin, Gh, P, Gw, P).permute(0, 2, 4, 1, 3, 5).reshape(B * L, K)
+        rows = patch_rows(x, P, w["Kp"])
         tok = torch.empty(B, S, C, dtype=torch.float32, device=x.device)
         tok[:, 0, :] = cls
-        ops.gemm_tc(patches.view(B, L, Kp), w["pe_w"].bf16, w["pe_b"], residual=pos.expand(B, L, C), out=tok[:, 1:, :])
+        patch_embed("bf16", rows, w["pe_w"], w["pe_b"], pos, tok[:, 1:, :])
         tok = tok.view(B * S, C)
-        act = ops.ACT_SWIGLU if self.ffn_layer == "swiglufused" else _ACT_GELU
+        act = ops.ACT_SWIGLU if self.ffn_layer == "swiglufused" else ops.ACT_GELU
         for bw in w["blocks"]:
-            xn = ops.layernorm_bf16(tok, bw["n1w"], bw["n1b"], eps=1e-6)
-            qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, S, slot=4)
-            att = self._attention(qk, vt, B, S, C)
-            tok = ops.gemm_tma(att, bw["proj"].bf16, bw["proj_b"], residual=tok)
-            xn = ops.layernorm_bf16(tok, bw["n2w"], bw["n2b"], eps=1e-6)
-            hid = ops.gemm_tma(xn, bw["f1"].bf16, bw["f1b"], act=act, out_dtype=torch.bfloat16)
-            tok = ops.gemm_tma(hid, bw["f2"].bf16, bw["f2b"], residual=tok)
+            def attend(xn):
+                qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, S, slot=4)
+                return self._attention(qk, vt, B, S, C)
+            tok = block("bf16", bw, tok, attend, act)
         xn = ops.layernorm(tok, w["nw"], w["nb"], eps=1e-6).view(B, S, C)
         return {"x_norm_clstoken": xn[:, 0], "x_norm_regtokens": xn[:, 1:1], "x_norm_patchtokens": xn[:, 1:], "x_prenorm": tok.view(B, S, C),
                 "masks": masks}

@@ -31,7 +31,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
-from .pem import _Packed, _param_key
+from .layers import _Packed
 
 bf = torch.bfloat16
 REG_MAX, NM, NC = 16, 32, 1
@@ -169,9 +169,9 @@ class YOLOv8Seg(nn.Module):
 
     # ---- packing ------------------------------------------------------------------------------------------------------
     def _weights(self):
-        key = _param_key(self)
-        if self._packed.key == key:
-            return self._packed.w
+        return self._packed.get(self._pack, self)
+
+    def _pack(self):
         m = self.model
         w = {}
         sw, sb = fold_conv_bn(m[0].conv, m[0].bn)
@@ -204,7 +204,6 @@ class YOLOv8Seg(nn.Module):
         up = p.upsample.weight.detach().float()                                     # (in, out, 2, 2)
         w["up"] = [[_CW(up[:, :, i, j].t().reshape(up.shape[1], up.shape[0], 1, 1), p.upsample.bias.detach().float()) for j in range(2)]
                    for i in range(2)]
-        self._packed.w, self._packed.key = w, key
         return w
 
     # ---- launches -----------------------------------------------------------------------------------------------------

@@ -184,6 +184,7 @@ def gemm_tma(A: Tensor, W: Tensor, bias: Optional[Tensor] = None, residual: Opti
     return out
 
 
+ACT_GELU = 2
 ACT_SWIGLU = 3
 
 

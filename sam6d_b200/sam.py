@@ -23,9 +23,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .pem import _W, _f32, _Packed, _param_key, _gemm, PRECISIONS
+from .layers import _W, _f32, _gemm, _Packed, PRECISIONS, block, pack_block, patch_embed, patch_rows
 
-_ACT_GELU = 2
 HEAD_DIMS = (64, 80)            # the head dims sam6d_attn_relpos / sam6d_attn_global_tc_ex / sam6d_attn_tc are built for
 
 # build_sam.py:14-46: embed_dim, depth, num_heads, global_attn_indexes per backbone (the keyword arguments of
@@ -125,28 +124,26 @@ class ImageEncoderViT(nn.Module):
 
     # ------------------------------------------------------------------------------------------------------------ weights
     def _weights(self):
-        key = _param_key(self)
-        if self._packed.key != key:
-            w = dict(pe_w=_W(self.patch_embed.proj.weight.reshape(self.embed_dim, -1)), pe_b=_f32(self.patch_embed.proj.bias),
-                     pos=_f32(self.pos_embed).reshape(-1, self.embed_dim) if self.pos_embed is not None else None, blocks=[])
-            for blk in self.blocks:
-                w["blocks"].append(dict(
-                    n1w=_f32(blk.norm1.weight), n1b=_f32(blk.norm1.bias), eps1=blk.norm1.eps,
-                    qkv=_W(blk.attn.qkv.weight), qkv_b=_f32(blk.attn.qkv.bias), proj=_W(blk.attn.proj.weight),
-                    proj_b=_f32(blk.attn.proj.bias), rh=_f32(blk.attn.rel_pos_h), rw=_f32(blk.attn.rel_pos_w),
-                    rel_blob=(ops.pack_rel_pos(_f32(blk.attn.rel_pos_h), _f32(blk.attn.rel_pos_w),
-                                               slab_rows=32 if blk.attn.rel_pos_h.shape[0] <= 32 else 128)
-                              if blk.attn.rel_pos_h.shape[0] <= 128 and blk.attn.rel_pos_h.is_cuda else None),
-                    n2w=_f32(blk.norm2.weight), n2b=_f32(blk.norm2.bias), eps2=blk.norm2.eps,
-                    l1=_W(blk.mlp.lin1.weight), l1b=_f32(blk.mlp.lin1.bias), l2=_W(blk.mlp.lin2.weight), l2b=_f32(blk.mlp.lin2.bias)))
-            oc = self.neck[0].out_channels
-            w["neck0"] = _W(self.neck[0].weight.reshape(oc, -1))
-            w["ln1"] = (_f32(self.neck[1].weight), _f32(self.neck[1].bias), self.neck[1].eps)
-            # 3x3 conv as 9 shifted 1x1 GEMMs: tap (kh,kw) -> weight[:, :, kh, kw]
-            w["neck2"] = [_W(self.neck[2].weight[:, :, kh, kw]) for kh in range(3) for kw in range(3)]
-            w["ln2"] = (_f32(self.neck[3].weight), _f32(self.neck[3].bias), self.neck[3].eps)
-            self._packed.w, self._packed.key = w, key
-        return self._packed.w
+        return self._packed.get(self._pack, self)
+
+    def _pack(self):
+        w = dict(pe_w=_W(self.patch_embed.proj.weight.reshape(self.embed_dim, -1)), pe_b=_f32(self.patch_embed.proj.bias),
+                 pos=_f32(self.pos_embed).reshape(-1, self.embed_dim) if self.pos_embed is not None else None, blocks=[])
+        for blk in self.blocks:
+            a = blk.attn
+            bw = pack_block(blk.norm1, a.qkv.weight, a.qkv.bias, a.proj.weight, a.proj.bias,
+                            blk.norm2, blk.mlp.lin1.weight, blk.mlp.lin1.bias, blk.mlp.lin2.weight, blk.mlp.lin2.bias)
+            bw.update(rh=_f32(a.rel_pos_h), rw=_f32(a.rel_pos_w),
+                      rel_blob=(ops.pack_rel_pos(_f32(a.rel_pos_h), _f32(a.rel_pos_w), slab_rows=32 if a.rel_pos_h.shape[0] <= 32 else 128)
+                                if a.rel_pos_h.shape[0] <= 128 and a.rel_pos_h.is_cuda else None))
+            w["blocks"].append(bw)
+        oc = self.neck[0].out_channels
+        w["neck0"] = _W(self.neck[0].weight.reshape(oc, -1))
+        w["ln1"] = (_f32(self.neck[1].weight), _f32(self.neck[1].bias), self.neck[1].eps)
+        # 3x3 conv as 9 shifted 1x1 GEMMs: tap (kh,kw) -> weight[:, :, kh, kw]
+        w["neck2"] = [_W(self.neck[2].weight[:, :, kh, kw]) for kh in range(3) for kw in range(3)]
+        w["ln2"] = (_f32(self.neck[3].weight), _f32(self.neck[3].bias), self.neck[3].eps)
+        return w
 
     # ------------------------------------------------------------------------------------------------------------ index maps
     def _index_maps(self, B: int, G: int, ws: int, device):
@@ -172,6 +169,37 @@ class ImageEncoderViT(nn.Module):
         return self._maps[key]
 
     # ------------------------------------------------------------------------------------------------------------ forward
+    def _attend(self, blk, bw, xn, B, G, maps):
+        """window partition (pad 64 -> 70 after norm1), relative-position attention, unpartition (drops the padded tokens;
+        proj is token-wise, so it runs after it).  bf16: the tensor cores read bf16 operands and attention writes bf16."""
+        C, nH = self.embed_dim, self.num_heads
+        bf16 = self.precision == "bf16"
+        gather = ops.gather_rows_bf16 if bf16 else ops.gather_rows
+        if blk.window_size > 0:
+            xn = gather(xn.view(B, G * G, C), maps["part"]).view(-1, C)                        # zero rows at the padding
+            nW, Hs = B * maps["nwin"] * maps["nwin"], blk.window_size
+        else:
+            nW, Hs = B, G
+        if not bf16:
+            qkv = ops.gemm(xn, bw["qkv"].f32, bw["qkv_b"])
+            att = ops.attn_relpos(qkv, nW, Hs, Hs, nH, bw["rh"], bw["rw"], blk.attn.scale)
+        elif Hs * Hs <= 256:
+            # windowed blocks: tensor-core attention (QK^T and PV on wgmma, decomposed rel-pos bias in the softmax warps)
+            qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs)                   # [q|k] rows and V^T per window
+            att = ops.attn_tc(qk, 0, qk, C, vt, nW, nH, Hs * Hs, Hs * Hs, C // nH, blk.attn.scale,
+                              rel=(bw["rel_blob"], Hs, Hs), out_dtype=torch.bfloat16)
+        elif Hs == 64 and bw["rel_blob"] is not None:
+            # global blocks of the 64 x 64 grid (4096 keys): wgmma attention with an online softmax, scores never leave registers
+            qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs, slot=2)
+            att = ops.attn_global_tc(qk, vt, bw["rel_blob"], nW, nH, Hs, blk.attn.scale, D=C // nH)
+        else:
+            # other grids: flash-style CUDA-core kernel with online softmax
+            qkv = ops.gemm_tma(xn, bw["qkv"].bf16, bw["qkv_b"])
+            att = ops.attn_relpos(qkv, nW, Hs, Hs, nH, bw["rh"], bw["rw"], blk.attn.scale, out_dtype=torch.bfloat16)
+        if blk.window_size > 0:
+            att = gather(att.view(B, -1, C), maps["unpart"]).view(-1, C)
+        return att
+
     @torch.no_grad()
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
@@ -183,35 +211,16 @@ class ImageEncoderViT(nn.Module):
         G = Himg // P
         L = G * G
         # PatchEmbed (image_encoder.py:364-395): non-overlapping conv == GEMM over (c, kh, kw)-flattened patches; + pos_embed
-        patches = x.float().reshape(B, Cin, G, P, G, P).permute(0, 2, 4, 1, 3, 5).reshape(B * L, Cin * P * P).contiguous()
-        tok = torch.empty(B * L, C, dtype=torch.float32, device=x.device)
+        rows = patch_rows(x, P)
         if w["pos"] is not None:
-            Wm = w["pe_w"]
-            gemm, pe_w = (ops.gemm_tc, Wm.bf16) if prec == "bf16" else (ops.gemm, Wm.f32)
-            gemm(patches.view(B, L, -1), pe_w, w["pe_b"], residual=w["pos"].expand(B, L, C), out=tok.view(B, L, C))
+            tok = torch.empty(B * L, C, dtype=torch.float32, device=x.device)
+            patch_embed(prec, rows, w["pe_w"], w["pe_b"], w["pos"], tok.view(B, L, C))
         else:
-            tok = _gemm(prec, patches, w["pe_w"], w["pe_b"])
+            tok = _gemm(prec, rows, w["pe_w"], w["pe_b"])
         ws = max((b.window_size for b in self.blocks), default=0) or 14
         maps = self._index_maps(B, G, ws, x.device)
         for blk, bw in zip(self.blocks, w["blocks"]):
-            if prec == "bf16":
-                tok = self._block_bf16(blk, bw, tok, B, L, C, G, maps)
-                continue
-            xn = ops.layernorm(tok, bw["n1w"], bw["n1b"], eps=bw["eps1"])
-            if blk.window_size > 0:
-                xw = ops.gather_rows(xn.view(B, L, C), maps["part"]).view(-1, C)            # zero rows at the padding
-                nW, Hs = B * maps["nwin"] * maps["nwin"], blk.window_size
-            else:
-                xw, nW, Hs = xn, B, G
-            qkv = _gemm(prec, xw, bw["qkv"], bw["qkv_b"])
-            att = ops.attn_relpos(qkv, nW, Hs, Hs, self.num_heads, bw["rh"], bw["rw"], blk.attn.scale)
-            if blk.window_size > 0:
-                # proj is token-wise, so un-partition first (drops the padded tokens) and fuse the residual into proj
-                att = ops.gather_rows(att.view(B, -1, C), maps["unpart"]).view(-1, C)
-            tok = _gemm(prec, att, bw["proj"], bw["proj_b"], residual=tok)
-            xn = ops.layernorm(tok, bw["n2w"], bw["n2b"], eps=bw["eps2"])
-            h = _gemm(prec, xn, bw["l1"], bw["l1b"], relu=_ACT_GELU)
-            tok = _gemm(prec, h, bw["l2"], bw["l2b"], residual=tok)
+            tok = block(prec, bw, tok, lambda xn: self._attend(blk, bw, xn, B, G, maps))
         # neck (image_encoder.py:88-104)
         y = _gemm(prec, tok, w["neck0"])
         y = ops.layernorm(y, w["ln1"][0], w["ln1"][1], eps=w["ln1"][2])
@@ -223,39 +232,6 @@ class ImageEncoderViT(nn.Module):
             acc = _gemm(prec, shifted, Wt, None, residual=acc)
         out = ops.layernorm(acc, w["ln2"][0], w["ln2"][1], eps=w["ln2"][2])
         return out.view(B, G, G, oc).permute(0, 3, 1, 2).contiguous()
-
-
-def _block_bf16(self, blk, bw, tok, B, L, C, G, maps):
-    """one Block with bf16 operands everywhere the tensor cores read them (the residual stream `tok` stays fp32):
-    LayerNorm -> bf16 rows -> TMA GEMM; attention writes bf16; the GELU hidden activations live in bf16."""
-    xn = ops.layernorm_bf16(tok, bw["n1w"], bw["n1b"], eps=bw["eps1"])
-    if blk.window_size > 0:
-        xw = ops.gather_rows_bf16(xn.view(B, L, C), maps["part"]).view(-1, C)
-        nW, Hs = B * maps["nwin"] * maps["nwin"], blk.window_size
-    else:
-        xw, nW, Hs = xn, B, G
-    if Hs * Hs <= 256:
-        # windowed blocks: tensor-core attention (QK^T and PV on wgmma, decomposed rel-pos bias in the softmax warps)
-        qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs)                   # [q|k] rows and V^T per window
-        att = ops.attn_tc(qk, 0, qk, C, vt, nW, self.num_heads, Hs * Hs, Hs * Hs, C // self.num_heads, blk.attn.scale,
-                          rel=(bw["rel_blob"], Hs, Hs), out_dtype=torch.bfloat16)
-    elif Hs == 64 and bw["rel_blob"] is not None:
-        # global blocks of the 64 x 64 grid (4096 keys): wgmma attention with an online softmax, scores never leave registers
-        qk, vt = ops.gemm_tma_vt(xw, bw["qkv"].bf16, bw["qkv_b"], 2 * C, Hs * Hs, slot=2)
-        att = ops.attn_global_tc(qk, vt, bw["rel_blob"], nW, self.num_heads, Hs, blk.attn.scale, D=C // self.num_heads)
-    else:
-        # other grids: flash-style CUDA-core kernel with online softmax
-        qkv = ops.gemm_tma(xw, bw["qkv"].bf16, bw["qkv_b"])
-        att = ops.attn_relpos(qkv, nW, Hs, Hs, self.num_heads, bw["rh"], bw["rw"], blk.attn.scale, out_dtype=torch.bfloat16)
-    if blk.window_size > 0:
-        att = ops.gather_rows_bf16(att.view(B, -1, C), maps["unpart"]).view(-1, C)
-    tok = ops.gemm_tma(att, bw["proj"].bf16, bw["proj_b"], residual=tok)
-    xn = ops.layernorm_bf16(tok, bw["n2w"], bw["n2b"], eps=bw["eps2"])
-    h = ops.gemm_tma(xn, bw["l1"].bf16, bw["l1b"], act=_ACT_GELU, out_dtype=torch.bfloat16)
-    return ops.gemm_tma(h, bw["l2"].bf16, bw["l2b"], residual=tok)
-
-
-ImageEncoderViT._block_bf16 = _block_bf16
 
 
 def build_image_encoder(name: str = "vit_h", precision: str = "bf16") -> ImageEncoderViT:

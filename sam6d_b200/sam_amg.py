@@ -29,15 +29,10 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .pem import _W, _f32, _Packed, _param_key
+from .layers import _W, _f32, _Packed
+from .sam import LayerNorm2d
 
 bf = torch.bfloat16
-
-
-class LayerNorm2d(nn.Module):
-    def __init__(self, c, eps=1e-6):
-        super().__init__()
-        self.weight, self.bias, self.eps = nn.Parameter(torch.ones(c)), nn.Parameter(torch.zeros(c)), eps
 
 
 class _PositionEmbeddingRandom(nn.Module):
@@ -93,12 +88,8 @@ class PromptEncoder(nn.Module):
     def _mask_params(self) -> torch.Tensor:
         """mask_downscaling's parameters in the order sam6d_sam_mask_embed reads them (include/sam6d_b200.h)"""
         md = self.mask_downscaling
-        key = _param_key(md)
-        if self._packed.key != key:
-            self._packed.w = torch.cat([_f32(t).reshape(-1) for t in (md[0].weight, md[0].bias, md[1].weight, md[1].bias, md[3].weight, md[3].bias,
-                                                                      md[4].weight, md[4].bias, md[6].weight, md[6].bias)]).contiguous()
-            self._packed.key = key
-        return self._packed.w
+        params = (md[0].weight, md[0].bias, md[1].weight, md[1].bias, md[3].weight, md[3].bias, md[4].weight, md[4].bias, md[6].weight, md[6].bias)
+        return self._packed.get(lambda: torch.cat([_f32(t).reshape(-1) for t in params]).contiguous(), md)
 
     def _pe(self, coords: torch.Tensor) -> torch.Tensor:
         """PositionEmbeddingRandom.forward_with_coords: (B,N,2) pixel coordinates, already shifted by 0.5 -> (B,N,256)"""
@@ -233,24 +224,23 @@ class MaskDecoder(nn.Module):
 
     # ---- weights in kernel form -----------------------------------------------------------------------------------------------
     def _weights(self):
-        key = _param_key(self)
-        if self._packed.key != key:
-            t = self.transformer
-            w = {}
-            for name, a in (("t2i0", t.layers[0].cross_attn_token_to_image), ("i2t0", t.layers[0].cross_attn_image_to_token),
-                            ("t2i1", t.layers[1].cross_attn_token_to_image), ("i2t1", t.layers[1].cross_attn_image_to_token),
-                            ("fin", t.final_attn_token_to_image)):
-                w[name] = dict(q=_W(a.q_proj.weight), qb=_f32(a.q_proj.bias), k=_W(a.k_proj.weight), kb=_f32(a.k_proj.bias),
-                               v=_W(a.v_proj.weight), vb=_f32(a.v_proj.bias), o=_W(a.out_proj.weight), ob=_f32(a.out_proj.bias))
-            up = self.output_upscaling
-            w["ct1"] = _W(_f32(up[0].weight).permute(2, 3, 1, 0).reshape(4 * up[0].out_channels, up[0].in_channels))     # rows (i, j, o)
-            w["ct1b"] = _f32(up[0].bias).repeat(4).contiguous()
-            w["ln2w"], w["ln2b"] = _f32(up[1].weight), _f32(up[1].bias)
-            w["ct2"] = _W(_f32(up[3].weight).permute(2, 3, 1, 0).reshape(4 * up[3].out_channels, up[3].in_channels))
-            w["ct2b"] = _f32(up[3].bias).repeat(4).contiguous()
-            self._packed.w, self._packed.key = w, key
-            self._frame = {}
-        return self._packed.w
+        return self._packed.get(self._pack, self)
+
+    def _pack(self):
+        t = self.transformer
+        w = {}
+        for name, a in (("t2i0", t.layers[0].cross_attn_token_to_image), ("i2t0", t.layers[0].cross_attn_image_to_token),
+                        ("t2i1", t.layers[1].cross_attn_token_to_image), ("i2t1", t.layers[1].cross_attn_image_to_token),
+                        ("fin", t.final_attn_token_to_image)):
+            w[name] = dict(q=_W(a.q_proj.weight), qb=_f32(a.q_proj.bias), k=_W(a.k_proj.weight), kb=_f32(a.k_proj.bias),
+                           v=_W(a.v_proj.weight), vb=_f32(a.v_proj.bias), o=_W(a.out_proj.weight), ob=_f32(a.out_proj.bias))
+        up = self.output_upscaling
+        w["ct1"] = _W(_f32(up[0].weight).permute(2, 3, 1, 0).reshape(4 * up[0].out_channels, up[0].in_channels))     # rows (i, j, o)
+        w["ct1b"] = _f32(up[0].bias).repeat(4).contiguous()
+        w["ln2w"], w["ln2b"] = _f32(up[1].weight), _f32(up[1].bias)
+        w["ct2"] = _W(_f32(up[3].weight).permute(2, 3, 1, 0).reshape(4 * up[3].out_channels, up[3].in_channels))
+        w["ct2b"] = _f32(up[3].bias).repeat(4).contiguous()
+        return w
 
     def _frame_terms(self, image_embeddings, pe_rows, no_mask):
         """everything that depends on the frame but not on the prompts (block 0 of the transformer sees the same image tokens for

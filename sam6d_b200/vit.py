@@ -23,29 +23,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .pem import _W, _f32, _Packed, _param_key, _cfg, sample_pts_feats, PRECISIONS
-
-_ACT_GELU = 2
-
-
-class _PatchEmbed(nn.Module):
-    def __init__(self, patch_size, in_chans, embed_dim):
-        super().__init__()
-        self.proj = nn.Conv2d(in_chans, embed_dim, kernel_size=patch_size, stride=patch_size)
-
-
-class _Attention(nn.Module):
-    def __init__(self, dim, qkv_bias):
-        super().__init__()
-        self.qkv = nn.Linear(dim, dim * 3, bias=qkv_bias)
-        self.proj = nn.Linear(dim, dim)
-
-
-class _Mlp(nn.Module):
-    def __init__(self, dim, hidden):
-        super().__init__()
-        self.fc1 = nn.Linear(dim, hidden)
-        self.fc2 = nn.Linear(hidden, dim)
+from .layers import _W, _f32, _Packed, _PatchEmbed, _Attention, _Mlp, PRECISIONS, block, pack_block, patch_embed, patch_rows
+from .pem import _cfg, sample_pts_feats
 
 
 class _Block(nn.Module):
@@ -79,44 +58,29 @@ class ViT(nn.Module):
         self._packed = _Packed()
 
     def _weights(self):
-        key = _param_key(self)
-        if self._packed.key != key:
-            C = self.embed_dim
-            w = dict(pe_w=_W(self.patch_embed.proj.weight.reshape(C, -1)), pe_b=_f32(self.patch_embed.proj.bias),
-                     cls=(_f32(self.cls_token).reshape(C) + _f32(self.pos_embed)[0, 0]).contiguous(),
-                     pos=_f32(self.pos_embed)[0, 1:].contiguous(), nw=_f32(self.norm.weight), nb=_f32(self.norm.bias),
-                     neps=self.norm.eps, blocks=[])
-            for blk in self.blocks:
-                w["blocks"].append(dict(
-                    n1w=_f32(blk.norm1.weight), n1b=_f32(blk.norm1.bias), eps1=blk.norm1.eps,
-                    qkv=_W(blk.attn.qkv.weight),
-                    qkv_b=_f32(blk.attn.qkv.bias) if blk.attn.qkv.bias is not None else torch.zeros(3 * C, device=self.cls_token.device),
-                    proj=_W(blk.attn.proj.weight), proj_b=_f32(blk.attn.proj.bias),
-                    n2w=_f32(blk.norm2.weight), n2b=_f32(blk.norm2.bias), eps2=blk.norm2.eps,
-                    f1=_W(blk.mlp.fc1.weight), f1b=_f32(blk.mlp.fc1.bias), f2=_W(blk.mlp.fc2.weight), f2b=_f32(blk.mlp.fc2.bias)))
-            self._packed.w, self._packed.key = w, key
-        return self._packed.w
+        return self._packed.get(self._pack, self)
 
-    def _block(self, bw, tok, B, S, C):
-        """x = x + proj(attn(norm1(x)));  x = x + fc2(gelu(fc1(norm2(x))))  on the fp32 residual stream tok (B*S, C)"""
+    def _pack(self):
+        C = self.embed_dim
+        return dict(pe_w=_W(self.patch_embed.proj.weight.reshape(C, -1)), pe_b=_f32(self.patch_embed.proj.bias),
+                    cls=(_f32(self.cls_token).reshape(C) + _f32(self.pos_embed)[0, 0]).contiguous(),
+                    pos=_f32(self.pos_embed)[0, 1:].contiguous(), nw=_f32(self.norm.weight), nb=_f32(self.norm.bias),
+                    neps=self.norm.eps,
+                    blocks=[pack_block(blk.norm1, blk.attn.qkv.weight, blk.attn.qkv.bias, blk.attn.proj.weight, blk.attn.proj.bias,
+                                       blk.norm2, blk.mlp.fc1.weight, blk.mlp.fc1.bias, blk.mlp.fc2.weight, blk.mlp.fc2.bias)
+                            for blk in self.blocks])
+
+    def _attend(self, bw, xn, B, S):
+        C = self.embed_dim
         H, d = self.num_heads, C // self.num_heads
         if self.precision == "bf16":
-            xn = ops.layernorm_bf16(tok, bw["n1w"], bw["n1b"], eps=bw["eps1"])
             qk, vt = ops.gemm_tma_vt(xn, bw["qkv"].bf16, bw["qkv_b"], 2 * C, S, slot=3)
-            att = ops.attn_tc(qk, 0, qk, C, vt, B, H, S, S, d, d ** -0.5, out_dtype=torch.bfloat16)
-            tok = ops.gemm_tma(att, bw["proj"].bf16, bw["proj_b"], residual=tok)
-            xn = ops.layernorm_bf16(tok, bw["n2w"], bw["n2b"], eps=bw["eps2"])
-            h = ops.gemm_tma(xn, bw["f1"].bf16, bw["f1b"], act=_ACT_GELU, out_dtype=torch.bfloat16)
-            return ops.gemm_tma(h, bw["f2"].bf16, bw["f2b"], residual=tok)
-        xn = ops.layernorm(tok, bw["n1w"], bw["n1b"], eps=bw["eps1"])
+            return ops.attn_tc(qk, 0, qk, C, vt, B, H, S, S, d, d ** -0.5, out_dtype=torch.bfloat16)
         qkv = ops.gemm(xn, bw["qkv"].f32, bw["qkv_b"])
-        att = torch.empty(B * S, C, dtype=torch.float32, device=tok.device)
+        att = torch.empty(B * S, C, dtype=torch.float32, device=xn.device)
         qkv = qkv.view(B, S, 3 * C)
         ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], None, d ** -0.5, att.view(B, S, C))
-        tok = ops.gemm(att, bw["proj"].f32, bw["proj_b"], residual=tok)
-        xn = ops.layernorm(tok, bw["n2w"], bw["n2b"], eps=bw["eps2"])
-        h = ops.gemm(xn, bw["f1"].f32, bw["f1b"], relu=_ACT_GELU)
-        return ops.gemm(h, bw["f2"].f32, bw["f2b"], residual=tok)
+        return att
 
     @torch.no_grad()
     def forward_tokens(self, x):
@@ -130,20 +94,18 @@ class ViT(nn.Module):
         L, S = G * G, G * G + 1
         if w["pos"].shape[0] != L:
             raise RuntimeError(f"pos_embed has {w['pos'].shape[0]} patch positions, the image gives {L}")
-        patches = x.float().reshape(B, Cin, G, P, G, P).permute(0, 2, 4, 1, 3, 5).reshape(B * L, Cin * P * P).contiguous()
+        rows = patch_rows(x, P)
         tok = torch.empty(B, S, C, dtype=torch.float32, device=x.device)
         tok[:, 0, :] = w["cls"]                                      # cls_token + pos_embed[0]
-        K = Cin * P * P
         # patch tokens = patches W^T + b + pos_embed[1:], written behind the cls row of every image
-        gemm, pe_w = (ops.gemm_tc, w["pe_w"].bf16) if self.precision == "bf16" else (ops.gemm, w["pe_w"].f32)
-        gemm(patches.view(B, L, K), pe_w, w["pe_b"], residual=w["pos"].expand(B, L, C), out=tok[:, 1:, :])
+        patch_embed(self.precision, rows, w["pe_w"], w["pe_b"], w["pos"], tok[:, 1:, :])
         tok = tok.view(B * S, C)
         d = self.depth
         n = d // 4
         taps = (d - 1, d - n - 1, d - 2 * n - 1, d - 3 * n - 1)
         outs = []
         for idx, bw in enumerate(w["blocks"]):
-            tok = self._block(bw, tok, B, S, C)
+            tok = block(self.precision, bw, tok, lambda xn: self._attend(bw, xn, B, S))
             if idx in taps:
                 if self.precision == "bf16":
                     outs.append(ops.layernorm_bf16(tok, w["nw"], w["nb"], eps=w["neps"]))
@@ -179,11 +141,8 @@ class ViT_AE(nn.Module):
         # (the reference downloads the MAE checkpoint when cfg.pretrained: weights come from load_state_dict here)
 
     def _weights(self):
-        key = _param_key(self.output_upscaling)
-        if self._packed.key != key:
-            self._packed.w = dict(up=_W(self.output_upscaling.weight), up_b=_f32(self.output_upscaling.bias))
-            self._packed.key = key
-        return self._packed.w
+        return self._packed.get(lambda: dict(up=_W(self.output_upscaling.weight), up_b=_f32(self.output_upscaling.bias)),
+                                self.output_upscaling)
 
     @torch.no_grad()
     def upscaled_tokens(self, x):
