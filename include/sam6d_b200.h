@@ -509,6 +509,57 @@ int sam6d_symmetry_agreement(const float* Rt, int C, const float* q, const float
  * NULL pointer. */
 int sam6d_point_diameter(const float* pts, int V, float* d2, void* stream);
 
+/* ---- object models from posed RGB-D views (not in the reference; csrc/fusion.cu, sam6d_b200/fusion.py, oracle/fusion_oracle.py) */
+/* A volume of nx x ny x nz voxels (each in [2, 512]), x fastest: voxel (i, j, k) is index (k ny + j) nx + i, its centre
+ * p = (bx + (i + 0.5) voxel, by + (j + 0.5) voxel, bz + (k + 0.5) voxel) in mm, each coordinate computed as
+ * b + ((float)i + 0.5) * voxel.  Fields: tsdf (N) f32 (start at 1), weight (N) i32 (start at 0), csum (N,3) u32 colour sums and
+ * ccount (N) i32 colour count (start at 0).  Every operation below is fp32 rounded to nearest, in the order written (no fused
+ * multiply-add), so a float32 restatement reproduces the results bit for bit. */
+/* Fuses T views into the volume.  rgb (T,H,W,3) u8, depth (T,H,W) f32 in mm (0 = missing), mask (T,H,W) u8 (non-zero = object)
+ * or NULL (every pixel is object), K (T,4) f32 = fx, fy, cx, cy, pose (T,12) f32 object -> camera (R row-major, then t in mm).
+ * One thread owns each voxel and visits the views in index order, so splitting the views over several calls gives the same
+ * bits as one call.  For view k:
+ *   q = R p + t, each row ((r0 px + r1 py) + r2 pz) + t;  q.z <= znear: skip the view;
+ *   u = (fx qx) / qz + cx, v = (fy qy) / qz + cy;  pixel c = floor(u + 0.5), r = floor(v + 0.5) (pixel c is the ray through
+ *   u = c); outside the image: skip;  d = depth at (r, c);
+ *   object pixel: d == 0: skip; sdf = d - qz; sdf < -trunc: skip; else update with obs = min(1, sdf / trunc), and when
+ *     |sdf| < trunc add the pixel's RGB to csum and 1 to ccount;
+ *   other pixel (silhouette carving): d > 0 and qz > d - trunc: skip (the voxel may be hidden behind what the pixel sees);
+ *     else update with obs = 1 (free space);
+ *   update: tsdf = (tsdf * (float)w + obs) / (float)(w + 1), then w = w + 1.
+ * -22 (nothing launched): a dimension < 2 or > 512, voxel or trunc not finite or <= 0, a bound or znear not finite, T < 1,
+ * H < 1, W < 1, a NULL pointer other than mask. */
+int sam6d_tsdf_integrate(const unsigned char* rgb, const float* depth, const unsigned char* mask, const float* K, const float* pose,
+                         int T, int H, int W, float bx, float by, float bz, float voxel, float trunc, float znear, int nx, int ny, int nz,
+                         float* tsdf, int* weight, unsigned* csum, int* ccount, void* stream);
+/* Marching tetrahedra over the volume, pass 1.  Each cube (lower corner at lattice point (i, j, k), i < nx - 1, ...; cube index
+ * (k (ny - 1) + j) (nx - 1) + i) is split into the 6 Kuhn tetrahedra: with corners numbered by bits x = 1, y = 2, z = 4, the
+ * path 0 -> e_a -> e_a + e_b -> 7 for the axis permutations (a, b, c) in lexicographic order.  Neighbouring cubes split their
+ * shared faces alike, and every tetrahedron edge is a lattice edge from a point p in one of the 7 positive directions
+ * d = 1..7 (bits as for the corners): vertex key (p, d).  A corner is inside when tsdf < 0 (0 is outside).  A tetrahedron
+ * emits triangles when its signs are mixed and all 4 corners have weight >= min_weight: one triangle with 1 or 3 corners
+ * inside, two (a quad) with 2.  emask (N) u32 (zeroed here): bit d - 1 of point p = edge (p, d) carries a vertex, i.e. it
+ * changes sign in an emitting tetrahedron; vcount (N) i32 = the set bits of emask; tcount (cubes) i32 = the cube's triangles.
+ * -22 (nothing launched): a dimension < 2 or > 512, min_weight < 1 (unobserved corners would carry surface), a NULL pointer. */
+int sam6d_tsdf_mesh_count(const float* tsdf, const int* weight, int nx, int ny, int nz, int min_weight, unsigned* emask, int* vcount,
+                          int* tcount, void* stream);
+/* Pass 2.  voff (N), toff (cubes) i32: the inclusive prefix sums of vcount and tcount.  Vertices in key order (point index,
+ * then d): for edge (p, p + d) with a = tsdf[p], b = tsdf[p + d], t = a / (a - b) and each coordinate
+ * b_axis + (((float)i + 0.5) + (t if d has the axis, else 0)) * voxel -> verts (V,3) f32 in mm.  Colour, per channel, with
+ * mean_x = (float)csum_x / (float)ccount_x: both ends observed (ccount > 0): mean_a + t (mean_b - mean_a); one: its mean;
+ * neither: 128; rounded half to even -> vcol (V,3) u8.  Faces (F,3) i32 in cube order, then tetrahedron order, then within the
+ * tetrahedron: with the tetrahedron's corners 0..3 along its path and (i, j, k, l) an even permutation of them, (x_ij, x_ik,
+ * x_il) for a lone inside corner i, (x_ij, x_il, x_ik) for a lone outside corner i, and for inside corners i, j the quad
+ * (x_ik, x_il, x_jl, x_jk) split along x_ik - x_jl into (x_ik, x_il, x_jl), (x_ik, x_jl, x_jk); each reversed (second and
+ * last vertex swapped) in the 3 tetrahedra of odd permutations.  So (b - a) x (c - a) points toward increasing tsdf (outward).
+ * The even permutations used: lone corner 0, 1, 2, 3 -> (0,1,2,3), (1,0,3,2), (2,0,1,3), (3,0,2,1); inside pair {0,1}
+ * (0,1,2,3), {0,2} (0,2,3,1), {0,3} (0,3,1,2), {1,2} (1,2,0,3), {1,3} (1,3,2,0), {2,3} (2,3,0,1).
+ * -22 (nothing launched): a dimension < 2 or > 512, min_weight < 1, voxel not finite or <= 0, a bound not finite, a NULL
+ * pointer. */
+int sam6d_tsdf_mesh_emit(const float* tsdf, const int* weight, const unsigned* csum, const int* ccount, int nx, int ny, int nz,
+                         float bx, float by, float bz, float voxel, int min_weight, const unsigned* emask, const int* voff,
+                         const int* toff, float* verts, unsigned char* vcol, int* faces, void* stream);
+
 /* ---- ISM template scoring (ISM/model/loss.py:21-44, ISM/model/detector.py:198-207,260-296) ------------------------ */
 /* Qn (P,C), Rn (O,T,C) F.normalize'd fp32, C % 4 == 0.  aggregation over the templates (matching_config.aggregation_function):
  * 0 mean, 1 median (torch.median's lower median), 2 max, 3 avg_5.  sim_out (P,O,T) optional; obj_score (P,O) f32 and obj_tmpl

@@ -71,7 +71,7 @@ _launches = 0
 _MULTI = {"sam6d_fine_assign": 6, "sam6d_coarse_select": 2, "sam6d_geo_embed_tc": 2, "sam6d_render_meshes": 4, "sam6d_yolo_masks": 2,
           "sam6d_mask_rle_count": 2, "sam6d_template_score_agg": 2, "sam6d_template_score": 2,
           "sam6d_pbr_reference_crops": 2, "sam6d_track_points": 4,
-          "sam6d_track_points_scene": 5, "sam6d_symmetry_agreement": 2}
+          "sam6d_track_points_scene": 5, "sam6d_symmetry_agreement": 2, "sam6d_tsdf_mesh_count": 2, "sam6d_tsdf_mesh_emit": 2}
 _timed = {}      # name -> list of (start_event, end_event); filled only for names registered with time_kernel()
 
 

@@ -145,3 +145,36 @@ def sample_surface(verts, faces, n, rng=None, return_normals: bool = False):
         return pts
     nrm = cross[f] / np.maximum(2.0 * area[f], np.finfo(np.float64).tiny)[:, None]
     return pts, nrm.astype(np.float32)
+
+
+def save_ply(path, mesh: Mesh) -> None:
+    """write a numpy Mesh as binary little-endian PLY: vertex x, y, z float (+ red, green, blue uchar when it has colours) and
+    face `list uchar int vertex_indices`, the layout BOP's models use.  load_ply_mesh reads it back exactly."""
+    v = np.asarray(mesh.vertices)
+    f = np.asarray(mesh.faces)
+    if v.ndim != 2 or v.shape[1] != 3 or f.ndim != 2 or f.shape[1] != 3:
+        raise ValueError(f"save_ply: vertices (V,3) and faces (F,3), got {v.shape} and {f.shape}")
+    if len(f) and (f.min() < 0 or f.max() >= len(v) or f.max() > np.iinfo(np.int32).max):
+        raise ValueError(f"save_ply: face indices outside [0, {len(v)})")
+    props = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if mesh.colors is not None:
+        c = np.asarray(mesh.colors)
+        if c.shape != v.shape or c.dtype != np.uint8:
+            raise ValueError(f"save_ply: colors (V,3) uint8, got {c.shape} {c.dtype}")
+        props += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    vrec = np.empty(len(v), dtype=np.dtype(props))
+    for k, name in enumerate("xyz"):
+        vrec[name] = v[:, k]
+    if mesh.colors is not None:
+        for k, name in enumerate(("red", "green", "blue")):
+            vrec[name] = c[:, k]
+    frec = np.empty(len(f), dtype=np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+    frec["n"] = 3
+    frec["i"] = f
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}"]
+    head += [f"property {'float' if t == '<f4' else 'uchar'} {n}" for n, t in props]
+    head += [f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(vrec.tobytes())
+        fh.write(frec.tobytes())

@@ -8,6 +8,7 @@ A "row view" is a 2-D (rows, C) or 3-D (batch, rows, C) tensor whose last stride
 projection or the rows behind a sequence's first token; its row and batch strides are read from .stride(), and a batch
 stride of 0 (expand) shares one matrix across the batch.
 """
+import math
 from typing import Optional, Tuple
 
 import numpy as np
@@ -1191,3 +1192,85 @@ def point_diameter(pts: Tensor) -> Tensor:
     d2 = torch.empty(1, dtype=torch.float32, device=pts.device)
     _lib.call("sam6d_point_diameter", pts, pts.shape[0], d2)
     return d2
+
+
+# ---------------------------------------------------------------------------------------------- TSDF fusion (fusion.py)
+TSDF_MAX_DIM = 512              # voxels per side that sam6d_tsdf_integrate / sam6d_tsdf_mesh_* accept
+
+
+def _tsdf_volume(tsdf: Tensor, weight: Tensor, csum: Tensor, ccount: Tensor):
+    """the volume's four fields -> (nz, ny, nx).  csum holds the u32 colour sums in an int32 tensor (the same bits)."""
+    _check(tsdf, torch.float32, "tsdf", 3)
+    _check(weight, torch.int32, "weight", 3)
+    _check(csum, torch.int32, "csum", 4)
+    _check(ccount, torch.int32, "ccount", 3)
+    dims = tuple(tsdf.shape)
+    if tuple(weight.shape) != dims or tuple(ccount.shape) != dims or tuple(csum.shape) != dims + (3,):
+        raise RuntimeError(f"tsdf volume: tsdf, weight, ccount (nz,ny,nx) and csum (nz,ny,nx,3), got {dims}, {tuple(weight.shape)}, "
+                           f"{tuple(ccount.shape)}, {tuple(csum.shape)}")
+    if min(dims) < 2 or max(dims) > TSDF_MAX_DIM:
+        raise RuntimeError(f"tsdf volume: every side in [2, {TSDF_MAX_DIM}] voxels, got {dims}")
+    return dims
+
+
+def _tsdf_box(bbox_min, voxel: float):
+    b = [float(x) for x in bbox_min]
+    if len(b) != 3 or not all(math.isfinite(x) for x in b):
+        raise RuntimeError(f"tsdf volume: bbox_min must be 3 finite numbers, got {bbox_min}")
+    if not (math.isfinite(voxel) and voxel > 0):
+        raise RuntimeError(f"tsdf volume: voxel must be finite and > 0, got {voxel}")
+    return b
+
+
+def tsdf_integrate(rgb: Tensor, depth: Tensor, mask: Optional[Tensor], K: Tensor, pose: Tensor, tsdf: Tensor, weight: Tensor,
+                   csum: Tensor, ccount: Tensor, bbox_min, voxel: float, trunc: float, znear: float):
+    """fuse T views into the volume in place (the rule: include/sam6d_b200.h, sam6d_tsdf_integrate).  rgb (T,H,W,3) u8, depth
+    (T,H,W) f32 mm (0 = missing), mask (T,H,W) u8 or None, K (T,4) f32 fx, fy, cx, cy, pose (T,12) f32 object -> camera (R
+    row-major, t mm); tsdf (nz,ny,nx) f32, weight i32, csum (nz,ny,nx,3) int32 holding u32 sums, ccount i32; bbox_min (3,)
+    the lattice's lower corner in mm, voxel, trunc in mm"""
+    nz, ny, nx = _tsdf_volume(tsdf, weight, csum, ccount)
+    _check(rgb, torch.uint8, "rgb", 4)
+    _check(depth, torch.float32, "depth", 3)
+    _check(K, torch.float32, "K", 2)
+    _check(pose, torch.float32, "pose", 2)
+    T, H, W = depth.shape
+    if T < 1 or H < 1 or W < 1 or tuple(rgb.shape) != (T, H, W, 3) or tuple(K.shape) != (T, 4) or tuple(pose.shape) != (T, 12):
+        raise RuntimeError(f"tsdf_integrate: rgb (T,H,W,3), depth (T,H,W), K (T,4), pose (T,12) with T, H, W >= 1, got "
+                           f"{tuple(rgb.shape)}, {tuple(depth.shape)}, {tuple(K.shape)}, {tuple(pose.shape)}")
+    if mask is not None:
+        _check(mask, torch.uint8, "mask", 3)
+        if tuple(mask.shape) != (T, H, W):
+            raise RuntimeError(f"tsdf_integrate: mask (T,H,W) = {(T, H, W)}, got {tuple(mask.shape)}")
+    if not bool(torch.isfinite(pose).all()) or not bool(torch.isfinite(K).all()):
+        raise RuntimeError("tsdf_integrate: K and pose must be finite")
+    b = _tsdf_box(bbox_min, float(voxel))
+    if not (math.isfinite(float(trunc)) and float(trunc) > 0) or not math.isfinite(float(znear)):
+        raise RuntimeError(f"tsdf_integrate: trunc must be finite and > 0 and znear finite, got {trunc}, {znear}")
+    _lib.call("sam6d_tsdf_integrate", rgb, depth, mask, K, pose, T, H, W, b[0], b[1], b[2], float(voxel), float(trunc), float(znear),
+              nx, ny, nz, tsdf, weight, csum, ccount)
+
+
+def tsdf_mesh(tsdf: Tensor, weight: Tensor, csum: Tensor, ccount: Tensor, bbox_min, voxel: float, min_weight: int = 1):
+    """marching tetrahedra over the volume (the rule: include/sam6d_b200.h, sam6d_tsdf_mesh_count / _emit) -> (verts (V,3) f32 mm,
+    colours (V,3) u8, faces (F,3) i32) on the device.  The prefix sums are torch.cumsum; one device-to-host copy reads the two
+    totals that size the outputs."""
+    nz, ny, nx = _tsdf_volume(tsdf, weight, csum, ccount)
+    b = _tsdf_box(bbox_min, float(voxel))
+    if int(min_weight) < 1:
+        raise RuntimeError(f"tsdf_mesh: min_weight must be >= 1 (a corner no view saw has no distance), got {min_weight}")
+    dev = tsdf.device
+    N, ncube = nx * ny * nz, (nx - 1) * (ny - 1) * (nz - 1)
+    emask = torch.empty(N, dtype=torch.int32, device=dev)
+    vcount = torch.empty(N, dtype=torch.int32, device=dev)
+    tcount = torch.empty(ncube, dtype=torch.int32, device=dev)
+    _lib.call("sam6d_tsdf_mesh_count", tsdf, weight, nx, ny, nz, int(min_weight), emask, vcount, tcount)
+    voff = torch.cumsum(vcount, 0, dtype=torch.int32)
+    toff = torch.cumsum(tcount, 0, dtype=torch.int32)
+    V, F = (int(x) for x in torch.stack([voff[-1], toff[-1]]).cpu())
+    verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
+    cols = torch.empty(V, 3, dtype=torch.uint8, device=dev)
+    faces = torch.empty(F, 3, dtype=torch.int32, device=dev)
+    if V > 0 and F > 0:
+        _lib.call("sam6d_tsdf_mesh_emit", tsdf, weight, csum, ccount, nx, ny, nz, b[0], b[1], b[2], float(voxel), int(min_weight),
+                  emask, voff, toff, verts, cols, faces)
+    return verts, cols, faces
